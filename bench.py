@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Benchmark of the PFN training hot path on B200 (contract: see task statement / DESIGN.md section "Measurement").
+"""Benchmark of the PFN training hot path on H100 (see DESIGN.md section "Measurement").
 
     python bench.py --gpus 1 --steps 6 --warmup 3                 # this repo's CUDA engine (default), config cfg2
     python bench.py --config cfg3|cfg4 ...                         # the other single-GPU BASELINE.json configurations
     torchrun --nproc-per-node N ... bench.py --gpus N ...          # data parallel, one rank per GPU
     python bench.py --impl reference --steps 3 --warmup 1          # the UNMODIFIED reference train.train on the host cores
+    python bench.py ... --dump-outputs DIR                         # also write the last timed step's outputs as DIR/*.npy
 
 One "step" = one full training step on one batch of synthetic prior data, driven through the public API
 (`train.build_trainer(...)` -> `Trainer.step`, batches from the prior's `DataLoader`):
@@ -38,14 +39,16 @@ CONFIGS = {
     # configs[2]: BNN tabular prior, 18 features, 12 layers, binary classification head
     "cfg3": dict(prior="mlp", T=512, F=18, E=512, H=4, nhid=1024, L=12, n_out=1, head="bce", sep=256, batch=512,
                  prior_kwargs={"batch_size_per_gp_sample": 8}),
-    # configs[3]: mixture-of-GPs hyperprior, seq_len 2000, 512 datasets per GPU (4096 global on 8 GPUs)
-    "cfg4": dict(prior="fast_gp_mix", T=2000, F=1, E=512, H=4, nhid=1024, L=6, n_out=100, head="bar", sep=1000, batch=512,
+    # configs[3]: mixture-of-GPs hyperprior, seq_len 2000; 256 datasets per GPU (2048 global on 8 GPUs): the activations kept
+    # for the backward at 512 per GPU (~75 GiB) do not fit an 80 GB H100 next to the step's temporaries
+    "cfg4": dict(prior="fast_gp_mix", T=2000, F=1, E=512, H=4, nhid=1024, L=6, n_out=100, head="bar", sep=1000, batch=256,
                  prior_kwargs={"batch_size_per_gp_sample": 64, "hyperparameters": {"fast_computations": (False, False, False)}}),
 }
 
 
 def step_flops(T, B, F, E, nhid, L, n_out, sep):
-    """Algorithmic (mask-aware) FLOPs of one training step, SURVEY.md section 8d."""
+    """Algorithmic (mask-aware) FLOPs of one training step: forward + backward (3x) of the dense layers, the masked attention
+    (sep train keys per row, plus its own key for each of the T - sep query rows), the decoder on the query rows and the embedding."""
     dense = T * B * L * (8 * E * E + 4 * E * nhid)
     attn = 4 * E * B * L * (T * sep + (T - sep))
     dec = (T - sep) * B * (2 * E * nhid + 2 * nhid * n_out)
@@ -59,7 +62,7 @@ def load_peaks():
         p = json.load(open(path))
         return dict(bf16_sustained=p.get("bf16_tflops_sustained"), bf16_burst=p.get("bf16_tflops"), hbm=p.get("hbm_gbs"),
                     source="MEASURED_PEAKS.json (measured)")
-    return dict(bf16_sustained=1400.0, bf16_burst=1590.0, hbm=6650.0, source="B200_PROFILING.md fallback")
+    return dict(bf16_sustained=989.0, bf16_burst=989.0, hbm=3350.0, source="H100 SXM data sheet (dense bf16, 700 W), not measured")
 
 
 class ClockSampler:
@@ -261,6 +264,22 @@ def gpu_eager_baseline(name, cfg, batch, dev, steps=4, warmup=2):
     return out
 
 
+DUMP_SAMPLE = 1 << 18          # elements kept of a larger output (fixed, seeded positions): 12 layers stay under 64 MB
+
+
+def dump_outputs(path, arrays):
+    """Writes each array as <path>/<name>.npy in float32; an array of more than DUMP_SAMPLE elements is reduced to a fixed,
+    seeded sample of its flattened elements, so that two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().float().flatten().cpu()
+        if t.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            t = t[torch.randperm(t.numel(), generator=g)[:DUMP_SAMPLE].sort().values]
+        np.save(os.path.join(path, name + ".npy"), t.numpy())
+
+
 def run_engine(args):
     import transformerscandobayesianinference_b200 as pkg
     from transformerscandobayesianinference_b200 import _lib as L, bar_distribution, encoders, parallel, priors, train as T_
@@ -287,9 +306,12 @@ def run_engine(args):
     sep = cfg["sep"]
     batches = iter(tr.dl)                                        # prefetching loader: next batch sampled on a side stream
 
+    last = {}
+
     def train_step():
         data, targets = next(batches)
-        loss, _ = tr.step(data, targets, sep)
+        loss, losses = tr.step(data, targets, sep)
+        last["loss"], last["losses"] = loss, losses
         return loss
 
     def barrier():
@@ -320,6 +342,10 @@ def run_engine(args):
     L.reset_launch_count()
     L.PROFILE_GEMM = [] if rank == 0 else None
     ms = timed(train_step, args.steps)
+    if args.dump_outputs and rank == 0:
+        # what the last timed step returned (loss, per-target losses) and the parameters its optimizer step produced
+        dump_outputs(args.dump_outputs, dict(loss=last["loss"], losses=last["losses"],
+                                             **{"param." + n: p for n, p in tr.model.named_parameters()}))
     gemm_prof_concurrent = L.PROFILE_GEMM
     L.PROFILE_GEMM = None
     launches = L.launch_count()
@@ -387,28 +413,16 @@ def run_engine(args):
         return
     flops = step_flops(cfg["T"], B, cfg["F"], cfg["E"], cfg["nhid"], cfg["L"], cfg["n_out"], sep)
     achieved_step = flops * args.steps / (ms / 1e3) / 1e12
-    # dominant kernel: the tcgen05 GEMM (all dense-layer launches of the timed region, CUDA events on the launch stream)
+    # dominant kernel: the wgmma GEMM (all dense-layer launches of the timed region, CUDA events on the launch stream)
     g_flops = sum(r[0] for r in gemm_prof)
     g_ms = sum(r[1].elapsed_time(r[2]) for r in gemm_prof)
     gemm_tf = g_flops / (g_ms / 1e3) / 1e12 if g_ms > 0 else None
     gc_ms = sum(r[1].elapsed_time(r[2]) for r in gemm_prof_concurrent)
     gemm_tf_concurrent = sum(r[0] for r in gemm_prof_concurrent) / (gc_ms / 1e3) / 1e12 if gc_ms > 0 else None
-    # DRAM traffic of the same kernel from the committed `ncu --set full` capture of this command (profiles/, not measured live)
-    traffic, traffic_src, traffic_alg = None, None, None
-    for tname in ("r2_gemm_traffic.json", "r1_gemm_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if os.path.exists(tpath) and name == "cfg2" and B == cfg["batch"] and args.precision == "bf16":
-            with open(tpath) as f:
-                tj = json.load(f)
-            traffic, traffic_src = tj["mean_dram_bytes_per_launch"], "profiles/" + tname
-            traffic_alg = tj.get("mean_algorithmic_bytes_per_launch")
-            break
     g_bytes = sum(r[3] for r in gemm_prof)
-    roofline = {"bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 GEMM, all launches of the timed steps)",
+    roofline = {"bound": "tensor", "kernel": "gemm_tc_kernel (wgmma GEMM, all launches of the timed steps)",
                 "achieved": gemm_tf, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
                 "frac": (gemm_tf / peaks["bf16_sustained"]) if gemm_tf else None,
-                "traffic": traffic, "traffic_unit": "bytes/launch (dram read+write, mean over the captured launches)",
-                "traffic_source": traffic_src, "traffic_algorithmic": traffic_alg,
                 "algorithmic_bytes_per_launch": g_bytes / max(len(gemm_prof), 1),
                 "launches": len(gemm_prof), "kernel_ms_per_step": g_ms / n_roof, "peak_source": peaks["source"] + ", sustained bf16",
                 "measured_in": f"{n_roof} extra steps with the prior sampled on the main stream ({ms_roof / n_roof:.2f} ms/step): nothing else runs "
@@ -459,11 +473,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="cfg2", choices=sorted(CONFIGS))
-    ap.add_argument("--batch", type=int, default=None, help="per-GPU batch (default: the config's 512)")
+    ap.add_argument("--batch", type=int, default=None, help="per-GPU batch (default: the config's)")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--ref-batch", type=int, default=4, help="bounded CPU sample: sequences per CPU step")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss, per-target losses and updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
     # The contract is ONE JSON line on stdout.  Libraries write there too (NCCL prints its version banner on fd 1 when
     # NCCL_DEBUG is set), so fd 1 points at stderr while the run is in progress and the line goes to the saved descriptor.

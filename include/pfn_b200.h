@@ -1,5 +1,5 @@
 /*
- * pfn_b200.h — C ABI of libpfn_b200.so, the sm_100a kernel library behind the PFN training hot path
+ * pfn_b200.h — C ABI of libpfn_b200.so, the sm_90a kernel library behind the PFN training hot path
  * (prior sample -> masked-attention transformer fwd+bwd -> BarDistribution NLL).
  *
  * The reference (automl/TransformersCanDoBayesianInference @ 9c20031) has no FFI of its own: its hot path is
@@ -39,16 +39,16 @@ int pfn_num_sms(void);
  *   K-major operand : element (i,k) at base + i*ld + k;   MN-major operand : element (i,k) at base + k*ld + i
  *   epilogue GELU      : C = gelu_erf(acc+bias), optional C2 = acc+bias (pre-activation, saved for backward)
  *   epilogue GELU_BWD  : C = acc * gelu_erf'(aux)
- *   epilogue MUL       : C = acc * aux   (tcgen05 path only).  With GELU's c2_gelu_grad = 1 the forward stores gelu'(pre)
+ *   epilogue MUL       : C = acc * aux   (tensor-core path only).  With GELU's c2_gelu_grad = 1 the forward stores gelu'(pre)
  *                        in C2 instead of the pre-activation, and the backward dgrad is this plain product: the ~14
  *                        instructions per element of gelu' leave the backward epilogue, whose cost is instruction issue.
  *   epilogue ROWDOT    : C = acc (+bias), and rowdot_out[m * ceil(N / rowdot_width) + n / rowdot_width] += sum over the
  *                        column group of C[m,n] * aux[m,n]   (fp32 atomics; aux is NOT added to C).  Used to produce
- *                        delta = rowsum(dO * O) per (token, head) in the out-projection dgrad (tcgen05 path only).
+ *                        delta = rowsum(dO * O) per (token, head) in the out-projection dgrad (tensor-core path only).
  *   accumulate / k_splits>1 : atomic fp32 accumulation into C (weight gradients)
  * Replaces: nn.Linear / in_proj / out_proj / linear1 / linear2 / decoder GEMMs and their autograd backward
  *   (reference transformer.py:17-18,23,84-85; torch:nn/functional.py:6478; torch:nn/modules/transformer.py:980-982).
- * pfn_gemm_bf16_tc : tcgen05 + TMA + TMEM path (bf16 operands; lda/ldb multiples of 8; 16-byte aligned bases).
+ * pfn_gemm_bf16_tc : TMA + wgmma path (bf16 operands; lda/ldb multiples of 8; 16-byte aligned bases).
  * pfn_gemm_simt    : fp32-FMA path for fp32 parity mode and shapes the tensor-core path does not take.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct pfn_gemm_desc {
@@ -65,7 +65,7 @@ typedef struct pfn_gemm_desc {
   int ab_dtype;            /* dtype of A, B, aux, C2 (simt path; the tc path is bf16 only) */
   float* rowdot_out;       /* epilogue ROWDOT: [M, ceil(N / rowdot_width)] fp32, accumulated (zero it first) */
   int rowdot_width;        /* columns per group (the head dimension); must be a multiple of 128 */
-  int c2_gelu_grad;        /* epilogue GELU with C2, tcgen05 path only: 1 = C2 receives gelu'(acc+bias) instead of acc+bias */
+  int c2_gelu_grad;        /* epilogue GELU with C2, tensor-core path only: 1 = C2 receives gelu'(acc+bias) instead of acc+bias */
 } pfn_gemm_desc;
 
 int pfn_gemm_bf16_tc(const pfn_gemm_desc* d, void* stream);
@@ -89,17 +89,17 @@ typedef struct pfn_attn_desc {
   const void* dout; int ld_dout;
   void* dqkv; int ld_dqkv;
   float* delta;            /* [B*H, T] fp32 scratch for backward: rowsum(dO * O) */
-  int batch_major;         /* 0: token row = t*B + b (reference layout); 1: token row = b*T + t (tcgen05 kernels only) */
+  int batch_major;         /* 0: token row = t*B + b (reference layout); 1: token row = b*T + t (tensor-core kernels only) */
   /* dropout on the attention probabilities (torch:nn/functional.py multi_head_attention_forward `dropout_p`; reference
    * train.py:22 default 0.2): drop_thr = round(256 p) in [0,255], 0 = off; the keep bit of (row i, key j) of head (b,h) is
    * pfn_dropout_keep_mask's bit for (row = (b*H + h)*T + i, col = j) under drop_seed. */
   uint32_t drop_seed;
   int drop_thr;
-  /* backward, tcgen05 kernels only, optional: dq_colsum[H*dh] += column sums of dQ (the q third of the in-projection bias
+  /* backward, tensor-core kernels only, optional: dq_colsum[H*dh] += column sums of dQ (the q third of the in-projection bias
    * gradient), accumulated from the staged dQ tiles so that dqkv need not be re-read.  (The k third is zero in exact
    * arithmetic -- every row of dS sums to zero -- and the v third equals colsum(dO) = colsum(dz) W_out; see engine.py.) */
   float* dq_colsum;
-  /* backward, tcgen05 kernels only: 1 = `delta` already holds rowsum(dO * O) in TOKEN-major layout [T*B, H] (produced by the
+  /* backward, tensor-core kernels only: 1 = `delta` already holds rowsum(dO * O) in TOKEN-major layout [T*B, H] (produced by the
    * ROWDOT epilogue of the out-projection dgrad GEMM); the kernels then skip their own delta pass.  0 = `delta` is [B*H, T]
    * scratch that the backward fills itself. */
   int delta_token_major;
@@ -109,8 +109,6 @@ int pfn_attention_fwd_simt(const pfn_attn_desc* d, void* stream);
 int pfn_attention_bwd_simt(const pfn_attn_desc* d, void* stream);
 int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream);
 int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream);
-/* debug: clock64 event log of CTA 0 of subsequent tcgen05 attention launches ([3][cap][4] int64; which: 0 fwd, 1 dq, 2 dkv; null = off) */
-int pfn_debug_attention_trace(long long* buf, int cap, int which);
 
 /* ------------------------------------------------------------------------------------------------
  * Embedding stage (reference transformer.py:68-74):

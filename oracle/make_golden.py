@@ -1,7 +1,7 @@
 """Generate the golden fixtures under tests/golden/ by running the UNMODIFIED reference modules
 (/root/reference/{transformer,bar_distribution,utils}.py) on CPU under this container's torch.
 
-Run here (the GPU box has no /root/reference):   python oracle/make_golden.py
+Run where the reference checkout exists:   python oracle/make_golden.py   (host-side fixtures: ... make_golden.py host)
 The fixtures are small: inputs, seeds and reference OUTPUTS only — model weights are re-created from the recorded
 seed by `build_case_weights` (same torch version on both boxes), and a per-tensor checksum of the reference's
 state_dict is stored so that tests can prove they rebuilt exactly the same weights.
@@ -230,5 +230,76 @@ def main():
     print("golden fixtures written to", OUT)
 
 
+# ---- host-side mirrors (positional_encodings.py, utils.py) and the shipped checkpoints' layouts: what the tests compare
+# this repo's modules against, recorded from the unmodified reference modules so that the tests need no reference checkout.
+POSENC_CLASSES = ("NoPositionalEncoding", "PositionalEncoding", "LearnedPositionalEncoding", "PairedScrambledPositionalEncodings")
+
+
+def posenc_record(mod):
+    """Same seed -> initial state, output and RNG consumption of every positional-encoding class of `mod`."""
+    torch.manual_seed(3)
+    x = torch.randn(7, 3, 12)
+    out = {}
+    for name in POSENC_CLASSES:
+        torch.manual_seed(11)
+        a = getattr(mod, name)(12, 20)
+        state = {k: v.detach().clone() for k, v in a.state_dict().items()}
+        torch.manual_seed(5)
+        y = a(x).detach()
+        torch.manual_seed(5)
+        a(x)
+        out[name] = {"keys": list(state), "state": state, "y": y, "rng_after": torch.rand(4)}
+    return out
+
+
+def utils_record(mod):
+    """Every step of both LR schedules, the single_eval_pos sampler streams and SeqBN of `mod`."""
+    lrs = {}
+    for warm, total, cycles in [(0, 10, 0.5), (3, 10, 0.5), (5, 40, 1.5), (10, 10, 0.5)]:
+        for fn, kw in (("get_cosine_schedule_with_warmup", dict(num_cycles=cycles)), ("get_linear_schedule_with_warmup", {})):
+            opt = torch.optim.SGD([torch.nn.Parameter(torch.zeros(1))], lr=0.7)
+            sch = getattr(mod, fn)(opt, warm, total, **kw)
+            cur = []
+            for _ in range(total + 5):
+                cur.append(sch.get_last_lr()[0]); opt.step(); sch.step()
+            lrs[f"{fn}/{warm}/{total}"] = cur
+    samplers = {}
+    for n in (1, 2, 37):
+        for fn in ("get_weighted_single_eval_pos_sampler", "get_uniform_single_eval_pos_sampler"):
+            random.seed(n)
+            samplers[f"{fn}/{n}"] = [getattr(mod, fn)(n)() for _ in range(3)] + [f() for f in [getattr(mod, fn)(n)] for _ in range(20)]
+    torch.manual_seed(0)
+    sb = mod.SeqBN(6)
+    torch.manual_seed(1)
+    x = torch.randn(5, 4, 6)
+    return {"lrs": lrs, "samplers": samplers, "seqbn_keys": list(sb.state_dict()),
+            "seqbn_state": {k: v.detach().clone() for k, v in sb.state_dict().items()}, "seqbn_y": sb(x).detach()}
+
+
+def host_goldens():
+    sys.path.insert(0, ROOT)
+    sys.path.insert(0, REF)
+    rec = {"posenc": posenc_record(_load_ref("positional_encodings")), "utils": utils_record(_load_ref("utils")),
+           "checkpoints": {}}
+    res = os.path.join(REF, "results")
+    for fn in sorted(os.listdir(res)):
+        sd = torch.load(os.path.join(res, fn), map_location="cpu", weights_only=False)[0]
+        rec["checkpoints"][fn] = {k: tuple(v.shape) for k, v in sd.items()}
+    # statistics of one batch of the reference BNN prior (priors/mlp.py through oracle/_ref) per seed of tests/test_mlp_prior.py
+    from oracle import ref_runner
+    spec = importlib.util.spec_from_file_location("_pfn_test_mlp_prior", os.path.join(ROOT, "tests", "test_mlp_prior.py"))
+    tm = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(tm)
+    mods = ref_runner.load()
+    rec["mlp_prior"] = {}
+    for seed in (1, 2):
+        tm._seed(seed)
+        x, y, _ = mods["priors"].mlp.get_batch(tm.B, tm.T, tm.F, device="cpu", hyperparameters=tm._hp(mods["priors"].utils),
+                                                batch_size_per_gp_sample=tm.G)
+        rec["mlp_prior"][seed] = tm._stats(x, y)
+    torch.save(rec, os.path.join(OUT, "host_reference.pt"))
+    print("host golden fixtures written to", OUT)
+
+
 if __name__ == "__main__":
-    main()
+    host_goldens() if sys.argv[1:] == ["host"] else main()

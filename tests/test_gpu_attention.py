@@ -1,4 +1,4 @@
-"""Masked attention kernels (fp32-FMA and tcgen05) vs the dense-mask oracle."""
+"""Masked attention kernels (fp32-FMA and tensor-core) vs the dense-mask oracle."""
 import pytest
 import torch
 
@@ -40,8 +40,8 @@ def test_attention_simt_fwd_bwd(cuda_device, dtype, T, B, H, dh, sep):
     assert err <= (5e-5 if dtype == torch.float32 else 5e-2) * (qr.grad.abs().max().item() + 1e-6), err
 
 
-# the last two cases give every persistent CTA SEVERAL tiles (B*H*ceil(T/128) = 384 / 320 work items > 148 SMs): the
-# multi-tile-per-CTA paths (barrier phase wrap-around, prefetch across tiles) must fail here in seconds, not only in
+# ragged tails (T, sep not multiples of the 64-row tiles / key blocks), sep = 0 and sep = T - 1, and in the last two cases
+# more CTAs (B*H*ceil(T/64)) than the GPU holds at once: a tiling error must fail here in seconds, not only in
 # tests/test_gpu_fullsize.py
 TC_CASES = [(128, 1, 1, 64), (256, 2, 2, 128), (200, 2, 4, 100), (1000, 2, 4, 500), (130, 1, 2, 0), (300, 3, 1, 299),
             (64, 2, 1, 64), (513, 1, 2, 257), (384, 32, 4, 200), (640, 16, 4, 300)]

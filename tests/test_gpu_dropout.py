@@ -109,7 +109,7 @@ def test_default_train_arguments_run_with_dropout(cuda_device):
 
 @pytest.mark.parametrize("T,B,H,sep,p", [(200, 2, 2, 100, 0.5), (384, 8, 4, 200, 0.2), (130, 1, 2, 0, 0.5), (256, 2, 1, 255, 0.2)])
 def test_tcgen05_attention_with_probability_dropout(cuda_device, T, B, H, sep, p):
-    """tcgen05 forward / dQ / dK,dV kernels (bf16, head dim 128) with dropout on the probabilities vs the dense fp64 oracle
+    """tensor-core forward / dQ / dK,dV kernels (bf16, head dim 128) with dropout on the probabilities vs the dense fp64 oracle
     that consumes the same keep mask: O = (softmax(S) m / (1-p)) V and its exact gradients."""
     dev = cuda_device
     torch.manual_seed(T + sep)
@@ -148,7 +148,7 @@ def test_tcgen05_attention_with_probability_dropout(cuda_device, T, B, H, sep, p
 
 
 def test_bf16_engine_training_step_with_dropout_on_tensor_cores(cuda_device):
-    """Whole bf16 step (tcgen05 GEMMs + tcgen05 attention, head dim 128) with dropout 0.5: loss within 1e-2 of the
+    """Whole bf16 step (wgmma GEMMs + tensor-core attention, head dim 128) with dropout 0.5: loss within 1e-2 of the
     mask-consuming fp64 oracle, gradient norms within 8 %."""
     dev = cuda_device
     T, B, F, E, H, nhid, NL, n_out, sep, p = 160, 4, 1, 256, 2, 512, 2, 20, 96, 0.5

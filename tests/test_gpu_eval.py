@@ -1,4 +1,4 @@
-"""Inference / evaluation path on the GPU (SURVEY.md section 8f rows 1, 2 and 4): BarDistribution helpers on device tensors
+"""Inference / evaluation path on the GPU: BarDistribution helpers on device tensors
 against the reference goldens, DataLoader.validate, the exact-GP baseline `fast_gp.evaluate`, and the other heads /
 encoders (BCE, CE + class-embedding y-encoder, positional encodings, wide feature encoder) through the CUDA stack."""
 import os

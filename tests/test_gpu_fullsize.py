@@ -16,7 +16,7 @@ DH = E // H
 
 
 def test_attention_fullsize_slices_match_oracle(cuda_device):
-    """tcgen05 attention fwd+bwd on the full [T*B, 3E] tensor; three (batch, head) slices re-done by the dense-mask oracle."""
+    """tensor-core attention fwd+bwd on the full [T*B, 3E] tensor; three (batch, head) slices re-done by the dense-mask oracle."""
     torch.manual_seed(11)
     qkv = torch.randn(T * B, 3 * E, device=cuda_device).to(torch.bfloat16)
     out = torch.empty(T * B, E, device=cuda_device, dtype=torch.bfloat16)
@@ -42,7 +42,7 @@ def test_attention_fullsize_slices_match_oracle(cuda_device):
 
 
 def test_gemm_fullsize_rows_match_reference(cuda_device):
-    """512000 x 1536 x 512 projection (cta_group::2 tcgen05 path): random output rows against fp64 dot products."""
+    """512000 x 1536 x 512 projection (wgmma path): random output rows against fp64 dot products."""
     torch.manual_seed(12)
     N = T * B
     x = torch.randn(N, E, device=cuda_device).to(torch.bfloat16)

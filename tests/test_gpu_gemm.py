@@ -1,4 +1,4 @@
-"""tcgen05 / SIMT GEMM vs a torch fp32 reference of the same (bf16-rounded) operands."""
+"""wgmma / SIMT GEMM vs a torch fp32 reference of the same (bf16-rounded) operands."""
 import pytest
 import torch
 
@@ -90,7 +90,7 @@ def test_gemm_tc_epilogues(cuda_device):
     L.gemm(A, B, C, aux=aux, epilogue=L.EPI_GELU_BWD, use_tc=True)
     ref, _ = _ref(A, B, False, False, None, aux, L.EPI_GELU_BWD)
     assert (C.float() - ref).abs().max().item() <= 2e-2 * ref.abs().max().item()
-    # gelu'(pre) in C2 (forward) + plain product with it (backward): the pair that replaces GELU_BWD on the tcgen05 path
+    # gelu'(pre) in C2 (forward) + plain product with it (backward): the pair that replaces GELU_BWD on the tensor-core path
     L.gemm(A, B, C, bias=bias, C2=C2, epilogue=L.EPI_GELU, c2_gelu_grad=True, use_tc=True)
     ref, pre = _ref(A, B, False, False, bias, None, L.EPI_GELU)
     cdf = 0.5 * (1 + torch.erf(pre / 2 ** 0.5))
@@ -172,8 +172,8 @@ def test_gemm_simt(cuda_device, dtype, M, N, K, a_mn, b_mn):
                                         (300, 96, 64, False), (129, 328, 128, True)])
 @pytest.mark.parametrize("epi", ["add", "mul"])
 def test_gemm_tc_aux_through_staging(cuda_device, M, N, K, b_mn, epi):
-    """aux tiles (residual / multiplier) reach the epilogue by TMA through the output staging buffer: many tiles per CTA (barrier
-    phases), ragged M and N (zero-filled boxes, clipped stores), padded aux / C leading dimensions, narrow and wide tiles."""
+    """aux (residual / multiplier) read by the epilogue next to the accumulator: many tiles and k-blocks (ring phases), ragged
+    M and N (zero-filled boxes, masked stores), padded aux / C leading dimensions, N narrower and wider than one tile."""
     torch.manual_seed(M + N)
     A = _operand(M, K, False, torch.bfloat16, cuda_device)
     B = (_operand(N, K, b_mn, torch.bfloat16, cuda_device).float() * K ** -0.5).to(torch.bfloat16)

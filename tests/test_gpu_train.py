@@ -36,7 +36,7 @@ def test_fast_gp_get_batch_contract_and_covariance(cuda_device):
 def test_gp_sampler_factorises_the_cfg2_kernel_without_jitter(cuda_device, Bn):
     """The BASELINE cfg-2 kernel matrix (1000 points, RBF lengthscale 0.6, noise 1e-4) has a condition number near 1e7: the
     factorisation must go through in fp32 with NO failing pivot and no jitter (a 3xTF32 tensor-core variant of the update with
-    an explicit-inverse panel solve failed 2-4 % of such datasets and was backed out: profiles/r2_gp_sampler_ablation.md)."""
+    an explicit-inverse panel solve failed 2-4 % of such datasets and was backed out)."""
     from transformerscandobayesianinference_b200 import _lib as L
     T = 1000
     ls = torch.full((Bn, 1), .6, device=cuda_device); os_ = torch.ones(Bn, device=cuda_device)

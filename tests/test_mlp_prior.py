@@ -1,13 +1,13 @@
-"""priors.mlp (BNN tabular prior) against the UNMODIFIED reference priors/mlp.py (oracle/_ref, vendored by oracle/build_ref.py):
-same host hyper-sampler stream, same per-dataset distribution.  The vectorised all-models-at-once formulation is checked on
+"""priors.mlp (BNN tabular prior) against the UNMODIFIED reference priors/mlp.py (statistics of its batches recorded in
+tests/golden/host_reference.pt by oracle/make_golden.py): same host hyper-sampler stream, same per-dataset distribution.  The vectorised all-models-at-once formulation is checked on
 CPU here (no kernels involved: it is batched torch ops) and on the GPU through the public `get_batch`."""
+import os
 import random
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import ref_runner as R
 from transformerscandobayesianinference_b200.priors import mlp, utils as su
 
 T, B, G, F = 64, 256, 8, 18
@@ -35,12 +35,9 @@ def _seed(s):
 
 
 def _reference_batch(seed):
-    if not R.available():
-        pytest.skip("oracle/_ref not built (run oracle/build_ref.py where /root/reference exists)")
-    mods = R.load()
-    _seed(seed)
-    x, y, _ = mods["priors"].mlp.get_batch(B, T, F, device='cpu', hyperparameters=_hp(mods["priors"].utils), batch_size_per_gp_sample=G)
-    return _stats(x, y)
+    """_stats of the reference prior's batch drawn after _seed(seed)."""
+    gold = os.path.join(os.path.dirname(__file__), "golden", "host_reference.pt")
+    return torch.load(gold, weights_only=False)["mlp_prior"][seed]
 
 
 def _check(ours, ref):

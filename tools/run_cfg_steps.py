@@ -42,7 +42,7 @@ which = sys.argv[1:] or ["cfg4", "cfg3"]
 if "cfg4" in which:
     run("cfg4 fast_gp_mix T=2000 B=512 L=6", priors.fast_gp_mix.get_batch, 2000, 512, 1, 6, 1000, batch_size_per_gp_sample=64)
 if "cfg3" in which:
-    su = priors.utils     # the shipped bnn config (TabularEvalSimple.ipynb:154-176 via SURVEY cfg 3)
+    su = priors.utils     # the shipped bnn config (TabularEvalSimple.ipynb:154-176)
     hp = (lambda: 3, su.scaled_beta_sampler_f(2, 4, 150, 2), torch.nn.Tanh, su.gamma_sampler_f(3.62, .0677),
           su.gamma_sampler_f(1.87, .0528), lambda: 0.0, True, su.scaled_beta_sampler_f(1, 1.6, 18, 2), None, False, None,
           None, None, True, True, lambda n: ([], []), 0.0)

@@ -1,4 +1,4 @@
-"""transformerscandobayesianinference_b200 — a B200-native (sm_100a) engine for the PFN training hot path of
+"""transformerscandobayesianinference_b200 — a H100-native (sm_90a) engine for the PFN training hot path of
 automl/TransformersCanDoBayesianInference, behind the reference's own Python module API.
 
     from transformerscandobayesianinference_b200 import train, transformer, bar_distribution, priors, encoders, utils

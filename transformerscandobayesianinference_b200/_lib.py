@@ -52,7 +52,6 @@ EXPORTED_SYMBOLS = [
     "pfn_last_error", "pfn_version", "pfn_num_sms",
     "pfn_gemm_bf16_tc", "pfn_gemm_simt",
     "pfn_attention_fwd_simt", "pfn_attention_bwd_simt", "pfn_attention_fwd_tc", "pfn_attention_bwd_tc",
-    "pfn_debug_attention_trace",
     "pfn_embed_fwd", "pfn_embed_bwd",
     "pfn_layernorm_fwd", "pfn_layernorm_bwd", "pfn_colsum",
     "pfn_bar_nll_fwd", "pfn_bar_nll_bwd", "pfn_bar_bucket_idx",
@@ -63,7 +62,7 @@ EXPORTED_SYMBOLS = [
 
 _lib = None
 _launches = 0          # kernel launches issued through this binding (bench.py reports it as gpu_launches)
-PROFILE_GEMM = None    # when a list: (flops, start_event, end_event, algorithmic operand+result bytes) is appended for every tcgen05 GEMM launch
+PROFILE_GEMM = None    # when a list: (flops, start_event, end_event, algorithmic operand+result bytes) is appended for every wgmma GEMM launch
 
 
 _NUM_SMS = {}
@@ -112,7 +111,6 @@ def load():
     lib.pfn_gemm_simt.argtypes = [ctypes.POINTER(GemmDesc), c_void_p]
     for n in ("pfn_attention_fwd_simt", "pfn_attention_bwd_simt", "pfn_attention_fwd_tc", "pfn_attention_bwd_tc"):
         getattr(lib, n).argtypes = [ctypes.POINTER(AttnDesc), c_void_p]
-    lib.pfn_debug_attention_trace.argtypes = [c_void_p, c_int, c_int]
     lib.pfn_embed_fwd.argtypes = [c_void_p] * 7 + [c_int] * 6 + [c_void_p]
     lib.pfn_embed_bwd.argtypes = [c_void_p, c_int] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p]
     lib.pfn_layernorm_fwd.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
@@ -187,7 +185,7 @@ def require_cuda(*tensors):
             continue
         if not t.is_cuda:
             raise RuntimeError(
-                "the PFN hot path runs on sm_100a CUDA kernels only; got a tensor on "
+                "the PFN hot path runs on sm_90a CUDA kernels only; got a tensor on "
                 f"{t.device}. Move the model and data to a CUDA device (no CPU fallback exists).")
         if dev is None:
             dev = t.device
@@ -315,7 +313,7 @@ def attention_fwd(qkv, out, lse, T, B, H, dh, sep, use_tc=None, batch_major=Fals
 @_guarded
 def attention_bwd(qkv, out, lse, dout, dqkv, delta, T, B, H, dh, sep, use_tc=None, batch_major=False, drop=None,
                   dq_colsum=None, delta_token_major=False):
-    """dq_colsum (fp32 [H*dh], tcgen05 path only): += column sums of dQ, taken from the staged tiles inside the kernel.
+    """dq_colsum (fp32 [H*dh], tensor-core path only): += column sums of dQ, taken from the staged tiles inside the kernel.
     delta_token_major: `delta` is a [T*B, H] tensor that already holds rowsum(dO * O) (GEMM ROWDOT epilogue)."""
     _count(2)
     lib = load()
@@ -324,10 +322,10 @@ def attention_bwd(qkv, out, lse, dout, dqkv, delta, T, B, H, dh, sep, use_tc=Non
     if use_tc is None:
         use_tc = tc_attention_ok(qkv, dh)
     if dq_colsum is not None:
-        assert use_tc, "dq_colsum is produced by the tcgen05 backward only"
+        assert use_tc, "dq_colsum is produced by the tensor-core backward only"
         d.dq_colsum = dq_colsum.data_ptr()
     if delta_token_major:
-        assert use_tc, "a precomputed token-major delta is consumed by the tcgen05 backward only"
+        assert use_tc, "a precomputed token-major delta is consumed by the tensor-core backward only"
         d.delta_token_major = 1
     fn = lib.pfn_attention_bwd_tc if use_tc else lib.pfn_attention_bwd_simt
     check(fn(ctypes.byref(d), stream_ptr()), "pfn_attention_bwd")

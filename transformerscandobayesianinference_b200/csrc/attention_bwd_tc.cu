@@ -1,32 +1,49 @@
-// tcgen05 backward of the single_eval_pos-masked attention (head dim 128, bf16), three kernels:
+// Tensor-core backward of the single_eval_pos-masked attention (head dim 128, bf16), three kernels:
 //
-//  (0) attn_bwd_delta_kernel   delta[b,h,i] = dO_i . O_i   (one warp per token row, HBM-bound, 16 B vectors)
+//  (0) attn_bwd_delta_kernel  delta[b,h,i] = dO_i . O_i   (one warp per token row, HBM-bound, 16 B vectors); skipped when
+//      the caller passes the token-major delta the out-projection dgrad's ROWDOT epilogue already produced
 //
-//  (1) attn_bwd_dq_tc_kernel   [attention_bwd_dq.cu] one CTA per (batch, head, 128-row query tile); blocks = 64-key blocks of the train keys
-//      followed by up to two "diagonal" blocks (the tile's own rows as keys; row i keeps only key i, cf. attention_tc.cu):
-//          S_j  = Q K_j^T          dP_j = dO V_j^T                      (SS MMAs, 128x64x128, TMEM double-buffered)
-//          dS_j = exp2(S_j c - lse) * (dP_j - delta) * scale   -> bf16 -> TMEM   (one thread per query row)
-//          dQ  += dS_j K_j                                                (TS MMA, K_j read MN-major from the same smem)
-//      For a query row the diagonal key is attended by that row only, so dK_i = dS_ii q_i and dV_i = P_ii dO_i are
-//      complete: the owning thread scales its own q / dO row (read back from the swizzled smem tiles) and stores them.
-//      Q and dO tiles are double-buffered so the next tile's loads overlap this tile's epilogue.
+//  (1) attn_bwd_dq_kernel     one CTA (4 warps) per (batch, head, 64-row query tile); loop over 64-key blocks of the train keys:
+//          S_j  = Q K_j^T      dP_j = dO V_j^T                                 (mma.sync, fp32)
+//          dS_j = exp2(S_j c - lse2) * (dP_j - delta) * scale  -> bf16 A fragments (registers)
+//          dQ  += dS_j K_j
+//      For a query row (i >= sep) the diagonal key is attended by that row only, so dK_i = dS_ii q_i and dV_i = P_ii dO_i are
+//      complete: the four lanes that own the row compute and store them, and add dS_ii k_i to dQ.
 //
-//  (2) attn_bwd_dkv_tc_kernel  one CTA per (batch, head, 128-key tile of the train keys), loop over 64-row blocks i:
-//          S^T_i = K Q_i^T         dP^T_i = V dO_i^T                      (lane = key, column = query row)
-//          P^T, dS^T -> bf16 -> TMEM ;  dV += P^T dO_i ;  dK += dS^T Q_i  (TS MMAs; Q_i / dO_i blocks read MN-major
-//                                                                          from the very smem bytes used K-major above)
+//  (2) attn_bwd_dkv_kernel    one CTA (4 warps) per (batch, head, 64-key tile of the train keys), loop over 32-row query blocks:
+//          S^T = K Q_i^T       dP^T = V dO_i^T     (row = key, column = query row)
+//          dV += (P^T . mask) dO_i ;   dK += dS^T Q_i
 //
-// Same warp roles / mbarrier protocol as the forward kernel (attention_tc.cu): warp 0 TMA, warp 1 MMA issue,
-// warps 2..5 one thread per TMEM lane.  All tiles come straight out of the packed [T*B, 3E] qkv / [T*B, E] dO
-// buffers through 3-D TMA maps (column, batch, time); no transposes, no atomics, deterministic.
-#include <stdlib.h>
-
-#include "attention_bwd_common.cuh"
-#include "dropout.cuh"
+// Q/K/V/dO rows come straight out of the packed [T*B, 3E] qkv / [T*B, E] dO buffers; no transposes, no atomics on dQKV.
+#include "attention_common.cuh"
 
 namespace pfn {
 
-int check_attn_desc_public(const pfn_attn_desc* d, bool bwd, const char* who);
+constexpr int AB_BM = 64;                                 // dQ kernel: query rows per CTA; key block size
+constexpr int AB_TILE = AB_BM * ATT_ROW_BYTES;            // 16 KB
+constexpr int AB_DQ_SMEM = 6 * AB_TILE;                   // Q + dO + 2 x K + 2 x V
+constexpr int AB_QB = 32;                                 // dK/dV kernel: query rows per block
+constexpr int AB_QTILE = AB_QB * ATT_ROW_BYTES;           // 8 KB
+constexpr int AB_DKV_SMEM = 2 * AB_TILE + 4 * AB_QTILE + 2 * 2 * AB_QB * 4;   // K + V + 2 x (Q, dO) + 2 x (lse2, delta)
+
+struct AttnBwdParams {
+  int T, B, H, sep;
+  float scale, scale_log2;
+  const __nv_bfloat16* qkv; int ld_qkv;
+  const __nv_bfloat16* dout; int ld_dout;
+  __nv_bfloat16* dqkv; int ld_dqkv;
+  const float* lse;
+  const float* delta;
+  int delta_tm;          // 1: delta is token-major [T*B, H] (GEMM ROWDOT epilogue); 0: [B*H, T]
+  float* dq_colsum;      // optional [H*dh]: += column sums of dQ
+  uint32_t drop_seed; int drop_thr;   // dropout on the attention probabilities (thr 0 = off), csrc/dropout.cuh
+  int n_tiles;
+  int batch_major;
+};
+
+__device__ __forceinline__ float ab_delta(const AttnBwdParams& p, int b, int h, int i) {
+  return p.delta_tm ? p.delta[att_tok(i, b, p.T, p.B, 0) * p.H + h] : p.delta[(static_cast<size_t>(b) * p.H + h) * p.T + i];
+}
 
 // =====================================================================================================================
 // Kernel 0: delta = rowsum(dO * O) per (batch, head, row)
@@ -46,7 +63,7 @@ attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ out, int ld_out, const _
       const int h = h0 + (lane >> 4);
       float acc = 0.f;
       if (h < H) {
-        const int col = h * AB_DH + (lane & 15) * 8;
+        const int col = h * ATT_DH + (lane & 15) * 8;
         const uint4 pa = *reinterpret_cast<const uint4*>(out + tok * ld_out + col);
         const uint4 pb = *reinterpret_cast<const uint4*>(dout + tok * ld_dout + col);
         const __nv_bfloat162* ha = reinterpret_cast<const __nv_bfloat162*>(&pa);
@@ -67,309 +84,301 @@ attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ out, int ld_out, const _
 }
 
 // =====================================================================================================================
-// Kernel 2: dK, dV of the train keys
+// Kernel 1: dQ (+ dK, dV of the query rows' own keys)
 // =====================================================================================================================
-__global__ void __launch_bounds__(AB_THREADS + 32, 1)
-attn_bwd_dkv_tc_kernel(const __grid_constant__ CUtensorMap tmQKV128, const __grid_constant__ CUtensorMap tmQKV64,
-                       const __grid_constant__ CUtensorMap tmDO64, const AttnBwdParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  // 1 KB alignment by an OFFSET on the __shared__ symbol (an integer round trip of the pointer makes every access through it a
-  // generic LD.E / ST.E instead of LDS / STS)
-  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sK = smem;
-  uint8_t* sV = smem + AB_TILE_BYTES;
-  uint8_t* sQD = smem + 2 * AB_TILE_BYTES;               // stage s: Q block at +s*32K, dO block at +16K
-  float* sStat = reinterpret_cast<float*>(smem + 2 * AB_TILE_BYTES + AB_KS * 2 * AB_BLK_BYTES);   // [2][2][64]: lse2, delta*scale
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * AB_TILE_BYTES + AB_KS * 2 * AB_BLK_BYTES + 1024);
-  uint64_t* kv_full = bars + 0;
-  uint64_t* kv_empty = bars + 1;
-  uint64_t* qd_full = bars + 2;                  // [AB_KS]
-  uint64_t* qd_empty = bars + 2 + AB_KS;         // [AB_KS]
-  uint64_t* st_full = bars + 2 + 2 * AB_KS;      // S^T / dP^T of a block are in TMEM (one phase per block)
-  uint64_t* s_consumed = st_full + 1;            // every row thread has read them into registers (one phase per block)
-  uint64_t* pds_ready = st_full + 2;             // [2] P^T / dS^T written (bf16, TMEM)
-  uint64_t* pd_free = st_full + 4;               // [2] the dV / dK MMAs that read that P^T / dS^T buffer are complete
-  uint64_t* acc_done = st_full + 6;
-  uint64_t* acc_empty = st_full + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(st_full + 8);
+__global__ void __launch_bounds__(128, 2)
+attn_bwd_dq_kernel(const AttnBwdParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint8_t* sQ = smem;
+  uint8_t* sD = smem + AB_TILE;
+  uint8_t* sK = smem + 2 * AB_TILE;                       // buffer s at + s * 16 KB
+  uint8_t* sV = smem + 4 * AB_TILE;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int qt = static_cast<int>(blockIdx.x) % p.n_tiles;
+  const int bh = static_cast<int>(blockIdx.x) / p.n_tiles;
+  const int h = bh % p.H, b = bh / p.H;
+  const int E = p.H * ATT_DH;
+  const int i0 = qt * AB_BM;
+  const int nblk = (p.sep + AB_BM - 1) / AB_BM;
+  const int r0 = 16 * warp;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int E = p.H * AB_DH;
+  att_load_tile<AB_BM>(sQ, p.qkv, p.ld_qkv, h * ATT_DH, i0, p.T, b, p.T, p.B, p.batch_major);
+  att_load_tile<AB_BM>(sD, p.dout, p.ld_dout, h * ATT_DH, i0, p.T, b, p.T, p.B, p.batch_major);
+  if (nblk > 0) {
+    att_load_tile<AB_BM>(sK, p.qkv, p.ld_qkv, E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
+    att_load_tile<AB_BM>(sV, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
+  }
+  tc::cp_async_commit();
 
-  if (warp == 0 && lane == 0) {
-    tc::tma_prefetch_desc(&tmQKV128);
-    tc::tma_prefetch_desc(&tmQKV64);
-    tc::tma_prefetch_desc(&tmDO64);
+  // per-row statistics of this lane's two rows
+  float lse2[2], dl[2];
+  uint32_t drow[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int i = i0 + r0 + (lane >> 2) + 8 * r;
+    const bool valid = i < p.T;
+    lse2[r] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+    dl[r] = valid ? ab_delta(p, b, h, i) : 0.f;
+    drow[r] = static_cast<uint32_t>(bh) * p.T + i;
   }
-  if (warp == 1 && lane == 0) {
-    tc::mbar_init(kv_full, 1);
-    tc::mbar_init(kv_empty, 1);
-    for (int s = 0; s < AB_KS; ++s) {
-      tc::mbar_init(&qd_full[s], 1);
-      tc::mbar_init(&qd_empty[s], 1);
-    }
-    tc::mbar_init(st_full, 1);
-    tc::mbar_init(s_consumed, AB_EW_WARPS);
-    for (int s = 0; s < 2; ++s) {
-      tc::mbar_init(&pds_ready[s], AB_EW_WARPS);
-      tc::mbar_init(&pd_free[s], 1);
-    }
-    tc::mbar_init(acc_done, 1);
-    tc::mbar_init(acc_empty, AB_EW_WARPS);
-    tc::mbar_fence_init();
-  }
-  if (warp == 2) {
-    tc::tmem_alloc(tmem_slot, 512);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int nq = (p.T + 63) / 64;
-  // TMEM columns: S^T @0 | dP^T @64 | P^T[2] @128,192 (32 cols, bf16) | dS^T[2] @160,224 | dV @256 | dK @384.
-  // The fp32 score buffer is single: it is free again as soon as the row threads have pulled it into registers
-  // (s_consumed), so the next block's score MMAs run under this block's exp/convert work, while the bf16 P^T / dS^T
-  // operands of the accumulate MMAs are double-buffered on their own columns.
+  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
 
-  if (warp == 0) {
-    {
-      uint32_t g = 0, tcount = 0;
-      for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++tcount) {
-        const int bh = w / p.n_tiles;
-        const int kt = w - bh * p.n_tiles;
-        const int b = bh / p.H, h = bh - b * p.H;
-        const int j0 = kt * 128;
-        tc::mbar_wait(kv_empty, (tcount & 1) ^ 1);
-        if (tc::elect_one()) {
-          tc::mbar_expect_tx(kv_full, 2 * AB_TILE_BYTES);
-          tc::tma_load_3d(sK, &tmQKV128, kv_full, E + h * AB_DH, b, j0);
-          tc::tma_load_3d(sK + 16384, &tmQKV128, kv_full, E + h * AB_DH + 64, b, j0);
-          tc::tma_load_3d(sV, &tmQKV128, kv_full, 2 * E + h * AB_DH, b, j0);
-          tc::tma_load_3d(sV + 16384, &tmQKV128, kv_full, 2 * E + h * AB_DH + 64, b, j0);
-        }
-        __syncwarp();
-        for (int i = 0; i < nq; ++i, ++g) {
-          const int st = g % AB_KS;
-          tc::mbar_wait(&qd_empty[st], ((g / AB_KS) & 1) ^ 1);
-          uint8_t* qdst = sQD + st * 2 * AB_BLK_BYTES;
-          uint8_t* ddst = qdst + AB_BLK_BYTES;
-          const int i0 = i * 64;
-          if (tc::elect_one()) {
-            tc::mbar_expect_tx(&qd_full[st], 2 * AB_BLK_BYTES);
-            tc::tma_load_3d(qdst, &tmQKV64, &qd_full[st], h * AB_DH, b, i0);
-            tc::tma_load_3d(qdst + 8192, &tmQKV64, &qd_full[st], h * AB_DH + 64, b, i0);
-            tc::tma_load_3d(ddst, &tmDO64, &qd_full[st], h * AB_DH, b, i0);
-            tc::tma_load_3d(ddst + 8192, &tmDO64, &qd_full[st], h * AB_DH + 64, b, i0);
-          }
-          __syncwarp();
-        }
+  float dq[16][4];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) dq[j][0] = dq[j][1] = dq[j][2] = dq[j][3] = 0.f;
+  const uint32_t q_s = tc::smem_u32(sQ), d_s = tc::smem_u32(sD);
+
+  for (int kb = 0; kb < nblk; ++kb) {
+    if (kb + 1 < nblk) {
+      const int nb = (kb + 1) & 1;
+      att_load_tile<AB_BM>(sK + nb * AB_TILE, p.qkv, p.ld_qkv, E + h * ATT_DH, (kb + 1) * AB_BM, p.sep, b, p.T, p.B, p.batch_major);
+      att_load_tile<AB_BM>(sV + nb * AB_TILE, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, (kb + 1) * AB_BM, p.sep, b, p.T, p.B, p.batch_major);
+      tc::cp_async_commit();
+      tc::cp_async_wait<1>();
+    } else {
+      tc::cp_async_wait<0>();
+    }
+    __syncthreads();
+    const uint32_t k_s = tc::smem_u32(sK + (kb & 1) * AB_TILE);
+    const uint32_t v_s = tc::smem_u32(sV + (kb & 1) * AB_TILE);
+
+    float s[8][4], dp[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = dp[j][0] = dp[j][1] = dp[j][2] = dp[j][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t aq[4], ad[4];
+      att_frag_a(aq, q_s, r0, kk * 16, lane);
+      att_frag_a(ad, d_s, r0, kk * 16, lane);
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        uint32_t bk[4], bv[4];
+        att_frag_b(bk, k_s, np * 16, kk * 16, lane);
+        att_frag_b(bv, v_s, np * 16, kk * 16, lane);
+        tc::mma_bf16_16816(s[2 * np], aq, bk[0], bk[1]);
+        tc::mma_bf16_16816(s[2 * np + 1], aq, bk[2], bk[3]);
+        tc::mma_bf16_16816(dp[2 * np], ad, bv[0], bv[1]);
+        tc::mma_bf16_16816(dp[2 * np + 1], ad, bv[2], bv[3]);
       }
     }
-  } else if (warp == 1) {
-    {
-      // Score issuer (S^T, dP^T of every 64-row block).  The accumulate MMAs are issued by warp 10: with a single issuing
-      // thread the score issue, the wait for P^T / dS^T, the accumulate issue and the barrier polls were served in series
-      // (see attention_bwd_dq.cu); nothing orders the two streams beyond the barriers that already exist (s_consumed guards
-      // the single fp32 score buffer, pd_free the bf16 operand buffers, qd_empty the Q / dO ring).
-      const uint32_t k_addr = tc::smem_u32(sK), v_addr = tc::smem_u32(sV);
-      const uint32_t qd_addr0 = tc::smem_u32(sQD);
-      int sst = 0;               // ring stage of the block whose scores are issued next
-      uint32_t sph = 0;
-      uint32_t nsc = 0;          // score batches issued so far
-      uint32_t tcount = 0;
-      tc::KernelTrace tr = tc::trace_make(p.trace, p.trace_cap, 1);
-      for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++tcount) {
-        tc::mbar_wait(kv_full, tcount & 1);
-        for (int i = 0; i < nq; ++i) {
-          const uint32_t q_addr = qd_addr0 + static_cast<uint32_t>(sst) * (2 * AB_BLK_BYTES);
-          tc::mbar_wait(&qd_full[sst], sph);
-          if (nsc > 0) tc::mbar_wait(s_consumed, (nsc - 1) & 1);      // the previous block's scores are in registers
-          tc::tc_fence_after();
-          if (lane == 0) tr.log(11, tcount, i);
-          if (tc::elect_one()) {
-            ab_mma_ss_128x64(tmem_base, k_addr, q_addr);                             // S^T  = K Q^T
-            ab_mma_ss_128x64(tmem_base + 64, v_addr, q_addr + AB_BLK_BYTES);         // dP^T = V dO^T
-            tc::umma_commit(st_full);
-            if (i + 1 == nq) tc::umma_commit(kv_empty);                              // K / V tile no longer read
-          }
-          __syncwarp();
-          if (lane == 0) tr.log(14, tcount, i);
-          ++nsc;
-          if (++sst == AB_KS) { sst = 0; sph ^= 1; }
-        }
+    // dS = P (mask dP - delta) scale  (keys >= sep of the last block get P = 0)
+    const int key0 = kb * AB_BM + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = key0 + 8 * j + (e & 1);
+        const float pr = key < p.sep ? fast_ex2(fmaf(s[j][e], p.scale_log2, -lse2[e >> 1])) : 0.f;
+        const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[e >> 1], key, p.drop_thr) ? dscale : 0.f) : 1.f;
+        s[j][e] = pr * fmaf(mk, dp[j][e], -dl[e >> 1]) * p.scale;
+      }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      a[0] = tc::pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
+      a[1] = tc::pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
+      a[2] = tc::pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+      a[3] = tc::pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+#pragma unroll
+      for (int dd = 0; dd < 8; ++dd) {
+        uint32_t bb[4];
+        att_frag_bt(bb, k_s, kk * 16, dd * 16, lane);
+        tc::mma_bf16_16816(dq[2 * dd], a, bb[0], bb[1]);
+        tc::mma_bf16_16816(dq[2 * dd + 1], a, bb[2], bb[3]);
       }
     }
-  } else if (warp == 10) {
-    {
-      // Accumulate issuer: dV += P^T dO_i, dK += dS^T Q_i
-      const uint32_t qd_addr0 = tc::smem_u32(sQD);
-      int ast = 0;
-      uint32_t g = 0, tcount = 0;
-      tc::KernelTrace tr = tc::trace_make(p.trace, p.trace_cap, 10);
-      for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++tcount) {
-        for (int i = 0; i < nq; ++i, ++g) {
-          const uint32_t buf = g & 1;
-          tc::mbar_wait(&pds_ready[buf], (g >> 1) & 1);
-          if (i == 0) tc::mbar_wait(acc_empty, (tcount & 1) ^ 1);
-          tc::tc_fence_after();
-          if (lane == 0) tr.log(12, tcount, i);
-          const uint32_t q_addr = qd_addr0 + static_cast<uint32_t>(ast) * (2 * AB_BLK_BYTES);
-          if (tc::elect_one()) {
-            ab_mma_ts_128x128(tmem_base + 256, tmem_base + 128 + buf * 64, q_addr + AB_BLK_BYTES, i > 0);   // dV += P^T dO
-            ab_mma_ts_128x128(tmem_base + 384, tmem_base + 160 + buf * 64, q_addr, i > 0);                  // dK += dS^T Q
-            tc::umma_commit(&qd_empty[ast]);
-            tc::umma_commit(&pd_free[buf]);
-            if (i + 1 == nq) tc::umma_commit(acc_done);    // one phase per tile
-          }
-          __syncwarp();
-          if (lane == 0) tr.log(13, tcount, i);
-          if (++ast == AB_KS) ast = 0;
-        }
+    __syncthreads();     // this buffer is refilled by the next iteration's loads
+  }
+  tc::cp_async_wait<0>();
+
+  // diagonal keys of the query rows, dQ stores, column sums
+  float cs[16][2];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) cs[j][0] = cs[j][1] = 0.f;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int i = i0 + r0 + (lane >> 2) + 8 * r;
+    const bool valid = i < p.T;
+    const bool diag = valid && i >= p.sep;
+    const size_t tok = att_tok(valid ? i : 0, b, p.T, p.B, p.batch_major);
+    const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + h * ATT_DH;
+    const __nv_bfloat16* drw = p.dout + tok * p.ld_dout + h * ATT_DH;
+    __nv_bfloat16* grow = p.dqkv + tok * p.ld_dqkv + h * ATT_DH;
+    float sd = 0.f, dpd = 0.f;
+    if (diag) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane);
+        const float2 g = att_ld2(drw, j, lane), v = att_ld2(qrow + 2 * E, j, lane);
+        sd = fmaf(q.x, k.x, fmaf(q.y, k.y, sd));
+        dpd = fmaf(g.x, v.x, fmaf(g.y, v.y, dpd));
       }
     }
-  } else {
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;              // which 32 of a block's 64 query-row columns this warp owns
-    const int row = quarter * 32 + lane;           // key within the tile
-    const int st_tid = threadIdx.x - 64;           // 0..255
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    tc::KernelTrace tr = tc::trace_make(p.trace, p.trace_cap, warp);
-    uint32_t g = 0, tcount = 0;
-    // Row statistics (lse * log2e, delta * scale) of a 64-row block, one value per thread 0..127.  They are fetched one
-    // block AHEAD into a register and parked in the other smem buffer after this block's bar.sync, so the global-load
-    // latency is off the per-block critical path.
-    // load_stat returns the RAW global value (no arithmetic on it, so nothing waits for the load where it is issued);
-    // finish_stat applies the scaling / row masking when the value is parked in shared memory a block later.
-    auto load_stat = [&](int ww, int ii) -> float {
-      if (st_tid >= 128 || ww >= p.total_work) return 0.f;
-      const int bh2 = ww / p.n_tiles;
-      const int r = min(ii * 64 + (st_tid & 63), p.T - 1);
-      if (st_tid >= 64 && p.delta_tm) return __ldg(p.delta + (static_cast<size_t>(r) * p.B + bh2 / p.H) * p.H + bh2 % p.H);
-      const float* src = st_tid < 64 ? p.lse : p.delta;
-      return __ldg(src + static_cast<size_t>(bh2) * p.T + r);
-    };
-    auto finish_stat = [&](float raw, int ii) -> float {
-      const bool ok = ii * 64 + (st_tid & 63) < p.T;
-      if (st_tid < 64) return ok ? raw * 1.4426950408889634f : INFINITY;
-      return ok ? raw * p.scale : 0.f;
-    };
-    if (st_tid < 128 && static_cast<int>(blockIdx.x) < p.total_work) sStat[st_tid] = finish_stat(load_stat(blockIdx.x, 0), 0);
-    for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++tcount) {
-      const int bh = w / p.n_tiles;
-      const int kt = w - bh * p.n_tiles;
-      const int b = bh / p.H, h = bh - b * p.H;
-      const int j = kt * 128 + row;
-      const bool key_ok = j < p.sep;               // sep <= T
-      for (int i = 0; i < nq; ++i, ++g) {
-        const uint32_t buf = g & 1;
-        float* stat = sStat + buf * 128;
-        const float stat_next = (i + 1 < nq) ? load_stat(w, i + 1) : load_stat(w + gridDim.x, 0);
-        asm volatile("bar.sync 1, 256;" ::: "memory");   // stat[buf] visible; everyone is done reading stat[buf ^ 1]
-        if (lane == 0) tr.log(24 + 100 * warp, tcount, i);
-        tc::mbar_wait_rows(st_full, g & 1);
-        if (lane == 0) tr.log(20 + 100 * warp, tcount, i);
-        tc::tc_fence_after();
-        {
-          uint32_t s[32], dp[32], pkp[16], pkd[16];
-          tc::tmem_ld_32x32b_x32(tmem_base + lane_off + half * 32, s);
-          tc::tmem_ld_32x32b_x32(tmem_base + lane_off + 64 + half * 32, dp);
-          tc::tmem_ld_wait();
-          if (lane == 0) tr.log(25 + 100 * warp, tcount, i);
-          tc::tc_fence_before();
-          tc::mbar_arrive_warp(s_consumed);          // the score buffer may be overwritten by the next block's MMAs
-          if (key_ok && p.drop_thr == 0) {
+    sd = quad_sum(sd);
+    dpd = quad_sum(dpd);
+    if (diag) {
+      const float pr = fast_ex2(fmaf(sd, p.scale_log2, -lse2[r]));
+      const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[r], i, p.drop_thr) ? dscale : 0.f) : 1.f;
+      const float ds = pr * fmaf(mk, dpd, -dl[r]) * p.scale;
+      const float pm = pr * mk;
 #pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              const int col = half * 32 + 4 * c;
-              const float4 l2 = *reinterpret_cast<const float4*>(&stat[col]);
-              const float4 dl = *reinterpret_cast<const float4*>(&stat[64 + col]);
-              const float p0 = tc::fast_exp2(fmaf(__uint_as_float(s[4 * c]), p.scale_log2, -l2.x));
-              const float p1 = tc::fast_exp2(fmaf(__uint_as_float(s[4 * c + 1]), p.scale_log2, -l2.y));
-              const float p2 = tc::fast_exp2(fmaf(__uint_as_float(s[4 * c + 2]), p.scale_log2, -l2.z));
-              const float p3 = tc::fast_exp2(fmaf(__uint_as_float(s[4 * c + 3]), p.scale_log2, -l2.w));
-              pkp[2 * c] = tc::pack_bf16x2(p0, p1);
-              pkp[2 * c + 1] = tc::pack_bf16x2(p2, p3);
-              pkd[2 * c] = tc::pack_bf16x2(p0 * fmaf(__uint_as_float(dp[4 * c]), p.scale, -dl.x),
-                                           p1 * fmaf(__uint_as_float(dp[4 * c + 1]), p.scale, -dl.y));
-              pkd[2 * c + 1] = tc::pack_bf16x2(p2 * fmaf(__uint_as_float(dp[4 * c + 2]), p.scale, -dl.z),
-                                               p3 * fmaf(__uint_as_float(dp[4 * c + 3]), p.scale, -dl.w));
-            }
-          } else if (key_ok) {
-            // dropout on the probabilities (csrc/dropout.cuh): the keep bit of (query row i, key j) is byte j & 3 of the hash
-            // of (row id (b*H + h)*T + i, j >> 2); Pd = P m / (1 - p) feeds dV, dS = P (m dP / (1 - p) - delta) scale feeds dK
-            const float dsc = drop_scale(p.drop_thr);
-            const uint32_t rowbase = static_cast<uint32_t>(bh) * p.T + i * 64 + half * 32;
-#pragma unroll
-            for (int c = 0; c < 16; ++c) {
-              float pv[2], dv[2];
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int cc = 2 * c + e;
-                const bool keep = drop_keep_byte(drop_hash(p.drop_seed, rowbase + cc, static_cast<uint32_t>(j) >> 2), j & 3, p.drop_thr);
-                const float mk = keep ? dsc : 0.f;
-                const float pr = tc::fast_exp2(fmaf(__uint_as_float(s[cc]), p.scale_log2, -stat[half * 32 + cc]));
-                pv[e] = pr * mk;
-                dv[e] = pr * fmaf(__uint_as_float(dp[cc]) * mk, p.scale, -stat[64 + half * 32 + cc]);
-              }
-              pkp[c] = tc::pack_bf16x2(pv[0], pv[1]);
-              pkd[c] = tc::pack_bf16x2(dv[0], dv[1]);
-            }
-          } else {
-#pragma unroll
-            for (int c = 0; c < 16; ++c) { pkp[c] = 0u; pkd[c] = 0u; }
-          }
-          if (lane == 0) tr.log(26 + 100 * warp, tcount, i);
-          tc::mbar_wait(&pd_free[buf], ((g >> 1) & 1) ^ 1);      // accumulate MMAs of block g-2 no longer read this buffer
-          if (lane == 0) tr.log(27 + 100 * warp, tcount, i);
-          tc::tc_fence_after();
-          tc::tmem_st_32x32b_x16(tmem_base + lane_off + 128 + buf * 64 + half * 16, pkp);
-          tc::tmem_st_32x32b_x16(tmem_base + lane_off + 160 + buf * 64 + half * 16, pkd);
-        }
-        tc::tmem_st_wait();
-        tc::tc_fence_before();
-        tc::mbar_arrive_warp(&pds_ready[buf]);
-        if (st_tid < 128) sStat[(buf ^ 1) * 128 + st_tid] = finish_stat(stat_next, i + 1 < nq ? i + 1 : 0);   // parked for the next block
-        if (lane == 0) tr.log(21 + 100 * warp, tcount, i);
+      for (int j = 0; j < 16; ++j) {
+        const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane), g = att_ld2(drw, j, lane);
+        dq[j][2 * r] = fmaf(ds, k.x, dq[j][2 * r]);
+        dq[j][2 * r + 1] = fmaf(ds, k.y, dq[j][2 * r + 1]);
+        att_st2(grow + E, j, lane, ds * q.x, ds * q.y);
+        att_st2(grow + 2 * E, j, lane, pm * g.x, pm * g.y);
       }
-      tc::mbar_wait(acc_done, tcount & 1);                    // committed once per tile, after its last dV/dK MMA
-      if (lane == 0) tr.log(22 + 100 * warp, tcount, 0);
-      tc::tc_fence_after();
-      const bool store_ok = j < p.sep && j < p.T;
-      const size_t krow = p.batch_major ? static_cast<size_t>(b) * p.T + (store_ok ? j : 0) : static_cast<size_t>(store_ok ? j : 0) * p.B + b;
-      __nv_bfloat16* drow = p.dqkv + krow * p.ld_dqkv + h * AB_DH;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t raw[32];
-        float acc[32];
-        // half 0 stores dV (TMEM columns 256..383), half 1 stores dK (384..511)
-        tc::tmem_ld_32x32b_x32(tmem_base + lane_off + 256 + half * 128 + c * 32, raw);
-        tc::tmem_ld_wait();
+    }
+    if (valid) {
 #pragma unroll
-        for (int e = 0; e < 32; ++e) acc[e] = __uint_as_float(raw[e]);
-        if (store_ok) ab_store32(drow + (half == 0 ? 2 * E : E) + c * 32, acc);
+      for (int j = 0; j < 16; ++j) {
+        att_st2(grow, j, lane, dq[j][2 * r], dq[j][2 * r + 1]);
+        cs[j][0] += __bfloat162float(__float2bfloat16_rn(dq[j][2 * r]));
+        cs[j][1] += __bfloat162float(__float2bfloat16_rn(dq[j][2 * r + 1]));
       }
-      tc::tc_fence_before();
-      tc::mbar_arrive_warp(acc_empty);
-      if (lane == 0) tr.log(23 + 100 * warp, tcount, 0);
     }
   }
-
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem_base, 512);
+  if (p.dq_colsum != nullptr) {
+    // reduce over the eight row groups of the warp (lanes with equal lane & 3), then one atomic per column and warp
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float v = cs[j][e];
+        v += __shfl_xor_sync(0xffffffffu, v, 4);
+        v += __shfl_xor_sync(0xffffffffu, v, 8);
+        v += __shfl_xor_sync(0xffffffffu, v, 16);
+        if (lane < 4) atomicAdd(p.dq_colsum + h * ATT_DH + 8 * j + 2 * lane + e, v);
+      }
   }
 }
 
-static int make_map3d(CUtensorMap* tm, const void* base, int ld, int width, int B, int T, int box_rows, int batch_major) {
-  uint64_t dims[3] = {static_cast<uint64_t>(width), static_cast<uint64_t>(B), static_cast<uint64_t>(T)};
-  uint64_t strides[3] = {0, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(ld) * 2 * B};
-  if (batch_major) { strides[1] = static_cast<uint64_t>(ld) * 2 * T; strides[2] = static_cast<uint64_t>(ld) * 2; }
-  uint32_t box[3] = {64, 1, static_cast<uint32_t>(box_rows)};
-  return make_tensor_map_bf16(tm, base, 3, dims, strides, box, true);
+// =====================================================================================================================
+// Kernel 2: dK, dV of the train keys
+// =====================================================================================================================
+__global__ void __launch_bounds__(128, 2)
+attn_bwd_dkv_kernel(const AttnBwdParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint8_t* sK = smem;
+  uint8_t* sV = smem + AB_TILE;
+  uint8_t* sQ = smem + 2 * AB_TILE;                       // buffer s at + s * 8 KB
+  uint8_t* sD = sQ + 2 * AB_QTILE;
+  float* sStat = reinterpret_cast<float*>(sD + 2 * AB_QTILE);   // [2][2][AB_QB]: lse2, delta
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int kt = static_cast<int>(blockIdx.x) % p.n_tiles;
+  const int bh = static_cast<int>(blockIdx.x) / p.n_tiles;
+  const int h = bh % p.H, b = bh / p.H;
+  const int E = p.H * ATT_DH;
+  const int j0 = kt * AB_BM;
+  const int r0 = 16 * warp;                               // this warp's keys: j0 + r0 .. + 15
+  const int nqb = (p.T + AB_QB - 1) / AB_QB;
+
+  auto load_block = [&](int qb, int buf) {
+    att_load_tile<AB_QB>(sQ + buf * AB_QTILE, p.qkv, p.ld_qkv, h * ATT_DH, qb * AB_QB, p.T, b, p.T, p.B, p.batch_major);
+    att_load_tile<AB_QB>(sD + buf * AB_QTILE, p.dout, p.ld_dout, h * ATT_DH, qb * AB_QB, p.T, b, p.T, p.B, p.batch_major);
+    if (threadIdx.x < AB_QB) {
+      const int i = qb * AB_QB + threadIdx.x;
+      const bool valid = i < p.T;
+      sStat[buf * 2 * AB_QB + threadIdx.x] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+      sStat[buf * 2 * AB_QB + AB_QB + threadIdx.x] = valid ? ab_delta(p, b, h, i) : 0.f;
+    }
+  };
+  att_load_tile<AB_BM>(sK, p.qkv, p.ld_qkv, E + h * ATT_DH, j0, p.sep, b, p.T, p.B, p.batch_major);
+  att_load_tile<AB_BM>(sV, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, j0, p.sep, b, p.T, p.B, p.batch_major);
+  load_block(0, 0);
+  tc::cp_async_commit();
+
+  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
+  float dk[16][4], dv[16][4];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) dk[j][0] = dk[j][1] = dk[j][2] = dk[j][3] = dv[j][0] = dv[j][1] = dv[j][2] = dv[j][3] = 0.f;
+  const uint32_t k_s = tc::smem_u32(sK), v_s = tc::smem_u32(sV);
+  const int key_a = j0 + r0 + (lane >> 2);                // this lane's keys: key_a, key_a + 8
+  const uint32_t drow_base = static_cast<uint32_t>(bh) * p.T;
+
+  for (int qb = 0; qb < nqb; ++qb) {
+    const int buf = qb & 1;
+    if (qb + 1 < nqb) {
+      load_block(qb + 1, buf ^ 1);
+      tc::cp_async_commit();
+      tc::cp_async_wait<1>();
+    } else {
+      tc::cp_async_wait<0>();
+    }
+    __syncthreads();
+    const uint32_t q_s = tc::smem_u32(sQ + buf * AB_QTILE), d_s = tc::smem_u32(sD + buf * AB_QTILE);
+    const float* st_lse = sStat + buf * 2 * AB_QB;
+    const float* st_dl = st_lse + AB_QB;
+
+    float s[4][4], dp[4][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = dp[j][0] = dp[j][1] = dp[j][2] = dp[j][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t ak[4], av[4];
+      att_frag_a(ak, k_s, r0, kk * 16, lane);
+      att_frag_a(av, v_s, r0, kk * 16, lane);
+#pragma unroll
+      for (int np = 0; np < 2; ++np) {
+        uint32_t bq[4], bd[4];
+        att_frag_b(bq, q_s, np * 16, kk * 16, lane);
+        att_frag_b(bd, d_s, np * 16, kk * 16, lane);
+        tc::mma_bf16_16816(s[2 * np], ak, bq[0], bq[1]);
+        tc::mma_bf16_16816(s[2 * np + 1], ak, bq[2], bq[3]);
+        tc::mma_bf16_16816(dp[2 * np], av, bd[0], bd[1]);
+        tc::mma_bf16_16816(dp[2 * np + 1], av, bd[2], bd[3]);
+      }
+    }
+    // element (key, query i): P^T = exp2(S^T c - lse2_i), P^T mask -> s, dS^T -> dp
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int ci = 8 * j + 2 * (lane & 3) + (e & 1);
+        const int i = qb * AB_QB + ci;
+        const float pr = fast_ex2(fmaf(s[j][e], p.scale_log2, -st_lse[ci]));
+        const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow_base + i, key_a + 8 * (e >> 1), p.drop_thr) ? dscale : 0.f) : 1.f;
+        dp[j][e] = pr * fmaf(mk, dp[j][e], -st_dl[ci]) * p.scale;
+        s[j][e] = pr * mk;
+      }
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk) {
+      uint32_t ap[4], as[4];
+      ap[0] = tc::pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
+      ap[1] = tc::pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
+      ap[2] = tc::pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+      ap[3] = tc::pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+      as[0] = tc::pack_bf16x2(dp[2 * kk][0], dp[2 * kk][1]);
+      as[1] = tc::pack_bf16x2(dp[2 * kk][2], dp[2 * kk][3]);
+      as[2] = tc::pack_bf16x2(dp[2 * kk + 1][0], dp[2 * kk + 1][1]);
+      as[3] = tc::pack_bf16x2(dp[2 * kk + 1][2], dp[2 * kk + 1][3]);
+#pragma unroll
+      for (int dd = 0; dd < 8; ++dd) {
+        uint32_t bd[4], bq[4];
+        att_frag_bt(bd, d_s, kk * 16, dd * 16, lane);
+        att_frag_bt(bq, q_s, kk * 16, dd * 16, lane);
+        tc::mma_bf16_16816(dv[2 * dd], ap, bd[0], bd[1]);
+        tc::mma_bf16_16816(dv[2 * dd + 1], ap, bd[2], bd[3]);
+        tc::mma_bf16_16816(dk[2 * dd], as, bq[0], bq[1]);
+        tc::mma_bf16_16816(dk[2 * dd + 1], as, bq[2], bq[3]);
+      }
+    }
+    __syncthreads();     // this buffer is refilled by the next iteration's loads
+  }
+
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int key = key_a + 8 * r;
+    if (key < p.sep) {
+      __nv_bfloat16* grow = p.dqkv + att_tok(key, b, p.T, p.B, p.batch_major) * p.ld_dqkv + h * ATT_DH;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        att_st2(grow + E, j, lane, dk[j][2 * r], dk[j][2 * r + 1]);
+        att_st2(grow + 2 * E, j, lane, dv[j][2 * r], dv[j][2 * r + 1]);
+      }
+    }
+  }
 }
 
 }  // namespace pfn
@@ -377,59 +386,40 @@ static int make_map3d(CUtensorMap* tm, const void* base, int ld, int width, int 
 using namespace pfn;
 
 extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
-  if (int rc = check_attn_desc_public(d, true, "attention_bwd_tc")) return rc;
-  PFN_CHECK_ARG(d->dtype == PFN_BF16, "attention_bwd_tc: bf16 only");
-  PFN_CHECK_ARG(d->dh == AB_DH, "attention_bwd_tc: head dim %d unsupported (built for 128)", d->dh);
-  PFN_CHECK_ARG(d->ld_qkv % 8 == 0 && d->ld_out % 8 == 0 && d->ld_dout % 8 == 0 && d->ld_dqkv % 8 == 0,
-                "attention_bwd_tc: leading dims must be multiples of 8");
-  PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->qkv) | reinterpret_cast<uintptr_t>(d->out) |
-                  reinterpret_cast<uintptr_t>(d->dout) | reinterpret_cast<uintptr_t>(d->dqkv)) & 15) == 0,
-                "attention_bwd_tc: buffers must be 16-byte aligned");
-  const int E = d->H * d->dh;
-  CUtensorMap tmQKV128, tmQKV64, tmDO128, tmDO64;
-  if (int rc = make_map3d(&tmQKV128, d->qkv, d->ld_qkv, 3 * E, d->B, d->T, 128, d->batch_major)) return rc;
-  if (int rc = make_map3d(&tmQKV64, d->qkv, d->ld_qkv, 3 * E, d->B, d->T, 64, d->batch_major)) return rc;
-  if (int rc = make_map3d(&tmDO128, d->dout, d->ld_dout, E, d->B, d->T, 128, d->batch_major)) return rc;
-  if (int rc = make_map3d(&tmDO64, d->dout, d->ld_dout, E, d->B, d->T, 64, d->batch_major)) return rc;
+  if (int rc = check_tc_attn(d, true, "attention_bwd_tc")) return rc;
+  PFN_CHECK_ARG(!(d->delta_token_major && d->batch_major), "attention_bwd_tc: a token-major delta implies the reference token order");
   AttnBwdParams p;
   p.T = d->T; p.B = d->B; p.H = d->H; p.sep = d->sep;
   p.scale = d->scale; p.scale_log2 = d->scale * 1.4426950408889634f;
   p.qkv = reinterpret_cast<const __nv_bfloat16*>(d->qkv); p.ld_qkv = d->ld_qkv;
-  p.out = reinterpret_cast<const __nv_bfloat16*>(d->out); p.ld_out = d->ld_out;
   p.dout = reinterpret_cast<const __nv_bfloat16*>(d->dout); p.ld_dout = d->ld_dout;
   p.dqkv = reinterpret_cast<__nv_bfloat16*>(d->dqkv); p.ld_dqkv = d->ld_dqkv;
   p.lse = d->lse; p.delta = d->delta; p.dq_colsum = d->dq_colsum; p.delta_tm = d->delta_token_major;
-  PFN_CHECK_ARG(!(d->delta_token_major && d->batch_major), "attention_bwd_tc: a token-major delta implies the reference token order");
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
   p.batch_major = d->batch_major;
-  p.trace = nullptr; p.trace_cap = g_trace_cap;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
-    PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dkv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+    PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_DQ_SMEM));
+    PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_DKV_SMEM));
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  // debug only (tools/time_kernels.py): pfn_debug_attention_trace(NULL, 0, 21|22|23) runs just dK/dV | dQ | delta
-  const int only = (g_trace_ptr == nullptr && g_trace_which >= 21 && g_trace_which <= 23) ? g_trace_which : 0;
-  if ((only == 0 || only == 23) && !d->delta_token_major) {
+  if (!d->delta_token_major) {
     const long long rows = static_cast<long long>(d->T) * d->B;
     long long grid = (rows + 7) / 8;
     if (grid > 8LL * num_sms()) grid = 8LL * num_sms();
-    attn_bwd_delta_kernel<<<static_cast<int>(grid), 256, 0, s>>>(p.out, p.ld_out, p.dout, p.ld_dout, p.delta, d->T, d->B, d->H, d->batch_major);
+    attn_bwd_delta_kernel<<<static_cast<int>(grid), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(d->out), d->ld_out,
+                                                                 p.dout, p.ld_dout, d->delta, d->T, d->B, d->H, d->batch_major);
     PFN_LAUNCH_OK();
   }
-  if (only == 0 || only == 22) {
-    p.trace = g_trace_which == 1 ? g_trace_ptr : nullptr;
-    if (int rc = launch_attn_bwd_dq(p, d, s)) return rc;
-    p.trace = nullptr;
-    PFN_LAUNCH_OK();
-  }
-  if (d->sep > 0 && (only == 0 || only == 21)) {
-    p.n_tiles = (d->sep + 127) / 128;
-    p.total_work = p.n_tiles * d->B * d->H;
-    int grid = num_sms() < p.total_work ? num_sms() : p.total_work;
-    p.trace = g_trace_which == 2 ? g_trace_ptr : nullptr;
-    attn_bwd_dkv_tc_kernel<<<grid, AB_THREADS + 32, AB_SMEM, s>>>(tmQKV128, tmQKV64, tmDO64, p);
-    p.trace = nullptr;
+  p.n_tiles = (d->T + AB_BM - 1) / AB_BM;
+  long long grid = static_cast<long long>(p.n_tiles) * d->B * d->H;
+  PFN_CHECK_ARG(grid < (1LL << 31), "attention_bwd_tc: too many tiles");
+  attn_bwd_dq_kernel<<<static_cast<unsigned>(grid), 128, AB_DQ_SMEM, s>>>(p);
+  PFN_LAUNCH_OK();
+  if (d->sep > 0) {
+    p.n_tiles = (d->sep + AB_BM - 1) / AB_BM;
+    grid = static_cast<long long>(p.n_tiles) * d->B * d->H;
+    attn_bwd_dkv_kernel<<<static_cast<unsigned>(grid), 128, AB_DKV_SMEM, s>>>(p);
     PFN_LAUNCH_OK();
   }
   return 0;

@@ -1,5 +1,5 @@
 // fp32-FMA masked attention (forward, dQ, dK/dV) for the fp32 parity mode and for head sizes / dtypes the
-// tcgen05 kernels do not take.  One warp per (batch, head, row); the head dimension is spread over the
+// tensor-core kernels do not take.  One warp per (batch, head, row); the head dimension is spread over the
 // lanes, scores are reduced with warp shuffles, softmax is computed online.  The single_eval_pos mask of
 // reference transformer.py:35-41 is implicit:  keys(i) = [0, sep)  U  {i if i >= sep}.
 #include "common.cuh"
@@ -228,15 +228,15 @@ using namespace pfn;
 
 extern "C" int pfn_attention_fwd_simt(const pfn_attn_desc* d, void* stream) {
   if (int rc = check_attn_desc(d, false, "attention_fwd_simt")) return rc;
-  PFN_CHECK_ARG(d->batch_major == 0, "attention_fwd_simt: batch-major token order is only implemented by the tcgen05 kernels");
+  PFN_CHECK_ARG(d->batch_major == 0, "attention_fwd_simt: batch-major token order is only implemented by the tensor-core kernels");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   return d->dtype == PFN_F32 ? dispatch_attn_simt<float>(d, false, s) : dispatch_attn_simt<__nv_bfloat16>(d, false, s);
 }
 
 extern "C" int pfn_attention_bwd_simt(const pfn_attn_desc* d, void* stream) {
   if (int rc = check_attn_desc(d, true, "attention_bwd_simt")) return rc;
-  PFN_CHECK_ARG(d->batch_major == 0, "attention_bwd_simt: batch-major token order is only implemented by the tcgen05 kernels");
-  PFN_CHECK_ARG(d->delta_token_major == 0, "attention_bwd_simt: a precomputed token-major delta is only consumed by the tcgen05 kernels");
+  PFN_CHECK_ARG(d->batch_major == 0, "attention_bwd_simt: batch-major token order is only implemented by the tensor-core kernels");
+  PFN_CHECK_ARG(d->delta_token_major == 0, "attention_bwd_simt: a precomputed token-major delta is only consumed by the tensor-core kernels");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   return d->dtype == PFN_F32 ? dispatch_attn_simt<float>(d, true, s) : dispatch_attn_simt<__nv_bfloat16>(d, true, s);
 }

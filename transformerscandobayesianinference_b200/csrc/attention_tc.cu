@@ -1,47 +1,23 @@
-// tcgen05 masked attention for the single_eval_pos mask (reference transformer.py:35-41), head dim 128, bf16.
+// Tensor-core masked attention for the single_eval_pos mask (reference transformer.py:35-41), head dim 128, bf16.
 //
 //   keys(i) = [0, sep)  U  {i if i >= sep}        o_i = softmax_j(q_i.k_j / sqrt(dh)) v_j
 //
-// The [T,T] mask is never built: the dense part (keys < sep) runs on the tensor cores in 64-key blocks and the
-// single diagonal key of a query row is a 128-wide dot product done by the thread that owns the row.
-// Q/K/V tiles are fetched straight out of the packed [T*B, 3E] in-projection output with 3-D TMA descriptors
-// (dims: column, batch, time), so there is no head-split / transpose kernel (the reference spends 22 % of its
-// CPU time in exactly those copies, SURVEY.md section 6).
+// The [T,T] mask is never built: the dense part (keys < sep) runs on the tensor cores in 64-key blocks and the single
+// diagonal key of a query row is a 128-wide dot product done by the four lanes that own the row.  Q/K/V rows are read
+// straight out of the packed [T*B, 3E] in-projection output, so there is no head-split / transpose kernel.
 //
-// Forward, per CTA (two CTAs per SM so one CTA's softmax overlaps the other's MMAs):
-//   warp 0      TMA producer: Q tile (128 rows) once per work item, K blocks (64 keys) through a 3-stage ring and V blocks
-//               through their own 2-stage ring.  K_j is needed a whole block before V_j (Q K_j^T is
-//               issued ahead of the softmax of block j-1, P_j V_j after the softmax of block j) and its stage is free as
-//               soon as Q K_j^T has completed, so separate rings let both loads run 2 blocks ahead inside the same 112 KB
-//               (a joint 2-stage K+V ring made every block wait ~1 300 clk for a load that could only be requested after
-//               P_{j-2} V_{j-2} had completed: profiles/r1_trace_attn_fwd_clock64.txt)
-//   warp 1      MMA issuer  : S_j = Q K_j^T  (SS, 128x64x128)  ->  TMEM S buffer (double buffered)
-//                             O  += P_j V_j  (TS, P read from TMEM, V MN-major from smem, 128x128x64)
-//   warps 2..5  softmax     : one thread per query row; tcgen05.ld S row, online softmax in the log2 domain with
-//                             lazy rescaling (O is only rescaled when the running max grows by > 2^8), P written
-//                             back to TMEM as packed bf16 over the S buffer; epilogue normalises O and stores.
-// TMEM map (256 columns): [0,64) S0 | [64,128) S1 | [128,256) O ; P_j aliases the first 32 columns of S_j.
-#include "common.cuh"
-#include "dropout.cuh"
-#include "tc_common.cuh"
-#include "../../include/pfn_b200.h"
+// One CTA (4 warps) per (batch, head, 64-row query tile); warp w owns query rows [16 w, 16 w + 16).  K and V blocks are
+// double-buffered with cp.async so the loads of block j+1 overlap the MMAs and softmax of block j:
+//   S_j = Q K_j^T (mma.sync, fp32)  ->  online softmax in the log2 domain  ->  P_j as bf16 A fragments  ->  O += P_j V_j
+// P_j never leaves the registers: the S accumulator layout of two n-tiles is the A fragment layout of one k-step.
+#include "attention_common.cuh"
 
 namespace pfn {
 
-int check_attn_desc_public(const pfn_attn_desc* d, bool bwd, const char* who);
-
-constexpr int ATT_BM = 128;
-constexpr int ATT_BN = 64;
-constexpr int ATT_DH = 128;
-constexpr int ATT_NK = 3;                                  // K ring depth
-constexpr int ATT_NV = 2;                                  // V ring depth
-constexpr int ATT_THREADS = 192;
-constexpr int ATT_Q_BYTES = ATT_BM * ATT_DH * 2;          // 32 KB (two 64-wide chunks of 16 KB)
-constexpr int ATT_KV_BYTES = ATT_BN * ATT_DH * 2;         // 16 KB per operand (two chunks of 8 KB)
-// No alignment slack: two CTAs of 112 KB + barriers must fit one SM, so the kernel relies on (and checks) a 1 KB-aligned
-// dynamic shared memory base instead of rounding the pointer up.
-constexpr int ATT_FWD_SMEM = ATT_Q_BYTES + (ATT_NK + ATT_NV) * ATT_KV_BYTES + 256;
-constexpr float kRescaleThreshold = 8.0f;                  // log2 units
+constexpr int ATT_BM = 64;                                // query rows per CTA
+constexpr int ATT_BN = 64;                                // keys per block
+constexpr int ATT_TILE_BYTES = ATT_BM * ATT_ROW_BYTES;    // 16 KB
+constexpr int ATT_FWD_SMEM = 5 * ATT_TILE_BYTES;          // Q + 2 x K + 2 x V
 
 struct AttnFwdParams {
   int T, B, H, sep;
@@ -50,455 +26,159 @@ struct AttnFwdParams {
   __nv_bfloat16* out; int ld_out;
   float* lse;
   int n_qtiles;
-  int total_work;
   int batch_major;
-  long long* trace;     // debug: clock64 event log of CTA 0 (null = off)
-  int trace_cap;
   uint32_t drop_seed; int drop_thr;   // dropout on the probabilities (thr 0 = off), csrc/dropout.cuh
 };
 
-// Block plan of one 128-row query tile: `nblk` dense blocks over the train keys [0, sep), followed by up to two
-// "diagonal" blocks whose keys are the tile's own rows [i0, i0+64) / [i0+64, i0+128) — needed only when that row range
-// holds query rows (>= sep).  In a diagonal block row i keeps exactly one key: itself.  All roles call this.
-__device__ __forceinline__ int tile_block_plan(int i0, int sep, int T, int nblk, int (&dstart)[2]) {
-  int nd = 0;
-#pragma unroll
-  for (int jj = 0; jj < 2; ++jj) {
-    const int lo = i0 + 64 * jj;
-    if (lo < T && lo + 63 >= sep) dstart[nd++] = lo;
-  }
-  return nblk + nd;
-}
-
-__device__ __forceinline__ void load_row128(const __nv_bfloat16* p, float (&v)[32], int chunk) {
-  // 32 consecutive bf16 -> fp32 (chunk selects which quarter of the 128-wide row)
-  const uint4* src = reinterpret_cast<const uint4*>(p + chunk * 32);
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const uint4 pk = src[q];
-    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&pk);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 t = __bfloat1622float2(h[j]);
-      v[q * 8 + 2 * j] = t.x;
-      v[q * 8 + 2 * j + 1] = t.y;
-    }
-  }
-}
-
-__device__ __forceinline__ float dot_rows128(const __nv_bfloat16* a, const __nv_bfloat16* b) {
-  float acc = 0.f;
-#pragma unroll
-  for (int c = 0; c < 16; ++c) {
-    const uint4 pa = reinterpret_cast<const uint4*>(a)[c];
-    const uint4 pb = reinterpret_cast<const uint4*>(b)[c];
-    const __nv_bfloat162* ha = reinterpret_cast<const __nv_bfloat162*>(&pa);
-    const __nv_bfloat162* hb = reinterpret_cast<const __nv_bfloat162*>(&pb);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 x = __bfloat1622float2(ha[j]);
-      const float2 y = __bfloat1622float2(hb[j]);
-      acc = fmaf(x.x, y.x, acc);
-      acc = fmaf(x.y, y.y, acc);
-    }
-  }
-  return acc;
-}
-
-__global__ void __launch_bounds__(ATT_THREADS, 2)
-attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
-                   const AttnFwdParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if ((tc::smem_u32(smem) & 1023u) != 0) __trap();        // the 128-byte-swizzled tiles need 1 KB alignment
+__global__ void __launch_bounds__(128, 2)
+attn_fwd_tc_kernel(const AttnFwdParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* sQ = smem;
-  uint8_t* sK = smem + ATT_Q_BYTES;                          // stage s at + s * 16 KB
-  uint8_t* sV = sK + ATT_NK * ATT_KV_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ATT_NV * ATT_KV_BYTES);
-  uint64_t* q_full = bars + 0;
-  uint64_t* q_empty = bars + 1;
-  uint64_t* k_full = bars + 2;                   // [ATT_NK]
-  uint64_t* k_empty = k_full + ATT_NK;           // [ATT_NK]
-  uint64_t* v_full = k_empty + ATT_NK;           // [ATT_NV]
-  uint64_t* v_empty = v_full + ATT_NV;           // [ATT_NV]
-  uint64_t* s_full = v_empty + ATT_NV;           // [2]
-  uint64_t* p_ready = s_full + 2;                // [2]
-  uint64_t* pv_done = p_ready + 2;
-  uint64_t* o_empty = pv_done + 1;
-  uint64_t* o_done = pv_done + 2;                // one phase per tile: committed after the tile's last P V
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 3);
-  static_assert((2 + 2 * ATT_NK + 2 * ATT_NV + 4 + 3) * 8 + 4 <= 256, "barrier block");
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  uint8_t* sK = smem + ATT_TILE_BYTES;                    // buffer s at + s * 16 KB
+  uint8_t* sV = smem + 3 * ATT_TILE_BYTES;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int qt = static_cast<int>(blockIdx.x) % p.n_qtiles;
+  const int bh = static_cast<int>(blockIdx.x) / p.n_qtiles;
+  const int h = bh % p.H, b = bh / p.H;
   const int E = p.H * ATT_DH;
-
-  if (warp == 0 && lane == 0) {
-    tc::tma_prefetch_desc(&tmQ);
-    tc::tma_prefetch_desc(&tmKV);
-  }
-  if (warp == 1 && lane == 0) {
-    tc::mbar_init(q_full, 1);
-    tc::mbar_init(q_empty, 1);
-    for (int s = 0; s < ATT_NK; ++s) { tc::mbar_init(&k_full[s], 1); tc::mbar_init(&k_empty[s], 1); }
-    for (int s = 0; s < ATT_NV; ++s) { tc::mbar_init(&v_full[s], 1); tc::mbar_init(&v_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) {
-      tc::mbar_init(&s_full[s], 1);
-      tc::mbar_init(&p_ready[s], 4);      // one arrival per softmax warp
-    }
-    tc::mbar_init(pv_done, 1);
-    tc::mbar_init(o_empty, 4);
-    tc::mbar_init(o_done, 1);
-    tc::mbar_fence_init();
-  }
-  if (warp == 2) {
-    tc::tmem_alloc(tmem_slot, 256);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  const int i0 = qt * ATT_BM;
   const int nblk = (p.sep + ATT_BN - 1) / ATT_BN;
 
-  if (warp == 0) {
-    // =============================================================== TMA producer (converged warp, elected lane issues)
-    // One warp feeds both rings.  The (tile, block) sequence is walked by two cursors, the K cursor two blocks ahead of the
-    // V cursor:  K0 K1 | V0 K2 | V1 K3 | ...   V_n waits for P_{n-2} V_{n-2} to complete, and by then Q K_{n-1}^T (which the
-    // MMA warp issues before P_{n-2} V_{n-2}) has freed the stage K_{n+2} goes to, so neither wait holds the other load back.
-    {
-      tc::KernelTrace tr = tc::trace_make(p.trace, p.trace_cap, 0);
-      struct Cursor { int w, j, nb, b, h, i0; int dstart[2]; uint32_t tcount; bool valid; };
-      auto enter = [&](Cursor& c) {
-        c.valid = c.w < p.total_work;
-        if (!c.valid) return;
-        const int bh = c.w / p.n_qtiles;
-        const int qt = c.w - bh * p.n_qtiles;
-        c.b = bh / p.H; c.h = bh - c.b * p.H;
-        c.i0 = qt * ATT_BM;
-        c.nb = tile_block_plan(c.i0, p.sep, p.T, nblk, c.dstart);
-        c.j = 0;
-      };
-      auto advance = [&](Cursor& c) {
-        if (++c.j == c.nb) { c.w += gridDim.x; ++c.tcount; enter(c); }
-      };
-      int kst = 0, vst = 0; uint32_t kph = 0, vph = 0;
-      auto issue_k = [&](Cursor& c) {
-        if (!c.valid) return;
-        if (c.j == 0) {
-          tc::mbar_wait(q_empty, (c.tcount & 1) ^ 1);
-          if (lane == 0) tr.log(1, c.tcount, 0);   // Q load issue
-          if (tc::elect_one()) {
-            tc::mbar_expect_tx(q_full, ATT_Q_BYTES);
-            tc::tma_load_3d(sQ, &tmQ, q_full, c.h * ATT_DH, c.b, c.i0);
-            tc::tma_load_3d(sQ + 16384, &tmQ, q_full, c.h * ATT_DH + 64, c.b, c.i0);
-          }
-          __syncwarp();
-        }
-        tc::mbar_wait(&k_empty[kst], kph ^ 1);
-        if (lane == 0) tr.log(2, c.tcount, c.j);   // K load issue
-        uint8_t* kdst = sK + kst * ATT_KV_BYTES;
-        const int j0 = c.j < nblk ? c.j * ATT_BN : c.dstart[c.j - nblk];
-        if (tc::elect_one()) {
-          tc::mbar_expect_tx(&k_full[kst], ATT_KV_BYTES);
-          tc::tma_load_3d(kdst, &tmKV, &k_full[kst], E + c.h * ATT_DH, c.b, j0);
-          tc::tma_load_3d(kdst + 8192, &tmKV, &k_full[kst], E + c.h * ATT_DH + 64, c.b, j0);
-        }
-        __syncwarp();
-        if (++kst == ATT_NK) { kst = 0; kph ^= 1; }
-        advance(c);
-      };
-      auto issue_v = [&](Cursor& c) {
-        tc::mbar_wait(&v_empty[vst], vph ^ 1);
-        if (lane == 0) tr.log(3, c.tcount, c.j);   // V load issue
-        uint8_t* vdst = sV + vst * ATT_KV_BYTES;
-        const int j0 = c.j < nblk ? c.j * ATT_BN : c.dstart[c.j - nblk];
-        if (tc::elect_one()) {
-          tc::mbar_expect_tx(&v_full[vst], ATT_KV_BYTES);
-          tc::tma_load_3d(vdst, &tmKV, &v_full[vst], 2 * E + c.h * ATT_DH, c.b, j0);
-          tc::tma_load_3d(vdst + 8192, &tmKV, &v_full[vst], 2 * E + c.h * ATT_DH + 64, c.b, j0);
-        }
-        __syncwarp();
-        if (++vst == ATT_NV) { vst = 0; vph ^= 1; }
-        advance(c);
-      };
-      Cursor ck, cv;
-      ck.w = cv.w = blockIdx.x; ck.tcount = cv.tcount = 0;
-      enter(ck); enter(cv);
-      issue_k(ck);
-      issue_k(ck);
-      while (cv.valid) {
-        issue_v(cv);
-        issue_k(ck);
+  att_load_tile<ATT_BM>(sQ, p.qkv, p.ld_qkv, h * ATT_DH, i0, p.T, b, p.T, p.B, p.batch_major);
+  if (nblk > 0) {
+    att_load_tile<ATT_BN>(sK, p.qkv, p.ld_qkv, E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
+    att_load_tile<ATT_BN>(sV, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
+  }
+  tc::cp_async_commit();
+
+  float o[16][4];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const int r0 = 16 * warp;
+  const uint32_t drow0 = static_cast<uint32_t>(bh) * p.T + i0 + r0 + (lane >> 2);   // dropout row of this lane's first row
+  const uint32_t q_s = tc::smem_u32(sQ);
+
+  for (int kb = 0; kb < nblk; ++kb) {
+    if (kb + 1 < nblk) {
+      const int nb = (kb + 1) & 1;
+      att_load_tile<ATT_BN>(sK + nb * ATT_TILE_BYTES, p.qkv, p.ld_qkv, E + h * ATT_DH, (kb + 1) * ATT_BN, p.sep, b, p.T, p.B, p.batch_major);
+      att_load_tile<ATT_BN>(sV + nb * ATT_TILE_BYTES, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, (kb + 1) * ATT_BN, p.sep, b, p.T, p.B, p.batch_major);
+      tc::cp_async_commit();
+      tc::cp_async_wait<1>();
+    } else {
+      tc::cp_async_wait<0>();
+    }
+    __syncthreads();
+    const uint32_t k_s = tc::smem_u32(sK + (kb & 1) * ATT_TILE_BYTES);
+    const uint32_t v_s = tc::smem_u32(sV + (kb & 1) * ATT_TILE_BYTES);
+
+    float s[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t a[4];
+      att_frag_a(a, q_s, r0, kk * 16, lane);
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        uint32_t bb[4];
+        att_frag_b(bb, k_s, np * 16, kk * 16, lane);
+        tc::mma_bf16_16816(s[2 * np], a, bb[0], bb[1]);
+        tc::mma_bf16_16816(s[2 * np + 1], a, bb[2], bb[3]);
       }
     }
-  } else if (warp == 1) {
-    // =============================================================== MMA issuer
-    // The whole warp runs the control flow (so addresses / descriptors stay warp-uniform and live in uniform registers);
-    // one elected lane issues the tcgen05 instructions.
-    {
-      constexpr uint32_t idesc_qk = tc::umma_idesc_bf16(ATT_BM, ATT_BN, 0, 0);
-      constexpr uint32_t idesc_pv = tc::umma_idesc_bf16(ATT_BM, ATT_DH, 0, 1);
-      const uint32_t q_addr = tc::smem_u32(sQ);
-      tc::KernelTrace tr = tc::trace_make(p.trace, p.trace_cap, 1);
-      uint32_t g = 0, tcount = 0;
-      int kst = 0; uint32_t kph = 0;     // K ring position of the NEXT Q K^T batch
-      int vst = 0; uint32_t vph = 0;     // V ring position of the NEXT P V batch
-      auto issue_qk = [&](uint32_t gg) {
-        tc::mbar_wait(&k_full[kst], kph);
-        if (lane == 0) tr.log(11, tcount, static_cast<int>(gg));   // K landed
-        tc::tc_fence_after();
-        const uint32_t k_addr = tc::smem_u32(sK + kst * ATT_KV_BYTES);
-        const uint32_t d_tmem = tmem_base + (gg & 1) * ATT_BN;
-        if (tc::elect_one()) {
+    // online softmax (log2 domain); keys >= sep of the last block are masked
+    const int key0 = kb * ATT_BN + 2 * (lane & 3);
+    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-          for (int kk = 0; kk < ATT_DH / 16; ++kk) {
-            const uint64_t a_desc = tc::umma_smem_desc(q_addr + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024);
-            const uint64_t b_desc = tc::umma_smem_desc(k_addr + (kk >> 2) * 8192 + (kk & 3) * 32, 16, 1024);
-            tc::umma_bf16_ss(d_tmem, a_desc, b_desc, idesc_qk, kk > 0 ? 1u : 0u);
-          }
-          tc::umma_commit(&s_full[gg & 1]);
-          tc::umma_commit(&k_empty[kst]);        // the K stage is free as soon as this batch has completed
-        }
-        __syncwarp();
-        if (++kst == ATT_NK) { kst = 0; kph ^= 1; }
-      };
-      for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++tcount) {
-        const int qt = w % p.n_qtiles;
-        int dstart[2];
-        const int nb = tile_block_plan(qt * ATT_BM, p.sep, p.T, nblk, dstart);
-        tc::mbar_wait(q_full, tcount & 1);
-        if (lane == 0) tr.log(10, tcount, 0);  // Q landed
-        issue_qk(g);
-        for (int j = 0; j < nb; ++j, ++g) {
-          bool p_ok = false;        // p_ready probed before the (blocking) Q K^T issue; see gemm_tc.cu on early probes
-          if (j + 1 < nb) {
-            p_ok = tc::mbar_try_wait(&p_ready[g & 1], (g >> 1) & 1);
-            issue_qk(g + 1);
-          } else {
-            if (tc::elect_one()) tc::umma_commit(q_empty);   // every QK^T of this tile has been issued
-            __syncwarp();
-          }
-          const bool v_ok = tc::mbar_try_wait(&v_full[vst], vph);
-          if (!p_ok) tc::mbar_wait(&p_ready[g & 1], (g >> 1) & 1);
-          if (lane == 0) tr.log(12, tcount, j);  // P ready seen by MMA warp
-          if (j == 0) tc::mbar_wait(o_empty, (tcount & 1) ^ 1);
-          if (!v_ok) tc::mbar_wait(&v_full[vst], vph);
-          tc::tc_fence_after();
-          const uint32_t v_addr = tc::smem_u32(sV + vst * ATT_KV_BYTES);
-          const uint32_t p_tmem = tmem_base + (g & 1) * ATT_BN;
-          const uint32_t o_tmem = tmem_base + 128;
-          if (tc::elect_one()) {
+    for (int j = 0; j < 8; ++j)
 #pragma unroll
-            for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-              const uint64_t b_desc = tc::umma_smem_desc(v_addr + kk * 2048, 8192, 1024);
-              tc::umma_bf16_ts(o_tmem, p_tmem + kk * 8, b_desc, idesc_pv, (j > 0 || kk > 0) ? 1u : 0u);
-            }
-            tc::umma_commit(&v_empty[vst]);
-            tc::umma_commit(pv_done);
-            if (j + 1 == nb) tc::umma_commit(o_done);
-          }
-          __syncwarp();
-          if (++vst == ATT_NV) { vst = 0; vph ^= 1; }
-          if (lane == 0) tr.log(13, tcount, j);  // PV issued
-        }
+      for (int e = 0; e < 4; ++e) {
+        const bool ok = key0 + 8 * j + (e & 1) < p.sep;
+        s[j][e] = ok ? s[j][e] * p.scale_log2 : -INFINITY;
+        mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
+      }
+    float corr[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float mn = fmaxf(m[r], quad_max(mx[r]));
+      corr[r] = fast_ex2(m[r] - mn);
+      m[r] = mn;
+      l[r] *= corr[r];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float pr = fast_ex2(s[j][e] - m[e >> 1]);
+        l[e >> 1] += pr;
+        if (p.drop_thr > 0 && !drop_keep(p.drop_seed, drow0 + 8 * (e >> 1), key0 + 8 * j + (e & 1), p.drop_thr)) s[j][e] = 0.f;
+        else s[j][e] = pr;
+      }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      o[j][0] *= corr[0]; o[j][1] *= corr[0];
+      o[j][2] *= corr[1]; o[j][3] *= corr[1];
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      a[0] = tc::pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
+      a[1] = tc::pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
+      a[2] = tc::pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+      a[3] = tc::pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+#pragma unroll
+      for (int dp = 0; dp < 8; ++dp) {
+        uint32_t bb[4];
+        att_frag_bt(bb, v_s, kk * 16, dp * 16, lane);
+        tc::mma_bf16_16816(o[2 * dp], a, bb[0], bb[1]);
+        tc::mma_bf16_16816(o[2 * dp + 1], a, bb[2], bb[3]);
       }
     }
-  } else {
-    // =============================================================== softmax / correction / epilogue
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    tc::KernelTrace tr = tc::trace_make(p.trace, p.trace_cap, 2);
-    bool s_ok = false;      // early probe result: the next block's scores are already complete
-    uint32_t g = 0, tcount = 0;
-    for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++tcount) {
-      const int bh = w / p.n_qtiles;
-      const int qt = w - bh * p.n_qtiles;
-      const int b = bh / p.H, h = bh - b * p.H;
-      const int i0 = qt * ATT_BM;
-      const int i = i0 + row;
-      const bool valid = i < p.T;
-      const bool is_query = valid && i >= p.sep;
-      int dstart[2];
-      const int nb = tile_block_plan(i0, p.sep, p.T, nblk, dstart);
-      float m = -INFINITY, l = 0.f;
-      for (int j = 0; j < nb; ++j, ++g) {
-        const uint32_t buf = g & 1;
-        if (!s_ok) tc::mbar_wait_rows(&s_full[buf], (g >> 1) & 1);
-        if (threadIdx.x == 64) tr.log(20, w, j);   // S visible to softmax
-        tc::tc_fence_after();
-        const uint32_t s_tmem = tmem_base + lane_off + buf * ATT_BN;
-        uint32_t r0[32], r1[32];
-        tc::tmem_ld_32x32b_x32(s_tmem, r0);
-        tc::tmem_ld_32x32b_x32(s_tmem + 32, r1);
-        tc::tmem_ld_wait();
-        // keys of this block the row may attend to: all 64 (full dense block), the first kmax (last dense block), or
-        // only the row's own key (diagonal block).  Three code paths so that the common one carries no masks.
-        const bool dense = j < nblk;
-        const int kmax = dense ? p.sep - j * ATT_BN : 0;
-        int c_self = -1;
-        if (!dense) {
-          const int c = i - dstart[j - nblk];
-          if (is_query && c >= 0 && c < ATT_BN) c_self = c;
-        }
-        float bm = -INFINITY;
-        if (dense && kmax >= ATT_BN) {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) bm = fmaxf(bm, fmaxf(__uint_as_float(r0[c]), __uint_as_float(r1[c])));
-        } else if (dense) {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            if (c < kmax) bm = fmaxf(bm, __uint_as_float(r0[c]));
-            if (c + 32 < kmax) bm = fmaxf(bm, __uint_as_float(r1[c]));
-          }
-        } else {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            bm = (c == c_self) ? __uint_as_float(r0[c]) : bm;
-            bm = (c + 32 == c_self) ? __uint_as_float(r1[c]) : bm;
-          }
-        }
-        bm *= p.scale_log2;
-        const bool need = bm > m + kRescaleThreshold;   // also true when m == -inf and the block has a visible key
-        if (__any_sync(0xffffffffu, need)) {
-          const float m_new = need ? bm : m;
-          const float factor = need ? tc::fast_exp2(m - m_new) : 1.0f;   // exp2(-inf) = 0
-          l *= factor;
-          m = m_new;
-          if (j > 0) {
-            // P V of block g-1 must be complete before O is rescaled.  Safe w.r.t. phase parity: this thread has seen
-            // S_g, which was issued after P V of block g-2, so pv_done is at phase g-1 or g.
-            tc::mbar_wait(pv_done, (g - 1) & 1);
-            tc::tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-              uint32_t o[32];
-              const uint32_t o_tmem = tmem_base + lane_off + 128 + c * 32;
-              tc::tmem_ld_32x32b_x32(o_tmem, o);
-              tc::tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < 32; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * factor);
-              tc::tmem_st_32x32b_x32(o_tmem, o);
-            }
-            tc::tmem_st_wait();
-          }
-        }
-        uint32_t pk[32];
-        float psum = 0.f;
-        if (dense && kmax >= ATT_BN) {
-          const float nm = -m;
-#pragma unroll
-          for (int c = 0; c < 16; ++c) {
-            const float a0 = tc::fast_exp2(fmaf(__uint_as_float(r0[2 * c]), p.scale_log2, nm));
-            const float a1 = tc::fast_exp2(fmaf(__uint_as_float(r0[2 * c + 1]), p.scale_log2, nm));
-            const float b0 = tc::fast_exp2(fmaf(__uint_as_float(r1[2 * c]), p.scale_log2, nm));
-            const float b1 = tc::fast_exp2(fmaf(__uint_as_float(r1[2 * c + 1]), p.scale_log2, nm));
-            psum += (a0 + a1) + (b0 + b1);
-            pk[c] = tc::pack_bf16x2(a0, a1);
-            pk[16 + c] = tc::pack_bf16x2(b0, b1);
-          }
-        } else if (dense) {
-#pragma unroll
-          for (int c = 0; c < 16; ++c) {
-            const float a0 = (2 * c < kmax) ? tc::fast_exp2(fmaf(__uint_as_float(r0[2 * c]), p.scale_log2, -m)) : 0.f;
-            const float a1 = (2 * c + 1 < kmax) ? tc::fast_exp2(fmaf(__uint_as_float(r0[2 * c + 1]), p.scale_log2, -m)) : 0.f;
-            const float b0 = (2 * c + 32 < kmax) ? tc::fast_exp2(fmaf(__uint_as_float(r1[2 * c]), p.scale_log2, -m)) : 0.f;
-            const float b1 = (2 * c + 33 < kmax) ? tc::fast_exp2(fmaf(__uint_as_float(r1[2 * c + 1]), p.scale_log2, -m)) : 0.f;
-            psum += (a0 + a1) + (b0 + b1);
-            pk[c] = tc::pack_bf16x2(a0, a1);
-            pk[16 + c] = tc::pack_bf16x2(b0, b1);
-          }
-        } else {
-          // bm is the row's own (scaled) score when it has one; everything else in the block is masked
-          const float pself = c_self >= 0 ? tc::fast_exp2(bm - m) : 0.f;
-          psum = pself;
-          const uint32_t lo = tc::pack_bf16x2(pself, 0.f), hi = tc::pack_bf16x2(0.f, pself);
-          const int cw = c_self >> 1;                      // packed column holding the key (-1 >> 1 == -1: none)
-          const uint32_t word = (c_self & 1) ? hi : lo;
-#pragma unroll
-          for (int c = 0; c < 32; ++c) pk[c] = (c == cw) ? word : 0u;
-        }
-        l += psum;                      // the normaliser is over ALL visible keys; dropout only zeroes entries of P
-        if (p.drop_thr > 0) {
-          // packed word w of pk holds keys (2w, 2w + 1) of this block; four keys share one hash (csrc/dropout.cuh)
-          const uint32_t rid = static_cast<uint32_t>(bh) * p.T + i;
-          const uint32_t kb4 = static_cast<uint32_t>(dense ? j * ATT_BN : dstart[j - nblk]) >> 2;
-#pragma unroll
-          for (int q4 = 0; q4 < 16; ++q4) {
-            const uint32_t hsh = drop_hash(p.drop_seed, rid, kb4 + q4);
-            const uint32_t m0 = (drop_keep_byte(hsh, 0, p.drop_thr) ? 0x0000FFFFu : 0u) | (drop_keep_byte(hsh, 1, p.drop_thr) ? 0xFFFF0000u : 0u);
-            const uint32_t m1 = (drop_keep_byte(hsh, 2, p.drop_thr) ? 0x0000FFFFu : 0u) | (drop_keep_byte(hsh, 3, p.drop_thr) ? 0xFFFF0000u : 0u);
-            pk[2 * q4] &= m0;
-            pk[2 * q4 + 1] &= m1;
-          }
-        }
-        // probe of the NEXT block's scores, issued before the P store and consumed at the top of the loop: the ~300-clock
-        // round trip of a probe of an already complete mbarrier then runs under the store instead of in front of the loads
-        s_ok = tc::mbar_try_wait(&s_full[buf ^ 1], ((g + 1) >> 1) & 1);
-        tc::tmem_st_32x32b_x32(tmem_base + lane_off + buf * ATT_BN, pk);
-        tc::tmem_st_wait();
-        tc::tc_fence_before();
-        tc::mbar_arrive_warp(&p_ready[buf]);
-        if (threadIdx.x == 64) tr.log(21, w, j);   // P published
-      }
-      // ---- epilogue: O / l, lse   (every valid row has seen at least one key: a train key or itself)
-      // o_done advances once per tile (and tile t+1's commit needs this thread's o_empty arrival), so its parity is unambiguous
-      tc::mbar_wait(o_done, tcount & 1);
-      if (threadIdx.x == 64) tr.log(22, w, 0);     // epilogue start
-      tc::tc_fence_after();
-      const float inv_l = (p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f) / l;     // kept probabilities are scaled by 1 / (1 - p)
-      const size_t tokrow = p.batch_major ? static_cast<size_t>(b) * p.T + (valid ? i : 0) : static_cast<size_t>(valid ? i : 0) * p.B + b;
-      __nv_bfloat16* orow = p.out + tokrow * p.ld_out + h * ATT_DH;
-      // software-pipelined: the TMEM load of chunk c+1 is in flight while chunk c is scaled, packed and stored
-      uint32_t raw[2][32];
-      tc::tmem_ld_32x32b_x32(tmem_base + lane_off + 128, raw[0]);
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        tc::tmem_ld_wait();
-        if (c + 1 < 4) tc::tmem_ld_32x32b_x32(tmem_base + lane_off + 128 + (c + 1) * 32, raw[(c + 1) & 1]);
-        if (valid) {
-#pragma unroll
-          for (int e = 0; e < 32; e += 8) {
-            uint4 pk4;
-            pk4.x = tc::pack_bf16x2(__uint_as_float(raw[c & 1][e]) * inv_l, __uint_as_float(raw[c & 1][e + 1]) * inv_l);
-            pk4.y = tc::pack_bf16x2(__uint_as_float(raw[c & 1][e + 2]) * inv_l, __uint_as_float(raw[c & 1][e + 3]) * inv_l);
-            pk4.z = tc::pack_bf16x2(__uint_as_float(raw[c & 1][e + 4]) * inv_l, __uint_as_float(raw[c & 1][e + 5]) * inv_l);
-            pk4.w = tc::pack_bf16x2(__uint_as_float(raw[c & 1][e + 6]) * inv_l, __uint_as_float(raw[c & 1][e + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + c * 32 + e) = pk4;
-          }
-        }
-      }
-      if (valid) p.lse[static_cast<size_t>(bh) * p.T + i] = (m + log2f(l)) * 0.6931471805599453f;
-      tc::tc_fence_before();
-      tc::mbar_arrive_warp(o_empty);
-      if (threadIdx.x == 64) tr.log(23, w, 0);     // epilogue end
-    }
+    __syncthreads();     // this buffer is refilled by the next iteration's loads
   }
 
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem_base, 256);
+  // diagonal key of the query rows (i >= sep), normalisation, stores
+  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int i = i0 + r0 + (lane >> 2) + 8 * r;
+    float lr = quad_sum(l[r]);
+    const bool valid = i < p.T;
+    const bool diag = valid && i >= p.sep;
+    const __nv_bfloat16* qrow = p.qkv + att_tok(valid ? i : 0, b, p.T, p.B, p.batch_major) * p.ld_qkv + h * ATT_DH;
+    float sd = 0.f;
+    if (diag) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane);
+        sd = fmaf(q.x, k.x, fmaf(q.y, k.y, sd));
+      }
+    }
+    sd = quad_sum(sd) * p.scale_log2;
+    if (diag) {
+      const float mn = fmaxf(m[r], sd);
+      const float c = fast_ex2(m[r] - mn);
+      const float pr = fast_ex2(sd - mn);
+      lr = lr * c + pr;
+      m[r] = mn;
+      const float pd = (p.drop_thr > 0 && !drop_keep(p.drop_seed, drow0 + 8 * r, i, p.drop_thr)) ? 0.f : pr;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 v = att_ld2(qrow + 2 * E, j, lane);
+        o[j][2 * r] = fmaf(pd, v.x, o[j][2 * r] * c);
+        o[j][2 * r + 1] = fmaf(pd, v.y, o[j][2 * r + 1] * c);
+      }
+    }
+    if (valid) {
+      const float inv = dscale / lr;
+      __nv_bfloat16* orow = p.out + att_tok(i, b, p.T, p.B, p.batch_major) * p.ld_out + h * ATT_DH;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) att_st2(orow, j, lane, o[j][2 * r] * inv, o[j][2 * r + 1] * inv);
+      if ((lane & 3) == 0) p.lse[static_cast<size_t>(bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+    }
   }
-}
-
-static int make_qkv_map(CUtensorMap* tm, const void* base, int ld, int width, int B, int T, int box_rows, int batch_major) {
-  uint64_t dims[3] = {static_cast<uint64_t>(width), static_cast<uint64_t>(B), static_cast<uint64_t>(T)};
-  uint64_t strides[3] = {0, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(ld) * 2 * B};
-  if (batch_major) { strides[1] = static_cast<uint64_t>(ld) * 2 * T; strides[2] = static_cast<uint64_t>(ld) * 2; }
-  uint32_t box[3] = {64, 1, static_cast<uint32_t>(box_rows)};
-  return make_tensor_map_bf16(tm, base, 3, dims, strides, box, true);
-}
-
-static int check_tc_attn(const pfn_attn_desc* d, const char* who) {
-  PFN_CHECK_ARG(d->dtype == PFN_BF16, "%s: bf16 only", who);
-  PFN_CHECK_ARG(d->dh == ATT_DH, "%s: head dim %d unsupported (tcgen05 path is built for 128)", who, d->dh);
-  PFN_CHECK_ARG(d->ld_qkv % 8 == 0 && d->ld_out % 8 == 0, "%s: leading dims must be multiples of 8", who);
-  PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->qkv) | reinterpret_cast<uintptr_t>(d->out)) & 15) == 0,
-                "%s: qkv/out must be 16-byte aligned", who);
-  return 0;
 }
 
 }  // namespace pfn
@@ -506,12 +186,7 @@ static int check_tc_attn(const pfn_attn_desc* d, const char* who) {
 using namespace pfn;
 
 extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
-  if (int rc = check_attn_desc_public(d, false, "attention_fwd_tc")) return rc;
-  if (int rc = check_tc_attn(d, "attention_fwd_tc")) return rc;
-  CUtensorMap tmQ, tmKV;
-  const int E = d->H * d->dh;
-  if (int rc = make_qkv_map(&tmQ, d->qkv, d->ld_qkv, 3 * E, d->B, d->T, ATT_BM, d->batch_major)) return rc;
-  if (int rc = make_qkv_map(&tmKV, d->qkv, d->ld_qkv, 3 * E, d->B, d->T, ATT_BN, d->batch_major)) return rc;
+  if (int rc = check_tc_attn(d, false, "attention_fwd_tc")) return rc;
   AttnFwdParams p;
   p.T = d->T; p.B = d->B; p.H = d->H; p.sep = d->sep;
   p.scale_log2 = d->scale * 1.4426950408889634f;
@@ -519,19 +194,15 @@ extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
   p.out = reinterpret_cast<__nv_bfloat16*>(d->out); p.ld_out = d->ld_out;
   p.lse = d->lse;
   p.n_qtiles = (d->T + ATT_BM - 1) / ATT_BM;
-  p.total_work = p.n_qtiles * d->B * d->H;
   p.batch_major = d->batch_major;
-  p.trace = g_trace_which == 0 ? g_trace_ptr : nullptr;
-  p.trace_cap = g_trace_cap;
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
+  const long long grid = static_cast<long long>(p.n_qtiles) * d->B * d->H;
+  PFN_CHECK_ARG(grid < (1LL << 31), "attention_fwd_tc: too many tiles");
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     PFN_CUDA_OK(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_FWD_SMEM));
-    PFN_CUDA_OK(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   }
-  int grid = 2 * num_sms();
-  if (grid > p.total_work) grid = p.total_work;
-  attn_fwd_tc_kernel<<<grid, ATT_THREADS, ATT_FWD_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(tmQ, tmKV, p);
+  attn_fwd_tc_kernel<<<static_cast<unsigned>(grid), 128, ATT_FWD_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   PFN_LAUNCH_OK();
   return 0;
 }

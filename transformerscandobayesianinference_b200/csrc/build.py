@@ -1,4 +1,4 @@
-"""In-tree build of libpfn_b200.so (sm_100a only) with plain nvcc; no JIT cache, no torch extension machinery.
+"""In-tree build of libpfn_b200.so (sm_90a only) with plain nvcc; no JIT cache, no torch extension machinery.
 
 `python -m transformerscandobayesianinference_b200.csrc.build` or `__graft_entry__.build()`.
 The shared object lands next to the package (`transformerscandobayesianinference_b200/libpfn_b200.so`) so it
@@ -20,20 +20,18 @@ SOURCES = [
     "runtime.cu",
     "optimizer.cu",
     "gemm_tc.cu",
-    "gemm_tc_c2g.cu",
     "gemm_simt.cu",
     "rowwise.cu",
     "bar_nll.cu",
     "attention_simt.cu",
     "attention_tc.cu",
     "attention_bwd_tc.cu",
-    "attention_bwd_dq.cu",
     "gp_sampler.cu",
     "dropout.cu",
 ]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -50,7 +48,6 @@ def _nvcc():
 
 def _headers():
     hs = [os.path.join(HERE, f) for f in os.listdir(HERE) if f.endswith((".cuh", ".h"))]
-    hs.append(os.path.join(HERE, "gemm_tc.cu"))          # included by gemm_tc_c2g.cu
     hs.append(os.path.join(ROOT, "include", "pfn_b200.h"))
     return hs
 
@@ -87,7 +84,7 @@ def build(force=False, verbose=True):
     need_link = bool(todo) or not os.path.exists(LIB_PATH) or any(
         os.path.getmtime(o) > os.path.getmtime(LIB_PATH) for o in objs)
     if need_link:
-        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         proc = subprocess.run(cmd, capture_output=True, text=True)
         if proc.returncode != 0:
             raise RuntimeError(f"link failed:\n{proc.stdout}\n{proc.stderr}")

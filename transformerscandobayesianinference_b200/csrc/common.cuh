@@ -1,4 +1,4 @@
-// Shared helpers for the PFN sm_100a kernels (error reporting, dtype traits, warp reductions).
+// Shared helpers for the PFN sm_90a kernels (error reporting, dtype traits, warp reductions).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -97,38 +97,7 @@ __device__ __forceinline__ float fast_tanh(float x) {
   return y;
 }
 constexpr float kGeluC0 = 0.7974228190582262f, kGeluC1 = 0.0370038563083048f, kGeluC2 = -0.0003475408844912201f;
-#ifdef PFN_GELU_TANH_F16X2
-// A/B variant (NOT the default; measured 0.81 ms GELU / 0.77 ms GELU' vs 0.72 / 0.77 for the default pair, so halving the
-// MUFU count buys nothing: the epilogue is not MUFU-bound): the transcendental runs on PAIRS of elements as
-// tanh.approx.f16x2 (one MUFU op per two elements; the argument
-// |u q| <= ~14 and the result in [-1, 1] are comfortably inside fp16, its 2^-11 relative error matches tanh.approx.f32).
-__device__ __forceinline__ void gelu_tanh_pair(float za, float zb, float& ta, float& tb) {
-  uint32_t packed, res;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(packed) : "f"(zb), "f"(za));      // low half = za, high half = zb
-  asm("tanh.approx.f16x2 %0, %1;" : "=r"(res) : "r"(packed));
-  asm("{\n\t.reg .f16 lo, hi;\n\tmov.b32 {lo, hi}, %2;\n\tcvt.f32.f16 %0, lo;\n\tcvt.f32.f16 %1, hi;\n\t}" : "=f"(ta), "=f"(tb) : "r"(res));
-}
-__device__ __forceinline__ void gelu_fast2(float& a, float& b) {
-  const float a2 = fminf(a * a, 80.0f), b2 = fminf(b * b, 80.0f);
-  float ta, tb;
-  gelu_tanh_pair(a * fmaf(a2, fmaf(a2, kGeluC2, kGeluC1), kGeluC0), b * fmaf(b2, fmaf(b2, kGeluC2, kGeluC1), kGeluC0), ta, tb);
-  const float ha = 0.5f * a, hb = 0.5f * b;
-  a = fmaf(ha, ta, ha);
-  b = fmaf(hb, tb, hb);
-}
-// returns GELU'(a), GELU'(b)
-__device__ __forceinline__ void gelu_grad_fast2(float& a, float& b) {
-  const float a2 = fminf(a * a, 80.0f), b2 = fminf(b * b, 80.0f);
-  float ta, tb;
-  gelu_tanh_pair(a * fmaf(a2, fmaf(a2, kGeluC2, kGeluC1), kGeluC0), b * fmaf(b2, fmaf(b2, kGeluC2, kGeluC1), kGeluC0), ta, tb);
-  const float da = fmaf(a2, fmaf(a2, 2.5f * kGeluC2, 1.5f * kGeluC1), 0.5f * kGeluC0);
-  const float db = fmaf(b2, fmaf(b2, 2.5f * kGeluC2, 1.5f * kGeluC1), 0.5f * kGeluC0);
-  a = fmaf(a * da, fmaf(-ta, ta, 1.0f), fmaf(0.5f, ta, 0.5f));
-  b = fmaf(b * db, fmaf(-tb, tb, 1.0f), fmaf(0.5f, tb, 0.5f));
-}
-#endif
-// Measured A/B on one B200 (tools/ab_gemm.py, 512000x1024x512): GELU epilogue 0.735 ms with the exp/rcp form vs 0.808 ms with
-// tanh.approx; GELU' epilogue 0.766 ms with tanh.approx vs 0.822 ms with exp/rcp -- so each uses the form that won.
+// GELU uses the exp/rcp form of the sigmoid, GELU' the tanh form (both the same approximant).
 constexpr float kGeluK = -2.8853900817779268f;   // -2 log2(e)
 __device__ __forceinline__ float gelu_fast(float u) {
   // u Phi(u), Phi = 1 / (1 + 2^(K u q(u^2)))  (identical to 0.5 (1 + tanh(u q)); relative accuracy kept in the tails)
@@ -153,76 +122,6 @@ __device__ __forceinline__ void gelu_and_grad_fast(float u, float& g, float& gp)
   const float dp2 = fmaf(u2, fmaf(u2, 10.0f * kGeluC2, 6.0f * kGeluC1), 2.0f * kGeluC0);     // 2 p'(u)
   g = u * phi;
   gp = fmaf(u * dp2, fmaf(-phi, phi, phi), phi);
-}
-
-// ---- packed fp32 pairs (sm_100 FFMA2 / FMUL2 / FADD2): one instruction for two elements.  Measured on one B200
-// (tools/ubench/ffma_rate.cu): scalar FFMA 84 FMA/clk/SM, FFMA2 114.  The GELU + GELU' epilogue of a 128 x 256 tile was
-// 482 instructions per 32 elements, 352 of them on the fma pipe -- more pipe clocks than the tile's MMAs take; in pairs it
-// is 307 / 176.  tools/ab_gemm.py, 512000 x 1024 x 512: GELU + gelu' output 0.94 -> 0.80 ms, GELU alone 0.71 -> 0.63 ms.
-// (Pairs in the bias / residual / MUL epilogues measured 2-10 % SLOWER -- they are not instruction-bound -- and stay scalar; a
-// one-MUFU tanh form of the pair GELU measured 0.87 ms: MUFU.TANH is slower than EX2 + RCP here.  Pairs in the softmax / dS
-// arithmetic of the three attention kernels: no change -- 0.94 / 1.25-1.28 / 1.36-1.38 ms either way -- so those stay scalar.)
-#ifndef PFN_EPI_F32X2
-#define PFN_EPI_F32X2 1
-#endif
-typedef unsigned long long f32x2_t;
-__device__ __forceinline__ f32x2_t pack2(float lo, float hi) {
-  f32x2_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ f32x2_t pack2u(uint32_t lo, uint32_t hi) {     // two fp32 bit patterns (e.g. tcgen05.ld words)
-  f32x2_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(f32x2_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2_t splat2(float c) { return pack2(c, c); }
-__device__ __forceinline__ f32x2_t mul2(f32x2_t a, f32x2_t b) {
-  f32x2_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2_t add2(f32x2_t a, f32x2_t b) {
-  f32x2_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2_t fma2(f32x2_t a, f32x2_t b, f32x2_t c) {
-  f32x2_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-// the shared front end of the pair GELUs: u, min(u^2, 80), Phi(u) = 1 / (1 + 2^(K u q(u^2)))
-__device__ __forceinline__ void gelu_phi2(f32x2_t u, f32x2_t& u2, f32x2_t& phi) {
-  float sa, sb;
-  unpack2(mul2(u, u), sa, sb);
-  u2 = pack2(fminf(sa, 80.0f), fminf(sb, 80.0f));
-  const f32x2_t q = fma2(u2, fma2(u2, splat2(kGeluC2 * kGeluK), splat2(kGeluC1 * kGeluK)), splat2(kGeluC0 * kGeluK));
-  float ea, eb;
-  unpack2(mul2(u, q), ea, eb);
-  float da, db;
-  unpack2(add2(pack2(fast_ex2(ea), fast_ex2(eb)), splat2(1.0f)), da, db);
-  phi = pack2(fast_rcp(da), fast_rcp(db));
-}
-// gelu on a pair (same approximant as gelu_fast)
-__device__ __forceinline__ void gelu_fast_pair(float& a, float& b) {
-  const f32x2_t u = pack2(a, b);
-  f32x2_t u2, phi;
-  gelu_phi2(u, u2, phi);
-  unpack2(mul2(u, phi), a, b);
-}
-// gelu and its derivative on a pair (same approximant as gelu_and_grad_fast; the derivative is evaluated as
-// Phi + (2 p'(u) * u Phi) * (1 - Phi), which differs from the scalar form only in the rounding of the last two products)
-__device__ __forceinline__ void gelu_and_grad_fast_pair(float& a, float& b, float& gpa, float& gpb) {
-  const f32x2_t u = pack2(a, b);
-  f32x2_t u2, phi;
-  gelu_phi2(u, u2, phi);
-  const f32x2_t dp2 = fma2(u2, fma2(u2, splat2(10.0f * kGeluC2), splat2(6.0f * kGeluC1)), splat2(2.0f * kGeluC0));   // 2 p'(u)
-  const f32x2_t g = mul2(u, phi);
-  const f32x2_t omp = fma2(phi, splat2(-1.0f), splat2(1.0f));
-  unpack2(fma2(mul2(dp2, g), omp, phi), gpa, gpb);
-  unpack2(g, a, b);
 }
 
 int num_sms();

@@ -1,4 +1,4 @@
-// fp32-FMA GEMM with the same contract as the tcgen05 path (pfn_gemm_desc): used for the fp32 parity
+// fp32-FMA GEMM with the same contract as the tensor-core path (pfn_gemm_desc): used for the fp32 parity
 // mode and for shapes/alignments the tensor-core kernel does not accept.  64x64x16 tiles, 4x4 micro-tiles.
 #include "common.cuh"
 #include "../../include/pfn_b200.h"
@@ -116,7 +116,7 @@ extern "C" int pfn_gemm_simt(const pfn_gemm_desc* d, void* stream) {
   PFN_CHECK_ARG(d->M > 0 && d->N > 0 && d->K > 0, "gemm_simt: empty problem %d x %d x %d", d->M, d->N, d->K);
   PFN_CHECK_ARG(d->ab_dtype == PFN_F32 || d->ab_dtype == PFN_BF16, "gemm_simt: bad ab_dtype %d", d->ab_dtype);
   PFN_CHECK_ARG(d->epilogue >= 0 && d->epilogue <= PFN_EPI_GELU_BWD, "gemm_simt: bad epilogue %d", d->epilogue);
-  PFN_CHECK_ARG(d->c2_gelu_grad == 0, "gemm_simt: c2_gelu_grad is a tcgen05-path option");
+  PFN_CHECK_ARG(d->c2_gelu_grad == 0, "gemm_simt: c2_gelu_grad is a tensor-core-path option");
   PFN_CHECK_ARG(d->epilogue != PFN_EPI_GELU_BWD || d->aux != nullptr, "gemm_simt: GELU' epilogue needs aux");
   const int num_kb = (d->K + 15) / 16;
   int splits = d->k_splits <= 0 ? 1 : d->k_splits;

@@ -1,6 +1,6 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a.
+// Warp-specialised TMA + wgmma GEMM for sm_90a.
 //
-//   C[M,N] (+)= epilogue( sum_k A(m,k) * B(n,k) )      bf16 operands, fp32 accumulation in TMEM
+//   C[M,N] (+)= epilogue( sum_k A(m,k) * B(n,k) )      bf16 operands, fp32 accumulation in registers
 //
 // Replaces the cuBLASLt addmm calls the reference reaches through nn.Linear / in_proj / out_proj
 // (reference transformer.py:17-18,23,84-85; torch nn/functional.py:6478 `_in_projection_packed`).
@@ -8,22 +8,14 @@
 // Operand storage ("major"):
 //   K-major  : element (i,k) at base + i*ld + k        (activations x, weights W[N,K] for y = x W^T)
 //   MN-major : element (i,k) at base + k*ld + i        (W used for dgrad, dY / X used for wgrad)
-// so forward, dgrad and wgrad all run on the same kernel without any transposed copies in HBM.
+// so forward, dgrad and wgrad all run on the same kernel without any transposed copies in HBM: wgmma reads either
+// layout straight from the 128-byte-swizzled tiles the TMA writes.
 //
-// Structure (one CTA per SM, persistent over work items = output tile x k-split):
-//   warp 0      : TMA producer   (cp.async.bulk.tensor, 128B swizzle, mbarrier complete_tx)
-//   warp 1      : MMA issuer     (one lane issues tcgen05.mma 128 x BLOCK_N x 16, commits to mbarriers)
-//   warps 2..9  : epilogue       (tcgen05.ld TMEM->regs, bias / GELU / residual / GELU'; bf16 tiles are staged in
-//                                 128B-swizzled smem and written with TMA stores, fp32/atomic outputs go direct)
-//   TMEM        : 2 accumulator stages x BLOCK_N fp32 columns (epilogue of tile i overlaps MMA of i+1)
-//
-// CTA2 = true (used whenever N > 128): clusters of two CTAs run tcgen05.mma.cta_group::2 with M = 256.  Each CTA loads its
-// own 128 rows of A and only HALF of the 256-wide B tile (the pair's tensor cores read both halves), which cuts the operand
-// traffic per MAC from 0.0234 to 0.0156 B — the 1-CTA kernel is bound by the ~12 TB/s L2->SM fabric at ~1000 TFLOP/s.
-// The leader CTA's MMA warp issues for the pair; its commits are multicast to the barriers of both CTAs; the leader's
-// `full` barriers collect the TMA bytes of both CTAs; both epilogues drain their own TMEM half and report to the leader.
-#include <stdlib.h>
-
+// Structure (one CTA per 128 x 128 output tile and k-split, two CTAs per SM so one CTA's epilogue overlaps the other's
+// main loop):
+//   warps 0..3, 4..7 : two consumer warpgroups; warpgroup g issues wgmma m64n128k16 for rows [64g, 64g + 64) of the tile
+//                      and runs the epilogue (bias / GELU / residual / GELU' / product / row dot) from its registers
+//   warp 8           : TMA producer (cp.async.bulk.tensor, 128B swizzle, mbarrier complete_tx) over a kStages ring
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "../../include/pfn_b200.h"
@@ -33,620 +25,204 @@ namespace pfn {
 struct GemmTcParams {
   int M, N, K;
   const float* bias;             // [N] fp32 or null
-  const __nv_bfloat16* aux;      // residual (epi add) or pre-activation u (GELU') : [M, ld_aux] bf16, or null
+  const __nv_bfloat16* aux;      // residual / pre-activation (GELU') / factor (MUL) / row-dot partner : [M, ld_aux] bf16, or null
   int ld_aux;
   void* C;                       // bf16 or fp32 [M, ldc]
   int ldc;
   int c_f32;                     // 1 => C is fp32
-  __nv_bfloat16* C2;             // optional second output: pre-activation (only with act == GELU)
+  __nv_bfloat16* C2;             // optional second output of the GELU epilogue
   int ldc2;
   int act;                       // PFN_EPI_*
   int accumulate;                // 1 => atomically add into fp32 C (split-K / grad accumulation)
-  int k_splits;
   int kb_per_split;              // k-blocks (of 64) per split
   int tiles_m, tiles_n;
-  int l2_prefetch;               // 1 => the producer prefetches the next work item's A tile into L2
-  long long* stall;              // debug: per-CTA [8] clock sums: producer wait-empty, MMA wait-full, MMA wait-tempty, epilogue wait-tfull, epilogue wait-staging (store read + group barrier), epilogue column loop, of which tcgen05.wait::ld
-  int tma_store;                 // 1 => bf16 C (and C2) leave through the smem staging buffer + TMA store
   float* rowdot_out;             // PFN_EPI_ROWDOT: [M, rowdot_groups] fp32, += sum over a column group of C * aux
   int rowdot_width, rowdot_groups;
   int c2_grad;                   // GELU with C2: C2 = gelu'(pre) instead of pre
-  int stages;                    // operand ring depth of this launch
-  int data_bytes;                // bytes of ring + staging in front of the barriers
 };
 
 constexpr int kBlockM = 128;
+constexpr int kBlockN = 128;
 constexpr int kBlockK = 64;
-// Epilogue warps: a warp can only read its own quarter (32 lanes) of TMEM, so the unit is 4 warps = 128 rows.  Two column
-// halves x kEpiSub warps per (quarter, half): with kEpiSub = 2 every 32-column step of a half is split into two 16-column
-// pieces handled by different warps (16 epilogue warps = 4 per scheduler instead of 2).  Measured A/B on one B200
-// (tools/ab_lib.sh + tools/time_kernels.py, round 2): 16 warps change NOTHING for the GELU / GELU' shapes (0.730 / 0.810 ms
-// vs 0.725 / 0.811 ms) and cost the plain K = 512 shapes 2-3 % -- the epilogues are not latency-bound.  What bounds them is
-// shared-memory / L1 bandwidth: per 128 x 256 tile and 8 k-blocks a CTA moves 256 KB of operands in (TMA writes) and out
-// (tensor-core reads), 64 KB per staged output in and out again, plus the aux rows through L1 -- 640 KB per 4096 MMA clocks
-// for a plain tile (156 B/clk, the K = 512 shapes' ~80 % of peak), 768 KB with the second GELU output.  Default stays 8.
-#ifndef PFN_GEMM_EPI_WARPS
-#define PFN_GEMM_EPI_WARPS 8
-#endif
-constexpr int kNumEpiWarps = PFN_GEMM_EPI_WARPS;
-static_assert(kNumEpiWarps == 8 || kNumEpiWarps == 16, "8 or 16 epilogue warps");
-constexpr int kEpiSub = kNumEpiWarps / 8;        // warps per (TMEM lane quarter, column half)
-constexpr int kCW = 32 / kEpiSub;                // columns one thread handles per 32-column step
-constexpr int kGroupThreads = 128 * kEpiSub;     // threads that share one column half (and its staging buffer)
-constexpr int kNumThreads = 64 + kNumEpiWarps * 32;
+constexpr int kStages = 3;
+constexpr int kABytes = kBlockM * kBlockK * 2;        // 16 KB
+constexpr int kBBytes = kBlockN * kBlockK * 2;        // 16 KB
+constexpr int kNumThreads = 2 * 128 + 32;
+constexpr int kSmemBytes = kStages * (kABytes + kBBytes) + 64 + 1024;   // ring + barriers + 1 KB alignment slack
+static_assert(2 * kSmemBytes <= 232448, "two CTAs per SM must fit the 227 KB of shared memory");
 
-template <int N> struct TmemLd;
-template <> struct TmemLd<32> { static __device__ __forceinline__ void ld(uint32_t a, uint32_t (&v)[32]) { tc::tmem_ld_32x32b_x32(a, v); } };
-template <> struct TmemLd<16> { static __device__ __forceinline__ void ld(uint32_t a, uint32_t (&v)[16]) { tc::tmem_ld_32x32b_x16(a, v); } };
-
-template <int BLOCK_N, bool CTA2 = false>
-struct GemmCfg {
-  static constexpr int kABytes = kBlockM * kBlockK * 2;                       // 16 KB
-  static constexpr int kBBytes = (CTA2 ? BLOCK_N / 2 : BLOCK_N) * kBlockK * 2;  // a CTA of a pair holds half of the B tile
-  static constexpr int kRingBudget = 212992;                                   // 208 KB of the 227 KB for operands + staging
-  static constexpr int kStagesMax = kRingBudget / (kABytes + kBBytes) > 6 ? 6 : kRingBudget / (kABytes + kBBytes);   // no staging buffer
-  static constexpr int kStagesStaged = (kRingBudget - kBlockM * BLOCK_N * 2) / (kABytes + kBBytes);
-  static constexpr int kTmemCols = 2 * BLOCK_N;
-  static constexpr int kStageOutBytes = kBlockM * BLOCK_N * 2;   // bf16 output tile (two column halves, one per epilogue group)
-  static constexpr int kRingBytes = kStagesMax * (kABytes + kBBytes);
-  static constexpr int kStagedBytes = kStagesStaged * (kABytes + kBBytes) + kStageOutBytes;
-  // Plain staged launches (no aux rows to read, one output): one more ring stage out of a 224 KB budget.  Measured on the
-  // 512000 x 1536 x 512 in-projection: 0.746 -> 0.722 ms -- its MMA warp waits for operands, not for the epilogue
-  // (tools/gemm_stalls.py).  Launches that read aux keep the smaller footprint: their rows travel through L1, i.e. through
-  // whatever of the 228 KB is NOT shared memory, and lost 2-4 % under the larger budget.
-  static constexpr int kPlainBudget = 229376;
-  static constexpr int kStagesPlainRaw = (kPlainBudget - kStageOutBytes) / (kABytes + kBBytes);
-  static constexpr int kStagesPlain = kStagesPlainRaw > 6 ? 6 : kStagesPlainRaw;
-  static constexpr int kPlainBytes = kStagesPlain * (kABytes + kBBytes) + kStageOutBytes;
-  static constexpr int kDataBytes = kRingBytes > kStagedBytes ? kRingBytes : kStagedBytes;       // default footprint
-  static constexpr int kDataBytesMax = kPlainBytes > kDataBytes ? kPlainBytes : kDataBytes;
-  static constexpr int kBarrierBytes = 512 + 1024;                                                 // barriers + 1 KB alignment slack
-  static constexpr int kSmemBytes = kDataBytes + kBarrierBytes;
-  static constexpr int kSmemBytesMax = kDataBytesMax + kBarrierBytes;
-  static_assert(kSmemBytesMax <= 232448, "exceeds the 227 KB of dynamic shared memory per CTA");
-};
-
-// C2G: the GELU epilogue stores gelu'(pre) in C2 (c2_gelu_grad).  A compile-time switch, instantiated only for the forward
-// linear layout: as a run-time flag its extra live values pushed every instantiation past the register cap (spills).
-template <int BLOCK_N, bool A_MN, bool B_MN, bool CTA2, bool C2G = false>
-__global__ void __launch_bounds__(kNumThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, const GemmTcParams p) {
-  using Cfg = GemmCfg<BLOCK_N, CTA2>;
-  const int STAGES = p.stages;         // ring depth chosen by the launcher (<= Cfg::kStagesMax barriers exist)
+template <bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(kNumThreads, 2)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmTcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  // 1 KB alignment by an OFFSET on the __shared__ symbol (an integer round trip of the pointer makes every access through it a
-  // generic LD.E / ST.E instead of LDS / STS)
+  // 1 KB alignment (128-byte swizzle atoms) by an offset on the __shared__ symbol
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * Cfg::kABytes;
-  uint8_t* sOut = smem + STAGES * (Cfg::kABytes + Cfg::kBBytes);      // only used when p.tma_store
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.data_bytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStagesMax;
-  uint64_t* tfull_bar = empty_bar + Cfg::kStagesMax;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint8_t* sB = smem + kStages * kABytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * (kABytes + kBBytes));
+  uint64_t* empty_bar = full_bar + kStages;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = CTA2 ? tc::cluster_ctarank() : 0u;     // 0 = leader of the pair
-  const bool is_leader = cta_rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    tc::tma_prefetch_desc(&tmA);
-    tc::tma_prefetch_desc(&tmB);
-    if (p.tma_store) { tc::tma_prefetch_desc(&tmC); if (p.C2 != nullptr) tc::tma_prefetch_desc(&tmC2); }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::kStagesMax; ++s) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) {
       tc::mbar_init(&full_bar[s], 1);
-      tc::mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      tc::mbar_init(&tfull_bar[s], 1);
-      tc::mbar_init(&tempty_bar[s], CTA2 ? 2 * kNumEpiWarps : kNumEpiWarps);   // pair: both CTAs' epilogues report to the leader
+      tc::mbar_init(&empty_bar[s], 2);          // one arrival per consumer warpgroup
     }
     tc::mbar_fence_init();
   }
-  if (warp == 2) {
-    if constexpr (CTA2) { tc::tmem_alloc_2cta(tmem_slot, Cfg::kTmemCols); tc::tmem_relinquish_2cta(); }
-    else { tc::tmem_alloc(tmem_slot, Cfg::kTmemCols); tc::tmem_relinquish(); }
-  }
-  tc::tc_fence_before();
-  if constexpr (CTA2) tc::cluster_sync_all(); else __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
+  const int tiles = p.tiles_m * p.tiles_n;
+  const int split = static_cast<int>(blockIdx.x) / tiles;
+  const int tile = static_cast<int>(blockIdx.x) - split * tiles;
+  const int m0 = (tile / p.tiles_n) * kBlockM;
+  const int n0 = (tile % p.tiles_n) * kBlockN;
   const int num_kb_total = (p.K + kBlockK - 1) / kBlockK;
-  const int tiles = p.tiles_m * p.tiles_n;             // tiles_m counts 256-row tiles when CTA2
-  const int total_work = tiles * p.k_splits;
-  const int work0 = CTA2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);   // work items are per pair
-  const int work_stride = CTA2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-  constexpr int kTileM = CTA2 ? 2 * kBlockM : kBlockM;
+  const int kb0 = split * p.kb_per_split;
+  const int kb1 = min(kb0 + p.kb_per_split, num_kb_total);
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (converged warp, elected lane issues)
-    {
-      long long st_prod = 0;
+  if (warp == 8) {
+    // ------------------------------------------------------------------ TMA producer
+    if (lane == 0) {
+      tc::tma_prefetch_desc(&tmA);
+      tc::tma_prefetch_desc(&tmB);
       int stage = 0;
       uint32_t phase = 0;
-      for (int w = work0; w < total_work; w += work_stride) {
-        const int split = w / tiles;
-        const int tile = w - split * tiles;
-        const int m0 = (tile / p.tiles_n) * kTileM + static_cast<int>(cta_rank) * kBlockM;
-        const int n0 = (tile % p.tiles_n) * BLOCK_N;
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(kb0 + p.kb_per_split, num_kb_total);
-        // Pull the NEXT work item's A tile (the streamed operand) into L2 now: its TMA loads then see L2 latency instead
-        // of DRAM latency, which the short smem ring cannot cover.
-        if (p.l2_prefetch && w + work_stride < total_work && tc::elect_one()) {
-          const int wn = w + work_stride;
-          const int splitn = wn / tiles;
-          const int tilen = wn - splitn * tiles;
-          const int mn = (tilen / p.tiles_n) * kTileM + static_cast<int>(cta_rank) * kBlockM;
-          const int kn0 = splitn * p.kb_per_split;
-          const int kn1 = min(kn0 + p.kb_per_split, num_kb_total);
-          for (int kb = kn0; kb < kn1; ++kb) {
-            if constexpr (!A_MN) {
-              tc::tma_prefetch_2d(&tmA, kb * kBlockK, mn);
-            } else {
-              tc::tma_prefetch_2d(&tmA, mn, kb * kBlockK);
-              tc::tma_prefetch_2d(&tmA, mn + 64, kb * kBlockK);
-            }
-          }
+      for (int kb = kb0; kb < kb1; ++kb) {
+        tc::mbar_wait_suspend(&empty_bar[stage], phase ^ 1);
+        uint8_t* a_dst = sA + stage * kABytes;
+        uint8_t* b_dst = sB + stage * kBBytes;
+        const int k0 = kb * kBlockK;
+        tc::mbar_expect_tx(&full_bar[stage], kABytes + kBBytes);
+        if constexpr (!A_MN) {
+          tc::tma_load_2d(a_dst, &tmA, &full_bar[stage], k0, m0);
+        } else {
+          tc::tma_load_2d(a_dst, &tmA, &full_bar[stage], m0, k0);
+          tc::tma_load_2d(a_dst + 8192, &tmA, &full_bar[stage], m0 + 64, k0);
         }
-        __syncwarp();
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if (p.stall != nullptr) { const long long t0 = clock64(); tc::mbar_wait(&empty_bar[stage], phase ^ 1); st_prod += clock64() - t0; }
-          else tc::mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* a_dst = sA + stage * Cfg::kABytes;
-          uint8_t* b_dst = sB + stage * Cfg::kBBytes;
-          const int k0 = kb * kBlockK;
-          if (tc::elect_one()) {
-            if constexpr (!CTA2) {
-              tc::mbar_expect_tx(&full_bar[stage], Cfg::kABytes + Cfg::kBBytes);
-              if constexpr (!A_MN) {
-                tc::tma_load_2d(a_dst, &tmA, &full_bar[stage], k0, m0);
-              } else {
-#pragma unroll
-                for (int c = 0; c < kBlockM / 64; ++c)
-                  tc::tma_load_2d(a_dst + c * 8192, &tmA, &full_bar[stage], m0 + c * 64, k0);
-              }
-              if constexpr (!B_MN) {
-                tc::tma_load_2d(b_dst, &tmB, &full_bar[stage], k0, n0);
-              } else {
-#pragma unroll
-                for (int c = 0; c < BLOCK_N / 64; ++c)
-                  tc::tma_load_2d(b_dst + c * 8192, &tmB, &full_bar[stage], n0 + c * 64, k0);
-              }
-            } else {
-              // pair: the leader arms its `full` barrier for the bytes of BOTH CTAs; each CTA loads its own A rows and its
-              // half (rank * BLOCK_N/2) of the B tile; all transaction bytes complete on the leader's barrier.
-              if (is_leader) tc::mbar_expect_tx(&full_bar[stage], 2 * (Cfg::kABytes + Cfg::kBBytes));
-              const int nh = n0 + static_cast<int>(cta_rank) * (BLOCK_N / 2);
-              if constexpr (!A_MN) {
-                tc::tma_load_2d_2cta(a_dst, &tmA, &full_bar[stage], k0, m0);
-              } else {
-#pragma unroll
-                for (int c = 0; c < kBlockM / 64; ++c)
-                  tc::tma_load_2d_2cta(a_dst + c * 8192, &tmA, &full_bar[stage], m0 + c * 64, k0);
-              }
-              if constexpr (!B_MN) {
-                tc::tma_load_2d_2cta(b_dst, &tmB, &full_bar[stage], k0, nh);
-              } else {
-#pragma unroll
-                for (int c = 0; c < BLOCK_N / 128; ++c)
-                  tc::tma_load_2d_2cta(b_dst + c * 8192, &tmB, &full_bar[stage], nh + c * 64, k0);
-              }
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if constexpr (!B_MN) {
+          tc::tma_load_2d(b_dst, &tmB, &full_bar[stage], k0, n0);
+        } else {
+          tc::tma_load_2d(b_dst, &tmB, &full_bar[stage], n0, k0);
+          tc::tma_load_2d(b_dst + 8192, &tmB, &full_bar[stage], n0 + 64, k0);
         }
-      }
-      if (p.stall != nullptr && lane == 0) p.stall[blockIdx.x * 8 + 0] = st_prod;
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (converged warp, elected lane issues)
-    if (!CTA2 || is_leader) {
-      constexpr uint32_t idesc = tc::umma_idesc_bf16(kTileM, BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0);
-      // The tcgen05 issue queue is shallow (tools/ubench/mma_queue.cu: an instruction-latency gap in this warp is tensor-pipe
-      // idle time, and a ready mbarrier probe costs ~125 clocks), so every barrier this warp needs is probed one step EARLY:
-      // the probe's shared-memory round trip overlaps the (blocking) issue of the current MMAs, and the slow spinning wait is
-      // only taken when the early probe said "not yet".
-      const bool timing = p.stall != nullptr;
-      long long st_full = 0, st_tempty = 0;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      bool full_ready = false;      // early probe result for full_bar[stage] / phase
-      bool tempty_ready = false;    // early probe result for the next tile's accumulator stage
-      for (int w = work0; w < total_work; w += work_stride, ++it) {
-        const int split = w / tiles;
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(kb0 + p.kb_per_split, num_kb_total);
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        if (!tempty_ready) {
-          const long long t0 = timing ? clock64() : 0;
-          tc::mbar_wait(&tempty_bar[as], aphase ^ 1);
-          if (timing) st_tempty += clock64() - t0;
-        }
-        tempty_ready = false;
-        tc::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BLOCK_N;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if (!full_ready) {
-            const long long t0 = timing ? clock64() : 0;
-            tc::mbar_wait(&full_bar[stage], phase);
-            if (timing) st_full += clock64() - t0;
-          }
-          tc::tc_fence_after();
-          {
-            // early probes, consumed after the MMAs below have been issued
-            const int ns = (stage + 1 == STAGES) ? 0 : stage + 1;
-            const uint32_t nph = (stage + 1 == STAGES) ? (phase ^ 1) : phase;
-            full_ready = tc::mbar_try_wait(&full_bar[ns], nph);
-            if (kb == kb1 - 1) tempty_ready = tc::mbar_try_wait(&tempty_bar[as ^ 1], (((it + 1) >> 1) & 1) ^ 1);
-          }
-          const uint32_t a_addr = tc::smem_u32(sA + stage * Cfg::kABytes);
-          const uint32_t b_addr = tc::smem_u32(sB + stage * Cfg::kBBytes);
-          if (tc::elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) {
-              // K-major: advance 16 elements (32 B) inside the 128 B swizzle row.
-              // MN-major: advance 16 k-rows (16 * 128 B); LBO = stride between 64-wide M/N chunks.
-              const uint64_t a_desc = A_MN ? tc::umma_smem_desc(a_addr + k * 2048, 8192, 1024)
-                                           : tc::umma_smem_desc(a_addr + k * 32, 16, 1024);
-              const uint64_t b_desc = B_MN ? tc::umma_smem_desc(b_addr + k * 2048, 8192, 1024)
-                                           : tc::umma_smem_desc(b_addr + k * 32, 16, 1024);
-              if constexpr (CTA2) tc::umma_bf16_ss_2cta(d_tmem, a_desc, b_desc, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-              else tc::umma_bf16_ss(d_tmem, a_desc, b_desc, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            }
-            if constexpr (CTA2) {
-              tc::umma_commit_2cta(&empty_bar[stage]);                     // frees the stage in BOTH CTAs
-              if (kb == kb1 - 1) tc::umma_commit_2cta(&tfull_bar[as]);     // wakes BOTH epilogues
-            } else {
-              tc::umma_commit(&empty_bar[stage]);
-              if (kb == kb1 - 1) tc::umma_commit(&tfull_bar[as]);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-      if (p.stall != nullptr && lane == 0) { p.stall[blockIdx.x * 8 + 1] = st_full; p.stall[blockIdx.x * 8 + 2] = st_tempty; }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps
-    // Two column halves; half `half` owns the left / right BLOCK_N/2 columns of the tile and its own staging buffer
-    // ([128 rows x 64 cols] bf16 chunks in the TMA 128-byte swizzle).  Within a half, warp `sub` of a lane quarter handles
-    // columns [sub * kCW, (sub + 1) * kCW) of every 32-column step.
-    const int ew = warp - 2;
-    const int q = warp & 3;              // TMEM lane quarter this warp may access
-    const int half = (ew >> 2) & 1;      // column half
-    const int sub = ew >> 3;             // which kCW-column piece of each 32-column step (0 when kEpiSub == 1)
-    constexpr int COLS_PER_GROUP = BLOCK_N / 2;
-    constexpr int OUT_CHUNKS = COLS_PER_GROUP / 64;
-    constexpr int NQ = kCW / 8;          // 16-byte units (8 bf16) per thread and step
-    uint8_t* stg = sOut + half * (Cfg::kStageOutBytes / 2);
-    const bool issuer = (ew & 3) == 0 && sub == 0 && lane == 0;   // the one thread per half that owns the bulk-store groups
-    const int nbar = 1 + half;                             // named barrier of this half (0 is __syncthreads)
-    // GELU with a second (pre-activation) output: BLOCK_N = 256 tiles run ONE pass over the accumulator in two rounds of 64
-    // columns, staging u in chunk slot 0 and GELU(u) in slot 1 (two bulk stores per round); the narrow tile keeps two passes.
-    const bool gelu_c2 = p.tma_store && p.act == PFN_EPI_GELU && p.C2 != nullptr;
-    const bool dual = gelu_c2 && OUT_CHUNKS >= 2;
-    const bool two_pass = gelu_c2 && !dual;
-    const bool use_aux = p.aux != nullptr;
-    bool store_pending = false;
-    long long st_tfull = 0, st_stage = 0, st_cols = 0, st_ldw = 0;
-    int it = 0;
-    for (int w = work0; w < total_work; w += work_stride, ++it) {
-      const int split = w / tiles;
-      const int tile = w - split * tiles;
-      const int m0 = (tile / p.tiles_n) * kTileM + static_cast<int>(cta_rank) * kBlockM;
-      const int n0 = (tile % p.tiles_n) * BLOCK_N;
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const int trow = q * 32 + lane;
-      const int row = m0 + trow;
-      const bool row_ok = row < p.M;
-      const bool add_bias = p.bias != nullptr && split == 0;
-      const bool aux_now = use_aux && row_ok && (p.act == PFN_EPI_GELU_BWD || split == 0);
-      float rowdot = 0.f;          // PFN_EPI_ROWDOT: this thread's share of sum_n C[row, n] * aux[row, n]
-      const int gcol0 = n0 + half * COLS_PER_GROUP + sub * kCW;          // first column this THREAD handles (step 0)
-      // Software pipeline: the aux (residual / pre-activation) row segment and the TMEM piece of step c+1 are requested
-      // before step c is computed; the very first aux request goes out before the accumulator is even complete.
-      uint4 aq[NQ];               // aux of the next step (two steps ahead measured slower: tools/ab_gemm.py)
-      auto aux_request = [&](int cc, uint4 (&dst)[NQ]) {
-        const __nv_bfloat16* src = p.aux + static_cast<size_t>(row) * p.ld_aux + gcol0 + cc;
-#pragma unroll
-        for (int i = 0; i < NQ; ++i) dst[i] = __ldg(reinterpret_cast<const uint4*>(src) + i);
-      };
-      auto aux_fast = [&](int cc) { return aux_now && gcol0 + cc + kCW <= p.N; };
-      if (aux_fast(0)) aux_request(0, aq);
-      if (use_aux && w + work_stride < total_work) {
-        // pull the NEXT tile's aux row segment (this thread's share of COLS_PER_GROUP bf16) towards L2 while this tile is processed
-        const int w2 = w + work_stride;
-        const int tile2 = w2 - (w2 / tiles) * tiles;
-        const int row2 = (tile2 / p.tiles_n) * kTileM + static_cast<int>(cta_rank) * kBlockM + trow;
-        const int col2 = (tile2 % p.tiles_n) * BLOCK_N + half * COLS_PER_GROUP;
-        if (row2 < p.M && col2 < p.N && sub == 0) {
-          const char* pa = reinterpret_cast<const char*>(p.aux + static_cast<size_t>(row2) * p.ld_aux + col2);
-#pragma unroll
-          for (int o = 0; o < COLS_PER_GROUP * 2; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pa + o));
-        }
-      }
-      if (p.stall != nullptr) { const long long t0 = clock64(); tc::mbar_wait(&tfull_bar[as], aphase); st_tfull += clock64() - t0; }
-      else tc::mbar_wait(&tfull_bar[as], aphase);
-      tc::tc_fence_after();
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) +
-                             static_cast<uint32_t>(as * BLOCK_N + half * COLS_PER_GROUP + sub * kCW);
-      const int npass = (dual || two_pass) ? 2 : 1;
-#pragma unroll 1
-      for (int pass = 0; pass < npass; ++pass) {
-        // two_pass: pass 0 writes the pre-activation (C2), pass 1 writes C.  dual: pass = 64-column round.
-        const bool write_pre_only = two_pass && pass == 0;
-        const int cc_begin = dual ? pass * 64 : 0;
-        const int cc_end = dual ? cc_begin + 64 : COLS_PER_GROUP;
-        if (p.tma_store && store_pending) {
-          // the previous bulk store must have finished READING the staging buffer before it is overwritten
-          const long long t0 = p.stall != nullptr ? clock64() : 0;
-          if (issuer) tc::tma_store_wait_read<0>();
-          asm volatile("bar.sync %0, %1;" ::"r"(nbar), "n"(kGroupThreads) : "memory");
-          if (p.stall != nullptr) st_stage += clock64() - t0;
-          store_pending = false;
-        }
-        const long long tc0 = p.stall != nullptr ? clock64() : 0;
-        uint32_t v[kCW];
-        if (gcol0 + cc_begin < p.N) TmemLd<kCW>::ld(tbase + cc_begin, v);
-        if (pass > 0) {           // (aux never accompanies a second pass today; kept correct)
-          if (aux_fast(cc_begin)) aux_request(cc_begin, aq);
-        }
-#pragma unroll 1
-        for (int cc = cc_begin; cc < cc_end; cc += 32) {
-          const int col0 = gcol0 + cc;
-          if (col0 >= p.N) break;  // warp-uniform
-          if (p.stall != nullptr) { const long long t0 = clock64(); tc::tmem_ld_wait(); st_ldw += clock64() - t0; }
-          else tc::tmem_ld_wait();
-          float f[kCW];
-#pragma unroll
-          for (int i = 0; i < kCW; ++i) f[i] = __uint_as_float(v[i]);
-          const bool have_aux = aux_fast(cc);
-          uint4 ac[NQ];
-#pragma unroll
-          for (int i = 0; i < NQ; ++i) ac[i] = aq[i];
-          if (cc + 32 < cc_end && col0 + 32 < p.N)
-            TmemLd<kCW>::ld(tbase + cc + 32, v);               // in flight while this step is computed
-          if (cc + 32 < cc_end && aux_fast(cc + 32)) aux_request(cc + 32, aq);
-          const bool full_chunk = (col0 + kCW <= p.N);
-          if (add_bias) {
-            if (full_chunk) {
-#pragma unroll
-              for (int i = 0; i < kCW; i += 4) {
-                const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + i));
-                if constexpr (C2G && PFN_EPI_F32X2) {     // the instruction-bound instantiation: bias in pairs as well (0.84 -> 0.80 ms)
-                  unpack2(add2(pack2(f[i], f[i + 1]), pack2(b4.x, b4.y)), f[i], f[i + 1]);
-                  unpack2(add2(pack2(f[i + 2], f[i + 3]), pack2(b4.z, b4.w)), f[i + 2], f[i + 3]);
-                } else {
-                  f[i] += b4.x; f[i + 1] += b4.y; f[i + 2] += b4.z; f[i + 3] += b4.w;
-                }
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < kCW; ++i)
-                if (col0 + i < p.N) f[i] += __ldg(p.bias + col0 + i);
-            }
-          }
-          // 16-byte unit (8 bf16) index of this thread's first column inside its 64-column staging chunk
-          const int u0 = ((cc & 63) >> 3) + sub * NQ;
-          if (C2G && p.act == PFN_EPI_GELU && write_pre_only) {
-#pragma unroll
-            for (int i = 0; i < kCW; ++i) f[i] = gelu_grad_fast(f[i]);       // two-pass layout: this pass stores C2 = gelu'(pre)
-          }
-          if (C2G && p.act == PFN_EPI_GELU && !write_pre_only) {
-            // C2 = gelu'(pre), C = gelu(pre): eight columns at a time so that only eight derivative values are live
-            if (dual) {
-              uint8_t* rowp = stg + trow * 128;
-#pragma unroll
-              for (int i = 0; i < NQ; ++i) {
-                float gp[8];
-#pragma unroll
-#if PFN_EPI_F32X2
-                for (int e = 0; e < 8; e += 2) gelu_and_grad_fast_pair(f[8 * i + e], f[8 * i + e + 1], gp[e], gp[e + 1]);
-#else
-                for (int e = 0; e < 8; ++e) gelu_and_grad_fast(f[8 * i + e], f[8 * i + e], gp[e]);
-#endif
-                uint4 pk;
-                pk.x = tc::pack_bf16x2(gp[0], gp[1]); pk.y = tc::pack_bf16x2(gp[2], gp[3]);
-                pk.z = tc::pack_bf16x2(gp[4], gp[5]); pk.w = tc::pack_bf16x2(gp[6], gp[7]);
-                *reinterpret_cast<uint4*>(rowp + (((u0 + i) ^ (trow & 7)) << 4)) = pk;
-              }
-            } else {
-              __nv_bfloat16* dst = p.C2 + static_cast<size_t>(row) * p.ldc2 + col0;
-              const bool direct = p.C2 != nullptr && row_ok && !p.tma_store;      // (two_pass stored C2 in pass 0)
-#pragma unroll
-              for (int i = 0; i < kCW; ++i) {
-                float gp;
-                gelu_and_grad_fast(f[i], f[i], gp);
-                if (direct && col0 + i < p.N) dst[i] = __float2bfloat16_rn(gp);
-              }
-            }
-          } else if (p.act == PFN_EPI_GELU && !write_pre_only) {
-            if (dual) {
-              // pre-activation goes to chunk slot 0 of the staging buffer (same swizzle as the main output below)
-              uint8_t* rowp = stg + trow * 128;
-#pragma unroll
-              for (int i = 0; i < NQ; ++i) {
-                uint4 pk;
-                pk.x = tc::pack_bf16x2(f[8 * i], f[8 * i + 1]); pk.y = tc::pack_bf16x2(f[8 * i + 2], f[8 * i + 3]);
-                pk.z = tc::pack_bf16x2(f[8 * i + 4], f[8 * i + 5]); pk.w = tc::pack_bf16x2(f[8 * i + 6], f[8 * i + 7]);
-                *reinterpret_cast<uint4*>(rowp + (((u0 + i) ^ (trow & 7)) << 4)) = pk;
-              }
-            } else if (p.C2 != nullptr && row_ok && !p.tma_store) {
-              __nv_bfloat16* dst = p.C2 + static_cast<size_t>(row) * p.ldc2 + col0;
-              if (full_chunk) {
-#pragma unroll
-                for (int i = 0; i < kCW; i += 8) {
-                  uint4 pk;
-                  pk.x = tc::pack_bf16x2(f[i], f[i + 1]); pk.y = tc::pack_bf16x2(f[i + 2], f[i + 3]);
-                  pk.z = tc::pack_bf16x2(f[i + 4], f[i + 5]); pk.w = tc::pack_bf16x2(f[i + 6], f[i + 7]);
-                  *reinterpret_cast<uint4*>(dst + i) = pk;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < kCW; ++i)
-                  if (col0 + i < p.N) dst[i] = __float2bfloat16_rn(f[i]);
-              }
-            }
-#ifdef PFN_GELU_TANH_F16X2
-#pragma unroll
-            for (int i = 0; i < kCW; i += 2) gelu_fast2(f[i], f[i + 1]);
-#else
-#if PFN_EPI_F32X2
-#pragma unroll
-            for (int i = 0; i < kCW; i += 2) gelu_fast_pair(f[i], f[i + 1]);
-#else
-#pragma unroll
-            for (int i = 0; i < kCW; ++i) f[i] = gelu_fast(f[i]);
-#endif
-#endif
-          }
-          if (aux_now && !write_pre_only) {
-            float a[kCW];
-            if (have_aux) {
-#pragma unroll
-              for (int i = 0; i < NQ; ++i) {
-                const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&ac[i]);
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) {
-                  const float2 t = __bfloat1622float2(h[jj]);
-                  a[8 * i + 2 * jj] = t.x; a[8 * i + 2 * jj + 1] = t.y;
-                }
-              }
-            } else {
-              const __nv_bfloat16* src = p.aux + static_cast<size_t>(row) * p.ld_aux + col0;
-#pragma unroll
-              for (int i = 0; i < kCW; ++i) a[i] = (col0 + i < p.N) ? __bfloat162float(src[i]) : 0.f;
-            }
-            if (p.act == PFN_EPI_GELU_BWD) {
-#ifdef PFN_GELU_TANH_F16X2
-#pragma unroll
-              for (int i = 0; i < kCW; i += 2) {
-                gelu_grad_fast2(a[i], a[i + 1]);
-                f[i] *= a[i]; f[i + 1] *= a[i + 1];
-              }
-#else
-#pragma unroll
-              for (int i = 0; i < kCW; ++i) f[i] *= gelu_grad_fast(a[i]);
-#endif
-            } else if (p.act == PFN_EPI_MUL) {
-#pragma unroll
-              for (int i = 0; i < kCW; ++i) f[i] *= a[i];
-            } else if (p.act == PFN_EPI_ROWDOT) {
-              // the products use the bf16-ROUNDED outputs (what the consumer of C will read), so that the row sum is
-              // exactly the dot product of the stored C with aux
-#pragma unroll
-              for (int i = 0; i < kCW; ++i) rowdot = fmaf(__bfloat162float(__float2bfloat16_rn(f[i])), a[i], rowdot);
-            } else {
-#pragma unroll
-              for (int i = 0; i < kCW; ++i) f[i] += a[i];
-            }
-          }
-          if (p.tma_store) {
-            // staging write: 64-column chunk (cc / 64), 16-byte units u0 .. u0 + NQ - 1 of row `trow`, XOR-swizzled
-            uint8_t* rowp = stg + (dual ? 1 : (cc >> 6)) * 16384 + trow * 128;
-#pragma unroll
-            for (int i = 0; i < NQ; ++i) {
-              uint4 pk;
-              pk.x = tc::pack_bf16x2(f[8 * i], f[8 * i + 1]); pk.y = tc::pack_bf16x2(f[8 * i + 2], f[8 * i + 3]);
-              pk.z = tc::pack_bf16x2(f[8 * i + 4], f[8 * i + 5]); pk.w = tc::pack_bf16x2(f[8 * i + 6], f[8 * i + 7]);
-              *reinterpret_cast<uint4*>(rowp + (((u0 + i) ^ (trow & 7)) << 4)) = pk;
-            }
-          } else if (row_ok) {
-            if (p.c_f32) {
-              float* dst = reinterpret_cast<float*>(p.C) + static_cast<size_t>(row) * p.ldc + col0;
-              if (p.accumulate) {
-#pragma unroll
-                for (int i = 0; i < kCW; ++i)
-                  if (col0 + i < p.N) atomicAdd(dst + i, f[i]);
-              } else if (full_chunk) {
-#pragma unroll
-                for (int i = 0; i < kCW; i += 4)
-                  *reinterpret_cast<float4*>(dst + i) = make_float4(f[i], f[i + 1], f[i + 2], f[i + 3]);
-              } else {
-#pragma unroll
-                for (int i = 0; i < kCW; ++i)
-                  if (col0 + i < p.N) dst[i] = f[i];
-              }
-            } else {
-              __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.C) + static_cast<size_t>(row) * p.ldc + col0;
-              if (full_chunk) {
-#pragma unroll
-                for (int i = 0; i < kCW; i += 8) {
-                  uint4 pk;
-                  pk.x = tc::pack_bf16x2(f[i], f[i + 1]); pk.y = tc::pack_bf16x2(f[i + 2], f[i + 3]);
-                  pk.z = tc::pack_bf16x2(f[i + 4], f[i + 5]); pk.w = tc::pack_bf16x2(f[i + 6], f[i + 7]);
-                  *reinterpret_cast<uint4*>(dst + i) = pk;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < kCW; ++i)
-                  if (col0 + i < p.N) dst[i] = __float2bfloat16_rn(f[i]);
-              }
-            }
-          }
-        }
-        if (p.stall != nullptr) st_cols += clock64() - tc0;
-        if (p.act == PFN_EPI_ROWDOT && row_ok && gcol0 < p.N)      // all columns this thread swept lie in ONE group (width % 128 == 0)
-          atomicAdd(p.rowdot_out + static_cast<size_t>(row) * p.rowdot_groups + gcol0 / p.rowdot_width, rowdot);
-        if (pass == npass - 1) {
-          // accumulator stage drained: hand it back to the MMA warp
-          tc::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) { if constexpr (CTA2) tc::mbar_arrive_leader(&tempty_bar[as]); else tc::mbar_arrive(&tempty_bar[as]); }
-        }
-        if (p.tma_store) {
-          tc::fence_proxy_async_smem();                       // generic-proxy staging writes -> visible to the TMA
-          asm volatile("bar.sync %0, %1;" ::"r"(nbar), "n"(kGroupThreads) : "memory");
-          if (issuer) {
-            const int hcol0 = n0 + half * COLS_PER_GROUP;      // first column of this half
-            if (dual) {
-              const int cbase = hcol0 + pass * 64;
-              if (cbase < p.N) {
-                tc::tma_store_2d(&tmC2, stg, cbase, m0);
-                tc::tma_store_2d(&tmC, stg + 16384, cbase, m0);
-              }
-            } else {
-              const CUtensorMap* tm = write_pre_only ? &tmC2 : &tmC;
-#pragma unroll
-              for (int c = 0; c < OUT_CHUNKS; ++c) {
-                const int cbase = hcol0 + c * 64;
-                if (cbase < p.N) tc::tma_store_2d(tm, stg + c * 16384, cbase, m0);   // rows >= M / cols >= N are clipped
-              }
-            }
-            tc::tma_store_commit();
-          }
-          store_pending = true;
-        }
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
     }
-    if (p.tma_store && issuer) tc::tma_store_wait<0>();        // all bulk stores complete before the CTA exits
-    if (p.stall != nullptr && warp == 2 && lane == 0) { p.stall[blockIdx.x * 8 + 3] = st_tfull; p.stall[blockIdx.x * 8 + 4] = st_stage; p.stall[blockIdx.x * 8 + 5] = st_cols; p.stall[blockIdx.x * 8 + 6] = st_ldw; }
+    return;
   }
 
-  tc::tc_fence_before();
-  if constexpr (CTA2) tc::cluster_sync_all(); else __syncthreads();   // pair: nobody frees TMEM / exits while the peer still uses it
-  if (warp == 2) {
-    tc::tc_fence_after();
-    if constexpr (CTA2) tc::tmem_dealloc_2cta(tmem_base, Cfg::kTmemCols); else tc::tmem_dealloc(tmem_base, Cfg::kTmemCols);
+  // -------------------------------------------------------------------- consumer warpgroups: main loop
+  const int g = warp >> 2;                 // warpgroup: rows [64 g, 64 g + 64) of the tile
+  // The first MMA of the tile writes the accumulator (scale-d = 0), so nothing but wgmma defines `acc` until the pipeline
+  // has drained: any other definition inside it makes ptxas serialise the wgmma instructions.
+  float acc[64];
+  {
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      tc::mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_addr = tc::smem_u32(sA + stage * kABytes) + g * 8192;   // K-major: 64 rows x 128 B; MN-major: chunk g
+      const uint32_t b_addr = tc::smem_u32(sB + stage * kBBytes);
+      tc::wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k) {
+        // K-major: advance 16 elements (32 B) inside the 128 B swizzle row.
+        // MN-major: advance 16 k-rows (16 * 128 B); LBO = stride between 64-wide M/N chunks.
+        const uint64_t a_desc = A_MN ? tc::wgmma_smem_desc(a_addr + k * 2048, 8192, 1024)
+                                     : tc::wgmma_smem_desc(a_addr + k * 32, 16, 1024);
+        const uint64_t b_desc = B_MN ? tc::wgmma_smem_desc(b_addr + k * 2048, 8192, 1024)
+                                     : tc::wgmma_smem_desc(b_addr + k * 32, 16, 1024);
+        tc::wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, a_desc, b_desc, (kb > kb0 || k > 0) ? 1u : 0u);
+      }
+      tc::wgmma_commit();
+      tc::wgmma_wait<1>();                 // the previous k-block's MMAs are done: its stage can be refilled
+      if (kb > kb0 && (threadIdx.x & 127) == 0) tc::mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    tc::wgmma_wait<0>();
+    tc::wgmma_fence_regs(acc);
+    if ((threadIdx.x & 127) == 0) tc::mbar_arrive(&empty_bar[prev]);
+  }
+
+  // -------------------------------------------------------------------- epilogue from the accumulator fragments
+  // acc[4 j + e]: row 64 g + 16 (warp & 3) + lane / 4 + 8 (e >> 1), column 8 j + 2 (lane & 3) + (e & 1)
+  const bool add_bias = p.bias != nullptr && split == 0;
+  const bool use_aux = p.aux != nullptr && (p.act == PFN_EPI_GELU_BWD || split == 0);
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = m0 + 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+    const bool row_ok = row < p.M;
+    float rowdot = 0.f;
+    if (row_ok) {
+#pragma unroll
+      for (int j = 0; j < kBlockN / 8; ++j) {
+        const int col = n0 + 8 * j + cq;
+        if (col >= p.N) continue;
+        const bool pair = col + 1 < p.N;
+        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+        if (add_bias) { f0 += __ldg(p.bias + col); if (pair) f1 += __ldg(p.bias + col + 1); }
+        if (p.act == PFN_EPI_GELU) {
+          if (p.C2 != nullptr) {
+            __nv_bfloat16* c2 = p.C2 + static_cast<size_t>(row) * p.ldc2 + col;
+            float s0 = f0, s1 = f1;
+            if (p.c2_grad) { gelu_and_grad_fast(f0, f0, s0); gelu_and_grad_fast(f1, f1, s1); }
+            else { f0 = gelu_fast(f0); f1 = gelu_fast(f1); }
+            if (pair) *reinterpret_cast<uint32_t*>(c2) = tc::pack_bf16x2(s0, s1);
+            else c2[0] = __float2bfloat16_rn(s0);
+          } else {
+            f0 = gelu_fast(f0); f1 = gelu_fast(f1);
+          }
+        }
+        if (use_aux) {
+          const __nv_bfloat16* ap = p.aux + static_cast<size_t>(row) * p.ld_aux + col;
+          float a0, a1 = 0.f;
+          if (pair) {
+            const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ap));
+            a0 = t.x; a1 = t.y;
+          } else {
+            a0 = __bfloat162float(ap[0]);
+          }
+          if (p.act == PFN_EPI_GELU_BWD) {
+            f0 *= gelu_grad_fast(a0); f1 *= gelu_grad_fast(a1);
+          } else if (p.act == PFN_EPI_MUL) {
+            f0 *= a0; f1 *= a1;
+          } else if (p.act == PFN_EPI_ROWDOT) {
+            // the products use the bf16-ROUNDED outputs (what the consumer of C will read), so that the row sum is
+            // exactly the dot product of the stored C with aux
+            rowdot = fmaf(__bfloat162float(__float2bfloat16_rn(f0)), a0, rowdot);
+            if (pair) rowdot = fmaf(__bfloat162float(__float2bfloat16_rn(f1)), a1, rowdot);
+          } else {
+            f0 += a0; f1 += a1;
+          }
+        }
+        if (p.c_f32) {
+          float* dst = reinterpret_cast<float*>(p.C) + static_cast<size_t>(row) * p.ldc + col;
+          if (p.accumulate) { atomicAdd(dst, f0); if (pair) atomicAdd(dst + 1, f1); }
+          else if (pair) *reinterpret_cast<float2*>(dst) = make_float2(f0, f1);
+          else dst[0] = f0;
+        } else {
+          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.C) + static_cast<size_t>(row) * p.ldc + col;
+          if (pair) *reinterpret_cast<uint32_t*>(dst) = tc::pack_bf16x2(f0, f1);
+          else dst[0] = __float2bfloat16_rn(f0);
+        }
+      }
+    }
+    if (p.act == PFN_EPI_ROWDOT) {
+      // the four lanes of a quad hold the same row; the tile's 128 columns lie in one group (width % 128 == 0)
+      rowdot += __shfl_xor_sync(0xffffffffu, rowdot, 1);
+      rowdot += __shfl_xor_sync(0xffffffffu, rowdot, 2);
+      if ((lane & 3) == 0 && row_ok)
+        atomicAdd(p.rowdot_out + static_cast<size_t>(row) * p.rowdot_groups + n0 / p.rowdot_width, rowdot);
+    }
   }
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool CTA2, bool C2G = false>
+template <bool A_MN, bool B_MN>
 static int launch_gemm_tc(const pfn_gemm_desc* d, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N, CTA2>;
-  constexpr int kBRows = CTA2 ? BLOCK_N / 2 : BLOCK_N;   // B rows one CTA loads per stage
   CUtensorMap tmA, tmB;
   {
     uint64_t dims[2], strides[2];
@@ -655,35 +231,12 @@ static int launch_gemm_tc(const pfn_gemm_desc* d, cudaStream_t stream) {
     else       { dims[0] = d->M; dims[1] = d->K; box[0] = 64; box[1] = 64; }
     strides[0] = 0; strides[1] = static_cast<uint64_t>(d->lda) * 2;
     if (int rc = make_tensor_map_bf16(&tmA, d->A, 2, dims, strides, box, true)) return rc;
-    if (!B_MN) { dims[0] = d->K; dims[1] = d->N; box[0] = 64; box[1] = kBRows; }
+    if (!B_MN) { dims[0] = d->K; dims[1] = d->N; box[0] = 64; box[1] = kBlockN; }
     else       { dims[0] = d->N; dims[1] = d->K; box[0] = 64; box[1] = 64; }
     strides[1] = static_cast<uint64_t>(d->ldb) * 2;
     if (int rc = make_tensor_map_bf16(&tmB, d->B, 2, dims, strides, box, true)) return rc;
   }
-  CUtensorMap tmC, tmC2;
-  memset(&tmC, 0, sizeof(tmC));
-  memset(&tmC2, 0, sizeof(tmC2));
-  // bf16 outputs without accumulation leave through smem staging + TMA store (needs 16 B aligned rows)
-  const bool tma_store = d->c_dtype == PFN_BF16 && !d->accumulate && (d->k_splits <= 1) && d->ldc % 8 == 0 &&
-                         (d->C2 == nullptr || d->ldc2 % 8 == 0);
-  if (tma_store) {
-    uint64_t dims[2] = {static_cast<uint64_t>(d->N), static_cast<uint64_t>(d->M)};
-    uint64_t strides[2] = {0, static_cast<uint64_t>(d->ldc) * 2};
-    uint32_t box[2] = {64, kBlockM};
-    if (int rc = make_tensor_map_bf16(&tmC, d->C, 2, dims, strides, box, true)) return rc;
-    if (d->C2 != nullptr) {
-      strides[1] = static_cast<uint64_t>(d->ldc2) * 2;
-      if (int rc = make_tensor_map_bf16(&tmC2, d->C2, 2, dims, strides, box, true)) return rc;
-    }
-  }
   GemmTcParams p;
-  p.tma_store = tma_store ? 1 : 0;
-  p.stall = g_trace_which == 10 ? g_trace_ptr : nullptr;
-  {
-    static int l2pf = -1;
-    if (l2pf < 0) { const char* e = getenv("PFN_GEMM_L2_PREFETCH"); l2pf = (e != nullptr && e[0] == '1') ? 1 : 0; }   // off by default: measured no gain
-    p.l2_prefetch = (l2pf && d->k_splits <= 1) ? 1 : 0;   // only for token-streaming GEMMs (K small, A = activations)
-  }
   p.M = d->M; p.N = d->N; p.K = d->K;
   p.bias = d->bias;
   p.aux = reinterpret_cast<const __nv_bfloat16*>(d->aux);
@@ -692,68 +245,32 @@ static int launch_gemm_tc(const pfn_gemm_desc* d, cudaStream_t stream) {
   p.C2 = reinterpret_cast<__nv_bfloat16*>(d->C2); p.ldc2 = d->ldc2;
   p.act = d->epilogue;
   p.c2_grad = d->c2_gelu_grad;
-  const bool plain = tma_store && d->aux == nullptr && d->C2 == nullptr;
-  p.stages = !tma_store ? Cfg::kStagesMax : (plain ? Cfg::kStagesPlain : Cfg::kStagesStaged);
-  p.data_bytes = plain ? Cfg::kPlainBytes : Cfg::kDataBytes;
-  const int smem_bytes = p.data_bytes + Cfg::kBarrierBytes;
   p.rowdot_out = d->rowdot_out; p.rowdot_width = d->rowdot_width > 0 ? d->rowdot_width : 1;
   p.rowdot_groups = (d->N + p.rowdot_width - 1) / p.rowdot_width;
-  constexpr int kTileM = CTA2 ? 2 * kBlockM : kBlockM;
-  p.tiles_m = (d->M + kTileM - 1) / kTileM;
-  p.tiles_n = (d->N + BLOCK_N - 1) / BLOCK_N;
+  p.tiles_m = (d->M + kBlockM - 1) / kBlockM;
+  p.tiles_n = (d->N + kBlockN - 1) / kBlockN;
   const int num_kb = (d->K + kBlockK - 1) / kBlockK;
   int splits = d->k_splits <= 0 ? 1 : d->k_splits;
   if (splits > num_kb) splits = num_kb;
   const int per = (num_kb + splits - 1) / splits;
   splits = (num_kb + per - 1) / per;
-  p.k_splits = splits;
   p.kb_per_split = per;
   p.accumulate = (d->accumulate || splits > 1) ? 1 : 0;
   PFN_CHECK_ARG(!p.accumulate || p.c_f32, "gemm_tc: accumulate / split-K requires an fp32 output");
-  const int total = p.tiles_m * p.tiles_n * splits;
-  auto kern = gemm_tc_kernel<BLOCK_N, A_MN, B_MN, CTA2, C2G>;
+  const long long total = static_cast<long long>(p.tiles_m) * p.tiles_n * splits;
+  PFN_CHECK_ARG(total < (1LL << 31), "gemm_tc: too many tiles");
+  auto kern = gemm_tc_kernel<A_MN, B_MN>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
-    PFN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytesMax));
+    PFN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
   }
-  if constexpr (!CTA2) {
-    const int grid = total < num_sms() ? total : num_sms();
-    kern<<<grid, kNumThreads, smem_bytes, stream>>>(tmA, tmB, tmC, tmC2, p);
-  } else {
-    const int pairs = num_sms() / 2;
-    const int grid = 2 * (total < pairs ? total : pairs);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kNumThreads);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    PFN_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, tmC2, p));
-  }
+  kern<<<static_cast<unsigned>(total), kNumThreads, kSmemBytes, stream>>>(tmA, tmB, p);
   PFN_LAUNCH_OK();
   return 0;
 }
 
-#ifdef PFN_GEMM_TC_C2G_TU
-// ---- second translation unit (gemm_tc_c2g.cu): ONLY the GELU + gelu' instantiations, built with 16 epilogue warps.  Their
-// epilogue is the critical path of the launch (tools/gemm_stalls.py) and four warps per scheduler hide more of its MUFU /
-// FFMA2 chains (0.84 -> 0.80 ms); every other instantiation stays at 8 warps, where 16 cost 2-3 %.
-__attribute__((visibility("hidden"))) int gemm_tc_launch_c2g(const pfn_gemm_desc* d, cudaStream_t s, bool wide, bool use_pair) {
-  if (wide && use_pair) return launch_gemm_tc<256, false, false, true, true>(d, s);
-  return wide ? launch_gemm_tc<256, false, false, false, true>(d, s) : launch_gemm_tc<128, false, false, false, true>(d, s);
-}
-#else
-__attribute__((visibility("hidden"))) int gemm_tc_launch_c2g(const pfn_gemm_desc* d, cudaStream_t s, bool wide, bool use_pair);   // gemm_tc_c2g.cu (library-internal)
-#endif
-
 }  // namespace pfn
 
-#ifndef PFN_GEMM_TC_C2G_TU
 extern "C" int pfn_gemm_bf16_tc(const pfn_gemm_desc* d, void* stream) {
   using namespace pfn;
   PFN_CHECK_ARG(d != nullptr, "gemm_tc: null descriptor");
@@ -776,31 +293,10 @@ extern "C" int pfn_gemm_bf16_tc(const pfn_gemm_desc* d, void* stream) {
                 "gemm_tc: C2 must be 16-byte aligned with ld multiple of 8");
   PFN_CHECK_ARG(d->bias == nullptr || (reinterpret_cast<uintptr_t>(d->bias) & 15) == 0, "gemm_tc: bias must be 16-byte aligned");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const bool wide = d->N > 128;
-  static int use_pair = -1;
-  if (use_pair < 0) { const char* e = getenv("PFN_GEMM_2CTA"); use_pair = (e == nullptr || e[0] != '0') ? 1 : 0; }
-  const int key = (wide ? 4 : 0) | (d->a_mn_major ? 2 : 0) | (d->b_mn_major ? 1 : 0);
-  if (d->c2_gelu_grad) {
-    PFN_CHECK_ARG((key & 3) == 0, "gemm_tc: c2_gelu_grad is built for K-major operands (the forward linear layout)");
-    return gemm_tc_launch_c2g(d, s, wide, use_pair != 0);
-  }
-  if (wide && use_pair) {
-    switch (key & 3) {
-      case 0: return launch_gemm_tc<256, false, false, true>(d, s);
-      case 1: return launch_gemm_tc<256, false, true, true>(d, s);
-      case 2: return launch_gemm_tc<256, true, false, true>(d, s);
-      default: return launch_gemm_tc<256, true, true, true>(d, s);
-    }
-  }
-  switch (key) {
-    case 0: return launch_gemm_tc<128, false, false, false>(d, s);
-    case 1: return launch_gemm_tc<128, false, true, false>(d, s);
-    case 2: return launch_gemm_tc<128, true, false, false>(d, s);
-    case 3: return launch_gemm_tc<128, true, true, false>(d, s);
-    case 4: return launch_gemm_tc<256, false, false, false>(d, s);
-    case 5: return launch_gemm_tc<256, false, true, false>(d, s);
-    case 6: return launch_gemm_tc<256, true, false, false>(d, s);
-    default: return launch_gemm_tc<256, true, true, false>(d, s);
+  switch ((d->a_mn_major ? 2 : 0) | (d->b_mn_major ? 1 : 0)) {
+    case 0: return launch_gemm_tc<false, false>(d, s);
+    case 1: return launch_gemm_tc<false, true>(d, s);
+    case 2: return launch_gemm_tc<true, false>(d, s);
+    default: return launch_gemm_tc<true, true>(d, s);
   }
 }
-#endif  // !PFN_GEMM_TC_C2G_TU

@@ -256,9 +256,7 @@ extern "C" int pfn_gp_sample(const float* x, const float* z, const float* ls, co
   PFN_CHECK_ARG(kernel_type >= PFN_KERNEL_RBF && kernel_type <= PFN_KERNEL_MATERN52, "gp_sample: bad kernel type %d", kernel_type);
   PFN_CHECK_ARG((reinterpret_cast<uintptr_t>(work) & 15) == 0, "gp_sample: work buffer must be 16-byte aligned");
   const int ldw = (T + 3) & ~3;
-  // Measured on one B200 (tools/time_kernels.py gp, T = 1000): 512 datasets 9.9 ms with TR = 128 vs 7.8 ms with TR = 64;
-  // 296 datasets 4.46 vs 4.94 ms; 148 datasets 2.94 vs 3.51 ms -> the small tile only once the batch no longer fits one
-  // wave of the large one.  (PFN_GP_TR pins one of them for A/B builds.)
+  // the small tile only once the batch no longer fills the GPU with the large one
 #ifdef PFN_GP_TR
   const bool small_tile = PFN_GP_TR == 64;
 #else

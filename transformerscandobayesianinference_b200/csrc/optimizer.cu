@@ -1,6 +1,6 @@
 // Optimizer step glue of the training inner loop (reference train.py:94-97: clip_grad_norm_(1.) then Adam.step()) as two
 // launches over ALL parameter tensors: (1) sum of squared gradients, (2) clip coefficient + Adam update + bf16 copy of the
-// updated weight (the operand the next step's tcgen05 GEMMs read, so no per-step cast pass).  HBM-bound: per element one
+// updated weight (the operand the next step's wgmma GEMMs read, so no per-step cast pass).  HBM-bound: per element one
 // read of g for the norm, then reads of p, g, m, v and writes of p, m, v (+ 2 bytes of shadow).
 // Work is cut into chunks of ADAM_CHUNK elements; `chunk_start[t]` is the first chunk of tensor t (prefix sums), so CTA b
 // finds its tensor by a short binary search -- no per-tensor launches, no host loop.

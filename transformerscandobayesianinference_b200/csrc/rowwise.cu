@@ -44,7 +44,7 @@ template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16*
 }
 
 // Raw (still packed) 8-element vectors: rows are requested one iteration ahead and unpacked when they are used, so a warp
-// keeps two rows of loads in flight (Little: ~44 KB per SM must be outstanding to cover HBM latency at 6.5 TB/s).
+// keeps two rows of loads in flight (by Little's law, tens of KB per SM must be outstanding to cover HBM latency).
 template <typename T> struct Raw8;
 template <> struct Raw8<float> { float4 a, b; };
 template <> struct Raw8<__nv_bfloat16> { uint4 a; };
@@ -334,7 +334,7 @@ layernorm_bwd_kernel(const T* __restrict__ dh, int lddh, const T* __restrict__ z
 
 // bf16 LayerNorm backward with the two input rows staged through a per-warp cp.async ring in shared memory: the bytes in
 // flight no longer live in registers (the register-prefetch kernel above holds 3 rows x 2 tensors = 6 KB per warp, 48 KB per
-// SM, and reaches ~4.0 TB/s), so a warp keeps LN_RING_D - 1 rows (x 2 tensors x 1 KB at E = 512) outstanding.
+// SM), so a warp keeps LN_RING_D - 1 rows (x 2 tensors x 1 KB at E = 512) outstanding.
 #ifndef PFN_LN_RING_D
 #define PFN_LN_RING_D 8
 #endif

@@ -9,9 +9,6 @@
 namespace pfn {
 
 static thread_local char g_err[1024] = "";
-long long* g_trace_ptr = nullptr;
-int g_trace_cap = 0;
-int g_trace_which = 0;
 
 void set_error(const char* fmt, ...) {
   va_list ap;
@@ -24,10 +21,10 @@ const char* get_error() { return g_err; }
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -86,12 +83,4 @@ extern "C" {
 const char* pfn_last_error(void) { return pfn::get_error(); }
 int pfn_version(void) { return PFN_B200_VERSION; }
 int pfn_num_sms(void) { return pfn::num_sms(); }
-// Debug hook (not part of the product surface): log clock64 events of CTA 0 of subsequent attention launches into `buf`
-// ([3 regions][cap][4] int64, zero it first).  which: 0 forward, 1 backward dQ, 2 backward dK/dV.  buf = null switches off.
-int pfn_debug_attention_trace(long long* buf, int cap, int which) {
-  pfn::g_trace_ptr = buf;
-  pfn::g_trace_cap = cap;
-  pfn::g_trace_which = which;
-  return 0;
-}
 }

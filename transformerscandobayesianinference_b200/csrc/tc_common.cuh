@@ -1,6 +1,6 @@
-// Blackwell (sm_100a) primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / fences) and UMMA shared-memory + instruction descriptors.
-// Everything is inline PTX; bit layouts follow the PTX ISA "tcgen05 matrix descriptor" tables.
+// Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma with its
+// shared-memory matrix descriptor, and the warp-level mma.sync / ldmatrix / cp.async used by the attention kernels.
+// Everything is inline PTX; bit layouts follow the PTX ISA "wgmma matrix descriptor" and "mma.m16n8k16" tables.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -15,16 +15,6 @@ namespace tc {
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -44,16 +34,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
-#ifdef PFN_MBAR_BLOCKING_TRY_WAIT
-  // potentially-blocking form: the hardware may suspend the warp; measured wake-up latency ~1000 clocks on B200
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-#else
   // non-blocking probe; the caller spins
   asm volatile(
       "{\n\t.reg .pred P;\n\t"
@@ -62,29 +42,22 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "=r"(ok)
       : "r"(smem_u32(bar)), "r"(parity)
       : "memory");
-#endif
   return ok != 0;
 }
-// Bounded wait: a pipeline bug must trap (=> a CUDA error the host reports) instead of hanging the GPU.
+// Bounded wait: a pipeline bug must trap (=> a CUDA error the host reports) instead of hanging the GPU.  A bare `trap`
+// rather than printf + __trap: a function call in a wgmma consumer would make ptxas serialise its wgmma pipeline.
 #ifndef PFN_MBAR_SPIN_LIMIT
 #define PFN_MBAR_SPIN_LIMIT (1u << 28)
 #endif
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > PFN_MBAR_SPIN_LIMIT) {
-      printf("pfn: mbarrier wait timed out (block %d thread %d bar %p parity %u)\n", blockIdx.x, threadIdx.x,
-             (void*)bar, parity);
-      __trap();
-    }
+    if (++spins > PFN_MBAR_SPIN_LIMIT) asm volatile("trap;");
   }
 }
 
-// Waiters that are NOT on the critical path (TMA producer waiting for a free ring stage, row warps waiting far ahead of the
-// tensor pipe) must not burn the issue slots of the scheduler they share with the MMA-issuing warp, nor hammer the
-// mbarrier unit: a spinning warp issues a probe + branch every few clocks.  `mbar_wait_suspend` uses the potentially
-// blocking mbarrier.try_wait (the hardware parks the warp; wake-up costs up to ~1000 clocks, measured), and
-// `mbar_wait_backoff` sleeps NS nanoseconds between probes after the first one failed.
+// Waiter that is NOT on the critical path (the TMA producer waiting for a free ring stage): the potentially blocking
+// mbarrier.try_wait lets the hardware park the warp instead of spinning on the issue slots the consumers need.
 __device__ __forceinline__ void mbar_wait_suspend(uint64_t* bar, uint32_t parity) {
   uint32_t ok = 0, spins = 0;
   while (true) {
@@ -96,46 +69,9 @@ __device__ __forceinline__ void mbar_wait_suspend(uint64_t* bar, uint32_t parity
         : "r"(smem_u32(bar)), "r"(parity)
         : "memory");
     if (ok) break;
-    if (++spins > PFN_MBAR_SPIN_LIMIT) { printf("pfn: mbarrier try_wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
+    if (++spins > PFN_MBAR_SPIN_LIMIT) asm volatile("trap;");
   }
 }
-template <int NS>
-__device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(NS);
-    if (++spins > PFN_MBAR_SPIN_LIMIT) { printf("pfn: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
-  }
-}
-
-// Warp-granular variants: one lane polls / arrives on behalf of a CONVERGED warp.  Arrivals on one mbarrier serialise
-// (~5 clk each, measured), so 8 warp arrivals instead of 256 thread arrivals take ~1000 clocks off every hand-off.
-__device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
-  if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
-  __syncwarp();
-}
-__device__ __forceinline__ void mbar_arrive_warp(uint64_t* bar) {
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
-}
-
-// Waits of the ROW warps (8-16 warps that all wait for the same barrier at about the same time): with every lane of every
-// warp probing, the probes of one barrier word queue up behind each other; PFN_ROW_POLL_ONE lets lane 0 probe for its warp.
-__device__ __forceinline__ void mbar_wait_rows(uint64_t* bar, uint32_t parity) {
-#if defined(PFN_ROW_POLL_ONE)
-  mbar_wait_warp(bar, parity);
-#elif defined(PFN_ROW_POLL_SLEEP)
-  mbar_wait_backoff<PFN_ROW_POLL_SLEEP>(bar, parity);     // fewer probes per wait (power), up to that many ns of extra latency
-#else
-  mbar_wait(bar, parity);
-#endif
-}
-
-// generic-proxy smem writes -> visible to the async proxy (TMA / UMMA reads)
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-
 // ---------------------------------------------------------------------------------------------
 // TMA
 // ---------------------------------------------------------------------------------------------
@@ -148,255 +84,92 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                            int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-// L2 prefetch of a tile (no smem, no barrier): later cp.async.bulk.tensor loads of the same box hit L2
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0),
-               "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, commit, mma, ld
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// MMA completion -> mbarrier arrive (implicitly fences before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp receives row (lane base + t)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  __syncwarp();   // .sync.aligned: the warp must be converged (callers may come out of divergent code)
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  __syncwarp();   // .sync.aligned: the warp must be converged (callers may come out of divergent code)
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  __syncwarp();
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 32 lanes x 16 consecutive 32-bit columns store (thread t -> lane base + t)
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  __syncwarp();   // .sync.aligned: the warp must be converged (callers may come out of divergent code)
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-      "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&v)[8]) {
-  __syncwarp();
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  __syncwarp();   // .sync.aligned: the warp must be converged (callers may come out of divergent code)
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-      "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-      "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-      "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ float fast_exp2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&t);
 }
-__device__ __forceinline__ void tmem_st_wait() {
-  __syncwarp();
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
 
 // ---------------------------------------------------------------------------------------------
-// 2-CTA (cta_group::2) variants: a cluster of two CTAs on one TPC cooperates on M=256 MMAs; each CTA holds its own
-// 128 rows of A and HALF of the B tile, so every SM receives one third less operand traffic per MAC.
-// shared::cluster addresses carry the CTA rank in bit 24: clearing it addresses the same offset in the even (leader) CTA.
-// ---------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load issued by either CTA of the pair; completes transaction bytes on the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_2d_2cta(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// MMA completion -> arrive on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-// arrive on the LEADER CTA's copy of a barrier (from either CTA)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// UMMA descriptors (sm_100 "version 1" matrix descriptor, 128-byte swizzle only)
+// wgmma shared-memory matrix descriptor (128-byte swizzle only)
 //   bits [0,14)  start address >> 4          bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4     bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
+//   bits [32,46) stride byte offset >> 4     bits [62,64) layout type (1 = SWIZZLE_128B)
 // K-major operand tile  : rows = M/N index, 128 B (64 bf16 of K) per row, 8-row groups SBO apart.
 // MN-major operand tile : rows = K index, 128 B (64 bf16 of M/N) per row, 8-row groups SBO apart,
 //                         next 64-wide M/N chunk LBO apart.
 // ---------------------------------------------------------------------------------------------
-__host__ __device__ constexpr uint64_t umma_smem_desc_hi(uint32_t sbo_bytes) {
-  return (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return umma_smem_desc_hi(sbo_bytes) | (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
+__device__ __forceinline__ uint64_t wgmma_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (1ull << 62) | (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32) |
+         (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16) | static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
 }
 
 // ---------------------------------------------------------------------------------------------
-// Debug event trace (CTA 0 only): private regions per role so that logging is a plain store.
-// Region r holds [ev, a, b, clock64] x cap entries at base + r*4*cap; the counter lives in a register of the role.
+// wgmma (sm_90a warpgroup MMA): one warpgroup (4 warps) computes a 64 x N tile with operands read from shared memory.
 // ---------------------------------------------------------------------------------------------
-struct KernelTrace {
-  long long* base; int cap; int n;
-  __device__ __forceinline__ void log(int ev, int a, int b) {
-    if (base != nullptr && n < cap) {
-      long long* e = base + static_cast<size_t>(n) * 4;
-      e[0] = ev; e[1] = a; e[2] = b; e[3] = clock64();
-      ++n;
-    }
-  }
-};
-__device__ __forceinline__ KernelTrace trace_make(long long* buf, int cap, int region) {
-  KernelTrace t;
-  t.base = (buf != nullptr && blockIdx.x == 0) ? buf + static_cast<size_t>(region) * 4 * cap : nullptr;
-  t.cap = cap; t.n = 0;
-  return t;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// register an accumulator array as live across the asynchronous wgmma (keeps the compiler from moving its uses)
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, bf16 in, fp32 accumulate; TA / TB = 1 for an MN-major operand
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+// ---------------------------------------------------------------------------------------------
+// Warp-level tensor-core MMA (mma.sync m16n8k16, bf16 in, fp32 accumulate) and ldmatrix, used by the attention kernels.
+// Fragment layouts follow the PTX ISA "mma.m16n8k16" figures: lane l holds rows l/4 and l/4 + 8, columns 2 (l % 4) + {0, 1}.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+// 16-byte global -> shared copy (cp.async); src_bytes = 0 zero-fills the destination
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
 }  // namespace tc
@@ -406,11 +179,6 @@ __device__ __forceinline__ KernelTrace trace_make(long long* buf, int cap, int r
 // so the library still loads on a CPU-only box for the symbol-export test).
 // ---------------------------------------------------------------------------------------------
 // dims/strides innermost first; strides in BYTES for dims 1..rank-1 (dim 0 is contiguous).
-// debug trace target shared by the attention kernels (see pfn_debug_attention_trace): which = 0 fwd, 1 dq, 2 dkv
-extern long long* g_trace_ptr;
-extern int g_trace_cap;
-extern int g_trace_which;
-
 int make_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                          const uint32_t* box, bool swizzle128);
 

@@ -3,7 +3,7 @@ the decoder head, expressed as sequences of C-ABI kernel calls (libpfn_b200.so) 
 `torch.autograd.Function`s so that `loss.backward()` in the reference-shaped `train.train` keeps working.
 
 Restates what the reference obtains from `nn.TransformerEncoder` (reference transformer.py:17-18,84;
-torch nn/modules/transformer.py:951-982) — see SURVEY.md Appendix A.1 for the maths.
+torch nn/modules/transformer.py:951-982).
 
 Layout: activations are [T*B, cols] row-major with token row = t*B + b (the reference's sequence-first layout,
 flattened), in the activation dtype (bf16 by default, fp32 in parity mode).  Parameters stay fp32 masters; the
@@ -42,16 +42,11 @@ def act_dtype(precision):
 
 
 def _wgrad_splits(n_tokens, out_rows, out_cols):
-    """Split-K factor of a wgrad GEMM (contraction over the tokens): ONE round of work items over the persistent grid.
-
-    Measured (tools/sweep_wgrad_splits.py, B200): the best factor is the one that gives ~one work item per CTA pair --
-    more splits only add fp32 atomic traffic on the same [out_rows, out_cols] block (qkv 6: 0.59 ms vs 24: 0.62;
-    mlp 9: 0.39 vs 37: 0.45; out-proj 18: 0.22 vs 74: 0.29)."""
-    sms = L.num_sms()
-    if out_cols > 128:      # cta_group::2 path: 256 x 256 tiles, one per CTA pair
-        tiles, units = ((out_rows + 255) // 256) * ((out_cols + 255) // 256), max(sms // 2, 1)
-    else:                   # single-CTA 128 x 128 tiles
-        tiles, units = ((out_rows + 127) // 128) * ((out_cols + 127) // 128), sms
+    """Split-K factor of a wgrad GEMM (contraction over the tokens): ONE round of work items over the GEMM's resident CTAs
+    (two 128 x 128 tiles per SM); more splits only add fp32 atomic traffic on the same [out_rows, out_cols] block
+    (tools/sweep_wgrad_splits.py times the alternatives)."""
+    tiles = ((out_rows + 127) // 128) * ((out_cols + 127) // 128)
+    units = 2 * L.num_sms()
     num_kb = (n_tokens + 63) // 64
     want = max(1, units // max(tiles, 1))
     return max(1, min(want, num_kb // 8 if num_kb >= 16 else 1))
@@ -84,7 +79,7 @@ _GELU_GRAD_FWD = os.environ.get("PFN_B200_GELU_GRAD_FWD", "1") != "0"     # A/B 
 
 def _gelu_linear_fwd(x, w_c, bias):
     """(gelu(x @ w_c^T + bias), s, s_is_grad): what the backward needs of the GELU is either the pre-activation u
-    (s_is_grad False: the dgrad epilogue evaluates gelu'(u)) or, on the tcgen05 path, gelu'(u) itself, produced by the
+    (s_is_grad False: the dgrad epilogue evaluates gelu'(u)) or, on the tensor-core path, gelu'(u) itself, produced by the
     forward epilogue from the sigmoid it has already computed -- the backward dgrad then only multiplies (the epilogues are
     bound by instruction issue, and gelu' alone is ~14 instructions per element)."""
     M, N = x.shape[0], w_c.shape[0]

@@ -7,7 +7,7 @@
 (`state[p] = {"step", "exp_avg", "exp_avg_sq"}`) and update rule, plus `max_grad_norm` (the clip the reference applies just
 before the step).  `step()` hands a device-resident table of (param, grad, exp_avg, exp_avg_sq, bf16 shadow) pointers to
 `pfn_adam_step` (csrc/optimizer.cu): one launch for the gradient norm, one for clip + update; the update also rewrites the
-bf16 copy of every 2-D weight that the next step's tcgen05 GEMMs read (engine._cast picks it up), so the per-step cast pass
+bf16 copy of every 2-D weight that the next step's wgmma GEMMs read (engine._cast picks it up), so the per-step cast pass
 disappears.  CUDA only: on other devices build torch.optim.Adam (train.py does)."""
 import ctypes
 

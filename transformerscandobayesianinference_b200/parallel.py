@@ -1,5 +1,5 @@
 """Data parallelism for the PFN step: one process per GPU (torchrun), independent prior draws per rank, ONE NCCL
-all-reduce of the flat gradient buffer per optimizer step (SURVEY.md section 8e).  The reference has no distributed
+all-reduce of the flat gradient buffer per optimizer step.  The reference has no distributed
 code at all; the semantics implemented here are the ones that reproduce its single-device gradient of the
 global-batch mean: grads are summed over ranks, divided by world size, THEN clipped (reference train.py:95-96),
 and `single_eval_pos` is identical on every rank for a given step (reference train.py:69 draws one per step).

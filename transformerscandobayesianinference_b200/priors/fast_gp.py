@@ -28,7 +28,7 @@ def _compute_device(device):
     if dev.type == 'cuda':
         return dev
     if not torch.cuda.is_available():
-        raise RuntimeError("priors.fast_gp samples with the sm_100a GP kernel; no CUDA device is available "
+        raise RuntimeError("priors.fast_gp samples with the sm_90a GP kernel; no CUDA device is available "
                            "(there is no CPU fallback)")
     return torch.device('cuda', torch.cuda.current_device())
 

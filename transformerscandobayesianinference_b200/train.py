@@ -1,4 +1,4 @@
-"""Drop-in `train.train` (reference train.py:22-135) on the sm_100a engine.
+"""Drop-in `train.train` (reference train.py:22-135) on the sm_90a engine.
 
 Same signature, defaults, prints and return value `(total_loss, positional_losses, model_on_cpu)`.  Differences that
 do not change results: the model forward/backward and the criterion run on hand-written CUDA kernels; the mask is
@@ -274,7 +274,7 @@ _CLI_SAMPLERS = {'weighted': get_weighted_single_eval_pos_sampler, 'uniform': ge
 
 def _cli_parser():
     import argparse
-    ap = argparse.ArgumentParser(prog='train', description='Train a PFN on a prior (sm_100a engine).')
+    ap = argparse.ArgumentParser(prog='train', description='Train a PFN on a prior (sm_90a engine).')
     ap.add_argument('prior', help='gp | mix_gp | ridge')
     ap.add_argument('--config', help='yaml file whose keys override the defaults below')
     ap.add_argument('--loss_function', default='barnll',

@@ -1,4 +1,4 @@
-"""Drop-in `transformer.TransformerModel` (reference transformer.py:13-91) whose forward runs on the sm_100a engine.
+"""Drop-in `transformer.TransformerModel` (reference transformer.py:13-91) whose forward runs on the sm_90a engine.
 
 The module keeps `self.transformer_encoder = nn.TransformerEncoder(...)` purely as the *parameter container*:
 identical state_dict keys (the five reference checkpoints under results/ load with strict=True), identical
@@ -88,11 +88,11 @@ class TransformerModel(nn.Module):
             expect = self.generate_D_q_matrix(T_chk, T_chk - sep_chk).to(src_mask.device)
             if src_mask.shape != expect.shape or not torch.equal(src_mask.to(expect.dtype), expect):
                 raise NotImplementedError(
-                    "src_mask differs from generate_D_q_matrix(T, T - single_eval_pos): the sm_100a attention kernels "
+                    "src_mask differs from generate_D_q_matrix(T, T - single_eval_pos): the sm_90a attention kernels "
                     "implement that mask implicitly and no other (reference transformer.py:60)")
         if not x_src.is_cuda:
             raise RuntimeError(
-                "TransformerModel.forward runs on hand-written sm_100a kernels only; inputs are on "
+                "TransformerModel.forward runs on hand-written sm_90a kernels only; inputs are on "
                 f"{x_src.device}. Move model and data to a CUDA device (there is no CPU fallback).")
         T, B = x_src.shape[0], x_src.shape[1]
         sep = int(single_eval_pos)
