@@ -2,7 +2,11 @@
 
 Debug/measurement aid: wraps the ctypes entry points of libpfn_b200.so with event recording, runs a few steps, prints the
 time per entry point (GEMMs grouped by shape/epilogue/operand layout) and the remainder (torch-side elementwise, Adam, ...).
-Event pairs add launch gaps, so the sum is an upper bound of the kernels' own time."""
+Event pairs add launch gaps, so the sum is an upper bound of the kernels' own time.
+
+For every wgmma GEMM row it also prints the algorithmic HBM bytes (operands, aux, C and C2 once each: the byte formula of
+_lib.PROFILE_GEMM), the achieved TFLOP/s and GB/s, and the share of the floor, floor = max(FLOP / peak, bytes / bandwidth)
+with the H100 SXM data-sheet peaks (dense BF16 989 TFLOP/s, HBM3 3.35 TB/s); the bound that sets the floor is named."""
 import sys, os, collections
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -13,6 +17,8 @@ dev = torch.device("cuda:0")
 T, B, F, E, NL, NH, H, NB, sep = 1000, int(os.environ.get("PFN_BENCH_B", 512)), 1, 512, 6, 1024, 4, 100, 500
 lib = L.load()
 REC = None
+PEAK_FLOPS, PEAK_BW = 989e12, 3.35e12
+GEMM_COST = {}      # label -> (flop, bytes) of one call
 NAMES = ["pfn_gemm_bf16_tc", "pfn_gemm_simt", "pfn_attention_fwd_tc", "pfn_attention_bwd_tc", "pfn_attention_fwd_simt",
          "pfn_attention_bwd_simt", "pfn_embed_fwd", "pfn_embed_bwd", "pfn_layernorm_fwd", "pfn_layernorm_bwd", "pfn_colsum",
          "pfn_bar_nll_fwd", "pfn_bar_nll_bwd", "pfn_gp_sample"]
@@ -26,6 +32,10 @@ def wrap(name):
         if name.startswith("pfn_gemm"):
             d = a[0]._obj
             label = f"gemm M={d.M} N={d.N} K={d.K} epi={d.epilogue} amn={d.a_mn_major} bmn={d.b_mn_major} c2={int(bool(d.C2))} aux={int(bool(d.aux))} cdt={d.c_dtype} ks={d.k_splits}"
+            if name == "pfn_gemm_bf16_tc":
+                esz = 4 if d.c_dtype == L.F32 else 2
+                nbytes = 2.0 * (d.M * d.K + d.N * d.K) + esz * d.M * d.N * (2 if d.C2 else 1) + (2.0 * d.M * d.N if d.aux else 0.0)
+                GEMM_COST[label] = (2.0 * d.M * d.N * d.K, nbytes)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); rc = orig(*a); e1.record()
         REC.append((label, e0, e1))
@@ -70,6 +80,14 @@ rows = sorted(agg.items(), key=lambda kv: -kv[1][1])
 s = 0.0
 print(f"step {total:.2f} ms (with event overhead)")
 for label, (n, t) in rows:
-    print(f"{t / NS:8.3f} ms/step  {n // NS:3d}x  {t / n:7.3f} ms each  {label}")
+    extra = ""
+    if label in GEMM_COST:
+        flop, nbytes = GEMM_COST[label]
+        sec = t / n * 1e-3
+        t_flop, t_bytes = flop / PEAK_FLOPS, nbytes / PEAK_BW
+        extra = (f"  | {nbytes / 1e9:6.3f} GB {flop / sec / 1e12:6.1f} TFLOP/s {nbytes / sec / 1e9:7.1f} GB/s"
+                 f"  floor {max(t_flop, t_bytes) * 1e3:6.3f} ms ({'tensor' if t_flop >= t_bytes else 'HBM'})"
+                 f"  {100 * max(t_flop, t_bytes) / sec:5.1f}% of floor")
+    print(f"{t / NS:8.3f} ms/step  {n // NS:3d}x  {t / n:7.3f} ms each  {label}{extra}")
     s += t / NS
 print(f"{s:8.3f} ms/step in C-ABI kernels; {total - s:.3f} ms/step elsewhere (torch elementwise, Adam, clip, launch gaps)")

@@ -16,7 +16,7 @@ for (M, Nn, name) in [(1536, 512, "qkv"), (1024, 512, "mlp1"), (512, 1024, "mlp2
     A = torch.randn(N, M, device=dev).to(torch.bfloat16); Bm = torch.randn(N, Nn, device=dev).to(torch.bfloat16)
     C = torch.zeros(M, Nn, device=dev)
     res = []
-    for ks in (2, 3, 4, 6, 9, 12, 18, 24, 37, 74):
+    for ks in (2, 3, 4, 5, 6, 8, 9, 11, 12, 16, 18, 24, 33, 37, 74):
         ms = t(lambda: L.gemm(A, Bm, C, a_mn_major=True, b_mn_major=True, M=M, N=Nn, K=N, accumulate=True, k_splits=ks, use_tc=True))
         res.append(f"{ks}:{ms:.3f}")
     print(f"{name} wgrad {M}x{Nn}: " + "  ".join(res), flush=True)

@@ -48,8 +48,8 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int make_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                         const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128) {
+int make_tensor_map(CUtensorMap* out, const void* base, bool f32, int rank, const uint64_t* dims,
+                    const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128) {
   EncodeTiledFn fn = get_encode_fn();
   PFN_CHECK_ARG(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
   PFN_CHECK_ARG((reinterpret_cast<uintptr_t>(base) & 15) == 0, "TMA base pointer %p not 16-byte aligned", base);
@@ -67,7 +67,8 @@ int make_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const uin
       gstr[i - 1] = strides_bytes[i];
     }
   }
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim,
+  CUresult r = fn(out, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                  static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim,
                   gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

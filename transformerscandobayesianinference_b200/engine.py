@@ -42,9 +42,11 @@ def act_dtype(precision):
 
 
 def _wgrad_splits(n_tokens, out_rows, out_cols):
-    """Split-K factor of a wgrad GEMM (contraction over the tokens): ONE round of work items over the GEMM's resident CTAs
-    (two 128 x 128 tiles per SM); more splits only add fp32 atomic traffic on the same [out_rows, out_cols] block
-    (tools/sweep_wgrad_splits.py times the alternatives)."""
+    """Split-K factor of a wgrad GEMM (contraction over the tokens): about two work units (128 x 128 tile, k-split) per
+    SM.  The persistent GEMM runs one CTA per SM whose two consumer warpgroups take the CTA's units in turn, so two units
+    per CTA keep the tensor pipe busy from the first main loop to the last while the first unit's fp32 reduce-add
+    epilogue overlaps the second's main loop; more splits only add reduce-add traffic on the same
+    [out_rows, out_cols] block (tools/sweep_wgrad_splits.py times the alternatives)."""
     tiles = ((out_rows + 127) // 128) * ((out_cols + 127) // 128)
     units = 2 * L.num_sms()
     num_kb = (n_tokens + 63) // 64
@@ -105,7 +107,7 @@ def _linear_dgrad(dy, w_c, *, aux=None, epilogue=L.EPI_NONE, rowdot=None):
 
 
 def _linear_wgrad(dy, x, dw, rows=None, cols=None):
-    """dw[N,K] += dy^T @ x.  dy [M,N], x [M,K] both read in place as MN-major operands; fp32 atomic split-K."""
+    """dw[N,K] += dy^T @ x.  dy [M,N], x [M,K] both read in place as MN-major operands; fp32 split-K (TMA reduce-add)."""
     n_tok = dy.shape[0]
     N = dw.shape[0] if rows is None else rows
     K = dw.shape[1] if cols is None else cols
