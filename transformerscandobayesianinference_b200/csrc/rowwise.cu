@@ -2,8 +2,6 @@
 // One warp per token row, 16-byte vector accesses, fp32 statistics; column reductions (dgamma, dbeta, bias
 // gradients) are accumulated per lane across the rows a warp owns, combined per CTA in shared memory and
 // flushed with one atomicAdd per column per CTA.
-#include <type_traits>
-
 #include "common.cuh"
 #include "../../include/pfn_b200.h"
 
@@ -41,27 +39,6 @@ template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16*
   pk.x = *reinterpret_cast<uint32_t*>(&t0); pk.y = *reinterpret_cast<uint32_t*>(&t1);
   pk.z = *reinterpret_cast<uint32_t*>(&t2); pk.w = *reinterpret_cast<uint32_t*>(&t3);
   *reinterpret_cast<uint4*>(p) = pk;
-}
-
-// Raw (still packed) 8-element vectors: rows are requested one iteration ahead and unpacked when they are used, so a warp
-// keeps two rows of loads in flight (by Little's law, tens of KB per SM must be outstanding to cover HBM latency).
-template <typename T> struct Raw8;
-template <> struct Raw8<float> { float4 a, b; };
-template <> struct Raw8<__nv_bfloat16> { uint4 a; };
-__device__ __forceinline__ void load_raw8(const float* p, Raw8<float>& r) {
-  r.a = *reinterpret_cast<const float4*>(p); r.b = *reinterpret_cast<const float4*>(p + 4);
-}
-__device__ __forceinline__ void load_raw8(const __nv_bfloat16* p, Raw8<__nv_bfloat16>& r) { r.a = *reinterpret_cast<const uint4*>(p); }
-__device__ __forceinline__ void unpack8(const Raw8<float>& r, float (&v)[8]) {
-  v[0] = r.a.x; v[1] = r.a.y; v[2] = r.a.z; v[3] = r.a.w; v[4] = r.b.x; v[5] = r.b.y; v[6] = r.b.z; v[7] = r.b.w;
-}
-__device__ __forceinline__ void unpack8(const Raw8<__nv_bfloat16>& r, float (&v)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&r.a);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 t = __bfloat1622float2(h[j]);
-    v[2 * j] = t.x; v[2 * j + 1] = t.y;
-  }
 }
 
 // --------------------------------------------------------------------------------------------
@@ -141,337 +118,46 @@ embed_bwd_kernel(const T* __restrict__ dout, const float* __restrict__ x, const 
 }
 
 // --------------------------------------------------------------------------------------------
-// LayerNorm forward / backward.  NCH = 8-element chunks per lane (E <= 256*NCH).
+// LayerNorm forward / backward.  One warp per row, NCH = 8-element chunks per lane (E <= 256*NCH).  Each warp stages its
+// input rows through a private cp.async ring in shared memory and reduces one row while the next DEPTH - 1 are in flight,
+// so the bytes in flight take no registers.  That matters most in the backward, whose three per-lane column accumulators
+// need twice the registers of the forward: it runs half the forward's 8-warp CTAs per SM.  A ring slot holds columns
+// [0, ROW) of one row as they lie in memory, so a lane's chunk sits at the same column offset in the slot as in the row.
 // --------------------------------------------------------------------------------------------
 template <typename T, int NCH>
-__global__ void __launch_bounds__(256)
+struct LnRing {
+  static constexpr int ROW = NCH * 256;                         // elements of one staged row
+  static constexpr int ROW_BYTES = ROW * sizeof(T);
+  // Two forward CTAs and one backward CTA per SM; rows of at most 512 B run twice as many, because with so little work
+  // per row the warps of one or two CTAs cannot hide each row's shuffle reductions, and no ring depth makes up for it
+  // (measured at bf16 E = 128 on an H100).
+  static constexpr int FWD_CTAS = ROW_BYTES <= 512 ? 4 : 2, BWD_CTAS = FWD_CTAS / 2;
+  // 128 KB of ring per SM in either direction (8 rows at bf16 E = 512), but at least 3 rows, so that two stay in flight
+  // beyond the one being reduced.
+  static constexpr int DEPTH = 8192 / (BWD_CTAS * ROW_BYTES) > 3 ? 8192 / (BWD_CTAS * ROW_BYTES) : 3;
+  static constexpr size_t WARP_BYTES = static_cast<size_t>(DEPTH) * ROW_BYTES;  // one tensor's ring of one warp
+};
+
+// One lane's 8-element chunk, global -> shared: one 16-byte cp.async for bf16, two for fp32.
+template <typename T>
+__device__ __forceinline__ void ln_cp_async8(T* smem_dst, const T* gsrc) {
+#pragma unroll
+  for (int k = 0; k < 8; k += 16 / static_cast<int>(sizeof(T)))
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;"
+                 ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(smem_dst + k))), "l"(gsrc + k) : "memory");
+}
+
+template <typename T, int NCH>
+__global__ void __launch_bounds__(256, LnRing<T, NCH>::FWD_CTAS)
 layernorm_fwd_kernel(const T* __restrict__ z, int ldz, const float* __restrict__ gamma, const float* __restrict__ beta,
                      T* __restrict__ h, int ldh, float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows,
                      int E, float eps) {
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  const float inv_e = 1.0f / static_cast<float>(E);
-  Raw8<T> nxt[NCH];
-  if (warp < rows) {
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) load_raw8(z + static_cast<size_t>(warp) * ldz + col, nxt[c]);
-    }
-  }
-  for (int row = warp; row < rows; row += nwarps) {
-    float v[NCH][8];
-    float s = 0.f;
-    Raw8<T> cur[NCH];
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) cur[c] = nxt[c];
-    if (row + nwarps < rows) {
-#pragma unroll
-      for (int c = 0; c < NCH; ++c) {
-        const int col = (c * 32 + lane) * 8;
-        if (col < E) load_raw8(z + static_cast<size_t>(row + nwarps) * ldz + col, nxt[c]);
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) {
-        unpack8(cur[c], v[c]);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s += v[c][i];
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[c][i] = 0.f;
-      }
-    }
-    const float mean = warp_sum(s) * inv_e;
-    float ss = 0.f;
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { const float dlt = v[c][i] - mean; ss = fmaf(dlt, dlt, ss); }
-      }
-    }
-    const float var = warp_sum(ss) * inv_e;
-    const float rstd = rsqrtf(var + eps);
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) {
-        float g[8], b[8], o[8];
-        load8<float>(gamma + col, g);
-        load8<float>(beta + col, b);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) o[i] = fmaf((v[c][i] - mean) * rstd, g[i], b[i]);
-        store8<T>(h + static_cast<size_t>(row) * ldh + col, o);
-      }
-    }
-    if (lane == 0) { mean_out[row] = mean; rstd_out[row] = rstd; }
-  }
-}
-
-#ifndef PFN_LN_BWD_MIN_CTAS
-#define PFN_LN_BWD_MIN_CTAS 1
-#endif
-template <typename T, int NCH>
-__global__ void __launch_bounds__(256, PFN_LN_BWD_MIN_CTAS)
-layernorm_bwd_kernel(const T* __restrict__ dh, int lddh, const T* __restrict__ z, int ldz,
-                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
-                     const float* __restrict__ gamma, T* __restrict__ dz, int lddz, float* __restrict__ dgamma,
-                     float* __restrict__ dbeta, float* __restrict__ colsum_out, int rows, int E) {
-  extern __shared__ float sred[];  // [3][E]
-  const int lane = threadIdx.x & 31;
-  const int warp_in_cta = threadIdx.x >> 5;
-  const int warps_per_cta = blockDim.x >> 5;
-  const int warp = blockIdx.x * warps_per_cta + warp_in_cta;
-  const int nwarps = gridDim.x * warps_per_cta;
-  const float inv_e = 1.0f / static_cast<float>(E);
-  for (int i = threadIdx.x; i < 3 * E; i += blockDim.x) sred[i] = 0.f;
-  __syncthreads();
-
-  float ag[NCH][8], ab[NCH][8], ac[NCH][8];
-#pragma unroll
-  for (int c = 0; c < NCH; ++c)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { ag[c][i] = 0.f; ab[c][i] = 0.f; ac[c][i] = 0.f; }
-  float gm[NCH][8];
-#pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < E) load8<float>(gamma + col, gm[c]);
-    else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) gm[c][i] = 0.f;
-    }
-  }
-
-  // The kernel needs ~190 registers (three column accumulators per lane), i.e. ONE 8-warp CTA per SM: occupancy cannot
-  // supply the bytes in flight, so every warp keeps TWO rows of loads outstanding beyond the one it is reducing
-  // (2 CTAs/SM via __launch_bounds__(256, 2) spills and halves the bandwidth: tools/ab_rowwise.py).
-  Raw8<T> nd[NCH], nz[NCH], md[NCH], mz[NCH];      // row + nwarps, row + 2 nwarps
-  float nmean = 0.f, nrstd = 0.f, mmean = 0.f, mrstd = 0.f;
-  auto request = [&](int r, Raw8<T> (&rd)[NCH], Raw8<T> (&rz)[NCH], float& rm, float& rs) {
-    if (r < rows) {
-      rm = mean_in[r]; rs = rstd_in[r];
-#pragma unroll
-      for (int c = 0; c < NCH; ++c) {
-        const int col = (c * 32 + lane) * 8;
-        if (col < E) {
-          load_raw8(dh + static_cast<size_t>(r) * lddh + col, rd[c]);
-          load_raw8(z + static_cast<size_t>(r) * ldz + col, rz[c]);
-        }
-      }
-    }
-  };
-  request(warp, nd, nz, nmean, nrstd);
-  request(warp + nwarps, md, mz, mmean, mrstd);
-  for (int row = warp; row < rows; row += nwarps) {
-    const float mean = nmean, rstd = nrstd;
-    Raw8<T> cd[NCH], cz[NCH];
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) { cd[c] = nd[c]; cz[c] = nz[c]; nd[c] = md[c]; nz[c] = mz[c]; }
-    nmean = mmean; nrstd = mrstd;
-    request(row + 2 * nwarps, md, mz, mmean, mrstd);      // goes out before this row's reductions
-    float xh[NCH][8], g[NCH][8];
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) {
-        float d[8], zz[8];
-        unpack8(cd[c], d);
-        unpack8(cz[c], zz);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          xh[c][i] = (zz[i] - mean) * rstd;
-          g[c][i] = d[i] * gm[c][i];
-          s1 += g[c][i];
-          s2 = fmaf(g[c][i], xh[c][i], s2);
-          ag[c][i] = fmaf(d[i], xh[c][i], ag[c][i]);
-          ab[c][i] += d[i];
-        }
-      }
-    }
-    s1 = warp_sum(s1) * inv_e;
-    s2 = warp_sum(s2) * inv_e;
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) {
-        float o[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          o[i] = rstd * (g[c][i] - s1 - xh[c][i] * s2);
-          ac[c][i] += o[i];
-        }
-        store8<T>(dz + static_cast<size_t>(row) * lddz + col, o);
-      }
-    }
-  }
-  // CTA-level combine, then one atomic per column per CTA
-#pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < E) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        atomicAdd(&sred[col + i], ag[c][i]);
-        atomicAdd(&sred[E + col + i], ab[c][i]);
-        atomicAdd(&sred[2 * E + col + i], ac[c][i]);
-      }
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < E; i += blockDim.x) {
-    if (dgamma != nullptr) atomicAdd(&dgamma[i], sred[i]);
-    if (dbeta != nullptr) atomicAdd(&dbeta[i], sred[E + i]);
-    if (colsum_out != nullptr) atomicAdd(&colsum_out[i], sred[2 * E + i]);
-  }
-}
-
-// bf16 LayerNorm backward with the two input rows staged through a per-warp cp.async ring in shared memory: the bytes in
-// flight no longer live in registers (the register-prefetch kernel above holds 3 rows x 2 tensors = 6 KB per warp, 48 KB per
-// SM), so a warp keeps LN_RING_D - 1 rows (x 2 tensors x 1 KB at E = 512) outstanding.
-#ifndef PFN_LN_RING_D
-#define PFN_LN_RING_D 8
-#endif
-constexpr int LN_RING_D = PFN_LN_RING_D;
-__device__ __forceinline__ void ln_cp_async16(void* smem_dst, const void* gsrc) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(smem_dst))), "l"(gsrc) : "memory");
-}
-template <int NCH>
-__global__ void __launch_bounds__(256, 1)
-layernorm_bwd_ring_kernel(const __nv_bfloat16* __restrict__ dh, int lddh, const __nv_bfloat16* __restrict__ z, int ldz,
-                          const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
-                          const float* __restrict__ gamma, __nv_bfloat16* __restrict__ dz, int lddz,
-                          float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ colsum_out, int rows, int E) {
+  using R = LnRing<T, NCH>;
   extern __shared__ __align__(16) uint8_t ln_smem[];
-  constexpr int ROWB = NCH * 512;                    // bytes of one staged row of one tensor (NCH x 32 lanes x 16 B)
-  float* sred = reinterpret_cast<float*>(ln_smem);   // [3][E]
   const int lane = threadIdx.x & 31;
   const int warp_in_cta = threadIdx.x >> 5;
   const int warps_per_cta = blockDim.x >> 5;
-  uint8_t* ring = ln_smem + ((3 * E * 4 + 15) & ~15) + static_cast<size_t>(warp_in_cta) * LN_RING_D * 2 * ROWB;
-  const int warp = blockIdx.x * warps_per_cta + warp_in_cta;
-  const int nwarps = gridDim.x * warps_per_cta;
-  const float inv_e = 1.0f / static_cast<float>(E);
-  for (int i = threadIdx.x; i < 3 * E; i += blockDim.x) sred[i] = 0.f;
-  __syncthreads();
-
-  float ag[NCH][8], ab[NCH][8], ac[NCH][8], gm[NCH][8];
-#pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { ag[c][i] = 0.f; ab[c][i] = 0.f; ac[c][i] = 0.f; gm[c][i] = 0.f; }
-    const int col = (c * 32 + lane) * 8;
-    if (col < E) load8<float>(gamma + col, gm[c]);
-  }
-  auto issue = [&](int r, int slot) {
-    if (r < rows) {
-#pragma unroll
-      for (int c = 0; c < NCH; ++c) {
-        const int col = (c * 32 + lane) * 8;
-        if (col < E) {
-          ln_cp_async16(ring + (slot * 2 + 0) * ROWB + (c * 32 + lane) * 16, dh + static_cast<size_t>(r) * lddh + col);
-          ln_cp_async16(ring + (slot * 2 + 1) * ROWB + (c * 32 + lane) * 16, z + static_cast<size_t>(r) * ldz + col);
-        }
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
-#pragma unroll
-  for (int k = 0; k < LN_RING_D - 1; ++k) issue(warp + k * nwarps, k);
-  float m_l = 0.f, s_l = 0.f;         // statistics of rows it .. it + 31 of this warp, one per lane
-  int it = 0;
-  for (int row = warp; row < rows; row += nwarps, ++it) {
-    if ((it & 31) == 0) {
-      const long long r = static_cast<long long>(row) + static_cast<long long>(lane) * nwarps;
-      m_l = r < rows ? __ldg(mean_in + r) : 0.f;
-      s_l = r < rows ? __ldg(rstd_in + r) : 0.f;
-    }
-    const float mean = __shfl_sync(0xffffffffu, m_l, it & 31), rstd = __shfl_sync(0xffffffffu, s_l, it & 31);
-    asm volatile("cp.async.wait_group %0;" ::"n"(LN_RING_D - 2) : "memory");
-    __syncwarp();                       // this row has landed for every lane; every lane is done with the slot refilled next
-    const int slot = it % LN_RING_D;
-    Raw8<__nv_bfloat16> cd[NCH], cz[NCH];
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      cd[c].a = *reinterpret_cast<const uint4*>(ring + (slot * 2 + 0) * ROWB + (c * 32 + lane) * 16);
-      cz[c].a = *reinterpret_cast<const uint4*>(ring + (slot * 2 + 1) * ROWB + (c * 32 + lane) * 16);
-    }
-    issue(row + (LN_RING_D - 1) * nwarps, (it + LN_RING_D - 1) % LN_RING_D);
-    float xh[NCH][8], g[NCH][8];
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) {
-        float d[8], zz[8];
-        unpack8(cd[c], d);
-        unpack8(cz[c], zz);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          xh[c][i] = (zz[i] - mean) * rstd;
-          g[c][i] = d[i] * gm[c][i];
-          s1 += g[c][i];
-          s2 = fmaf(g[c][i], xh[c][i], s2);
-          ag[c][i] = fmaf(d[i], xh[c][i], ag[c][i]);
-          ab[c][i] += d[i];
-        }
-      }
-    }
-    s1 = warp_sum(s1) * inv_e;
-    s2 = warp_sum(s2) * inv_e;
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < E) {
-        float o[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          o[i] = rstd * (g[c][i] - s1 - xh[c][i] * s2);
-          ac[c][i] += o[i];
-        }
-        store8<__nv_bfloat16>(dz + static_cast<size_t>(row) * lddz + col, o);
-      }
-    }
-  }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-#pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < E) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        atomicAdd(&sred[col + i], ag[c][i]);
-        atomicAdd(&sred[E + col + i], ab[c][i]);
-        atomicAdd(&sred[2 * E + col + i], ac[c][i]);
-      }
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < E; i += blockDim.x) {
-    if (dgamma != nullptr) atomicAdd(&dgamma[i], sred[i]);
-    if (dbeta != nullptr) atomicAdd(&dbeta[i], sred[E + i]);
-    if (colsum_out != nullptr) atomicAdd(&colsum_out[i], sred[2 * E + i]);
-  }
-}
-
-// bf16 LayerNorm forward with the input rows staged through the same per-warp cp.async ring as the backward.
-template <int NCH>
-__global__ void __launch_bounds__(256, 2)
-layernorm_fwd_ring_kernel(const __nv_bfloat16* __restrict__ z, int ldz, const float* __restrict__ gamma,
-                          const float* __restrict__ beta, __nv_bfloat16* __restrict__ h, int ldh, float* __restrict__ mean_out,
-                          float* __restrict__ rstd_out, int rows, int E, float eps) {
-  extern __shared__ __align__(16) uint8_t ln_smem[];
-  constexpr int ROWB = NCH * 512;
-  const int lane = threadIdx.x & 31;
-  const int warp_in_cta = threadIdx.x >> 5;
-  const int warps_per_cta = blockDim.x >> 5;
-  uint8_t* ring = ln_smem + static_cast<size_t>(warp_in_cta) * LN_RING_D * ROWB;
+  T* ring = reinterpret_cast<T*>(ln_smem) + static_cast<size_t>(warp_in_cta) * R::DEPTH * R::ROW;
   const int warp = blockIdx.x * warps_per_cta + warp_in_cta;
   const int nwarps = gridDim.x * warps_per_cta;
   const float inv_e = 1.0f / static_cast<float>(E);
@@ -488,29 +174,26 @@ layernorm_fwd_ring_kernel(const __nv_bfloat16* __restrict__ z, int ldz, const fl
 #pragma unroll
       for (int c = 0; c < NCH; ++c) {
         const int col = (c * 32 + lane) * 8;
-        if (col < E) ln_cp_async16(ring + slot * ROWB + (c * 32 + lane) * 16, z + static_cast<size_t>(r) * ldz + col);
+        if (col < E) ln_cp_async8(ring + slot * R::ROW + col, z + static_cast<size_t>(r) * ldz + col);
       }
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
 #pragma unroll
-  for (int k = 0; k < LN_RING_D - 1; ++k) issue(warp + k * nwarps, k);
+  for (int k = 0; k < R::DEPTH - 1; ++k) issue(warp + k * nwarps, k);
   int it = 0;
   for (int row = warp; row < rows; row += nwarps, ++it) {
-    asm volatile("cp.async.wait_group %0;" ::"n"(LN_RING_D - 2) : "memory");
-    __syncwarp();
-    const int slot = it % LN_RING_D;
-    Raw8<__nv_bfloat16> cz[NCH];
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) cz[c].a = *reinterpret_cast<const uint4*>(ring + slot * ROWB + (c * 32 + lane) * 16);
-    issue(row + (LN_RING_D - 1) * nwarps, (it + LN_RING_D - 1) % LN_RING_D);
+    asm volatile("cp.async.wait_group %0;" ::"n"(R::DEPTH - 2) : "memory");
+    __syncwarp();                       // this row has landed for every lane; every lane is done with the slot refilled next
+    const T* zr = ring + (it % R::DEPTH) * R::ROW;
+    issue(row + (R::DEPTH - 1) * nwarps, (it + R::DEPTH - 1) % R::DEPTH);
     float v[NCH][8];
     float s = 0.f;
 #pragma unroll
     for (int c = 0; c < NCH; ++c) {
       const int col = (c * 32 + lane) * 8;
       if (col < E) {
-        unpack8(cz[c], v[c]);
+        load8<T>(zr + col, v[c]);
 #pragma unroll
         for (int i = 0; i < 8; ++i) s += v[c][i];
       } else {
@@ -536,12 +219,128 @@ layernorm_fwd_ring_kernel(const __nv_bfloat16* __restrict__ z, int ldz, const fl
         float o[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) o[i] = fmaf((v[c][i] - mean) * rstd, gm[c][i], bt[c][i]);
-        store8<__nv_bfloat16>(h + static_cast<size_t>(row) * ldh + col, o);
+        store8<T>(h + static_cast<size_t>(row) * ldh + col, o);
       }
     }
     if (lane == 0) { mean_out[row] = mean; rstd_out[row] = rstd; }
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
+}
+
+// Shared memory: sred [3][E] for the CTA's column sums, then each warp's ring, whose slot k holds dh in half 2k and z in
+// half 2k + 1.
+template <typename T, int NCH>
+__global__ void __launch_bounds__(256, LnRing<T, NCH>::BWD_CTAS)
+layernorm_bwd_kernel(const T* __restrict__ dh, int lddh, const T* __restrict__ z, int ldz,
+                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
+                     const float* __restrict__ gamma, T* __restrict__ dz, int lddz, float* __restrict__ dgamma,
+                     float* __restrict__ dbeta, float* __restrict__ colsum_out, int rows, int E) {
+  using R = LnRing<T, NCH>;
+  extern __shared__ __align__(16) uint8_t ln_smem[];
+  float* sred = reinterpret_cast<float*>(ln_smem);
+  const int lane = threadIdx.x & 31;
+  const int warp_in_cta = threadIdx.x >> 5;
+  const int warps_per_cta = blockDim.x >> 5;
+  T* ring = reinterpret_cast<T*>(ln_smem + ((3 * E * 4 + 15) & ~15)) + static_cast<size_t>(warp_in_cta) * R::DEPTH * 2 * R::ROW;
+  const int warp = blockIdx.x * warps_per_cta + warp_in_cta;
+  const int nwarps = gridDim.x * warps_per_cta;
+  const float inv_e = 1.0f / static_cast<float>(E);
+  for (int i = threadIdx.x; i < 3 * E; i += blockDim.x) sred[i] = 0.f;
+  __syncthreads();
+
+  float ag[NCH][8], ab[NCH][8], ac[NCH][8], gm[NCH][8];
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { ag[c][i] = 0.f; ab[c][i] = 0.f; ac[c][i] = 0.f; gm[c][i] = 0.f; }
+    const int col = (c * 32 + lane) * 8;
+    if (col < E) load8<float>(gamma + col, gm[c]);
+  }
+  auto issue = [&](int r, int slot) {
+    if (r < rows) {
+#pragma unroll
+      for (int c = 0; c < NCH; ++c) {
+        const int col = (c * 32 + lane) * 8;
+        if (col < E) {
+          ln_cp_async8(ring + (slot * 2 + 0) * R::ROW + col, dh + static_cast<size_t>(r) * lddh + col);
+          ln_cp_async8(ring + (slot * 2 + 1) * R::ROW + col, z + static_cast<size_t>(r) * ldz + col);
+        }
+      }
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+#pragma unroll
+  for (int k = 0; k < R::DEPTH - 1; ++k) issue(warp + k * nwarps, k);
+  float m_l = 0.f, s_l = 0.f;         // statistics of rows it .. it + 31 of this warp, one per lane
+  int it = 0;
+  for (int row = warp; row < rows; row += nwarps, ++it) {
+    if ((it & 31) == 0) {
+      const long long r = static_cast<long long>(row) + static_cast<long long>(lane) * nwarps;
+      m_l = r < rows ? __ldg(mean_in + r) : 0.f;
+      s_l = r < rows ? __ldg(rstd_in + r) : 0.f;
+    }
+    const float mean = __shfl_sync(0xffffffffu, m_l, it & 31), rstd = __shfl_sync(0xffffffffu, s_l, it & 31);
+    asm volatile("cp.async.wait_group %0;" ::"n"(R::DEPTH - 2) : "memory");
+    __syncwarp();                       // this row has landed for every lane; every lane is done with the slot refilled next
+    const T* dr = ring + (it % R::DEPTH) * 2 * R::ROW;
+    const T* zr = dr + R::ROW;
+    float xh[NCH][8], g[NCH][8];
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      const int col = (c * 32 + lane) * 8;
+      if (col < E) {
+        float d[8], zz[8];
+        load8<T>(dr + col, d);
+        load8<T>(zr + col, zz);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          xh[c][i] = (zz[i] - mean) * rstd;
+          g[c][i] = d[i] * gm[c][i];
+          s1 += g[c][i];
+          s2 = fmaf(g[c][i], xh[c][i], s2);
+          ag[c][i] = fmaf(d[i], xh[c][i], ag[c][i]);
+          ab[c][i] += d[i];
+        }
+      }
+    }
+    issue(row + (R::DEPTH - 1) * nwarps, (it + R::DEPTH - 1) % R::DEPTH);   // after the reads of this row's slot
+    s1 = warp_sum(s1) * inv_e;
+    s2 = warp_sum(s2) * inv_e;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      const int col = (c * 32 + lane) * 8;
+      if (col < E) {
+        float o[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          o[i] = rstd * (g[c][i] - s1 - xh[c][i] * s2);
+          ac[c][i] += o[i];
+        }
+        store8<T>(dz + static_cast<size_t>(row) * lddz + col, o);
+      }
+    }
+  }
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  // CTA-level combine, then one atomic per column per CTA
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+    const int col = (c * 32 + lane) * 8;
+    if (col < E) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        atomicAdd(&sred[col + i], ag[c][i]);
+        atomicAdd(&sred[E + col + i], ab[c][i]);
+        atomicAdd(&sred[2 * E + col + i], ac[c][i]);
+      }
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < E; i += blockDim.x) {
+    if (dgamma != nullptr) atomicAdd(&dgamma[i], sred[i]);
+    if (dbeta != nullptr) atomicAdd(&dbeta[i], sred[E + i]);
+    if (colsum_out != nullptr) atomicAdd(&colsum_out[i], sred[2 * E + i]);
+  }
 }
 
 // Generic (any E) fallbacks: one warp per row, scalar accesses, re-reading the row from cache.
@@ -702,6 +501,43 @@ extern "C" int pfn_embed_bwd(const void* dout, int dtype, const float* x, const 
   return 0;
 }
 
+// Vector-path launches: LnRing's CTAs per SM, no more than the rows need.  An SM has 228 KB of shared memory, of which
+// 1 KB is reserved per CTA.
+template <typename T, int NCH>
+static int layernorm_fwd_vec(const T* z, int ldz, const float* gamma, const float* beta, T* h, int ldh, float* mean,
+                             float* rstd, int rows, int E, float eps, cudaStream_t s) {
+  using R = LnRing<T, NCH>;
+  constexpr size_t smem = 8 * R::WARP_BYTES;
+  static_assert(R::FWD_CTAS * (smem + 1024) <= 228 * 1024, "the forward CTAs must fit on an SM");
+  static bool attr_set[64] = {};
+  if (first_use_on_device(attr_set))
+    PFN_CUDA_OK(cudaFuncSetAttribute(layernorm_fwd_kernel<T, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  int grid = R::FWD_CTAS * num_sms();
+  if (grid > (rows + 7) / 8) grid = (rows + 7) / 8;
+  layernorm_fwd_kernel<T, NCH><<<grid, 256, smem, s>>>(z, ldz, gamma, beta, h, ldh, mean, rstd, rows, E, eps);
+  PFN_LAUNCH_OK();
+  return 0;
+}
+
+template <typename T, int NCH>
+static int layernorm_bwd_vec(const T* dh, int lddh, const T* z, int ldz, const float* mean, const float* rstd,
+                             const float* gamma, T* dz, int lddz, float* dgamma, float* dbeta, float* colsum_out, int rows,
+                             int E, cudaStream_t s) {
+  using R = LnRing<T, NCH>;
+  constexpr size_t rings = 8 * 2 * R::WARP_BYTES;
+  constexpr size_t max_smem = 3 * R::ROW * sizeof(float) + rings;
+  static_assert(R::BWD_CTAS * (max_smem + 1024) <= 228 * 1024, "the backward CTAs must fit on an SM");
+  static bool attr_set[64] = {};
+  if (first_use_on_device(attr_set))
+    PFN_CUDA_OK(cudaFuncSetAttribute(layernorm_bwd_kernel<T, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(max_smem)));
+  const size_t smem = ((3 * static_cast<size_t>(E) * 4 + 15) & ~size_t(15)) + rings;
+  int grid = R::BWD_CTAS * num_sms();
+  if (grid > (rows + 7) / 8) grid = (rows + 7) / 8;
+  layernorm_bwd_kernel<T, NCH><<<grid, 256, smem, s>>>(dh, lddh, z, ldz, mean, rstd, gamma, dz, lddz, dgamma, dbeta, colsum_out, rows, E);
+  PFN_LAUNCH_OK();
+  return 0;
+}
+
 template <typename T>
 static int layernorm_fwd_dispatch(const void* z, int ldz, const float* gamma, const float* beta, void* h, int ldh,
                                   float* mean, float* rstd, int rows, int E, float eps, cudaStream_t s) {
@@ -710,33 +546,14 @@ static int layernorm_fwd_dispatch(const void* z, int ldz, const float* gamma, co
   const bool vec = (E % 8 == 0) && (ldz % 8 == 0) && (ldh % 8 == 0) && E <= 1024 &&
                    ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(h) |
                      reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0;
-  const int warps = 8;
-  int grid = (rows + warps - 1) / warps;
-  const int max_grid = num_sms() * 8;
-  if (grid > max_grid) grid = max_grid;
-#ifndef PFN_LN_FWD_NO_RING
-  if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-    if (vec && E > 256 && E <= 512) {
-      constexpr int NCH = 2;
-      const size_t smem = static_cast<size_t>(warps) * LN_RING_D * NCH * 512;          // 64 KB at depth 8: two CTAs per SM
-      static bool attr_set[64] = {};
-      if (first_use_on_device(attr_set))
-        PFN_CUDA_OK(cudaFuncSetAttribute(layernorm_fwd_ring_kernel<NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-      int g1 = 2 * num_sms();
-      if (g1 > (rows + warps - 1) / warps) g1 = (rows + warps - 1) / warps;
-      layernorm_fwd_ring_kernel<NCH><<<g1, 256, smem, s>>>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps);
-      PFN_LAUNCH_OK();
-      return 0;
-    }
-  }
-#endif
   if (vec) {
-    if (E <= 256) layernorm_fwd_kernel<T, 1><<<grid, 256, 0, s>>>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps);
-    else if (E <= 512) layernorm_fwd_kernel<T, 2><<<grid, 256, 0, s>>>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps);
-    else layernorm_fwd_kernel<T, 4><<<grid, 256, 0, s>>>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps);
-  } else {
-    layernorm_fwd_generic<T><<<grid, 256, 0, s>>>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps);
+    if (E <= 256) return layernorm_fwd_vec<T, 1>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps, s);
+    if (E <= 512) return layernorm_fwd_vec<T, 2>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps, s);
+    return layernorm_fwd_vec<T, 4>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps, s);
   }
+  int grid = (rows + 7) / 8;
+  if (grid > num_sms() * 8) grid = num_sms() * 8;
+  layernorm_fwd_generic<T><<<grid, 256, 0, s>>>(zp, ldz, gamma, beta, hp, ldh, mean, rstd, rows, E, eps);
   PFN_LAUNCH_OK();
   return 0;
 }
@@ -759,35 +576,14 @@ static int layernorm_bwd_dispatch(const void* dh, int lddh, const void* z, int l
   const bool vec = (E % 8 == 0) && (ldz % 8 == 0) && (lddh % 8 == 0) && (lddz % 8 == 0) && E <= 1024 &&
                    ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(dh) | reinterpret_cast<uintptr_t>(dz) |
                      reinterpret_cast<uintptr_t>(gamma)) & 15) == 0;
-  const int warps = 8;
-  int grid = (rows + warps - 1) / warps;
-  const int max_grid = num_sms() * 4;
-  if (grid > max_grid) grid = max_grid;
-#ifndef PFN_LN_BWD_NO_RING
-  if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-    if (vec && E > 256 && E <= 512) {
-      // one persistent CTA per SM, the rows staged through the per-warp cp.async rings
-      constexpr int NCH = 2;
-      const size_t smem = ((3 * static_cast<size_t>(E) * 4 + 15) & ~size_t(15)) + static_cast<size_t>(warps) * LN_RING_D * 2 * NCH * 512;
-      static bool attr_set[64] = {};
-      if (first_use_on_device(attr_set))
-        PFN_CUDA_OK(cudaFuncSetAttribute(layernorm_bwd_ring_kernel<NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      int g1 = num_sms();
-      if (g1 > (rows + warps - 1) / warps) g1 = (rows + warps - 1) / warps;
-      layernorm_bwd_ring_kernel<NCH><<<g1, 256, smem, s>>>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E);
-      PFN_LAUNCH_OK();
-      return 0;
-    }
-  }
-#endif
   if (vec) {
-    const size_t smem = 3 * static_cast<size_t>(E) * sizeof(float);
-    if (E <= 256) layernorm_bwd_kernel<T, 1><<<grid, 256, smem, s>>>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E);
-    else if (E <= 512) layernorm_bwd_kernel<T, 2><<<grid, 256, smem, s>>>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E);
-    else layernorm_bwd_kernel<T, 4><<<grid, 256, smem, s>>>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E);
-  } else {
-    layernorm_bwd_generic<T><<<grid, 256, 0, s>>>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E);
+    if (E <= 256) return layernorm_bwd_vec<T, 1>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E, s);
+    if (E <= 512) return layernorm_bwd_vec<T, 2>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E, s);
+    return layernorm_bwd_vec<T, 4>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E, s);
   }
+  int grid = (rows + 7) / 8;
+  if (grid > num_sms() * 4) grid = num_sms() * 4;
+  layernorm_bwd_generic<T><<<grid, 256, 0, s>>>(dhp, lddh, zp, ldz, mean, rstd, gamma, dzp, lddz, dgamma, dbeta, colsum_out, rows, E);
   PFN_LAUNCH_OK();
   return 0;
 }
