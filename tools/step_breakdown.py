@@ -6,7 +6,8 @@ Event pairs add launch gaps, so the sum is an upper bound of the kernels' own ti
 
 For every wgmma GEMM row it also prints the algorithmic HBM bytes (operands, aux, C and C2 once each: the byte formula of
 _lib.PROFILE_GEMM), the achieved TFLOP/s and GB/s, and the share of the floor, floor = max(FLOP / peak, bytes / bandwidth)
-with the H100 SXM data-sheet peaks (dense BF16 989 TFLOP/s, HBM3 3.35 TB/s); the bound that sets the floor is named."""
+with the H100 SXM data-sheet peaks (dense BF16 989 TFLOP/s, HBM3 3.35 TB/s); the bound that sets the floor is named.
+Tensor-core attention rows print their algorithmic FLOPs (mask-aware) and the achieved TFLOP/s."""
 import sys, os, collections
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -19,6 +20,7 @@ lib = L.load()
 REC = None
 PEAK_FLOPS, PEAK_BW = 989e12, 3.35e12
 GEMM_COST = {}      # label -> (flop, bytes) of one call
+ATTN_COST = {}      # label -> algorithmic flop of one call
 NAMES = ["pfn_gemm_bf16_tc", "pfn_gemm_simt", "pfn_attention_fwd_tc", "pfn_attention_bwd_tc", "pfn_attention_fwd_simt",
          "pfn_attention_bwd_simt", "pfn_embed_fwd", "pfn_embed_bwd", "pfn_layernorm_fwd", "pfn_layernorm_bwd", "pfn_colsum",
          "pfn_bar_nll_fwd", "pfn_bar_nll_bwd", "pfn_gp_sample"]
@@ -36,6 +38,13 @@ def wrap(name):
                 esz = 4 if d.c_dtype == L.F32 else 2
                 nbytes = 2.0 * (d.M * d.K + d.N * d.K) + esz * d.M * d.N * (2 if d.C2 else 1) + (2.0 * d.M * d.N if d.aux else 0.0)
                 GEMM_COST[label] = (2.0 * d.M * d.N * d.K, nbytes)
+        elif name in ("pfn_attention_fwd_tc", "pfn_attention_bwd_tc"):
+            # matmul passes over the attended (query, key) pairs: every row attends the sep train keys, rows >= sep also
+            # their own key; forward S and PV (2 passes), backward S, dP, dV, dK, dQ (5 passes; recomputed S / dP not counted)
+            d = a[0]._obj
+            label = f"{name} T={d.T} B={d.B} H={d.H} sep={d.sep}"
+            pairs = d.T * d.sep + (d.T - d.sep)
+            ATTN_COST[label] = (2 if name.endswith("fwd_tc") else 5) * 2.0 * pairs * d.dh * d.B * d.H
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); rc = orig(*a); e1.record()
         REC.append((label, e0, e1))
@@ -88,6 +97,8 @@ for label, (n, t) in rows:
         extra = (f"  | {nbytes / 1e9:6.3f} GB {flop / sec / 1e12:6.1f} TFLOP/s {nbytes / sec / 1e9:7.1f} GB/s"
                  f"  floor {max(t_flop, t_bytes) * 1e3:6.3f} ms ({'tensor' if t_flop >= t_bytes else 'HBM'})"
                  f"  {100 * max(t_flop, t_bytes) / sec:5.1f}% of floor")
+    if label in ATTN_COST:
+        extra = f"  | {ATTN_COST[label] / 1e9:8.1f} GFLOP {ATTN_COST[label] / (t / n * 1e-3) / 1e12:6.1f} TFLOP/s"
     print(f"{t / NS:8.3f} ms/step  {n // NS:3d}x  {t / n:7.3f} ms each  {label}{extra}")
     s += t / NS
 print(f"{s:8.3f} ms/step in C-ABI kernels; {total - s:.3f} ms/step elsewhere (torch elementwise, Adam, clip, launch gaps)")

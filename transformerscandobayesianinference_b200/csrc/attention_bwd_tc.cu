@@ -3,28 +3,45 @@
 //  (0) attn_bwd_delta_kernel  delta[b,h,i] = dO_i . O_i   (one warp per token row, HBM-bound, 16 B vectors); skipped when
 //      the caller passes the token-major delta the out-projection dgrad's ROWDOT epilogue already produced
 //
-//  (1) attn_bwd_dq_kernel     one CTA (4 warps) per (batch, head, 64-row query tile); loop over 64-key blocks of the train keys:
-//          S_j  = Q K_j^T      dP_j = dO V_j^T                                 (mma.sync, fp32)
+//  (1) attn_bwd_dq_kernel     persistent: one CTA per SM walks the (batch, head, 128-row query tile) list; per tile, loop
+//      over 64-key blocks of the train keys:
+//          S_j  = Q K_j^T      dP_j = dO V_j^T                                 (wgmma m64n64k16, fp32)
 //          dS_j = exp2(S_j c - lse2) * (dP_j - delta) * scale  -> bf16 A fragments (registers)
-//          dQ  += dS_j K_j
+//          dQ  += dS_j K_j                                                      (wgmma m64n128k16, A from registers)
 //      For a query row (i >= sep) the diagonal key is attended by that row only, so dK_i = dS_ii q_i and dV_i = P_ii dO_i are
 //      complete: the four lanes that own the row compute and store them, and add dS_ii k_i to dQ.
 //
-//  (2) attn_bwd_dkv_kernel    one CTA (4 warps) per (batch, head, 64-key tile of the train keys), loop over 32-row query blocks:
-//          S^T = K Q_i^T       dP^T = V dO_i^T     (row = key, column = query row)
-//          dV += (P^T . mask) dO_i ;   dK += dS^T Q_i
+//  (2) attn_bwd_dkv_kernel    one CTA per (batch, head, 128-key tile of the train keys), K and V resident, loop over 64-row
+//      Q/dO blocks:
+//          S^T = K Q_i^T       dP^T = V dO_i^T     (row = key, column = query row; m64n64k16)
+//          dV += (P^T . mask) dO_i ;   dK += dS^T Q_i                           (m64n128k16, A from registers)
 //
-// Q/K/V/dO rows come straight out of the packed [T*B, 3E] qkv / [T*B, E] dO buffers; no transposes, no atomics on dQKV.
+// Both are warp-specialised: warpgroup 2 (producer, 40 registers) issues the TMA loads into a ring of stages, warpgroups 0
+// and 1 (consumers, 232 registers) each own 64 rows of the tile (query rows in (1), keys in (2)).  The fp32 S / dP
+// accumulators are packed to bf16 in place as the A operand of the second pair of MMAs, so P and dS never touch shared
+// memory.  Q/K/V/dO rows come straight out of the packed [T*B, 3E] qkv / [T*B, E] dO buffers through 3-D tensor maps
+// (columns, batch, time) whose two row strides encode the token order; the TMA zero-fills rows past T (Q, dO) and keys
+// past sep (K, V).  One 128-byte-swizzled tile serves as a K-major operand (S = Q K^T) and as an MN-major one
+// (dQ += dS K), so nothing is transposed.  No atomics on dQKV: every element is written exactly once.
 #include "attention_common.cuh"
 
 namespace pfn {
 
-constexpr int AB_BM = 64;                                 // dQ kernel: query rows per CTA; key block size
-constexpr int AB_TILE = AB_BM * ATT_ROW_BYTES;            // 16 KB
-constexpr int AB_DQ_SMEM = 6 * AB_TILE;                   // Q + dO + 2 x K + 2 x V
-constexpr int AB_QB = 32;                                 // dK/dV kernel: query rows per block
-constexpr int AB_QTILE = AB_QB * ATT_ROW_BYTES;           // 8 KB
-constexpr int AB_DKV_SMEM = 2 * AB_TILE + 4 * AB_QTILE + 2 * 2 * AB_QB * 4;   // K + V + 2 x (Q, dO) + 2 x (lse2, delta)
+constexpr int AB_ROWS = 64;                               // rows of one consumer warpgroup; key / query block size
+constexpr int AB_TILE = AB_ROWS * ATT_ROW_BYTES;          // 16 KB: 64 rows x 128 bf16 = two 8 KB boxes of 64 columns
+constexpr int AB_THREADS = 3 * 128;
+constexpr int AB_DQ_STAGES = 4;                           // K/V blocks in flight (dQ kernel)
+constexpr int AB_DKV_STAGES = 3;                          // Q/dO blocks in flight (dK/dV kernel)
+// dQ kernel: Q, dO of the tile (2 x 2 x 16 KB), ring of (K, V), barriers
+constexpr int AB_DQ_OFF_RING = 4 * AB_TILE;
+constexpr int AB_DQ_OFF_BAR = AB_DQ_OFF_RING + AB_DQ_STAGES * 2 * AB_TILE;
+constexpr int AB_DQ_SMEM = AB_DQ_OFF_BAR + (2 * AB_DQ_STAGES + 2) * 8 + 1024;   // + 1 KB alignment slack
+// dK/dV kernel: K, V of the tile (2 x 2 x 16 KB), ring of (Q, dO), ring of (lse2, delta), barriers
+constexpr int AB_DKV_OFF_RING = 4 * AB_TILE;
+constexpr int AB_DKV_OFF_STAT = AB_DKV_OFF_RING + AB_DKV_STAGES * 2 * AB_TILE;
+constexpr int AB_DKV_OFF_BAR = AB_DKV_OFF_STAT + AB_DKV_STAGES * 2 * AB_ROWS * 4;
+constexpr int AB_DKV_SMEM = AB_DKV_OFF_BAR + (2 * AB_DKV_STAGES + 1) * 8 + 1024;
+static_assert(AB_DQ_SMEM <= 232448 && AB_DKV_SMEM <= 232448, "the tiles and rings must fit the 227 KB of shared memory");
 
 struct AttnBwdParams {
   int T, B, H, sep;
@@ -37,12 +54,38 @@ struct AttnBwdParams {
   int delta_tm;          // 1: delta is token-major [T*B, H] (GEMM ROWDOT epilogue); 0: [B*H, T]
   float* dq_colsum;      // optional [H*dh]: += column sums of dQ
   uint32_t drop_seed; int drop_thr;   // dropout on the attention probabilities (thr 0 = off), csrc/dropout.cuh
-  int n_tiles;
+  int n_tiles;           // 128-row tiles per (batch, head): query rows (dQ kernel) or train keys (dK/dV kernel)
   int batch_major;
 };
 
 __device__ __forceinline__ float ab_delta(const AttnBwdParams& p, int b, int h, int i) {
   return p.delta_tm ? p.delta[att_tok(i, b, p.T, p.B, 0) * p.H + h] : p.delta[(static_cast<size_t>(b) * p.H + h) * p.T + i];
+}
+
+// wgmma descriptors of a 64-row tile (two 64-column boxes 8 KB apart, 128-byte swizzle), k16 step kk:
+// K-major (the tile's columns are the k index, kk < 8) and MN-major (its rows are the k index, kk < 4)
+__device__ __forceinline__ uint64_t ab_desc_k(uint32_t tile, int kk) {
+  return tc::wgmma_smem_desc(tile + (kk >> 2) * 8192 + (kk & 3) * 32, 16, 1024);
+}
+__device__ __forceinline__ uint64_t ab_desc_mn(uint32_t tile, int kk) {
+  return tc::wgmma_smem_desc(tile + kk * 2048, 8192, 1024);
+}
+// The address of a tile that stays resident across a loop, made opaque in every iteration so that the descriptors of its
+// k16 steps are formed next to their MMAs instead of being hoisted out of the loop and held in registers throughout.
+__device__ __forceinline__ uint32_t ab_opaque(uint32_t addr) {
+  asm volatile("" : "+r"(addr));
+  return addr;
+}
+// k16 step kk of a 64 x 64 score block; the first step writes the accumulator
+__device__ __forceinline__ void ab_mma_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, int kk) {
+  if (kk == 0) tc::wgmma_m64n64k16<0>(d, a_desc, b_desc);
+  else tc::wgmma_m64n64k16<1>(d, a_desc, b_desc);
+}
+
+// TMA of rows [t0, t0 + 64) of one head (columns col0 .. col0 + 127) into a 16 KB tile
+__device__ __forceinline__ void ab_load_tile(uint8_t* dst, const CUtensorMap* m, uint64_t* bar, int col0, int b, int t0) {
+  tc::tma_load_3d(dst, m, bar, col0, b, t0);
+  tc::tma_load_3d(dst + 8192, m, bar, col0 + 64, b, t0);
 }
 
 // =====================================================================================================================
@@ -86,287 +129,358 @@ attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ out, int ld_out, const _
 // =====================================================================================================================
 // Kernel 1: dQ (+ dK, dV of the query rows' own keys)
 // =====================================================================================================================
-__global__ void __launch_bounds__(128, 2)
-attn_bwd_dq_kernel(const AttnBwdParams p) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* sQ = smem;
-  uint8_t* sD = smem + AB_TILE;
-  uint8_t* sK = smem + 2 * AB_TILE;                       // buffer s at + s * 16 KB
-  uint8_t* sV = smem + 4 * AB_TILE;
+__global__ void __launch_bounds__(AB_THREADS, 1)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
+                   const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* sQ = smem;                                     // warpgroup g's 64 rows at + g * 16 KB
+  uint8_t* sD = smem + 2 * AB_TILE;
+  uint8_t* sRing = smem + AB_DQ_OFF_RING;                 // stage s: K at + 2 s * 16 KB, V at + (2 s + 1) * 16 KB
+  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + AB_DQ_OFF_BAR);
+  uint64_t* kv_empty = kv_full + AB_DQ_STAGES;
+  uint64_t* q_full = kv_empty + AB_DQ_STAGES;             // Q, dO of the CTA's current tile have landed
+  uint64_t* q_empty = q_full + 1;                         // both warpgroups have finished their last S / dP MMAs of it
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qt = static_cast<int>(blockIdx.x) % p.n_tiles;
-  const int bh = static_cast<int>(blockIdx.x) / p.n_tiles;
-  const int h = bh % p.H, b = bh / p.H;
   const int E = p.H * ATT_DH;
-  const int i0 = qt * AB_BM;
-  const int nblk = (p.sep + AB_BM - 1) / AB_BM;
-  const int r0 = 16 * warp;
-
-  att_load_tile<AB_BM>(sQ, p.qkv, p.ld_qkv, h * ATT_DH, i0, p.T, b, p.T, p.B, p.batch_major);
-  att_load_tile<AB_BM>(sD, p.dout, p.ld_dout, h * ATT_DH, i0, p.T, b, p.T, p.B, p.batch_major);
-  if (nblk > 0) {
-    att_load_tile<AB_BM>(sK, p.qkv, p.ld_qkv, E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
-    att_load_tile<AB_BM>(sV, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
+  const int nblk = (p.sep + AB_ROWS - 1) / AB_ROWS;
+  const int n_units = p.n_tiles * p.B * p.H;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < AB_DQ_STAGES; ++s) {
+      tc::mbar_init(&kv_full[s], 1);
+      tc::mbar_init(&kv_empty[s], 2);
+    }
+    tc::mbar_init(q_full, 1);
+    tc::mbar_init(q_empty, 2);
+    tc::mbar_fence_init();
   }
-  tc::cp_async_commit();
+  __syncthreads();
 
-  // per-row statistics of this lane's two rows
-  float lse2[2], dl[2];
-  uint32_t drow[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int i = i0 + r0 + (lane >> 2) + 8 * r;
-    const bool valid = i < p.T;
-    lse2[r] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
-    dl[r] = valid ? ab_delta(p, b, h, i) : 0.f;
-    drow[r] = static_cast<uint32_t>(bh) * p.T + i;
+  if (warp >= 8) {
+    // ------------------------------------------------------------------ TMA producer
+    tc::setmaxnreg_dec<40>();
+    if (threadIdx.x == 256) {
+      tc::tma_prefetch_desc(&tmQ);
+      tc::tma_prefetch_desc(&tmKV);
+      tc::tma_prefetch_desc(&tmDO);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
+        const int qt = u % p.n_tiles, bh = u / p.n_tiles;
+        const int h = bh % p.H, b = bh / p.H;
+        // The next tile's Q / dO go in once the consumers are done with the current one, which is before its last key
+        // block is (so the first key blocks of the next tile are already in flight by then).
+        auto load_q = [&]() {
+          if (it > 0) tc::mbar_wait_suspend(q_empty, (it - 1) & 1);
+          tc::mbar_expect_tx(q_full, 4 * AB_TILE);
+          for (int g = 0; g < 2; ++g) {
+            ab_load_tile(sQ + g * AB_TILE, &tmQ, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
+            ab_load_tile(sD + g * AB_TILE, &tmDO, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
+          }
+        };
+        const int claim_at = min(AB_DQ_STAGES - 1, nblk - 1);
+        if (nblk == 0) load_q();
+        for (int kb = 0; kb < nblk; ++kb) {
+          if (kb == claim_at) load_q();
+          tc::mbar_wait_suspend(&kv_empty[stage], phase ^ 1);
+          uint8_t* dst = sRing + stage * 2 * AB_TILE;
+          tc::mbar_expect_tx(&kv_full[stage], 2 * AB_TILE);
+          ab_load_tile(dst, &tmKV, &kv_full[stage], E + h * ATT_DH, b, kb * AB_ROWS);
+          ab_load_tile(dst + AB_TILE, &tmKV, &kv_full[stage], 2 * E + h * ATT_DH, b, kb * AB_ROWS);
+          if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
   }
+
+  // -------------------------------------------------------------------- consumer warpgroups
+  tc::setmaxnreg_inc<232>();
+  const int g = warp >> 2, wq = warp & 3;
+  const int tid = threadIdx.x & 127;
+  const uint32_t q_tile = tc::smem_u32(sQ + g * AB_TILE), d_tile = tc::smem_u32(sD + g * AB_TILE);
   const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
+  int stage = 0;
+  uint32_t phase = 0;
+  bool timed_out = false;
+  for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
+    const int qt = u % p.n_tiles, bh = u / p.n_tiles;
+    const int h = bh % p.H, b = bh / p.H;
+    const int i0 = qt * 128 + 64 * g + 16 * wq + (lane >> 2);    // this lane's rows: i0, i0 + 8
 
-  float dq[16][4];
+    // per-row statistics of this lane's two rows
+    float lse2[2], dl[2];
+    uint32_t drow[2];
 #pragma unroll
-  for (int j = 0; j < 16; ++j) dq[j][0] = dq[j][1] = dq[j][2] = dq[j][3] = 0.f;
-  const uint32_t q_s = tc::smem_u32(sQ), d_s = tc::smem_u32(sD);
-
-  for (int kb = 0; kb < nblk; ++kb) {
-    if (kb + 1 < nblk) {
-      const int nb = (kb + 1) & 1;
-      att_load_tile<AB_BM>(sK + nb * AB_TILE, p.qkv, p.ld_qkv, E + h * ATT_DH, (kb + 1) * AB_BM, p.sep, b, p.T, p.B, p.batch_major);
-      att_load_tile<AB_BM>(sV + nb * AB_TILE, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, (kb + 1) * AB_BM, p.sep, b, p.T, p.B, p.batch_major);
-      tc::cp_async_commit();
-      tc::cp_async_wait<1>();
-    } else {
-      tc::cp_async_wait<0>();
+    for (int r = 0; r < 2; ++r) {
+      const int i = i0 + 8 * r;
+      const bool valid = i < p.T;
+      lse2[r] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+      dl[r] = valid ? ab_delta(p, b, h, i) : 0.f;
+      drow[r] = static_cast<uint32_t>(bh) * p.T + i;
     }
-    __syncthreads();
-    const uint32_t k_s = tc::smem_u32(sK + (kb & 1) * AB_TILE);
-    const uint32_t v_s = tc::smem_u32(sV + (kb & 1) * AB_TILE);
+    if (!tc::mbar_wait_bounded(q_full, it & 1)) { timed_out = true; break; }
 
-    float s[8][4], dp[8][4];
+    // The first MMA of the tile writes dq (scale-d = 0), so nothing but wgmma defines it until the loop has drained.
+    float dq[64];
+    for (int kb = 0; kb < nblk; ++kb) {
+      if (!tc::mbar_wait_bounded(&kv_full[stage], phase)) { timed_out = true; break; }
+      const uint32_t k_s = tc::smem_u32(sRing + stage * 2 * AB_TILE);
+      const uint32_t v_s = k_s + AB_TILE;
+      const uint32_t q_s = ab_opaque(q_tile), d_s = ab_opaque(d_tile);
+      float s[32], dp[32];
+      tc::wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = dp[j][0] = dp[j][1] = dp[j][2] = dp[j][3] = 0.f;
+      for (int kk = 0; kk < 8; ++kk) ab_mma_n64(s, ab_desc_k(q_s, kk), ab_desc_k(k_s, kk), kk);
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t aq[4], ad[4];
-      att_frag_a(aq, q_s, r0, kk * 16, lane);
-      att_frag_a(ad, d_s, r0, kk * 16, lane);
+      for (int kk = 0; kk < 8; ++kk) ab_mma_n64(dp, ab_desc_k(d_s, kk), ab_desc_k(v_s, kk), kk);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      tc::wgmma_fence_regs(s);
+      tc::wgmma_fence_regs(dp);
+      if (kb == nblk - 1 && tid == 0) tc::mbar_arrive(q_empty);
+
+      // dS = P (mask dP - delta) scale  (keys >= sep of the last block get P = 0); element 4 j + e is row i0 + 8 (e >> 1),
+      // key kb * 64 + 8 j + 2 (lane & 3) + (e & 1)
+      uint32_t ads[16];
+      const int key0 = kb * AB_ROWS + 2 * (lane & 3);
 #pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t bk[4], bv[4];
-        att_frag_b(bk, k_s, np * 16, kk * 16, lane);
-        att_frag_b(bv, v_s, np * 16, kk * 16, lane);
-        tc::mma_bf16_16816(s[2 * np], aq, bk[0], bk[1]);
-        tc::mma_bf16_16816(s[2 * np + 1], aq, bk[2], bk[3]);
-        tc::mma_bf16_16816(dp[2 * np], ad, bv[0], bv[1]);
-        tc::mma_bf16_16816(dp[2 * np + 1], ad, bv[2], bv[3]);
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; e += 2) {
+          float v[2];
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int key = key0 + 8 * j + c;
+            const float pr = key < p.sep ? fast_ex2(fmaf(s[4 * j + e + c], p.scale_log2, -lse2[e >> 1])) : 0.f;
+            const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[e >> 1], key, p.drop_thr) ? dscale : 0.f) : 1.f;
+            v[c] = pr * fmaf(mk, dp[4 * j + e + c], -dl[e >> 1]) * p.scale;
+          }
+          ads[2 * j + (e >> 1)] = tc::pack_bf16x2(v[0], v[1]);
+        }
+      tc::wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(dq, ads + 4 * kk, ab_desc_mn(k_s, kk), kb > 0 || kk > 0);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      if (tid == 0) tc::mbar_arrive(&kv_empty[stage]);
+      if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
+    }
+    tc::wgmma_fence_regs(dq);
+    if (nblk == 0 && tid == 0) tc::mbar_arrive(q_empty);
+
+    // diagonal keys of the query rows, dQ stores, column sums; dq[4 j + 2 r + c] is row i0 + 8 r, column 8 j + 2 (lane & 3) + c
+    float cs[16][2];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) cs[j][0] = cs[j][1] = 0.f;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int i = i0 + 8 * r;
+      const bool valid = i < p.T;
+      const bool diag = valid && i >= p.sep;
+      const size_t tok = att_tok(valid ? i : 0, b, p.T, p.B, p.batch_major);
+      const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + h * ATT_DH;
+      const __nv_bfloat16* drw = p.dout + tok * p.ld_dout + h * ATT_DH;
+      __nv_bfloat16* grow = p.dqkv + tok * p.ld_dqkv + h * ATT_DH;
+      float sd = 0.f, dpd = 0.f;
+      if (diag) {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane);
+          const float2 gr = att_ld2(drw, j, lane), v = att_ld2(qrow + 2 * E, j, lane);
+          sd = fmaf(q.x, k.x, fmaf(q.y, k.y, sd));
+          dpd = fmaf(gr.x, v.x, fmaf(gr.y, v.y, dpd));
+        }
+      }
+      sd = quad_sum(sd);
+      dpd = quad_sum(dpd);
+      float ds = 0.f;
+      if (diag) {
+        const float pr = fast_ex2(fmaf(sd, p.scale_log2, -lse2[r]));
+        const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[r], i, p.drop_thr) ? dscale : 0.f) : 1.f;
+        ds = pr * fmaf(mk, dpd, -dl[r]) * p.scale;
+        const float pm = pr * mk;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float2 q = att_ld2(qrow, j, lane), gr = att_ld2(drw, j, lane);
+          att_st2(grow + E, j, lane, ds * q.x, ds * q.y);
+          att_st2(grow + 2 * E, j, lane, pm * gr.x, pm * gr.y);
+        }
+      }
+      if (valid) {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          float x = nblk > 0 ? dq[4 * j + 2 * r] : 0.f, y = nblk > 0 ? dq[4 * j + 2 * r + 1] : 0.f;
+          if (diag) {
+            const float2 k = att_ld2(qrow + E, j, lane);
+            x = fmaf(ds, k.x, x);
+            y = fmaf(ds, k.y, y);
+          }
+          att_st2(grow, j, lane, x, y);
+          cs[j][0] += __bfloat162float(__float2bfloat16_rn(x));
+          cs[j][1] += __bfloat162float(__float2bfloat16_rn(y));
+        }
       }
     }
-    // dS = P (mask dP - delta) scale  (keys >= sep of the last block get P = 0)
-    const int key0 = kb * AB_BM + 2 * (lane & 3);
+    if (p.dq_colsum != nullptr) {
+      // reduce over the eight row groups of the warp (lanes with equal lane & 3), then one atomic per column and warp
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+      for (int j = 0; j < 16; ++j)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = key0 + 8 * j + (e & 1);
-        const float pr = key < p.sep ? fast_ex2(fmaf(s[j][e], p.scale_log2, -lse2[e >> 1])) : 0.f;
-        const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[e >> 1], key, p.drop_thr) ? dscale : 0.f) : 1.f;
-        s[j][e] = pr * fmaf(mk, dp[j][e], -dl[e >> 1]) * p.scale;
-      }
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      a[0] = tc::pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
-      a[1] = tc::pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
-      a[2] = tc::pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-      a[3] = tc::pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-      for (int dd = 0; dd < 8; ++dd) {
-        uint32_t bb[4];
-        att_frag_bt(bb, k_s, kk * 16, dd * 16, lane);
-        tc::mma_bf16_16816(dq[2 * dd], a, bb[0], bb[1]);
-        tc::mma_bf16_16816(dq[2 * dd + 1], a, bb[2], bb[3]);
-      }
+        for (int e = 0; e < 2; ++e) {
+          float v = cs[j][e];
+          v += __shfl_xor_sync(0xffffffffu, v, 4);
+          v += __shfl_xor_sync(0xffffffffu, v, 8);
+          v += __shfl_xor_sync(0xffffffffu, v, 16);
+          if (lane < 4) atomicAdd(p.dq_colsum + h * ATT_DH + 8 * j + 2 * lane + e, v);
+        }
     }
-    __syncthreads();     // this buffer is refilled by the next iteration's loads
   }
-  tc::cp_async_wait<0>();
-
-  // diagonal keys of the query rows, dQ stores, column sums
-  float cs[16][2];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) cs[j][0] = cs[j][1] = 0.f;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int i = i0 + r0 + (lane >> 2) + 8 * r;
-    const bool valid = i < p.T;
-    const bool diag = valid && i >= p.sep;
-    const size_t tok = att_tok(valid ? i : 0, b, p.T, p.B, p.batch_major);
-    const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + h * ATT_DH;
-    const __nv_bfloat16* drw = p.dout + tok * p.ld_dout + h * ATT_DH;
-    __nv_bfloat16* grow = p.dqkv + tok * p.ld_dqkv + h * ATT_DH;
-    float sd = 0.f, dpd = 0.f;
-    if (diag) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane);
-        const float2 g = att_ld2(drw, j, lane), v = att_ld2(qrow + 2 * E, j, lane);
-        sd = fmaf(q.x, k.x, fmaf(q.y, k.y, sd));
-        dpd = fmaf(g.x, v.x, fmaf(g.y, v.y, dpd));
-      }
-    }
-    sd = quad_sum(sd);
-    dpd = quad_sum(dpd);
-    if (diag) {
-      const float pr = fast_ex2(fmaf(sd, p.scale_log2, -lse2[r]));
-      const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[r], i, p.drop_thr) ? dscale : 0.f) : 1.f;
-      const float ds = pr * fmaf(mk, dpd, -dl[r]) * p.scale;
-      const float pm = pr * mk;
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane), g = att_ld2(drw, j, lane);
-        dq[j][2 * r] = fmaf(ds, k.x, dq[j][2 * r]);
-        dq[j][2 * r + 1] = fmaf(ds, k.y, dq[j][2 * r + 1]);
-        att_st2(grow + E, j, lane, ds * q.x, ds * q.y);
-        att_st2(grow + 2 * E, j, lane, pm * g.x, pm * g.y);
-      }
-    }
-    if (valid) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        att_st2(grow, j, lane, dq[j][2 * r], dq[j][2 * r + 1]);
-        cs[j][0] += __bfloat162float(__float2bfloat16_rn(dq[j][2 * r]));
-        cs[j][1] += __bfloat162float(__float2bfloat16_rn(dq[j][2 * r + 1]));
-      }
-    }
-  }
-  if (p.dq_colsum != nullptr) {
-    // reduce over the eight row groups of the warp (lanes with equal lane & 3), then one atomic per column and warp
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        float v = cs[j][e];
-        v += __shfl_xor_sync(0xffffffffu, v, 4);
-        v += __shfl_xor_sync(0xffffffffu, v, 8);
-        v += __shfl_xor_sync(0xffffffffu, v, 16);
-        if (lane < 4) atomicAdd(p.dq_colsum + h * ATT_DH + 8 * j + 2 * lane + e, v);
-      }
-  }
+  if (timed_out) asm volatile("trap;");
 }
 
 // =====================================================================================================================
 // Kernel 2: dK, dV of the train keys
 // =====================================================================================================================
-__global__ void __launch_bounds__(128, 2)
-attn_bwd_dkv_kernel(const AttnBwdParams p) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* sK = smem;
-  uint8_t* sV = smem + AB_TILE;
-  uint8_t* sQ = smem + 2 * AB_TILE;                       // buffer s at + s * 8 KB
-  uint8_t* sD = sQ + 2 * AB_QTILE;
-  float* sStat = reinterpret_cast<float*>(sD + 2 * AB_QTILE);   // [2][2][AB_QB]: lse2, delta
+__global__ void __launch_bounds__(AB_THREADS, 1)
+attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
+                    const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* sK = smem;                                     // warpgroup g's 64 keys at + g * 16 KB
+  uint8_t* sV = smem + 2 * AB_TILE;
+  uint8_t* sRing = smem + AB_DKV_OFF_RING;                // stage s: Q at + 2 s * 16 KB, dO at + (2 s + 1) * 16 KB
+  float* sStat = reinterpret_cast<float*>(smem + AB_DKV_OFF_STAT);   // stage s: lse2 at [128 s], delta at [128 s + 64]
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + AB_DKV_OFF_BAR);
+  uint64_t* empty = full + AB_DKV_STAGES;
+  uint64_t* kv_bar = empty + AB_DKV_STAGES;               // K, V of the tile have landed
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kt = static_cast<int>(blockIdx.x) % p.n_tiles;
   const int bh = static_cast<int>(blockIdx.x) / p.n_tiles;
   const int h = bh % p.H, b = bh / p.H;
   const int E = p.H * ATT_DH;
-  const int j0 = kt * AB_BM;
-  const int r0 = 16 * warp;                               // this warp's keys: j0 + r0 .. + 15
-  const int nqb = (p.T + AB_QB - 1) / AB_QB;
-
-  auto load_block = [&](int qb, int buf) {
-    att_load_tile<AB_QB>(sQ + buf * AB_QTILE, p.qkv, p.ld_qkv, h * ATT_DH, qb * AB_QB, p.T, b, p.T, p.B, p.batch_major);
-    att_load_tile<AB_QB>(sD + buf * AB_QTILE, p.dout, p.ld_dout, h * ATT_DH, qb * AB_QB, p.T, b, p.T, p.B, p.batch_major);
-    if (threadIdx.x < AB_QB) {
-      const int i = qb * AB_QB + threadIdx.x;
-      const bool valid = i < p.T;
-      sStat[buf * 2 * AB_QB + threadIdx.x] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
-      sStat[buf * 2 * AB_QB + AB_QB + threadIdx.x] = valid ? ab_delta(p, b, h, i) : 0.f;
+  const int nqb = (p.T + AB_ROWS - 1) / AB_ROWS;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < AB_DKV_STAGES; ++s) {
+      tc::mbar_init(&full[s], 1 + AB_ROWS);              // the TMA thread's expect_tx + one arrival per statistics row
+      tc::mbar_init(&empty[s], 2);
     }
-  };
-  att_load_tile<AB_BM>(sK, p.qkv, p.ld_qkv, E + h * ATT_DH, j0, p.sep, b, p.T, p.B, p.batch_major);
-  att_load_tile<AB_BM>(sV, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, j0, p.sep, b, p.T, p.B, p.batch_major);
-  load_block(0, 0);
-  tc::cp_async_commit();
+    tc::mbar_init(kv_bar, 1);
+    tc::mbar_fence_init();
+  }
+  __syncthreads();
 
-  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
-  float dk[16][4], dv[16][4];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) dk[j][0] = dk[j][1] = dk[j][2] = dk[j][3] = dv[j][0] = dv[j][1] = dv[j][2] = dv[j][3] = 0.f;
-  const uint32_t k_s = tc::smem_u32(sK), v_s = tc::smem_u32(sV);
-  const int key_a = j0 + r0 + (lane >> 2);                // this lane's keys: key_a, key_a + 8
-  const uint32_t drow_base = static_cast<uint32_t>(bh) * p.T;
-
-  for (int qb = 0; qb < nqb; ++qb) {
-    const int buf = qb & 1;
-    if (qb + 1 < nqb) {
-      load_block(qb + 1, buf ^ 1);
-      tc::cp_async_commit();
-      tc::cp_async_wait<1>();
-    } else {
-      tc::cp_async_wait<0>();
-    }
-    __syncthreads();
-    const uint32_t q_s = tc::smem_u32(sQ + buf * AB_QTILE), d_s = tc::smem_u32(sD + buf * AB_QTILE);
-    const float* st_lse = sStat + buf * 2 * AB_QB;
-    const float* st_dl = st_lse + AB_QB;
-
-    float s[4][4], dp[4][4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = dp[j][0] = dp[j][1] = dp[j][2] = dp[j][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t ak[4], av[4];
-      att_frag_a(ak, k_s, r0, kk * 16, lane);
-      att_frag_a(av, v_s, r0, kk * 16, lane);
-#pragma unroll
-      for (int np = 0; np < 2; ++np) {
-        uint32_t bq[4], bd[4];
-        att_frag_b(bq, q_s, np * 16, kk * 16, lane);
-        att_frag_b(bd, d_s, np * 16, kk * 16, lane);
-        tc::mma_bf16_16816(s[2 * np], ak, bq[0], bq[1]);
-        tc::mma_bf16_16816(s[2 * np + 1], ak, bq[2], bq[3]);
-        tc::mma_bf16_16816(dp[2 * np], av, bd[0], bd[1]);
-        tc::mma_bf16_16816(dp[2 * np + 1], av, bd[2], bd[3]);
+  if (warp >= 8) {
+    // ------------------------------------------------------------------ producer: TMA (warp 8), lse2 / delta (warps 10, 11)
+    tc::setmaxnreg_dec<40>();
+    const int pt = threadIdx.x - 256;
+    int stage = 0;
+    uint32_t phase = 0;
+    if (pt == 0) {
+      tc::tma_prefetch_desc(&tmQ);
+      tc::tma_prefetch_desc(&tmKV);
+      tc::tma_prefetch_desc(&tmDO);
+      tc::mbar_expect_tx(kv_bar, 4 * AB_TILE);
+      for (int g = 0; g < 2; ++g) {
+        const int j0 = kt * 128 + 64 * g;
+        ab_load_tile(sK + g * AB_TILE, &tmKV, kv_bar, E + h * ATT_DH, b, j0);
+        ab_load_tile(sV + g * AB_TILE, &tmKV, kv_bar, 2 * E + h * ATT_DH, b, j0);
+      }
+      for (int qb = 0; qb < nqb; ++qb) {
+        tc::mbar_wait_suspend(&empty[stage], phase ^ 1);
+        uint8_t* dst = sRing + stage * 2 * AB_TILE;
+        tc::mbar_expect_tx(&full[stage], 2 * AB_TILE);
+        ab_load_tile(dst, &tmQ, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
+        ab_load_tile(dst + AB_TILE, &tmDO, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
+        if (++stage == AB_DKV_STAGES) { stage = 0; phase ^= 1; }
+      }
+    } else if (pt >= 64) {
+      const int r = pt - 64;
+      for (int qb = 0; qb < nqb; ++qb) {
+        const int i = qb * AB_ROWS + r;
+        const bool valid = i < p.T;
+        const float l2 = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+        const float dl = valid ? ab_delta(p, b, h, i) : 0.f;
+        tc::mbar_wait_suspend(&empty[stage], phase ^ 1);
+        sStat[stage * 2 * AB_ROWS + r] = l2;
+        sStat[stage * 2 * AB_ROWS + AB_ROWS + r] = dl;
+        tc::mbar_arrive(&full[stage]);
+        if (++stage == AB_DKV_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-    // element (key, query i): P^T = exp2(S^T c - lse2_i), P^T mask -> s, dS^T -> dp
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int ci = 8 * j + 2 * (lane & 3) + (e & 1);
-        const int i = qb * AB_QB + ci;
-        const float pr = fast_ex2(fmaf(s[j][e], p.scale_log2, -st_lse[ci]));
-        const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow_base + i, key_a + 8 * (e >> 1), p.drop_thr) ? dscale : 0.f) : 1.f;
-        dp[j][e] = pr * fmaf(mk, dp[j][e], -st_dl[ci]) * p.scale;
-        s[j][e] = pr * mk;
-      }
-#pragma unroll
-    for (int kk = 0; kk < 2; ++kk) {
-      uint32_t ap[4], as[4];
-      ap[0] = tc::pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
-      ap[1] = tc::pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
-      ap[2] = tc::pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-      ap[3] = tc::pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-      as[0] = tc::pack_bf16x2(dp[2 * kk][0], dp[2 * kk][1]);
-      as[1] = tc::pack_bf16x2(dp[2 * kk][2], dp[2 * kk][3]);
-      as[2] = tc::pack_bf16x2(dp[2 * kk + 1][0], dp[2 * kk + 1][1]);
-      as[3] = tc::pack_bf16x2(dp[2 * kk + 1][2], dp[2 * kk + 1][3]);
-#pragma unroll
-      for (int dd = 0; dd < 8; ++dd) {
-        uint32_t bd[4], bq[4];
-        att_frag_bt(bd, d_s, kk * 16, dd * 16, lane);
-        att_frag_bt(bq, q_s, kk * 16, dd * 16, lane);
-        tc::mma_bf16_16816(dv[2 * dd], ap, bd[0], bd[1]);
-        tc::mma_bf16_16816(dv[2 * dd + 1], ap, bd[2], bd[3]);
-        tc::mma_bf16_16816(dk[2 * dd], as, bq[0], bq[1]);
-        tc::mma_bf16_16816(dk[2 * dd + 1], as, bq[2], bq[3]);
-      }
-    }
-    __syncthreads();     // this buffer is refilled by the next iteration's loads
+    return;
   }
 
+  // -------------------------------------------------------------------- consumer warpgroups
+  tc::setmaxnreg_inc<232>();
+  const int g = warp >> 2, wq = warp & 3;
+  const int tid = threadIdx.x & 127;
+  const uint32_t k_tile = tc::smem_u32(sK + g * AB_TILE), v_tile = tc::smem_u32(sV + g * AB_TILE);
+  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
+  const int key_a = kt * 128 + 64 * g + 16 * wq + (lane >> 2);   // this lane's keys: key_a, key_a + 8
+  const uint32_t drow_base = static_cast<uint32_t>(bh) * p.T;
+  tc::mbar_wait(kv_bar, 0);
+
+  // The first MMAs write dk / dv (scale-d = 0), so nothing but wgmma defines them until the loop has drained.
+  float dk[64], dv[64];
+  int stage = 0;
+  uint32_t phase = 0;
+  bool timed_out = false;
+  for (int qb = 0; qb < nqb; ++qb) {
+    if (!tc::mbar_wait_bounded(&full[stage], phase)) { timed_out = true; break; }
+    const uint32_t q_s = tc::smem_u32(sRing + stage * 2 * AB_TILE);
+    const uint32_t d_s = q_s + AB_TILE;
+    const uint32_t k_s = ab_opaque(k_tile), v_s = ab_opaque(v_tile);
+    const float* st_lse = sStat + stage * 2 * AB_ROWS;
+    const float* st_dl = st_lse + AB_ROWS;
+    float s[32], dp[32];
+    tc::wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) ab_mma_n64(s, ab_desc_k(k_s, kk), ab_desc_k(q_s, kk), kk);
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) ab_mma_n64(dp, ab_desc_k(v_s, kk), ab_desc_k(d_s, kk), kk);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::wgmma_fence_regs(s);
+    tc::wgmma_fence_regs(dp);
+
+    // element 4 j + e is (key key_a + 8 (e >> 1), query row qb * 64 + 8 j + 2 (lane & 3) + (e & 1)).  Per 16 query rows
+    // kk: P^T . mask -> ap, dS^T -> as, then dV += ap dO and dK += as Q for those rows, so the MMAs of one slice run while
+    // the next is computed and the A fragments take the registers that S^T and dP^T free.
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t ap[4], as[4];
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; e += 2) {
+          const int j = 2 * kk + jj;
+          float pm[2], ds[2];
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int ci = 8 * j + 2 * (lane & 3) + c;
+            const int i = qb * AB_ROWS + ci;
+            const float pr = fast_ex2(fmaf(s[4 * j + e + c], p.scale_log2, -st_lse[ci]));
+            const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow_base + i, key_a + 8 * (e >> 1), p.drop_thr) ? dscale : 0.f) : 1.f;
+            ds[c] = pr * fmaf(mk, dp[4 * j + e + c], -st_dl[ci]) * p.scale;
+            pm[c] = pr * mk;
+          }
+          ap[2 * jj + (e >> 1)] = tc::pack_bf16x2(pm[0], pm[1]);
+          as[2 * jj + (e >> 1)] = tc::pack_bf16x2(ds[0], ds[1]);
+        }
+      tc::wgmma_fence();
+      tc::wgmma_m64n128k16_rs(dv, ap, ab_desc_mn(d_s, kk), qb > 0 || kk > 0);
+      tc::wgmma_m64n128k16_rs(dk, as, ab_desc_mn(q_s, kk), qb > 0 || kk > 0);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    if (tid == 0) tc::mbar_arrive(&empty[stage]);
+    if (++stage == AB_DKV_STAGES) { stage = 0; phase ^= 1; }
+  }
+  tc::wgmma_fence_regs(dk);
+  tc::wgmma_fence_regs(dv);
+
+  // dk[4 j + 2 r + c] is key key_a + 8 r, column 8 j + 2 (lane & 3) + c
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int key = key_a + 8 * r;
@@ -374,11 +488,22 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
       __nv_bfloat16* grow = p.dqkv + att_tok(key, b, p.T, p.B, p.batch_major) * p.ld_dqkv + h * ATT_DH;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        att_st2(grow + E, j, lane, dk[j][2 * r], dk[j][2 * r + 1]);
-        att_st2(grow + 2 * E, j, lane, dv[j][2 * r], dv[j][2 * r + 1]);
+        att_st2(grow + E, j, lane, dk[4 * j + 2 * r], dk[4 * j + 2 * r + 1]);
+        att_st2(grow + 2 * E, j, lane, dv[4 * j + 2 * r], dv[4 * j + 2 * r + 1]);
       }
     }
   }
+  if (timed_out) asm volatile("trap;");
+}
+
+// 3-D tensor map (columns, batch, time) over a [T*B, ld] bf16 activation, token row t*B + b (or b*T + t when batch-major),
+// with a box of 64 columns x 1 x 64 rows and the 128-byte swizzle; rows at t >= t_extent read as zeros
+static int ab_tensor_map(CUtensorMap* m, const void* base, int cols, int ld, int T, int B, int t_extent, int batch_major) {
+  const uint64_t row = static_cast<uint64_t>(ld) * 2;
+  const uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(B), static_cast<uint64_t>(t_extent)};
+  const uint64_t strides[3] = {0, batch_major ? row * T : row, batch_major ? row : row * B};
+  const uint32_t box[3] = {64, 1, AB_ROWS};
+  return make_tensor_map(m, base, false, 3, dims, strides, box, true);
 }
 
 }  // namespace pfn
@@ -397,6 +522,12 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
   p.lse = d->lse; p.delta = d->delta; p.dq_colsum = d->dq_colsum; p.delta_tm = d->delta_token_major;
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
   p.batch_major = d->batch_major;
+  const int E = d->H * ATT_DH;
+  CUtensorMap tmQ, tmKV, tmDO;
+  if (int rc = ab_tensor_map(&tmQ, d->qkv, 3 * E, d->ld_qkv, d->T, d->B, d->T, d->batch_major)) return rc;
+  // K / V: keys past sep read as zeros (the map needs a non-empty extent; with sep = 0 no key block is loaded)
+  if (int rc = ab_tensor_map(&tmKV, d->qkv, 3 * E, d->ld_qkv, d->T, d->B, d->sep > 0 ? d->sep : 1, d->batch_major)) return rc;
+  if (int rc = ab_tensor_map(&tmDO, d->dout, E, d->ld_dout, d->T, d->B, d->T, d->batch_major)) return rc;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_DQ_SMEM));
@@ -411,15 +542,16 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
                                                                  p.dout, p.ld_dout, d->delta, d->T, d->B, d->H, d->batch_major);
     PFN_LAUNCH_OK();
   }
-  p.n_tiles = (d->T + AB_BM - 1) / AB_BM;
-  long long grid = static_cast<long long>(p.n_tiles) * d->B * d->H;
-  PFN_CHECK_ARG(grid < (1LL << 31), "attention_bwd_tc: too many tiles");
-  attn_bwd_dq_kernel<<<static_cast<unsigned>(grid), 128, AB_DQ_SMEM, s>>>(p);
+  p.n_tiles = (d->T + 127) / 128;
+  const long long units = static_cast<long long>(p.n_tiles) * d->B * d->H;
+  PFN_CHECK_ARG(units < (1LL << 31), "attention_bwd_tc: too many tiles");
+  const int grid_dq = units < num_sms() ? static_cast<int>(units) : num_sms();
+  attn_bwd_dq_kernel<<<static_cast<unsigned>(grid_dq), AB_THREADS, AB_DQ_SMEM, s>>>(tmQ, tmKV, tmDO, p);
   PFN_LAUNCH_OK();
   if (d->sep > 0) {
-    p.n_tiles = (d->sep + AB_BM - 1) / AB_BM;
-    grid = static_cast<long long>(p.n_tiles) * d->B * d->H;
-    attn_bwd_dkv_kernel<<<static_cast<unsigned>(grid), 128, AB_DKV_SMEM, s>>>(p);
+    p.n_tiles = (d->sep + 127) / 128;
+    const long long grid = static_cast<long long>(p.n_tiles) * d->B * d->H;
+    attn_bwd_dkv_kernel<<<static_cast<unsigned>(grid), AB_THREADS, AB_DKV_SMEM, s>>>(tmQ, tmKV, tmDO, p);
     PFN_LAUNCH_OK();
   }
   return 0;

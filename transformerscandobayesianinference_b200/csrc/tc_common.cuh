@@ -55,6 +55,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > PFN_MBAR_SPIN_LIMIT) asm volatile("trap;");
   }
 }
+// The same bound, reported to the caller (false = timed out) so that it can leave its loop and trap outside it.  A trap
+// inside a loop that keeps wgmma accumulators live makes ptxas limit that loop to the launch-time register budget
+// instead of the one setmaxnreg raised it to.
+__device__ __forceinline__ bool mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > PFN_MBAR_SPIN_LIMIT) return false;
+  }
+  return true;
+}
 
 // Waiter that is NOT on the critical path (the TMA producer waiting for a free ring stage): the potentially blocking
 // mbarrier.try_wait lets the hardware park the warp instead of spinning on the issue slots the consumers need.
@@ -82,6 +92,12 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
 // shared -> global tile store / fp32 reduce-add (clipped at the tensor bounds), tracked by bulk async-groups
@@ -176,6 +192,52 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both operands K-major in shared memory.  ACCUMULATE = 0 overwrites D and
+// declares it write-only, so the previous contents are dead before the MMA (an accumulator that is rebuilt every
+// iteration then does not hold its registers across the rest of the loop).
+#define PFN_WGMMA_D32(C)                                                                                          \
+  C(d[0]), C(d[1]), C(d[2]), C(d[3]), C(d[4]), C(d[5]), C(d[6]), C(d[7]), C(d[8]), C(d[9]), C(d[10]), C(d[11]),   \
+      C(d[12]), C(d[13]), C(d[14]), C(d[15]), C(d[16]), C(d[17]), C(d[18]), C(d[19]), C(d[20]), C(d[21]),         \
+      C(d[22]), C(d[23]), C(d[24]), C(d[25]), C(d[26]), C(d[27]), C(d[28]), C(d[29]), C(d[30]), C(d[31])
+#define PFN_WGMMA_M64N64K16(SCALE_D)                                                                              \
+  "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "                                                         \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                       \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, " SCALE_D ", 1, 1, 0, 0;"
+template <int ACCUMULATE>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+  if constexpr (ACCUMULATE) {
+    asm volatile(PFN_WGMMA_M64N64K16("1") : PFN_WGMMA_D32("+f") : "l"(a_desc), "l"(b_desc));
+  } else {
+    asm volatile(PFN_WGMMA_M64N64K16("0") : PFN_WGMMA_D32("=f") : "l"(a_desc), "l"(b_desc));
+  }
+}
+#undef PFN_WGMMA_M64N64K16
+#undef PFN_WGMMA_D32
+
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T with A in registers and B MN-major in shared memory.  The A fragment of
+// warp w is rows 16 w .. 16 w + 15 in the mma.m16n8k16 A layout, which is the layout of columns 16 k .. 16 k + 15 of a
+// 64 x N wgmma accumulator packed to bf16: a = {acc[8k] acc[8k+1], acc[8k+2] acc[8k+3], acc[8k+4] acc[8k+5], acc[8k+6] acc[8k+7]}.
+__device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
 
 // ---------------------------------------------------------------------------------------------
