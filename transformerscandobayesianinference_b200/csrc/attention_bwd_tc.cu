@@ -27,8 +27,8 @@
 
 namespace pfn {
 
-constexpr int AB_ROWS = 64;                               // rows of one consumer warpgroup; key / query block size
-constexpr int AB_TILE = AB_ROWS * ATT_ROW_BYTES;          // 16 KB: 64 rows x 128 bf16 = two 8 KB boxes of 64 columns
+constexpr int AB_ROWS = ATT_TILE_ROWS;                    // rows of one consumer warpgroup; key / query block size
+constexpr int AB_TILE = ATT_TILE;                         // 16 KB: 64 rows x 128 bf16 = two 8 KB boxes of 64 columns
 constexpr int AB_THREADS = 3 * 128;
 constexpr int AB_DQ_STAGES = 4;                           // K/V blocks in flight (dQ kernel)
 constexpr int AB_DKV_STAGES = 3;                          // Q/dO blocks in flight (dK/dV kernel)
@@ -60,32 +60,6 @@ struct AttnBwdParams {
 
 __device__ __forceinline__ float ab_delta(const AttnBwdParams& p, int b, int h, int i) {
   return p.delta_tm ? p.delta[att_tok(i, b, p.T, p.B, 0) * p.H + h] : p.delta[(static_cast<size_t>(b) * p.H + h) * p.T + i];
-}
-
-// wgmma descriptors of a 64-row tile (two 64-column boxes 8 KB apart, 128-byte swizzle), k16 step kk:
-// K-major (the tile's columns are the k index, kk < 8) and MN-major (its rows are the k index, kk < 4)
-__device__ __forceinline__ uint64_t ab_desc_k(uint32_t tile, int kk) {
-  return tc::wgmma_smem_desc(tile + (kk >> 2) * 8192 + (kk & 3) * 32, 16, 1024);
-}
-__device__ __forceinline__ uint64_t ab_desc_mn(uint32_t tile, int kk) {
-  return tc::wgmma_smem_desc(tile + kk * 2048, 8192, 1024);
-}
-// The address of a tile that stays resident across a loop, made opaque in every iteration so that the descriptors of its
-// k16 steps are formed next to their MMAs instead of being hoisted out of the loop and held in registers throughout.
-__device__ __forceinline__ uint32_t ab_opaque(uint32_t addr) {
-  asm volatile("" : "+r"(addr));
-  return addr;
-}
-// k16 step kk of a 64 x 64 score block; the first step writes the accumulator
-__device__ __forceinline__ void ab_mma_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, int kk) {
-  if (kk == 0) tc::wgmma_m64n64k16<0>(d, a_desc, b_desc);
-  else tc::wgmma_m64n64k16<1>(d, a_desc, b_desc);
-}
-
-// TMA of rows [t0, t0 + 64) of one head (columns col0 .. col0 + 127) into a 16 KB tile
-__device__ __forceinline__ void ab_load_tile(uint8_t* dst, const CUtensorMap* m, uint64_t* bar, int col0, int b, int t0) {
-  tc::tma_load_3d(dst, m, bar, col0, b, t0);
-  tc::tma_load_3d(dst + 8192, m, bar, col0 + 64, b, t0);
 }
 
 // =====================================================================================================================
@@ -174,8 +148,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           if (it > 0) tc::mbar_wait_suspend(q_empty, (it - 1) & 1);
           tc::mbar_expect_tx(q_full, 4 * AB_TILE);
           for (int g = 0; g < 2; ++g) {
-            ab_load_tile(sQ + g * AB_TILE, &tmQ, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
-            ab_load_tile(sD + g * AB_TILE, &tmDO, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
+            att_load_tile(sQ + g * AB_TILE, &tmQ, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
+            att_load_tile(sD + g * AB_TILE, &tmDO, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
           }
         };
         const int claim_at = min(AB_DQ_STAGES - 1, nblk - 1);
@@ -185,8 +159,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           tc::mbar_wait_suspend(&kv_empty[stage], phase ^ 1);
           uint8_t* dst = sRing + stage * 2 * AB_TILE;
           tc::mbar_expect_tx(&kv_full[stage], 2 * AB_TILE);
-          ab_load_tile(dst, &tmKV, &kv_full[stage], E + h * ATT_DH, b, kb * AB_ROWS);
-          ab_load_tile(dst + AB_TILE, &tmKV, &kv_full[stage], 2 * E + h * ATT_DH, b, kb * AB_ROWS);
+          att_load_tile(dst, &tmKV, &kv_full[stage], E + h * ATT_DH, b, kb * AB_ROWS);
+          att_load_tile(dst + AB_TILE, &tmKV, &kv_full[stage], 2 * E + h * ATT_DH, b, kb * AB_ROWS);
           if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -227,13 +201,13 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       if (!tc::mbar_wait_bounded(&kv_full[stage], phase)) { timed_out = true; break; }
       const uint32_t k_s = tc::smem_u32(sRing + stage * 2 * AB_TILE);
       const uint32_t v_s = k_s + AB_TILE;
-      const uint32_t q_s = ab_opaque(q_tile), d_s = ab_opaque(d_tile);
+      const uint32_t q_s = att_opaque(q_tile), d_s = att_opaque(d_tile);
       float s[32], dp[32];
       tc::wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) ab_mma_n64(s, ab_desc_k(q_s, kk), ab_desc_k(k_s, kk), kk);
+      for (int kk = 0; kk < 8; ++kk) att_mma_n64(s, att_desc_k(q_s, kk), att_desc_k(k_s, kk), kk);
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) ab_mma_n64(dp, ab_desc_k(d_s, kk), ab_desc_k(v_s, kk), kk);
+      for (int kk = 0; kk < 8; ++kk) att_mma_n64(dp, att_desc_k(d_s, kk), att_desc_k(v_s, kk), kk);
       tc::wgmma_commit();
       tc::wgmma_wait<0>();
       tc::wgmma_fence_regs(s);
@@ -260,7 +234,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         }
       tc::wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(dq, ads + 4 * kk, ab_desc_mn(k_s, kk), kb > 0 || kk > 0);
+      for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(dq, ads + 4 * kk, att_desc_mn(k_s, kk), kb > 0 || kk > 0);
       tc::wgmma_commit();
       tc::wgmma_wait<0>();
       if (tid == 0) tc::mbar_arrive(&kv_empty[stage]);
@@ -383,15 +357,15 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       tc::mbar_expect_tx(kv_bar, 4 * AB_TILE);
       for (int g = 0; g < 2; ++g) {
         const int j0 = kt * 128 + 64 * g;
-        ab_load_tile(sK + g * AB_TILE, &tmKV, kv_bar, E + h * ATT_DH, b, j0);
-        ab_load_tile(sV + g * AB_TILE, &tmKV, kv_bar, 2 * E + h * ATT_DH, b, j0);
+        att_load_tile(sK + g * AB_TILE, &tmKV, kv_bar, E + h * ATT_DH, b, j0);
+        att_load_tile(sV + g * AB_TILE, &tmKV, kv_bar, 2 * E + h * ATT_DH, b, j0);
       }
       for (int qb = 0; qb < nqb; ++qb) {
         tc::mbar_wait_suspend(&empty[stage], phase ^ 1);
         uint8_t* dst = sRing + stage * 2 * AB_TILE;
         tc::mbar_expect_tx(&full[stage], 2 * AB_TILE);
-        ab_load_tile(dst, &tmQ, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
-        ab_load_tile(dst + AB_TILE, &tmDO, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
+        att_load_tile(dst, &tmQ, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
+        att_load_tile(dst + AB_TILE, &tmDO, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
         if (++stage == AB_DKV_STAGES) { stage = 0; phase ^= 1; }
       }
     } else if (pt >= 64) {
@@ -430,15 +404,15 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     if (!tc::mbar_wait_bounded(&full[stage], phase)) { timed_out = true; break; }
     const uint32_t q_s = tc::smem_u32(sRing + stage * 2 * AB_TILE);
     const uint32_t d_s = q_s + AB_TILE;
-    const uint32_t k_s = ab_opaque(k_tile), v_s = ab_opaque(v_tile);
+    const uint32_t k_s = att_opaque(k_tile), v_s = att_opaque(v_tile);
     const float* st_lse = sStat + stage * 2 * AB_ROWS;
     const float* st_dl = st_lse + AB_ROWS;
     float s[32], dp[32];
     tc::wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) ab_mma_n64(s, ab_desc_k(k_s, kk), ab_desc_k(q_s, kk), kk);
+    for (int kk = 0; kk < 8; ++kk) att_mma_n64(s, att_desc_k(k_s, kk), att_desc_k(q_s, kk), kk);
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) ab_mma_n64(dp, ab_desc_k(v_s, kk), ab_desc_k(d_s, kk), kk);
+    for (int kk = 0; kk < 8; ++kk) att_mma_n64(dp, att_desc_k(v_s, kk), att_desc_k(d_s, kk), kk);
     tc::wgmma_commit();
     tc::wgmma_wait<0>();
     tc::wgmma_fence_regs(s);
@@ -469,8 +443,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
           as[2 * jj + (e >> 1)] = tc::pack_bf16x2(ds[0], ds[1]);
         }
       tc::wgmma_fence();
-      tc::wgmma_m64n128k16_rs(dv, ap, ab_desc_mn(d_s, kk), qb > 0 || kk > 0);
-      tc::wgmma_m64n128k16_rs(dk, as, ab_desc_mn(q_s, kk), qb > 0 || kk > 0);
+      tc::wgmma_m64n128k16_rs(dv, ap, att_desc_mn(d_s, kk), qb > 0 || kk > 0);
+      tc::wgmma_m64n128k16_rs(dk, as, att_desc_mn(q_s, kk), qb > 0 || kk > 0);
     }
     tc::wgmma_commit();
     tc::wgmma_wait<0>();
@@ -496,16 +470,6 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   if (timed_out) asm volatile("trap;");
 }
 
-// 3-D tensor map (columns, batch, time) over a [T*B, ld] bf16 activation, token row t*B + b (or b*T + t when batch-major),
-// with a box of 64 columns x 1 x 64 rows and the 128-byte swizzle; rows at t >= t_extent read as zeros
-static int ab_tensor_map(CUtensorMap* m, const void* base, int cols, int ld, int T, int B, int t_extent, int batch_major) {
-  const uint64_t row = static_cast<uint64_t>(ld) * 2;
-  const uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(B), static_cast<uint64_t>(t_extent)};
-  const uint64_t strides[3] = {0, batch_major ? row * T : row, batch_major ? row : row * B};
-  const uint32_t box[3] = {64, 1, AB_ROWS};
-  return make_tensor_map(m, base, false, 3, dims, strides, box, true);
-}
-
 }  // namespace pfn
 
 using namespace pfn;
@@ -524,10 +488,8 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
   p.batch_major = d->batch_major;
   const int E = d->H * ATT_DH;
   CUtensorMap tmQ, tmKV, tmDO;
-  if (int rc = ab_tensor_map(&tmQ, d->qkv, 3 * E, d->ld_qkv, d->T, d->B, d->T, d->batch_major)) return rc;
-  // K / V: keys past sep read as zeros (the map needs a non-empty extent; with sep = 0 no key block is loaded)
-  if (int rc = ab_tensor_map(&tmKV, d->qkv, 3 * E, d->ld_qkv, d->T, d->B, d->sep > 0 ? d->sep : 1, d->batch_major)) return rc;
-  if (int rc = ab_tensor_map(&tmDO, d->dout, E, d->ld_dout, d->T, d->B, d->T, d->batch_major)) return rc;
+  if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
+  if (int rc = att_tensor_map(&tmDO, d->dout, E, d->ld_dout, d->T, d->B, d->T, d->batch_major)) return rc;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_DQ_SMEM));

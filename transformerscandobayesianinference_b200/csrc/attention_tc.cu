@@ -6,179 +6,267 @@
 // diagonal key of a query row is a 128-wide dot product done by the four lanes that own the row.  Q/K/V rows are read
 // straight out of the packed [T*B, 3E] in-projection output, so there is no head-split / transpose kernel.
 //
-// One CTA (4 warps) per (batch, head, 64-row query tile); warp w owns query rows [16 w, 16 w + 16).  K and V blocks are
-// double-buffered with cp.async so the loads of block j+1 overlap the MMAs and softmax of block j:
-//   S_j = Q K_j^T (mma.sync, fp32)  ->  online softmax in the log2 domain  ->  P_j as bf16 A fragments  ->  O += P_j V_j
-// P_j never leaves the registers: the S accumulator layout of two n-tiles is the A fragment layout of one k-step.
+// attn_fwd_kernel is persistent: one CTA per SM walks the (batch, head, 128-row query tile) units, query tile fastest,
+// so the tiles of one (batch, head) run at the same time and share its K/V in L2.  It is warp-specialised like the dQ
+// backward kernel: warpgroup 2 (producer, 40 registers) TMA-loads the tile's Q and a 4-stage ring of (K, V) 64-key blocks;
+// warpgroups 0 and 1 (consumers, 232 registers) each own 64 query rows and run, per key block j,
+//   S_j = Q K_j^T (wgmma m64n64k16, fp32)  ->  online softmax in the log2 domain  ->  P_j as bf16 A fragments (registers)
+//   ->  O += P_j V_j (wgmma m64n128k16, A from registers, V read MN-major)
+// with S_j and the PV MMAs of block j-1 issued together, so the softmax of block j runs under the previous P V.  A row's
+// diagonal key is folded in before the loop: m = s_ii, l = 1, O = keep_ii v_i (rows < sep start from -inf, 0, 0).
+// O / l is packed to bf16 into a 128-byte-swizzled staging tile per warpgroup and written with TMA tile stores, which
+// clip rows past T.
 #include "attention_common.cuh"
 
 namespace pfn {
 
-constexpr int ATT_BM = 64;                                // query rows per CTA
-constexpr int ATT_BN = 64;                                // keys per block
-constexpr int ATT_TILE_BYTES = ATT_BM * ATT_ROW_BYTES;    // 16 KB
-constexpr int ATT_FWD_SMEM = 5 * ATT_TILE_BYTES;          // Q + 2 x K + 2 x V
+constexpr int AF_THREADS = 3 * 128;
+constexpr int AF_STAGES = 4;                              // (K, V) blocks in flight
+// Q of the tile (2 x 16 KB), output staging (2 x 16 KB), ring of (K, V), barriers
+constexpr int AF_OFF_STG = 2 * ATT_TILE;
+constexpr int AF_OFF_RING = 4 * ATT_TILE;
+constexpr int AF_OFF_BAR = AF_OFF_RING + AF_STAGES * 2 * ATT_TILE;
+constexpr int AF_SMEM = AF_OFF_BAR + (2 * AF_STAGES + 2) * 8 + 1024;   // + 1 KB alignment slack
+static_assert(AF_SMEM <= 232448, "the tiles and the ring must fit the 227 KB of shared memory");
 
 struct AttnFwdParams {
   int T, B, H, sep;
   float scale_log2;   // scale * log2(e)
   const __nv_bfloat16* qkv; int ld_qkv;
-  __nv_bfloat16* out; int ld_out;
   float* lse;
-  int n_qtiles;
+  int n_tiles;        // 128-row query tiles per (batch, head)
   int batch_major;
   uint32_t drop_seed; int drop_thr;   // dropout on the probabilities (thr 0 = off), csrc/dropout.cuh
 };
 
-__global__ void __launch_bounds__(128, 2)
-attn_fwd_tc_kernel(const AttnFwdParams p) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* sQ = smem;
-  uint8_t* sK = smem + ATT_TILE_BYTES;                    // buffer s at + s * 16 KB
-  uint8_t* sV = smem + 3 * ATT_TILE_BYTES;
+__global__ void __launch_bounds__(AF_THREADS, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
+                const __grid_constant__ CUtensorMap tmO, const AttnFwdParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* sQ = smem;                                     // warpgroup g's 64 rows at + g * 16 KB
+  uint8_t* sStg = smem + AF_OFF_STG;                      // warpgroup g's output staging at + g * 16 KB
+  uint8_t* sRing = smem + AF_OFF_RING;                    // stage s: K at + 2 s * 16 KB, V at + (2 s + 1) * 16 KB
+  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + AF_OFF_BAR);
+  uint64_t* kv_empty = kv_full + AF_STAGES;
+  uint64_t* q_full = kv_empty + AF_STAGES;                // Q of the CTA's current tile has landed
+  uint64_t* q_empty = q_full + 1;                         // both warpgroups have finished their last S MMAs of it
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qt = static_cast<int>(blockIdx.x) % p.n_qtiles;
-  const int bh = static_cast<int>(blockIdx.x) / p.n_qtiles;
-  const int h = bh % p.H, b = bh / p.H;
   const int E = p.H * ATT_DH;
-  const int i0 = qt * ATT_BM;
-  const int nblk = (p.sep + ATT_BN - 1) / ATT_BN;
-
-  att_load_tile<ATT_BM>(sQ, p.qkv, p.ld_qkv, h * ATT_DH, i0, p.T, b, p.T, p.B, p.batch_major);
-  if (nblk > 0) {
-    att_load_tile<ATT_BN>(sK, p.qkv, p.ld_qkv, E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
-    att_load_tile<ATT_BN>(sV, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, 0, p.sep, b, p.T, p.B, p.batch_major);
+  const int nblk = (p.sep + ATT_TILE_ROWS - 1) / ATT_TILE_ROWS;
+  const int n_units = p.n_tiles * p.B * p.H;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < AF_STAGES; ++s) {
+      tc::mbar_init(&kv_full[s], 1);
+      tc::mbar_init(&kv_empty[s], 2);
+    }
+    tc::mbar_init(q_full, 1);
+    tc::mbar_init(q_empty, 2);
+    tc::mbar_fence_init();
   }
-  tc::cp_async_commit();
+  __syncthreads();
 
-  float o[16][4];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  const int r0 = 16 * warp;
-  const uint32_t drow0 = static_cast<uint32_t>(bh) * p.T + i0 + r0 + (lane >> 2);   // dropout row of this lane's first row
-  const uint32_t q_s = tc::smem_u32(sQ);
-
-  for (int kb = 0; kb < nblk; ++kb) {
-    if (kb + 1 < nblk) {
-      const int nb = (kb + 1) & 1;
-      att_load_tile<ATT_BN>(sK + nb * ATT_TILE_BYTES, p.qkv, p.ld_qkv, E + h * ATT_DH, (kb + 1) * ATT_BN, p.sep, b, p.T, p.B, p.batch_major);
-      att_load_tile<ATT_BN>(sV + nb * ATT_TILE_BYTES, p.qkv, p.ld_qkv, 2 * E + h * ATT_DH, (kb + 1) * ATT_BN, p.sep, b, p.T, p.B, p.batch_major);
-      tc::cp_async_commit();
-      tc::cp_async_wait<1>();
-    } else {
-      tc::cp_async_wait<0>();
-    }
-    __syncthreads();
-    const uint32_t k_s = tc::smem_u32(sK + (kb & 1) * ATT_TILE_BYTES);
-    const uint32_t v_s = tc::smem_u32(sV + (kb & 1) * ATT_TILE_BYTES);
-
-    float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t a[4];
-      att_frag_a(a, q_s, r0, kk * 16, lane);
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t bb[4];
-        att_frag_b(bb, k_s, np * 16, kk * 16, lane);
-        tc::mma_bf16_16816(s[2 * np], a, bb[0], bb[1]);
-        tc::mma_bf16_16816(s[2 * np + 1], a, bb[2], bb[3]);
+  if (warp >= 8) {
+    // ------------------------------------------------------------------ TMA producer
+    tc::setmaxnreg_dec<40>();
+    if (threadIdx.x == 256) {
+      tc::tma_prefetch_desc(&tmQ);
+      tc::tma_prefetch_desc(&tmKV);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
+        const int qt = u % p.n_tiles, bh = u / p.n_tiles;
+        const int h = bh % p.H, b = bh / p.H;
+        // The next tile's Q goes in once the consumers are done with the current one, which is before its last key
+        // block is (so the first key blocks of the next tile are already in flight by then).
+        auto load_q = [&]() {
+          if (it > 0) tc::mbar_wait_suspend(q_empty, (it - 1) & 1);
+          tc::mbar_expect_tx(q_full, 2 * ATT_TILE);
+          for (int g = 0; g < 2; ++g) att_load_tile(sQ + g * ATT_TILE, &tmQ, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
+        };
+        const int claim_at = min(AF_STAGES - 1, nblk - 1);
+        if (nblk == 0) load_q();
+        for (int kb = 0; kb < nblk; ++kb) {
+          if (kb == claim_at) load_q();
+          tc::mbar_wait_suspend(&kv_empty[stage], phase ^ 1);
+          uint8_t* dst = sRing + stage * 2 * ATT_TILE;
+          tc::mbar_expect_tx(&kv_full[stage], 2 * ATT_TILE);
+          att_load_tile(dst, &tmKV, &kv_full[stage], E + h * ATT_DH, b, kb * ATT_TILE_ROWS);
+          att_load_tile(dst + ATT_TILE, &tmKV, &kv_full[stage], 2 * E + h * ATT_DH, b, kb * ATT_TILE_ROWS);
+          if (++stage == AF_STAGES) { stage = 0; phase ^= 1; }
+        }
       }
     }
-    // online softmax (log2 domain); keys >= sep of the last block are masked
-    const int key0 = kb * ATT_BN + 2 * (lane & 3);
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const bool ok = key0 + 8 * j + (e & 1) < p.sep;
-        s[j][e] = ok ? s[j][e] * p.scale_log2 : -INFINITY;
-        mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
-      }
-    float corr[2];
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups
+  tc::setmaxnreg_inc<232>();
+  const int g = warp >> 2, wq = warp & 3;
+  const int tid = threadIdx.x & 127;
+  const uint32_t q_tile = tc::smem_u32(sQ + g * ATT_TILE);
+  uint8_t* stg = sStg + g * ATT_TILE;
+  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
+  int stage = 0;
+  uint32_t phase = 0;
+  bool timed_out = false;
+  for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
+    const int qt = u % p.n_tiles, bh = u / p.n_tiles;
+    const int h = bh % p.H, b = bh / p.H;
+    const int t0 = qt * 128 + 64 * g;
+    const int i0 = t0 + 16 * wq + (lane >> 2);            // this lane's rows: i0, i0 + 8
+
+    // Diagonal key first: o[4 j + 2 r + c] is row i0 + 8 r, column 8 j + 2 (lane & 3) + c.  A row i >= sep starts from
+    // m = s_ii, l = 1 (this lane's share of l: 1 in lane 0 of the quad) and O = keep_ii v_i; the loads are in flight
+    // while the first TMA waits run.
+    float o[64], m[2], l[2];
+    uint32_t drow[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const float mn = fmaxf(m[r], quad_max(mx[r]));
-      corr[r] = fast_ex2(m[r] - mn);
-      m[r] = mn;
-      l[r] *= corr[r];
-    }
+      const int i = i0 + 8 * r;
+      const bool diag = i < p.T && i >= p.sep;
+      drow[r] = static_cast<uint32_t>(bh) * p.T + i;
+      const __nv_bfloat16* qrow = p.qkv + att_tok(diag ? i : 0, b, p.T, p.B, p.batch_major) * p.ld_qkv + h * ATT_DH;
+      float sd = 0.f;
+      if (diag) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float pr = fast_ex2(s[j][e] - m[e >> 1]);
-        l[e >> 1] += pr;
-        if (p.drop_thr > 0 && !drop_keep(p.drop_seed, drow0 + 8 * (e >> 1), key0 + 8 * j + (e & 1), p.drop_thr)) s[j][e] = 0.f;
-        else s[j][e] = pr;
+        for (int j = 0; j < 16; ++j) {
+          const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane);
+          sd = fmaf(q.x, k.x, fmaf(q.y, k.y, sd));
+        }
       }
+      sd = quad_sum(sd) * p.scale_log2;
+      m[r] = diag ? sd : -INFINITY;
+      l[r] = diag && (lane & 3) == 0 ? 1.f : 0.f;
+      const bool keep = diag && (p.drop_thr == 0 || drop_keep(p.drop_seed, drow[r], i, p.drop_thr));
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      o[j][0] *= corr[0]; o[j][1] *= corr[0];
-      o[j][2] *= corr[1]; o[j][3] *= corr[1];
-    }
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      a[0] = tc::pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
-      a[1] = tc::pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
-      a[2] = tc::pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-      a[3] = tc::pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-      for (int dp = 0; dp < 8; ++dp) {
-        uint32_t bb[4];
-        att_frag_bt(bb, v_s, kk * 16, dp * 16, lane);
-        tc::mma_bf16_16816(o[2 * dp], a, bb[0], bb[1]);
-        tc::mma_bf16_16816(o[2 * dp + 1], a, bb[2], bb[3]);
+      for (int j = 0; j < 16; ++j) {
+        const float2 v = keep ? att_ld2(qrow + 2 * E, j, lane) : make_float2(0.f, 0.f);
+        o[4 * j + 2 * r] = v.x;
+        o[4 * j + 2 * r + 1] = v.y;
       }
     }
-    __syncthreads();     // this buffer is refilled by the next iteration's loads
-  }
+    if (!tc::mbar_wait_bounded(q_full, it & 1)) { timed_out = true; break; }
 
-  // diagonal key of the query rows (i >= sep), normalisation, stores
-  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
+    // Key loop.  Block kb issues S_kb = Q K_kb^T and PV_{kb-1} (O += P_{kb-1} V_{kb-1}) back to back, waits for S_kb
+    // only and runs its softmax while PV_{kb-1} is on the tensor pipe, then waits for PV_{kb-1}, rescales O and packs
+    // P_kb.  O and the S accumulator are written only when no MMA that owns them is in flight: otherwise ptxas
+    // serialises the whole wgmma pipeline.  For the same reason a timed-out wait inside the loop is recorded and the
+    // block runs on; the tile is abandoned once the pipeline has drained.
+    float s[32];
+    uint32_t ap[16];
+    float corr[2];
+    auto issue_s = [&](int st) {
+      const uint32_t k_s = tc::smem_u32(sRing + st * 2 * ATT_TILE);
+      const uint32_t q_s = att_opaque(q_tile);
+      tc::wgmma_fence();
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int i = i0 + r0 + (lane >> 2) + 8 * r;
-    float lr = quad_sum(l[r]);
-    const bool valid = i < p.T;
-    const bool diag = valid && i >= p.sep;
-    const __nv_bfloat16* qrow = p.qkv + att_tok(valid ? i : 0, b, p.T, p.B, p.batch_major) * p.ld_qkv + h * ATT_DH;
-    float sd = 0.f;
-    if (diag) {
+      for (int kk = 0; kk < 8; ++kk) att_mma_n64(s, att_desc_k(q_s, kk), att_desc_k(k_s, kk), kk);
+      tc::wgmma_commit();
+    };
+    auto issue_pv = [&](int st) {
+      const uint32_t v_s = tc::smem_u32(sRing + st * 2 * ATT_TILE) + ATT_TILE;
+      tc::wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane);
-        sd = fmaf(q.x, k.x, fmaf(q.y, k.y, sd));
+      for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(o, ap + 4 * kk, att_desc_mn(v_s, kk), 1);
+      tc::wgmma_commit();
+    };
+    // Online softmax of block kb in s.  Element 4 j + e of S is row i0 + 8 (e >> 1), key kb * 64 + 8 j + 2 (lane & 3) +
+    // (e & 1); keys >= sep (only in the last block) are masked.  The running max m is in the scaled log2 domain; the
+    // scale > 0 is applied to the block max and inside the exp2 argument, p = 2^(s c - m).  l sums the probabilities
+    // before dropout; s is left holding them after dropout.
+    auto softmax = [&](int kb) {
+      const int key0 = kb * ATT_TILE_ROWS + 2 * (lane & 3);
+      if (kb * ATT_TILE_ROWS + ATT_TILE_ROWS > p.sep) {
+#pragma unroll
+        for (int e = 0; e < 32; ++e)
+          if (key0 + 8 * (e >> 2) + (e & 1) >= p.sep) s[e] = -INFINITY;
       }
-    }
-    sd = quad_sum(sd) * p.scale_log2;
-    if (diag) {
-      const float mn = fmaxf(m[r], sd);
-      const float c = fast_ex2(m[r] - mn);
-      const float pr = fast_ex2(sd - mn);
-      lr = lr * c + pr;
-      m[r] = mn;
-      const float pd = (p.drop_thr > 0 && !drop_keep(p.drop_seed, drow0 + 8 * r, i, p.drop_thr)) ? 0.f : pr;
+      float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float2 v = att_ld2(qrow + 2 * E, j, lane);
-        o[j][2 * r] = fmaf(pd, v.x, o[j][2 * r] * c);
-        o[j][2 * r + 1] = fmaf(pd, v.y, o[j][2 * r + 1] * c);
+      for (int e = 0; e < 32; ++e) mx[(e >> 1) & 1] = fmaxf(mx[(e >> 1) & 1], s[e]);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float mn = fmaxf(m[r], quad_max(mx[r]) * p.scale_log2);
+        corr[r] = fast_ex2(m[r] - mn);
+        m[r] = mn;
+        l[r] *= corr[r];
       }
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        const int r = (e >> 1) & 1;
+        const float pr = fast_ex2(fmaf(s[e], p.scale_log2, -m[r]));
+        l[r] += pr;
+        s[e] = p.drop_thr > 0 && !drop_keep(p.drop_seed, drow[r], key0 + 8 * (e >> 2) + (e & 1), p.drop_thr) ? 0.f : pr;
+      }
+    };
+    auto rescale_pack = [&]() {
+#pragma unroll
+      for (int e = 0; e < 64; ++e) o[e] *= corr[(e >> 1) & 1];
+#pragma unroll
+      for (int e = 0; e < 16; ++e) ap[e] = tc::pack_bf16x2(s[2 * e], s[2 * e + 1]);
+    };
+    if (nblk > 0) {
+      if (!tc::mbar_wait_bounded(&kv_full[stage], phase)) { timed_out = true; break; }
+      issue_s(stage);
+      tc::wgmma_wait<0>();
+      tc::wgmma_fence_regs(s);
+      if (nblk == 1 && tid == 0) tc::mbar_arrive(q_empty);
+      softmax(0);
+      rescale_pack();
+      int cur = stage;                      // ring stage of the block whose PV is next
+      if (++stage == AF_STAGES) { stage = 0; phase ^= 1; }
+      for (int kb = 1; kb < nblk; ++kb) {
+        if (!timed_out && !tc::mbar_wait_bounded(&kv_full[stage], phase)) timed_out = true;
+        issue_s(stage);
+        issue_pv(cur);
+        tc::wgmma_wait<1>();
+        tc::wgmma_fence_regs(s);
+        if (kb == nblk - 1 && tid == 0) tc::mbar_arrive(q_empty);
+        softmax(kb);
+        tc::wgmma_wait<0>();
+        tc::wgmma_fence_regs(o);
+        if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
+        cur = stage;
+        if (++stage == AF_STAGES) { stage = 0; phase ^= 1; }
+        rescale_pack();
+      }
+      issue_pv(cur);
+      tc::wgmma_wait<0>();
+      tc::wgmma_fence_regs(o);
+      if (timed_out) break;
+      if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
+    } else if (tid == 0) {
+      tc::mbar_arrive(q_empty);
     }
-    if (valid) {
+
+    // epilogue: O / l -> bf16 into the staging tile (two 64-column boxes, 128-byte swizzle: 16-byte chunk c of row rr at
+    // c ^ (rr & 7)), then one thread stores it with the TMA; lse = ln(sum_j exp(s_ij)) from one lane per row
+    if (tid == 0) tc::bulk_wait_read<0>();                // the previous tile's store has read the staging tile
+    tc::named_bar_sync(1 + g, 128);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int i = i0 + 8 * r;
+      const float lr = quad_sum(l[r]);
       const float inv = dscale / lr;
-      __nv_bfloat16* orow = p.out + att_tok(i, b, p.T, p.B, p.batch_major) * p.ld_out + h * ATT_DH;
+      const int rr = 16 * wq + (lane >> 2) + 8 * r;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) att_st2(orow, j, lane, o[j][2 * r] * inv, o[j][2 * r + 1] * inv);
-      if ((lane & 3) == 0) p.lse[static_cast<size_t>(bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+      for (int j = 0; j < 16; ++j) {
+        const uint32_t off = (j >> 3) * 8192 + rr * 128 + (((j & 7) ^ (rr & 7)) << 4) + (lane & 3) * 4;
+        *reinterpret_cast<uint32_t*>(stg + off) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+      }
+      if (i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+    }
+    tc::fence_proxy_async_smem();
+    tc::named_bar_sync(1 + g, 128);
+    if (tid == 0 && t0 < p.T) {
+      tc::tma_store_3d(&tmO, stg, h * ATT_DH, b, t0);
+      tc::tma_store_3d(&tmO, stg + 8192, h * ATT_DH + 64, b, t0);
+      tc::bulk_commit();
     }
   }
+  if (tid == 0) tc::bulk_wait<0>();
+  if (timed_out) asm volatile("trap;");
 }
 
 }  // namespace pfn
@@ -191,18 +279,23 @@ extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
   p.T = d->T; p.B = d->B; p.H = d->H; p.sep = d->sep;
   p.scale_log2 = d->scale * 1.4426950408889634f;
   p.qkv = reinterpret_cast<const __nv_bfloat16*>(d->qkv); p.ld_qkv = d->ld_qkv;
-  p.out = reinterpret_cast<__nv_bfloat16*>(d->out); p.ld_out = d->ld_out;
   p.lse = d->lse;
-  p.n_qtiles = (d->T + ATT_BM - 1) / ATT_BM;
+  p.n_tiles = (d->T + 127) / 128;
   p.batch_major = d->batch_major;
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
-  const long long grid = static_cast<long long>(p.n_qtiles) * d->B * d->H;
-  PFN_CHECK_ARG(grid < (1LL << 31), "attention_fwd_tc: too many tiles");
+  const int E = d->H * ATT_DH;
+  CUtensorMap tmQ, tmKV, tmO;
+  if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
+  // out: rows past T are not written
+  if (int rc = att_tensor_map(&tmO, d->out, E, d->ld_out, d->T, d->B, d->T, d->batch_major)) return rc;
+  const long long units = static_cast<long long>(p.n_tiles) * d->B * d->H;
+  PFN_CHECK_ARG(units < (1LL << 31), "attention_fwd_tc: too many tiles");
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
-    PFN_CUDA_OK(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_FWD_SMEM));
+    PFN_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AF_SMEM));
   }
-  attn_fwd_tc_kernel<<<static_cast<unsigned>(grid), 128, ATT_FWD_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  const int grid = units < num_sms() ? static_cast<int>(units) : num_sms();
+  attn_fwd_kernel<<<static_cast<unsigned>(grid), AF_THREADS, AF_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(tmQ, tmKV, tmO, p);
   PFN_LAUNCH_OK();
   return 0;
 }
