@@ -8,16 +8,20 @@
 //          S_j  = Q K_j^T      dP_j = dO V_j^T                                 (wgmma m64n64k16, fp32)
 //          dS_j = exp2(S_j c - lse2) * (dP_j - delta) * scale  -> bf16 A fragments (registers)
 //          dQ  += dS_j K_j                                                      (wgmma m64n128k16, A from registers)
-//      For a query row (i >= sep) the diagonal key is attended by that row only, so dK_i = dS_ii q_i and dV_i = P_ii dO_i are
-//      complete: the four lanes that own the row compute and store them, and add dS_ii k_i to dQ.
+//      software-pipelined like the forward: S_j / dP_j and dQ += dS_{j-1} K_{j-1} are issued together and dS_j is computed
+//      while the dQ MMAs of block j-1 run.  For a query row (i >= sep) the diagonal key is attended by that row only, so
+//      dK_i = dS_ii q_i and dV_i = P_ii dO_i are complete: producer warps 9-11 compute them one tile ahead, together with
+//      every row's lse2 and delta, and hand lse2, delta and dS_ii to the consumers through a double-buffered array in
+//      shared memory; the consumers add dS_ii k_i to dQ.
 //
 //  (2) attn_bwd_dkv_kernel    one CTA per (batch, head, 128-key tile of the train keys), K and V resident, loop over 64-row
 //      Q/dO blocks:
 //          S^T = K Q_i^T       dP^T = V dO_i^T     (row = key, column = query row; m64n64k16)
 //          dV += (P^T . mask) dO_i ;   dK += dS^T Q_i                           (m64n128k16, A from registers)
 //
-// Both are warp-specialised: warpgroup 2 (producer, 40 registers) issues the TMA loads into a ring of stages, warpgroups 0
-// and 1 (consumers, 232 registers) each own 64 rows of the tile (query rows in (1), keys in (2)).  The fp32 S / dP
+// Both are warp-specialised: warpgroup 2 (producer; 64 registers in (1), 40 in (2)) issues the TMA loads into a ring of
+// stages, warpgroups 0 and 1 (consumers; 208 registers in (1), 232 in (2)) each own 64 rows of the tile (query rows in
+// (1), keys in (2)).  The fp32 S / dP
 // accumulators are packed to bf16 in place as the A operand of the second pair of MMAs, so P and dS never touch shared
 // memory.  Q/K/V/dO rows come straight out of the packed [T*B, 3E] qkv / [T*B, E] dO buffers through 3-D tensor maps
 // (columns, batch, time) whose two row strides encode the token order; the TMA zero-fills rows past T (Q, dO) and keys
@@ -32,10 +36,12 @@ constexpr int AB_TILE = ATT_TILE;                         // 16 KB: 64 rows x 12
 constexpr int AB_THREADS = 3 * 128;
 constexpr int AB_DQ_STAGES = 4;                           // K/V blocks in flight (dQ kernel)
 constexpr int AB_DKV_STAGES = 3;                          // Q/dO blocks in flight (dK/dV kernel)
-// dQ kernel: Q, dO of the tile (2 x 2 x 16 KB), ring of (K, V), barriers
+constexpr int AB_DQ_STAT_WARPS = 3;                       // producer warps 9-11: per-row statistics of the next tile
+// dQ kernel: Q, dO of the tile (2 x 2 x 16 KB), ring of (K, V), two buffers of per-row (lse2, delta, ds_ii), barriers
 constexpr int AB_DQ_OFF_RING = 4 * AB_TILE;
-constexpr int AB_DQ_OFF_BAR = AB_DQ_OFF_RING + AB_DQ_STAGES * 2 * AB_TILE;
-constexpr int AB_DQ_SMEM = AB_DQ_OFF_BAR + (2 * AB_DQ_STAGES + 2) * 8 + 1024;   // + 1 KB alignment slack
+constexpr int AB_DQ_OFF_STAT = AB_DQ_OFF_RING + AB_DQ_STAGES * 2 * AB_TILE;
+constexpr int AB_DQ_OFF_BAR = AB_DQ_OFF_STAT + 2 * 3 * 128 * 4;
+constexpr int AB_DQ_SMEM = AB_DQ_OFF_BAR + (2 * AB_DQ_STAGES + 2 + 4) * 8 + 1024;   // + 1 KB alignment slack
 // dK/dV kernel: K, V of the tile (2 x 2 x 16 KB), ring of (Q, dO), ring of (lse2, delta), barriers
 constexpr int AB_DKV_OFF_RING = 4 * AB_TILE;
 constexpr int AB_DKV_OFF_STAT = AB_DKV_OFF_RING + AB_DKV_STAGES * 2 * AB_TILE;
@@ -115,10 +121,15 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint64_t* kv_empty = kv_full + AB_DQ_STAGES;
   uint64_t* q_full = kv_empty + AB_DQ_STAGES;             // Q, dO of the CTA's current tile have landed
   uint64_t* q_empty = q_full + 1;                         // both warpgroups have finished their last S / dP MMAs of it
+  // tile it's statistics are in buffer it & 1: [0, 128) lse2, [128, 256) delta, [256, 384) ds_ii of the tile's rows
+  float* sStat = reinterpret_cast<float*>(smem + AB_DQ_OFF_STAT);
+  uint64_t* st_full = q_empty + 1;                        // [2] written by the statistics warps
+  uint64_t* st_empty = st_full + 2;                       // [2] read by every consumer thread
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int E = p.H * ATT_DH;
   const int nblk = (p.sep + AB_ROWS - 1) / AB_ROWS;
   const int n_units = p.n_tiles * p.B * p.H;
+  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
   if (threadIdx.x == 0) {
     for (int s = 0; s < AB_DQ_STAGES; ++s) {
       tc::mbar_init(&kv_full[s], 1);
@@ -126,14 +137,91 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
     tc::mbar_init(q_full, 1);
     tc::mbar_init(q_empty, 2);
+    for (int s = 0; s < 2; ++s) {
+      tc::mbar_init(&st_full[s], 32 * AB_DQ_STAT_WARPS);
+      tc::mbar_init(&st_empty[s], 256);
+    }
     tc::mbar_fence_init();
   }
   __syncthreads();
 
   if (warp >= 8) {
-    // ------------------------------------------------------------------ TMA producer
-    tc::setmaxnreg_dec<40>();
-    if (threadIdx.x == 256) {
+    // ------------------------------------------------------------------ producer: TMA (thread 256), statistics (warps 9-11)
+    // 64 registers: the statistics warps keep two rows in flight (with 40 or 48 they spill), so the consumers get 208:
+    // 2 x 128 x 208 + 128 x 64 <= 64 K
+    tc::setmaxnreg_dec<64>();
+    if (warp > 8) {
+      // Per tile: lse2 and delta of its 128 rows, and for each row i >= sep its diagonal key: s_ii = q_i.k_i,
+      // dp_ii = dO_i.v_i, ds_ii = P_ii (mask dp_ii - delta_i) scale, which completes dK_i = ds_ii q_i and dV_i = P_ii mask
+      // dO_i (stored here) and leaves ds_ii k_i for the consumers' dQ.  Warp pw owns the rows r = pw (mod 3).  A row is
+      // read by the whole warp with 16-byte loads: lanes 0-15 take q_i and k_i, lanes 16-31 dO_i and v_i, eight columns
+      // each; the two halves then store dK_i and dV_i.  Two rows are in flight at a time.
+      const int pw = warp - 9;
+      for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
+        const int qt = u % p.n_tiles, bh = u / p.n_tiles;
+        const int h = bh % p.H, b = bh / p.H;
+        const int sb = it & 1;
+        float* st = sStat + sb * 3 * 128;
+        tc::mbar_wait_suspend(&st_empty[sb], ((it >> 1) & 1) ^ 1);
+#pragma unroll 1
+        for (int r = pw + AB_DQ_STAT_WARPS * lane; r < 128; r += 32 * AB_DQ_STAT_WARPS) {
+          const int i = qt * 128 + r;
+          const bool valid = i < p.T;
+          st[r] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+          st[128 + r] = valid ? ab_delta(p, b, h, i) : 0.f;
+        }
+        __syncwarp();
+        // the lane's half and columns come from an opaque lane index in every row, so that the address arithmetic built on
+        // them is formed next to its loads instead of being hoisted out of the loops and held in registers throughout
+        auto tok_of = [&](int r) { return att_tok(qt * 128 + r, b, p.T, p.B, p.batch_major); };
+        auto load_row = [&](int r, uint4& xv, uint4& yv) {
+          const int l = static_cast<int>(att_opaque(lane)), half = l >> 4, c8 = (l & 15) * 8;
+          const size_t tok = tok_of(r);
+          const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + h * ATT_DH + c8;
+          xv = *reinterpret_cast<const uint4*>(half ? p.dout + tok * p.ld_dout + h * ATT_DH + c8 : qrow);   // q_i | dO_i
+          yv = *reinterpret_cast<const uint4*>(qrow + (1 + half) * E);                                      // k_i | v_i
+        };
+        auto finish_row = [&](int r, uint4 xv, uint4 yv) {
+          const int l = static_cast<int>(att_opaque(lane)), half = l >> 4, c8 = (l & 15) * 8;
+          const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&xv);
+          const __nv_bfloat162* y2 = reinterpret_cast<const __nv_bfloat162*>(&yv);
+          float dot = 0.f;
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const float2 a = __bfloat1622float2(x2[c]), bb = __bfloat1622float2(y2[c]);
+            dot = fmaf(a.x, bb.x, fmaf(a.y, bb.y, dot));
+          }
+#pragma unroll
+          for (int o = 8; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+          const float sd = __shfl_sync(0xffffffffu, dot, 0), dpd = __shfl_sync(0xffffffffu, dot, 16);
+          const int i = qt * 128 + r;
+          const float pr = fast_ex2(fmaf(sd, p.scale_log2, -st[r]));
+          const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, static_cast<uint32_t>(bh) * p.T + i, i, p.drop_thr) ? dscale : 0.f) : 1.f;
+          const float ds = pr * fmaf(mk, dpd, -st[128 + r]) * p.scale;
+          const float f = half ? pr * mk : ds;
+          uint4 o;
+          uint32_t* o32 = reinterpret_cast<uint32_t*>(&o);
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const float2 a = __bfloat1622float2(x2[c]);
+            o32[c] = tc::pack_bf16x2(f * a.x, f * a.y);
+          }
+          *reinterpret_cast<uint4*>(p.dqkv + tok_of(r) * p.ld_dqkv + h * ATT_DH + (1 + half) * E + c8) = o;   // dK_i | dV_i
+          if (lane == 0) st[256 + r] = ds;
+        };
+        const int r_lo = max(0, p.sep - qt * 128), r_hi = min(128, p.T - qt * 128);
+        for (int r = r_lo + (pw - r_lo % AB_DQ_STAT_WARPS + AB_DQ_STAT_WARPS) % AB_DQ_STAT_WARPS; r < r_hi;
+             r += 2 * AB_DQ_STAT_WARPS) {
+          const int r2 = r + AB_DQ_STAT_WARPS < r_hi ? r + AB_DQ_STAT_WARPS : r;
+          uint4 xa, ya, xb, yb;
+          load_row(r, xa, ya);
+          load_row(r2, xb, yb);
+          finish_row(r, xa, ya);
+          if (r2 != r) finish_row(r2, xb, yb);
+        }
+        tc::mbar_arrive(&st_full[sb]);
+      }
+    } else if (threadIdx.x == 256) {
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
       tc::tma_prefetch_desc(&tmDO);
@@ -169,11 +257,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
 
   // -------------------------------------------------------------------- consumer warpgroups
-  tc::setmaxnreg_inc<232>();
+  tc::setmaxnreg_inc<208>();
   const int g = warp >> 2, wq = warp & 3;
   const int tid = threadIdx.x & 127;
   const uint32_t q_tile = tc::smem_u32(sQ + g * AB_TILE), d_tile = tc::smem_u32(sD + g * AB_TILE);
-  const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
   int stage = 0;
   uint32_t phase = 0;
   bool timed_out = false;
@@ -182,113 +269,134 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const int h = bh % p.H, b = bh / p.H;
     const int i0 = qt * 128 + 64 * g + 16 * wq + (lane >> 2);    // this lane's rows: i0, i0 + 8
 
-    // per-row statistics of this lane's two rows
-    float lse2[2], dl[2];
+    // per-row statistics of this lane's two rows (and ds_ii of its diagonal keys), prepared by the statistics warps
+    const int sb = it & 1;
+    if (!tc::mbar_wait_bounded(&st_full[sb], (it >> 1) & 1)) { timed_out = true; break; }
+    float lse2[2], dl[2], dsd[2];
     uint32_t drow[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const int i = i0 + 8 * r;
-      const bool valid = i < p.T;
-      lse2[r] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
-      dl[r] = valid ? ab_delta(p, b, h, i) : 0.f;
-      drow[r] = static_cast<uint32_t>(bh) * p.T + i;
+      const int rr = i0 + 8 * r - qt * 128;
+      lse2[r] = sStat[sb * 3 * 128 + rr];
+      dl[r] = sStat[sb * 3 * 128 + 128 + rr];
+      dsd[r] = sStat[sb * 3 * 128 + 256 + rr];
+      drow[r] = static_cast<uint32_t>(bh) * p.T + i0 + 8 * r;
     }
+    tc::mbar_arrive(&st_empty[sb]);
     if (!tc::mbar_wait_bounded(q_full, it & 1)) { timed_out = true; break; }
 
-    // The first MMA of the tile writes dq (scale-d = 0), so nothing but wgmma defines it until the loop has drained.
-    float dq[64];
-    for (int kb = 0; kb < nblk; ++kb) {
-      if (!tc::mbar_wait_bounded(&kv_full[stage], phase)) { timed_out = true; break; }
-      const uint32_t k_s = tc::smem_u32(sRing + stage * 2 * AB_TILE);
+    // Key loop.  Block kb issues S_kb = Q K_kb^T and dP_kb = dO V_kb^T as one commit group and dQ += dS_{kb-1} K_{kb-1}
+    // as a second, waits for the first only and computes dS_kb while dQ_{kb-1} is on the tensor pipe, then waits for
+    // dQ_{kb-1}, releases its ring stage and packs dS_kb into the A fragments.  dq and the S / dP accumulators are written
+    // only when no MMA that owns them is in flight: otherwise ptxas serialises the whole wgmma pipeline.  For the same
+    // reason a timed-out wait inside the loop is recorded and the block runs on; the tile is abandoned once the pipeline
+    // has drained.  The first dQ MMA of the tile writes dq (scale-d = 0), so nothing but wgmma defines it until then.
+    float dq[64], s[32], dp[32];
+    uint32_t ads[16];
+    auto issue_sdp = [&](int st) {
+      const uint32_t k_s = tc::smem_u32(sRing + st * 2 * AB_TILE);
       const uint32_t v_s = k_s + AB_TILE;
       const uint32_t q_s = att_opaque(q_tile), d_s = att_opaque(d_tile);
-      float s[32], dp[32];
       tc::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) att_mma_n64(s, att_desc_k(q_s, kk), att_desc_k(k_s, kk), kk);
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) att_mma_n64(dp, att_desc_k(d_s, kk), att_desc_k(v_s, kk), kk);
       tc::wgmma_commit();
+    };
+    auto issue_dq = [&](int st, bool accumulate) {
+      const uint32_t k_s = tc::smem_u32(sRing + st * 2 * AB_TILE);
+      tc::wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(dq, ads + 4 * kk, att_desc_mn(k_s, kk), accumulate || kk > 0);
+      tc::wgmma_commit();
+    };
+    // dS = P (mask dP - delta) scale into s (keys >= sep of the last block get P = 0); element 4 j + e is row
+    // i0 + 8 (e >> 1), key kb * 64 + 8 j + 2 (lane & 3) + (e & 1)
+    auto compute_ds = [&](int kb) {
+      const int key0 = kb * AB_ROWS + 2 * (lane & 3);
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        const int r = (e >> 1) & 1;
+        const int key = key0 + 8 * (e >> 2) + (e & 1);
+        const float pr = key < p.sep ? fast_ex2(fmaf(s[e], p.scale_log2, -lse2[r])) : 0.f;
+        const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[r], key, p.drop_thr) ? dscale : 0.f) : 1.f;
+        s[e] = pr * fmaf(mk, dp[e], -dl[r]) * p.scale;
+      }
+    };
+    auto pack_ds = [&]() {
+#pragma unroll
+      for (int e = 0; e < 16; ++e) ads[e] = tc::pack_bf16x2(s[2 * e], s[2 * e + 1]);
+    };
+    // k_i of this lane's diagonal keys (rows i >= sep), loaded while the tile's last dQ MMAs run; dq[4 j + 2 r + c] is
+    // row i0 + 8 r, column 8 j + 2 (lane & 3) + c
+    uint32_t kd[2][16];
+    auto load_kd = [&]() {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int i = i0 + 8 * r;
+        const bool diag = i < p.T && i >= p.sep;
+        const __nv_bfloat16* krow = p.qkv + att_tok(diag ? i : 0, b, p.T, p.B, p.batch_major) * p.ld_qkv + E + h * ATT_DH;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+          kd[r][j] = diag ? *reinterpret_cast<const uint32_t*>(krow + 8 * j + 2 * (lane & 3)) : 0u;
+      }
+    };
+    if (nblk > 0) {
+      if (!tc::mbar_wait_bounded(&kv_full[stage], phase)) { timed_out = true; break; }
+      issue_sdp(stage);
       tc::wgmma_wait<0>();
       tc::wgmma_fence_regs(s);
       tc::wgmma_fence_regs(dp);
-      if (kb == nblk - 1 && tid == 0) tc::mbar_arrive(q_empty);
-
-      // dS = P (mask dP - delta) scale  (keys >= sep of the last block get P = 0); element 4 j + e is row i0 + 8 (e >> 1),
-      // key kb * 64 + 8 j + 2 (lane & 3) + (e & 1)
-      uint32_t ads[16];
-      const int key0 = kb * AB_ROWS + 2 * (lane & 3);
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; e += 2) {
-          float v[2];
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int key = key0 + 8 * j + c;
-            const float pr = key < p.sep ? fast_ex2(fmaf(s[4 * j + e + c], p.scale_log2, -lse2[e >> 1])) : 0.f;
-            const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[e >> 1], key, p.drop_thr) ? dscale : 0.f) : 1.f;
-            v[c] = pr * fmaf(mk, dp[4 * j + e + c], -dl[e >> 1]) * p.scale;
-          }
-          ads[2 * j + (e >> 1)] = tc::pack_bf16x2(v[0], v[1]);
-        }
-      tc::wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(dq, ads + 4 * kk, att_desc_mn(k_s, kk), kb > 0 || kk > 0);
-      tc::wgmma_commit();
-      tc::wgmma_wait<0>();
-      if (tid == 0) tc::mbar_arrive(&kv_empty[stage]);
+      if (nblk == 1 && tid == 0) tc::mbar_arrive(q_empty);
+      compute_ds(0);
+      pack_ds();
+      int cur = stage;                      // ring stage of the block whose dQ MMAs are next
       if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
+      for (int kb = 1; kb < nblk; ++kb) {
+        if (!timed_out && !tc::mbar_wait_bounded(&kv_full[stage], phase)) timed_out = true;
+        issue_sdp(stage);
+        issue_dq(cur, kb > 1);
+        tc::wgmma_wait<1>();
+        tc::wgmma_fence_regs(s);
+        tc::wgmma_fence_regs(dp);
+        if (kb == nblk - 1 && tid == 0) tc::mbar_arrive(q_empty);
+        compute_ds(kb);
+        tc::wgmma_wait<0>();
+        tc::wgmma_fence_regs(dq);
+        if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
+        cur = stage;
+        if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
+        pack_ds();
+      }
+      issue_dq(cur, nblk > 1);
+      load_kd();
+      tc::wgmma_wait<0>();
+      tc::wgmma_fence_regs(dq);
+      if (timed_out) break;
+      if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
+    } else {
+      if (tid == 0) tc::mbar_arrive(q_empty);
+      load_kd();
     }
-    tc::wgmma_fence_regs(dq);
-    if (nblk == 0 && tid == 0) tc::mbar_arrive(q_empty);
 
-    // diagonal keys of the query rows, dQ stores, column sums; dq[4 j + 2 r + c] is row i0 + 8 r, column 8 j + 2 (lane & 3) + c
+    // dQ = dq + ds_ii k_i, stores, column sums over the bf16-rounded values
     float cs[16][2];
 #pragma unroll
     for (int j = 0; j < 16; ++j) cs[j][0] = cs[j][1] = 0.f;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int i = i0 + 8 * r;
-      const bool valid = i < p.T;
-      const bool diag = valid && i >= p.sep;
-      const size_t tok = att_tok(valid ? i : 0, b, p.T, p.B, p.batch_major);
-      const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + h * ATT_DH;
-      const __nv_bfloat16* drw = p.dout + tok * p.ld_dout + h * ATT_DH;
-      __nv_bfloat16* grow = p.dqkv + tok * p.ld_dqkv + h * ATT_DH;
-      float sd = 0.f, dpd = 0.f;
-      if (diag) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float2 q = att_ld2(qrow, j, lane), k = att_ld2(qrow + E, j, lane);
-          const float2 gr = att_ld2(drw, j, lane), v = att_ld2(qrow + 2 * E, j, lane);
-          sd = fmaf(q.x, k.x, fmaf(q.y, k.y, sd));
-          dpd = fmaf(gr.x, v.x, fmaf(gr.y, v.y, dpd));
-        }
-      }
-      sd = quad_sum(sd);
-      dpd = quad_sum(dpd);
-      float ds = 0.f;
-      if (diag) {
-        const float pr = fast_ex2(fmaf(sd, p.scale_log2, -lse2[r]));
-        const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[r], i, p.drop_thr) ? dscale : 0.f) : 1.f;
-        ds = pr * fmaf(mk, dpd, -dl[r]) * p.scale;
-        const float pm = pr * mk;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float2 q = att_ld2(qrow, j, lane), gr = att_ld2(drw, j, lane);
-          att_st2(grow + E, j, lane, ds * q.x, ds * q.y);
-          att_st2(grow + 2 * E, j, lane, pm * gr.x, pm * gr.y);
-        }
-      }
-      if (valid) {
+      if (i < p.T) {
+        const bool diag = i >= p.sep;
+        __nv_bfloat16* grow = p.dqkv + att_tok(i, b, p.T, p.B, p.batch_major) * p.ld_dqkv + h * ATT_DH;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           float x = nblk > 0 ? dq[4 * j + 2 * r] : 0.f, y = nblk > 0 ? dq[4 * j + 2 * r + 1] : 0.f;
           if (diag) {
-            const float2 k = att_ld2(qrow + E, j, lane);
-            x = fmaf(ds, k.x, x);
-            y = fmaf(ds, k.y, y);
+            const float2 k = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&kd[r][j]));
+            x = fmaf(dsd[r], k.x, x);
+            y = fmaf(dsd[r], k.y, y);
           }
           att_st2(grow, j, lane, x, y);
           cs[j][0] += __bfloat162float(__float2bfloat16_rn(x));
