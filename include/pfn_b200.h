@@ -195,6 +195,41 @@ int pfn_bar_bucket_idx(const float* y, const float* borders, int n_bars, int64_t
 int pfn_gp_sample(const float* x, const float* z, const float* ls, const float* os, const float* noise, float jitter,
                   int kernel_type, float* y, float* work, int* info, int Bn, int T, int F, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Stroke prior (reference priors/stroke.py:9-116): per dataset, C classes of 1..3 random strokes; per image, the strokes of
+ * its class drawn with a random width, offset and end-point jitter like PIL's ImageDraw.line, ink filled with U{200..254},
+ * ImageFilter.GaussianBlur(0.2), ToTensor (k / 255) and optionally per-image standardisation.
+ * All ranges are inclusive integer ranges (random.randint), already scaled by the image side S (int(S * fraction)).
+ * pfn_stroke_geometry : the rejection loop of every (dataset, class, stroke), capped at max_iters iterations (a capped stroke
+ *   sets *cap_flag = 1 and keeps its last draw; the flag is never cleared here).  geom [B, C, strokes_max, 4] int32 receives
+ *   (start x, start y, length, active) and turns [B, C, strokes_max] fp64 the direction as a fraction of a full turn
+ *   (radians = 2 pi turns).
+ * pfn_stroke_render : x [T, B, S*S] fp32 (sequence-first) for the class table cls [T, B] int32 (values in [0, C)).
+ * Both draw their random numbers from counter-based hashes of `seed` (no device RNG state).
+ * pfn_stroke_raster : the oracle hook.  Rasterises N images of side S, image i being the union of segs[i, 0..nseg[i]-1]
+ *   (segs [N, K, 4] int32 end points x0, y0, x1, y1; x = column) at width widths[i]; mask [N, S*S] uint8 receives 1 on ink
+ *   pixels, blurred [N, S*S] uint8 the GaussianBlur(0.2) of the image whose ink pixels hold fill [N, S*S] (NULL: 128).
+ * S <= PFN_STROKE_MAX_SIDE, strokes per class and K <= PFN_STROKE_MAX_STROKES.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_STROKE_MAX_STROKES = 16, PFN_STROKE_MAX_SIDE = 112 };
+typedef struct pfn_stroke_desc {
+  int S;                           /* image side; an image has S*S pixels */
+  int C;                           /* classes per dataset */
+  int strokes_min, strokes_max;    /* strokes per class */
+  int len_min, len_max;            /* stroke length */
+  int start_min, start_max;        /* start point coordinate */
+  int width_min, width_max;        /* line width per image */
+  int offset_min, offset_max;      /* per-image offset of every start point */
+  int jitter_min, jitter_max;      /* per-image, per-stroke integer jitter of each velocity component */
+  int max_iters;                   /* rejection cap per stroke */
+} pfn_stroke_desc;
+int pfn_stroke_geometry(const pfn_stroke_desc* d, uint32_t seed, int B, int* geom, double* turns, int* cap_flag,
+                        void* stream);
+int pfn_stroke_render(const pfn_stroke_desc* d, uint32_t seed, const int* cls, const int* geom, const double* turns,
+                      float* x, int T, int B, int normalize, void* stream);
+int pfn_stroke_raster(const int* segs, const int* nseg, const int* widths, const uint8_t* fill, uint8_t* mask,
+                      uint8_t* blurred, int N, int K, int S, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -33,6 +33,15 @@ class GemmDesc(ctypes.Structure):
     ]
 
 
+class StrokeDesc(ctypes.Structure):
+    _fields_ = [(n, c_int) for n in ("S", "C", "strokes_min", "strokes_max", "len_min", "len_max", "start_min", "start_max",
+                                     "width_min", "width_max", "offset_min", "offset_max", "jitter_min", "jitter_max",
+                                     "max_iters")]
+
+
+STROKE_MAX_STROKES, STROKE_MAX_SIDE = 16, 112
+
+
 class AttnDesc(ctypes.Structure):
     _fields_ = [
         ("T", c_int), ("B", c_int), ("H", c_int), ("dh", c_int), ("sep", c_int),
@@ -58,6 +67,7 @@ EXPORTED_SYMBOLS = [
     "pfn_gp_sample",
     "pfn_dropout", "pfn_dropout_keep_mask",
     "pfn_adam_step", "pfn_adam_chunk_elems",
+    "pfn_stroke_geometry", "pfn_stroke_render", "pfn_stroke_raster",
 ]
 
 _lib = None
@@ -128,6 +138,11 @@ def load():
     lib.pfn_dropout.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_uint32, c_int,
                                 c_void_p]
     lib.pfn_dropout_keep_mask.argtypes = [c_void_p, c_int, c_int, ctypes.c_uint32, c_int, c_void_p]
+    lib.pfn_stroke_geometry.argtypes = [ctypes.POINTER(StrokeDesc), ctypes.c_uint32, c_int, c_void_p, c_void_p, c_void_p,
+                                        c_void_p]
+    lib.pfn_stroke_render.argtypes = [ctypes.POINTER(StrokeDesc), ctypes.c_uint32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_int, c_int, c_int, c_void_p]
+    lib.pfn_stroke_raster.argtypes = [c_void_p] * 6 + [c_int, c_int, c_int, c_void_p]
     _lib = lib
     return lib
 
@@ -448,3 +463,34 @@ def gp_sample(x, z, ls, os_, noise, jitter, kernel_type, y, work, info):
     Bn, T, F = x.shape
     check(load().pfn_gp_sample(ptr(x), ptr(z), ptr(ls), ptr(os_), ptr(noise), float(jitter), int(kernel_type), ptr(y),
                                ptr(work), ptr(info), Bn, T, F, stream_ptr()), "pfn_gp_sample")
+
+
+@_guarded
+def stroke_geometry(desc, seed, geom, turns, cap_flag):
+    """geom [B, C, strokes_max, 4] int32, turns [B, C, strokes_max] fp64 <- the class strokes of B datasets; cap_flag [1]
+    int32 is set to 1 (never cleared) when a stroke's rejection loop hits desc.max_iters."""
+    _count(1)
+    require_cuda(geom, turns, cap_flag)
+    check(load().pfn_stroke_geometry(ctypes.byref(desc), int(seed) & 0xFFFFFFFF, geom.shape[0], ptr(geom), ptr(turns),
+                                     ptr(cap_flag), stream_ptr()), "pfn_stroke_geometry")
+
+
+@_guarded
+def stroke_render(desc, seed, cls, geom, turns, x, normalize):
+    """x [T, B, S*S] fp32 <- the images of the class table cls [T, B] int32."""
+    _count(1)
+    require_cuda(cls, geom, turns, x)
+    T, B = cls.shape
+    check(load().pfn_stroke_render(ctypes.byref(desc), int(seed) & 0xFFFFFFFF, ptr(cls), ptr(geom), ptr(turns), ptr(x), T, B,
+                                   int(bool(normalize)), stream_ptr()), "pfn_stroke_render")
+
+
+@_guarded
+def stroke_raster(segs, nseg, widths, fill, mask, blurred, S):
+    """Oracle hook: mask / blurred [N, S*S] uint8 <- segment sets segs [N, K, 4] int32 (nseg [N], widths [N] int32), ink
+    filled with fill [N, S*S] uint8 (None: 128) before the blur."""
+    _count(1)
+    require_cuda(segs, nseg, widths, fill, mask, blurred)
+    N, K, _ = segs.shape
+    check(load().pfn_stroke_raster(ptr(segs), ptr(nseg), ptr(widths), ptr(fill), ptr(mask), ptr(blurred), N, K, S,
+                                   stream_ptr()), "pfn_stroke_raster")

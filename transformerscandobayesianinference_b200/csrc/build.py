@@ -28,6 +28,7 @@ SOURCES = [
     "attention_bwd_tc.cu",
     "gp_sampler.cu",
     "dropout.cu",
+    "stroke_prior.cu",
 ]
 
 NVCC_FLAGS = [
