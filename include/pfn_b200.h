@@ -196,6 +196,47 @@ int pfn_gp_sample(const float* x, const float* z, const float* ls, const float* 
                   int kernel_type, float* y, float* work, int* info, int Bn, int T, int F, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Fitted-hyperparameter GP baseline (reference priors/fast_gp_mix.py:24-55,156-169 with priors/fast_gp.py:88-120:
+ * botorch SingleTaskGP + fit_gpytorch_model per prefix).  Problem p = i * B + b conditions on rows < ts[i] of dataset b and
+ * minimises, by L-BFGS with a More-Thuente line search, the MAP objective in theta = (rho_1..F, rho_s, noise, mean):
+ *   f = -(1/t) [ log N(y | mean 1, K) + sum_d log Gamma(ls_d; ls_conc, ls_rate) + log Gamma(s; os_conc, os_rate)
+ *                + log Gamma(noise; noise_conc, noise_rate) ],   K = s k_nu(x, x; ls) + noise I,
+ *   ls_d = softplus(rho_d), s = softplus(rho_s), noise >= noise_lb (projected), Gamma in rate form.
+ * Then, where ts[i] < T, the latent predictive of row ts[i]: mean + k*^T K^-1 (y - mean) and s - k*^T K^-1 k*.
+ * One CTA per problem holds the t x t matrix in fp64 shared memory: t <= T <= PFN_GP_FIT_MAX_T, F <= PFN_GP_FIT_MAX_F.
+ * max_iter = 0 only evaluates f, its gradient and the predictive at the starting point.
+ * x [B, T, F], y [B, T] fp32 (DEVICE); ts (HOST) [n_ts], 1 <= ts[i] <= T; theta0 (DEVICE, optional) [n_ts * B, F + 3];
+ * outputs (DEVICE) indexed by problem p: theta [P, F + 3], f [P], grad [P, F + 3] (optional), mean / var [P] (optional; NaN where
+ * no predictive is formed), iters / nevals / status [P] int (status: PFN_GP_FIT_*).  Each problem depends on its own inputs only.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_GP_FIT_MAX_T = 128, PFN_GP_FIT_MAX_F = 32 };
+enum { PFN_GP_FIT_CONVERGED = 0, PFN_GP_FIT_MAX_ITER = 1, PFN_GP_FIT_LINE_SEARCH = 2, PFN_GP_FIT_NOT_PD = 3 };
+typedef struct pfn_gp_fit_desc {
+  int B, T, F;
+  const float* x;
+  const float* y;
+  int n_ts;
+  const int* ts;
+  int kernel_type;                       /* PFN_KERNEL_MATERN12 / 32 / 52 (nu = 0.5 / 1.5 / 2.5) */
+  double ls_conc, ls_rate, os_conc, os_rate, noise_conc, noise_rate;
+  double noise_lb;                       /* lower bound of the noise */
+  const double* theta0;                  /* NULL: rho = 0, noise = noise_init, mean = 0 */
+  double noise_init;
+  int max_iter, max_eval;                /* caps on accepted iterations and on objective evaluations */
+  double ftol;                           /* stop when (f_old - f) <= ftol * max(|f_old|, |f|, 1) */
+  double gtol;                           /* stop when the projected gradient's inf-norm <= gtol */
+  double* theta;
+  double* f;
+  double* grad;
+  double* mean;
+  double* var;
+  int* iters;
+  int* nevals;
+  int* status;
+} pfn_gp_fit_desc;
+int pfn_gp_fit(const pfn_gp_fit_desc* d, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Stroke prior (reference priors/stroke.py:9-116): per dataset, C classes of 1..3 random strokes; per image, the strokes of
  * its class drawn with a random width, offset and end-point jitter like PIL's ImageDraw.line, ink filled with U{200..254},
  * ImageFilter.GaussianBlur(0.2), ToTensor (k / 255) and optionally per-image standardisation.

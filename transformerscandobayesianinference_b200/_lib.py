@@ -42,6 +42,30 @@ class StrokeDesc(ctypes.Structure):
 STROKE_MAX_STROKES, STROKE_MAX_SIDE = 16, 112
 
 
+c_double = ctypes.c_double
+
+
+class GpFitDesc(ctypes.Structure):
+    _fields_ = [
+        ("B", c_int), ("T", c_int), ("F", c_int),
+        ("x", c_void_p), ("y", c_void_p),
+        ("n_ts", c_int), ("ts", ctypes.POINTER(c_int)),
+        ("kernel_type", c_int),
+        ("ls_conc", c_double), ("ls_rate", c_double), ("os_conc", c_double), ("os_rate", c_double),
+        ("noise_conc", c_double), ("noise_rate", c_double),
+        ("noise_lb", c_double),
+        ("theta0", c_void_p), ("noise_init", c_double),
+        ("max_iter", c_int), ("max_eval", c_int),
+        ("ftol", c_double), ("gtol", c_double),
+        ("theta", c_void_p), ("f", c_void_p), ("grad", c_void_p), ("mean", c_void_p), ("var", c_void_p),
+        ("iters", c_void_p), ("nevals", c_void_p), ("status", c_void_p),
+    ]
+
+
+GP_FIT_MAX_T, GP_FIT_MAX_F = 128, 32
+GP_FIT_CONVERGED, GP_FIT_MAX_ITER, GP_FIT_LINE_SEARCH, GP_FIT_NOT_PD = 0, 1, 2, 3
+
+
 class AttnDesc(ctypes.Structure):
     _fields_ = [
         ("T", c_int), ("B", c_int), ("H", c_int), ("dh", c_int), ("sep", c_int),
@@ -64,7 +88,7 @@ EXPORTED_SYMBOLS = [
     "pfn_embed_fwd", "pfn_embed_bwd",
     "pfn_layernorm_fwd", "pfn_layernorm_bwd", "pfn_colsum",
     "pfn_bar_nll_fwd", "pfn_bar_nll_bwd", "pfn_bar_bucket_idx",
-    "pfn_gp_sample",
+    "pfn_gp_sample", "pfn_gp_fit",
     "pfn_dropout", "pfn_dropout_keep_mask",
     "pfn_adam_step", "pfn_adam_chunk_elems",
     "pfn_stroke_geometry", "pfn_stroke_render", "pfn_stroke_raster",
@@ -135,6 +159,7 @@ def load():
     lib.pfn_bar_bucket_idx.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]
     lib.pfn_gp_sample.argtypes = [c_void_p] * 5 + [c_float, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                   c_void_p]
+    lib.pfn_gp_fit.argtypes = [ctypes.POINTER(GpFitDesc), c_void_p]
     lib.pfn_dropout.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_uint32, c_int,
                                 c_void_p]
     lib.pfn_dropout_keep_mask.argtypes = [c_void_p, c_int, c_int, ctypes.c_uint32, c_int, c_void_p]
@@ -463,6 +488,36 @@ def gp_sample(x, z, ls, os_, noise, jitter, kernel_type, y, work, info):
     Bn, T, F = x.shape
     check(load().pfn_gp_sample(ptr(x), ptr(z), ptr(ls), ptr(os_), ptr(noise), float(jitter), int(kernel_type), ptr(y),
                                ptr(work), ptr(info), Bn, T, F, stream_ptr()), "pfn_gp_sample")
+
+
+def gp_fit_desc(B, T, F, ts, kernel_type, hyper, noise_lb, noise_init, max_iter, max_eval, ftol, gtol):
+    """Descriptor of a pfn_gp_fit call without its device pointers.  hyper = (ls_conc, ls_rate, os_conc, os_rate,
+    noise_conc, noise_rate).  The prefix list is kept alive on the descriptor (it is read on the host)."""
+    d = GpFitDesc()
+    d.B, d.T, d.F = int(B), int(T), int(F)
+    d._ts = (c_int * max(len(ts), 1))(*[int(t) for t in ts])
+    d.n_ts, d.ts = len(ts), d._ts
+    d.kernel_type = int(kernel_type)
+    d.ls_conc, d.ls_rate, d.os_conc, d.os_rate, d.noise_conc, d.noise_rate = (float(v) for v in hyper)
+    d.noise_lb, d.noise_init = float(noise_lb), float(noise_init)
+    d.max_iter, d.max_eval, d.ftol, d.gtol = int(max_iter), int(max_eval), float(ftol), float(gtol)
+    return d
+
+
+@_guarded
+def gp_fit(x, y, desc, theta, f, iters, nevals, status, theta0=None, grad=None, mean=None, var=None):
+    """One launch fits every (prefix in desc.ts, dataset) problem.  x [B,T,F], y [B,T] fp32; outputs indexed by problem
+    p = i * B + b: theta / grad [P, F+3], f / mean / var [P] fp64, iters / nevals / status [P] int32."""
+    _count(1)
+    require_cuda(x, y, theta, f, iters, nevals, status, theta0, grad, mean, var)
+    desc.x, desc.y = x.data_ptr(), y.data_ptr()
+    desc.theta0 = None if theta0 is None else theta0.data_ptr()
+    desc.theta, desc.f = theta.data_ptr(), f.data_ptr()
+    desc.grad = None if grad is None else grad.data_ptr()
+    desc.mean = None if mean is None else mean.data_ptr()
+    desc.var = None if var is None else var.data_ptr()
+    desc.iters, desc.nevals, desc.status = iters.data_ptr(), nevals.data_ptr(), status.data_ptr()
+    check(load().pfn_gp_fit(ctypes.byref(desc), stream_ptr()), "pfn_gp_fit")
 
 
 @_guarded

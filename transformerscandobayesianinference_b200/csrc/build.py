@@ -27,6 +27,7 @@ SOURCES = [
     "attention_tc.cu",
     "attention_bwd_tc.cu",
     "gp_sampler.cu",
+    "gp_fit.cu",
     "dropout.cu",
     "stroke_prior.cu",
 ]

@@ -144,16 +144,20 @@ class _Predictive:
 
 
 class GaussianLikelihood:
-    """likelihood(f): adds the observation noise to the latent predictive (gpytorch GaussianLikelihood.__call__)."""
+    """likelihood(f): adds the observation noise to the latent predictive (gpytorch GaussianLikelihood.__call__).
+    `noise` is one float for every dataset or a tensor [B] with one noise per dataset (fitted models)."""
 
     def __init__(self, noise):
-        self.noise = float(noise)
+        self.noise = noise if torch.is_tensor(noise) else float(noise)
 
     def eval(self):
         return self
 
     def __call__(self, f):
-        return _Predictive(f.mean, f.variance + self.noise)
+        noise = self.noise
+        if torch.is_tensor(noise):
+            noise = noise.to(f.variance.device, f.variance.dtype).reshape(-1, *([1] * (f.variance.dim() - 1)))
+        return _Predictive(f.mean, f.variance + noise)
 
 
 class ExactGPModel:

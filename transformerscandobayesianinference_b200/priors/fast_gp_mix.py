@@ -6,8 +6,14 @@ and is then sampled from a Matern-nu ARD GP (nu default 2.5) by the same fused C
 The botorch/pyro model objects the reference builds per group only serve to draw those hyperparameters; here they
 are drawn directly with torch.distributions.Gamma on the device (botorch 0.6.0 / pyro 1.7.0 are not installed:
 the hyper-prior restatement is validated distributionally — parity unpinned, see oracle/pfn_oracle.py).
+
+The fitted-hyperparameter baseline (`get_model`, `get_fitted_model`, `evaluate`; reference :24-55, :156-169) restates
+botorch's MAP fit (SingleTaskGP + Gamma priors + fit_gpytorch_model) as csrc/gp_fit.cu: one CTA per (dataset, prefix)
+problem runs the whole L-BFGS fit in fp64 and forms the predictive, all problems of a call in one launch (t <= 128).
 """
+import math
 import random
+import time
 
 import torch
 from torch import nn
@@ -15,6 +21,7 @@ from torch import nn
 from .. import _lib as L
 from ..bar_distribution import BarDistribution
 from ..utils import default_device
+from . import fast_gp
 from .fast_gp import _compute_device, sample_gp
 from .utils import get_batch_to_dataloader, _Deferred
 
@@ -134,3 +141,195 @@ class DataLoader(get_batch_to_dataloader(get_batch)):
             model.train()
             return torch.stack(losses)
         return 123.
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# fitted-hyperparameter GP baseline (reference :24-55 get_model(sample=False), :156-169 get_fitted_model / evaluate)
+# ----------------------------------------------------------------------------------------------------------------------
+MAX_FIT_T = L.GP_FIT_MAX_T
+FIT_FTOL, FIT_GTOL, FIT_MAX_ITER = 2.220446049250313e-09, 1e-5, 15000     # scipy L-BFGS-B defaults (fit_gpytorch_model)
+_STATUS_NAMES = {L.GP_FIT_CONVERGED: "converged", L.GP_FIT_MAX_ITER: "iteration cap",
+                 L.GP_FIT_LINE_SEARCH: "line-search failure", L.GP_FIT_NOT_PD: "not positive definite"}
+
+
+def _fit_settings(hyperparameters):
+    """(kernel type, Gamma prior parameters, initial noise) from the same keys and defaults as sample_hyperparameters.
+    The initial noise is the noise prior's mode (reference :27-35); below the bound it is clamped to the bound."""
+    hp = hyperparameters or {}
+    prior = tuple(float(hp.get(k, v)) for k, v in (
+        ('lengthscale_concentration', 3.0), ('lengthscale_rate', 6.0), ('outputscale_concentration', .5),
+        ('outputscale_rate', 0.15), ('noise_concentration', 1.1), ('noise_rate', 0.05)))
+    noise_init = max((prior[4] - 1.0) / prior[5], MIN_INFERRED_NOISE_LEVEL)
+    return _NU_TO_KERNEL[float(hp.get('nu', 2.5))], prior, noise_init
+
+
+def _check_fit_args(hyperparameters):
+    hp = hyperparameters or {}
+    assert not (hp.get('sigmoid', False)) and not (hp.get('y_minmax_norm', False)), \
+        "Sigmoid and y_minmax_norm can only be used to sample models..."
+
+
+def _fit_device(device):
+    dev = torch.device(device)
+    if dev.type != 'cuda':
+        raise RuntimeError(f"priors.fast_gp_mix fits with the sm_90a GP-fit kernel; device {dev} is not a CUDA device "
+                           "(there is no CPU fallback)")
+    return dev
+
+
+def default_theta(n, num_features, hyperparameters, device):
+    """The fit's starting point per problem: rho = 0 (lengthscales and outputscale softplus(0) = ln 2), noise at the
+    noise prior's mode, constant mean 0.  Layout of theta: (rho_1..F, rho_outputscale, noise, mean)."""
+    theta = torch.zeros(n, num_features + 3, dtype=torch.float64, device=device)
+    theta[:, num_features + 1] = _fit_settings(hyperparameters)[2]
+    return theta
+
+
+@torch.no_grad()
+def fit_map(x, y, ts, hyperparameters=None, theta0=None, max_iter=FIT_MAX_ITER, grad=False):
+    """One pfn_gp_fit launch over every (prefix t in ts, dataset b): x [B,T,F], y [B,T] on a CUDA device.
+    Returns a dict of tensors with leading dims [len(ts), B]: theta [.., F+3], f, mean / var (latent predictive of row t,
+    NaN where t == T), iters, nevals, status (L.GP_FIT_*), and grad [.., F+3] when asked.  theta0 [len(ts), B, F+3]
+    replaces the default start; max_iter = 0 only evaluates f, its gradient and the predictive at the start."""
+    Bn, T, F = x.shape
+    if T > MAX_FIT_T:
+        raise ValueError(f"the GP fit keeps the t x t matrix in shared memory: T={T} exceeds the limit of {MAX_FIT_T}")
+    kt, prior, noise_init = _fit_settings(hyperparameters)
+    dev = x.device
+    P = len(ts) * Bn
+    f64 = dict(dtype=torch.float64, device=dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    out = {"theta": torch.empty(P, F + 3, **f64), "f": torch.empty(P, **f64), "mean": torch.empty(P, **f64),
+           "var": torch.empty(P, **f64), "iters": torch.empty(P, **i32), "nevals": torch.empty(P, **i32),
+           "status": torch.empty(P, **i32)}
+    if grad:
+        out["grad"] = torch.empty(P, F + 3, **f64)
+    desc = L.gp_fit_desc(Bn, T, F, ts, kt, prior, MIN_INFERRED_NOISE_LEVEL, noise_init, max_iter, FIT_MAX_ITER,
+                         FIT_FTOL, FIT_GTOL)
+    th0 = None if theta0 is None else theta0.to(dev, torch.float64).reshape(P, F + 3).contiguous()
+    L.gp_fit(x.to(torch.float32).contiguous(), y.to(torch.float32).contiguous(), desc, out["theta"], out["f"],
+             out["iters"], out["nevals"], out["status"], theta0=th0, grad=out.get("grad"), mean=out["mean"],
+             var=out["var"])
+    return {k: v.view(len(ts), Bn, *v.shape[1:]) for k, v in out.items()}
+
+
+class FittedGP:
+    """Gpytorch-free stand-in for the reference's SingleTaskGP (constant mean, outputscale * Matern-nu ARD kernel, Gamma
+    priors) on train_x [B,t,F], train_y [B,t], at the parameters `theta` [B, F+3] (raw: rho_1..F, rho_s, noise, mean).
+    Calling it on test inputs [B,m,F] returns the latent predictive of each test point, formed by the same kernel that
+    fits (one max_iter = 0 launch per test point), so it agrees bitwise with the predictive `evaluate` forms."""
+
+    def __init__(self, train_x, train_y, theta, hyperparameters, likelihood, fit=None):
+        self.train_x, self.train_y, self.theta = train_x, train_y, theta
+        self.hyperparameters, self.likelihood = hyperparameters, likelihood
+        F = train_x.shape[-1]
+        self.lengthscale = torch.nn.functional.softplus(theta[:, :F])
+        self.outputscale = torch.nn.functional.softplus(theta[:, F])
+        self.noise = theta[:, F + 1]
+        self.mean_constant = theta[:, F + 2]
+        fit = fit or {}
+        self.f, self.status = fit.get("f"), fit.get("status")
+        self.iters, self.nevals = fit.get("iters"), fit.get("nevals")
+
+    def eval(self):
+        return self
+
+    def train(self, mode=True):
+        return self
+
+    def to(self, device):
+        self.train_x, self.train_y, self.theta = self.train_x.to(device), self.train_y.to(device), self.theta.to(device)
+        return self
+
+    @torch.no_grad()
+    def __call__(self, x):
+        dev = self.train_x.device
+        if dev.type != 'cuda':
+            raise RuntimeError("FittedGP predicts with the sm_90a GP-fit kernel; move the model to a CUDA device "
+                               "(there is no CPU fallback)")
+        Bn, t, F = self.train_x.shape
+        xs = x.to(dev, torch.float32)
+        ycat = torch.cat([self.train_y.to(torch.float32), torch.zeros(Bn, 1, device=dev)], 1).contiguous()
+        means, variances = [], []
+        for j in range(xs.shape[1]):
+            xcat = torch.cat([self.train_x.to(torch.float32), xs[:, j:j + 1]], 1).contiguous()
+            r = fit_map(xcat, ycat, [t], self.hyperparameters, theta0=self.theta.unsqueeze(0), max_iter=0)
+            means.append(r["mean"][0])
+            variances.append(r["var"][0])
+        return fast_gp._Predictive(torch.stack(means, 1), torch.stack(variances, 1))
+
+
+def get_model(x, y, hyperparameters, sample=False):
+    """(model, likelihood) at the fit's starting point (reference :24-55 with sample=False).  x [B,t,F], y [B,t]."""
+    if sample:
+        raise NotImplementedError("priors.fast_gp_mix.get_model(sample=True): models drawn from the hyper-priors are "
+                                  "sampled inside get_batch (sample_hyperparameters); use get_batch")
+    _check_fit_args(hyperparameters)
+    theta = default_theta(x.shape[0], x.shape[-1], hyperparameters, x.device)
+    F = x.shape[-1]
+    likelihood = fast_gp.GaussianLikelihood(theta[:, F + 1])
+    return FittedGP(x, y, theta, hyperparameters, likelihood), likelihood
+
+
+@torch.no_grad()
+def get_fitted_model(x, y, hyperparameters, device):
+    """MAP-fitted (model, likelihood) on x [B,t,F], y [B,t] (reference :156-166): one pfn_gp_fit launch for all B.
+    The model exposes the fitted lengthscale / outputscale / noise / mean_constant and f / status / iters per dataset."""
+    _check_fit_args(hyperparameters)
+    dev = _fit_device(device)
+    xb, yb = x.to(dev, torch.float32).contiguous(), y.to(dev, torch.float32).contiguous()
+    r = fit_map(xb, yb, [xb.shape[1]], hyperparameters)
+    r = {k: v[0] for k, v in r.items()}
+    F = xb.shape[-1]
+    likelihood = fast_gp.GaussianLikelihood(r["theta"][:, F + 1])
+    return FittedGP(xb, yb, r["theta"], hyperparameters, likelihood, fit=r), likelihood
+
+
+def _report_unconverged(status):
+    bad = status != L.GP_FIT_CONVERGED
+    n_bad = int(bad.sum())
+    if n_bad:
+        parts = ", ".join(f"{name}: {int((status == code).sum())}" for code, name in _STATUS_NAMES.items()
+                          if code != L.GP_FIT_CONVERGED and int((status == code).sum()))
+        print(f"fast_gp_mix.evaluate: {n_bad} of {status.numel()} GP fits did not converge ({parts})")
+
+
+@torch.no_grad()
+def evaluate(x, y, y_non_noisy, use_mse=False, hyperparameters={}, get_model_on_device=None, device=default_device,
+             step_size=1, start_pos=0):
+    """Fitted-GP baseline (reference :169 = fast_gp.evaluate with get_fitted_model): for each t, fit on rows < t and score
+    row t with the Gaussian predictive NLL (or the squared error of the predictive mean).  Returns
+    (all_losses [n_t, B], mean losses with a leading 0 when start_pos == 0, seconds), like fast_gp.evaluate.
+
+    Every (prefix, dataset) fit runs in ONE launch.  The losses are formed from the kernel's predictive by the same
+    expressions as fast_gp's per-t loop, so `fast_gp.evaluate(..., get_model_on_device=get_fitted_model)` returns the
+    same losses bit for bit.  A caller-supplied `get_model_on_device` is handed to fast_gp.evaluate."""
+    if get_model_on_device is not None:
+        return fast_gp.evaluate(x, y, y_non_noisy, use_mse=use_mse, hyperparameters=hyperparameters,
+                                get_model_on_device=get_model_on_device, device=device, step_size=step_size,
+                                start_pos=start_pos)
+    start = time.time()
+    _check_fit_args(hyperparameters)
+    T = len(x)
+    if T > MAX_FIT_T:
+        raise ValueError(f"fast_gp_mix.evaluate keeps the t x t matrix of every fit in shared memory: T={T} exceeds "
+                         f"the limit of {MAX_FIT_T}")
+    dev = _fit_device(device)
+    ts = list(range(max(start_pos, 1), T, step_size))
+    means_list = [.0] if start_pos == 0 else []
+    if not ts:
+        return torch.zeros(0, x.shape[1]), torch.tensor(means_list), time.time() - start
+    xb = x.to(dev, torch.float32).transpose(0, 1).contiguous()
+    yb = y.to(dev, torch.float32).transpose(0, 1).contiguous()
+    r = fit_map(xb, yb, ts, hyperparameters)
+    _report_unconverged(r["status"])
+    F = xb.shape[-1]
+    noise = r["theta"][..., F + 1]
+    pred = fast_gp._Predictive(r["mean"].unsqueeze(-1), (r["var"] + noise).unsqueeze(-1))
+    y_t = y[ts].to(dev)
+    if use_mse:
+        losses = (pred.mean.squeeze(-1) - y_t) ** 2
+    else:
+        losses = -pred.log_prob(y_t.unsqueeze(-1))
+    means_list += losses.mean(1).tolist()
+    return losses.float().to('cpu'), torch.tensor(means_list).to('cpu'), time.time() - start
