@@ -113,17 +113,13 @@ __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                    const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = att_smem_base(smem_raw);
   uint8_t* sQ = smem;                                     // warpgroup g's 64 rows at + g * 16 KB
   uint8_t* sD = smem + 2 * AB_TILE;
-  uint8_t* sRing = smem + AB_DQ_OFF_RING;                 // stage s: K at + 2 s * 16 KB, V at + (2 s + 1) * 16 KB
-  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + AB_DQ_OFF_BAR);
-  uint64_t* kv_empty = kv_full + AB_DQ_STAGES;
-  uint64_t* q_full = kv_empty + AB_DQ_STAGES;             // Q, dO of the CTA's current tile have landed
-  uint64_t* q_empty = q_full + 1;                         // both warpgroups have finished their last S / dP MMAs of it
+  const AttPipe<AB_DQ_STAGES> pp(smem + AB_DQ_OFF_RING, reinterpret_cast<uint64_t*>(smem + AB_DQ_OFF_BAR));
   // tile it's statistics are in buffer it & 1: [0, 128) lse2, [128, 256) delta, [256, 384) ds_ii of the tile's rows
   float* sStat = reinterpret_cast<float*>(smem + AB_DQ_OFF_STAT);
-  uint64_t* st_full = q_empty + 1;                        // [2] written by the statistics warps
+  uint64_t* st_full = pp.q_empty + 1;                     // [2] written by the statistics warps
   uint64_t* st_empty = st_full + 2;                       // [2] read by every consumer thread
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int E = p.H * ATT_DH;
@@ -131,12 +127,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int n_units = p.n_tiles * p.B * p.H;
   const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < AB_DQ_STAGES; ++s) {
-      tc::mbar_init(&kv_full[s], 1);
-      tc::mbar_init(&kv_empty[s], 2);
-    }
-    tc::mbar_init(q_full, 1);
-    tc::mbar_init(q_empty, 2);
+    pp.init();
     for (int s = 0; s < 2; ++s) {
       tc::mbar_init(&st_full[s], 32 * AB_DQ_STAT_WARPS);
       tc::mbar_init(&st_empty[s], 256);
@@ -158,27 +149,26 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       // each; the two halves then store dK_i and dV_i.  Two rows are in flight at a time.
       const int pw = warp - 9;
       for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
-        const int qt = u % p.n_tiles, bh = u / p.n_tiles;
-        const int h = bh % p.H, b = bh / p.H;
+        const AttUnit unit = att_unit(u, p.n_tiles, p.H);
         const int sb = it & 1;
         float* st = sStat + sb * 3 * 128;
         tc::mbar_wait_suspend(&st_empty[sb], ((it >> 1) & 1) ^ 1);
 #pragma unroll 1
         for (int r = pw + AB_DQ_STAT_WARPS * lane; r < 128; r += 32 * AB_DQ_STAT_WARPS) {
-          const int i = qt * 128 + r;
+          const int i = unit.tile * 128 + r;
           const bool valid = i < p.T;
-          st[r] = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
-          st[128 + r] = valid ? ab_delta(p, b, h, i) : 0.f;
+          st[r] = valid ? p.lse[static_cast<size_t>(unit.bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+          st[128 + r] = valid ? ab_delta(p, unit.b, unit.h, i) : 0.f;
         }
         __syncwarp();
         // the lane's half and columns come from an opaque lane index in every row, so that the address arithmetic built on
         // them is formed next to its loads instead of being hoisted out of the loops and held in registers throughout
-        auto tok_of = [&](int r) { return att_tok(qt * 128 + r, b, p.T, p.B, p.batch_major); };
+        auto tok_of = [&](int r) { return att_tok(unit.tile * 128 + r, unit.b, p.T, p.B, p.batch_major); };
         auto load_row = [&](int r, uint4& xv, uint4& yv) {
           const int l = static_cast<int>(att_opaque(lane)), half = l >> 4, c8 = (l & 15) * 8;
           const size_t tok = tok_of(r);
-          const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + h * ATT_DH + c8;
-          xv = *reinterpret_cast<const uint4*>(half ? p.dout + tok * p.ld_dout + h * ATT_DH + c8 : qrow);   // q_i | dO_i
+          const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + unit.h * ATT_DH + c8;
+          xv = *reinterpret_cast<const uint4*>(half ? p.dout + tok * p.ld_dout + unit.h * ATT_DH + c8 : qrow);   // q_i | dO_i
           yv = *reinterpret_cast<const uint4*>(qrow + (1 + half) * E);                                      // k_i | v_i
         };
         auto finish_row = [&](int r, uint4 xv, uint4 yv) {
@@ -194,9 +184,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
           for (int o = 8; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
           const float sd = __shfl_sync(0xffffffffu, dot, 0), dpd = __shfl_sync(0xffffffffu, dot, 16);
-          const int i = qt * 128 + r;
+          const int i = unit.tile * 128 + r;
           const float pr = fast_ex2(fmaf(sd, p.scale_log2, -st[r]));
-          const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, static_cast<uint32_t>(bh) * p.T + i, i, p.drop_thr) ? dscale : 0.f) : 1.f;
+          const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, static_cast<uint32_t>(unit.bh) * p.T + i, i, p.drop_thr) ? dscale : 0.f) : 1.f;
           const float ds = pr * fmaf(mk, dpd, -st[128 + r]) * p.scale;
           const float f = half ? pr * mk : ds;
           uint4 o;
@@ -206,10 +196,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             const float2 a = __bfloat1622float2(x2[c]);
             o32[c] = tc::pack_bf16x2(f * a.x, f * a.y);
           }
-          *reinterpret_cast<uint4*>(p.dqkv + tok_of(r) * p.ld_dqkv + h * ATT_DH + (1 + half) * E + c8) = o;   // dK_i | dV_i
+          *reinterpret_cast<uint4*>(p.dqkv + tok_of(r) * p.ld_dqkv + unit.h * ATT_DH + (1 + half) * E + c8) = o;   // dK_i | dV_i
           if (lane == 0) st[256 + r] = ds;
         };
-        const int r_lo = max(0, p.sep - qt * 128), r_hi = min(128, p.T - qt * 128);
+        const int r_lo = max(0, p.sep - unit.tile * 128), r_hi = min(128, p.T - unit.tile * 128);
         for (int r = r_lo + (pw - r_lo % AB_DQ_STAT_WARPS + AB_DQ_STAT_WARPS) % AB_DQ_STAT_WARPS; r < r_hi;
              r += 2 * AB_DQ_STAT_WARPS) {
           const int r2 = r + AB_DQ_STAT_WARPS < r_hi ? r + AB_DQ_STAT_WARPS : r;
@@ -225,33 +215,13 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
       tc::tma_prefetch_desc(&tmDO);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
-        const int qt = u % p.n_tiles, bh = u / p.n_tiles;
-        const int h = bh % p.H, b = bh / p.H;
-        // The next tile's Q / dO go in once the consumers are done with the current one, which is before its last key
-        // block is (so the first key blocks of the next tile are already in flight by then).
-        auto load_q = [&]() {
-          if (it > 0) tc::mbar_wait_suspend(q_empty, (it - 1) & 1);
-          tc::mbar_expect_tx(q_full, 4 * AB_TILE);
-          for (int g = 0; g < 2; ++g) {
-            att_load_tile(sQ + g * AB_TILE, &tmQ, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
-            att_load_tile(sD + g * AB_TILE, &tmDO, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
-          }
-        };
-        const int claim_at = min(AB_DQ_STAGES - 1, nblk - 1);
-        if (nblk == 0) load_q();
-        for (int kb = 0; kb < nblk; ++kb) {
-          if (kb == claim_at) load_q();
-          tc::mbar_wait_suspend(&kv_empty[stage], phase ^ 1);
-          uint8_t* dst = sRing + stage * 2 * AB_TILE;
-          tc::mbar_expect_tx(&kv_full[stage], 2 * AB_TILE);
-          att_load_tile(dst, &tmKV, &kv_full[stage], E + h * ATT_DH, b, kb * AB_ROWS);
-          att_load_tile(dst + AB_TILE, &tmKV, &kv_full[stage], 2 * E + h * ATT_DH, b, kb * AB_ROWS);
-          if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
+      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk, 4 * AB_TILE, [&](const AttUnit& unit) {
+        for (int g = 0; g < 2; ++g) {
+          const int t0 = unit.tile * 128 + 64 * g;
+          att_load_tile(sQ + g * AB_TILE, &tmQ, pp.q_full, unit.h * ATT_DH, unit.b, t0);
+          att_load_tile(sD + g * AB_TILE, &tmDO, pp.q_full, unit.h * ATT_DH, unit.b, t0);
         }
-      }
+      });
     }
     return;
   }
@@ -259,15 +229,12 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   // -------------------------------------------------------------------- consumer warpgroups
   tc::setmaxnreg_inc<208>();
   const int g = warp >> 2, wq = warp & 3;
-  const int tid = threadIdx.x & 127;
   const uint32_t q_tile = tc::smem_u32(sQ + g * AB_TILE), d_tile = tc::smem_u32(sD + g * AB_TILE);
-  int stage = 0;
-  uint32_t phase = 0;
+  AttRing<AB_DQ_STAGES> ring;
   bool timed_out = false;
   for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
-    const int qt = u % p.n_tiles, bh = u / p.n_tiles;
-    const int h = bh % p.H, b = bh / p.H;
-    const int i0 = qt * 128 + 64 * g + 16 * wq + (lane >> 2);    // this lane's rows: i0, i0 + 8
+    const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+    const int i0 = unit.tile * 128 + 64 * g + 16 * wq + (lane >> 2);    // this lane's rows: i0, i0 + 8
 
     // per-row statistics of this lane's two rows (and ds_ii of its diagonal keys), prepared by the statistics warps
     const int sb = it & 1;
@@ -276,25 +243,21 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     uint32_t drow[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const int rr = i0 + 8 * r - qt * 128;
+      const int rr = i0 + 8 * r - unit.tile * 128;
       lse2[r] = sStat[sb * 3 * 128 + rr];
       dl[r] = sStat[sb * 3 * 128 + 128 + rr];
       dsd[r] = sStat[sb * 3 * 128 + 256 + rr];
-      drow[r] = static_cast<uint32_t>(bh) * p.T + i0 + 8 * r;
+      drow[r] = static_cast<uint32_t>(unit.bh) * p.T + i0 + 8 * r;
     }
     tc::mbar_arrive(&st_empty[sb]);
-    if (!tc::mbar_wait_bounded(q_full, it & 1)) { timed_out = true; break; }
 
-    // Key loop.  Block kb issues S_kb = Q K_kb^T and dP_kb = dO V_kb^T as one commit group and dQ += dS_{kb-1} K_{kb-1}
-    // as a second, waits for the first only and computes dS_kb while dQ_{kb-1} is on the tensor pipe, then waits for
-    // dQ_{kb-1}, releases its ring stage and packs dS_kb into the A fragments.  dq and the S / dP accumulators are written
-    // only when no MMA that owns them is in flight: otherwise ptxas serialises the whole wgmma pipeline.  For the same
-    // reason a timed-out wait inside the loop is recorded and the block runs on; the tile is abandoned once the pipeline
-    // has drained.  The first dQ MMA of the tile writes dq (scale-d = 0), so nothing but wgmma defines it until then.
+    // Key loop (att_key_loop): S_kb = Q K_kb^T and dP_kb = dO V_kb^T as the first MMA group, dS_kb computed while
+    // dQ += dS_{kb-1} K_{kb-1} runs, then packed into the A fragments.  The first dQ MMA of the tile writes dq
+    // (scale-d = 0), so nothing but wgmma defines it until then.
     float dq[64], s[32], dp[32];
     uint32_t ads[16];
     auto issue_sdp = [&](int st) {
-      const uint32_t k_s = tc::smem_u32(sRing + st * 2 * AB_TILE);
+      const uint32_t k_s = tc::smem_u32(pp.ring + st * 2 * AB_TILE);
       const uint32_t v_s = k_s + AB_TILE;
       const uint32_t q_s = att_opaque(q_tile), d_s = att_opaque(d_tile);
       tc::wgmma_fence();
@@ -305,7 +268,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       tc::wgmma_commit();
     };
     auto issue_dq = [&](int st, bool accumulate) {
-      const uint32_t k_s = tc::smem_u32(sRing + st * 2 * AB_TILE);
+      const uint32_t k_s = tc::smem_u32(pp.ring + st * 2 * AB_TILE);
       tc::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(dq, ads + 4 * kk, att_desc_mn(k_s, kk), accumulate || kk > 0);
@@ -336,48 +299,16 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       for (int r = 0; r < 2; ++r) {
         const int i = i0 + 8 * r;
         const bool diag = i < p.T && i >= p.sep;
-        const __nv_bfloat16* krow = p.qkv + att_tok(diag ? i : 0, b, p.T, p.B, p.batch_major) * p.ld_qkv + E + h * ATT_DH;
+        const __nv_bfloat16* krow = p.qkv + att_tok(diag ? i : 0, unit.b, p.T, p.B, p.batch_major) * p.ld_qkv + E + unit.h * ATT_DH;
 #pragma unroll
         for (int j = 0; j < 16; ++j)
           kd[r][j] = diag ? *reinterpret_cast<const uint32_t*>(krow + 8 * j + 2 * (lane & 3)) : 0u;
       }
     };
-    if (nblk > 0) {
-      if (!tc::mbar_wait_bounded(&kv_full[stage], phase)) { timed_out = true; break; }
-      issue_sdp(stage);
-      tc::wgmma_wait<0>();
-      tc::wgmma_fence_regs(s);
-      tc::wgmma_fence_regs(dp);
-      if (nblk == 1 && tid == 0) tc::mbar_arrive(q_empty);
-      compute_ds(0);
-      pack_ds();
-      int cur = stage;                      // ring stage of the block whose dQ MMAs are next
-      if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
-      for (int kb = 1; kb < nblk; ++kb) {
-        if (!timed_out && !tc::mbar_wait_bounded(&kv_full[stage], phase)) timed_out = true;
-        issue_sdp(stage);
-        issue_dq(cur, kb > 1);
-        tc::wgmma_wait<1>();
-        tc::wgmma_fence_regs(s);
-        tc::wgmma_fence_regs(dp);
-        if (kb == nblk - 1 && tid == 0) tc::mbar_arrive(q_empty);
-        compute_ds(kb);
-        tc::wgmma_wait<0>();
-        tc::wgmma_fence_regs(dq);
-        if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
-        cur = stage;
-        if (++stage == AB_DQ_STAGES) { stage = 0; phase ^= 1; }
-        pack_ds();
-      }
-      issue_dq(cur, nblk > 1);
-      load_kd();
-      tc::wgmma_wait<0>();
-      tc::wgmma_fence_regs(dq);
-      if (timed_out) break;
-      if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
-    } else {
-      if (tid == 0) tc::mbar_arrive(q_empty);
-      load_kd();
+    if (att_key_loop(pp, ring, it, nblk, issue_sdp, issue_dq, [&] { tc::wgmma_fence_regs(s); tc::wgmma_fence_regs(dp); },
+                     [&] { tc::wgmma_fence_regs(dq); }, compute_ds, pack_ds, load_kd)) {
+      timed_out = true;
+      break;
     }
 
     // dQ = dq + ds_ii k_i, stores, column sums over the bf16-rounded values
@@ -389,7 +320,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       const int i = i0 + 8 * r;
       if (i < p.T) {
         const bool diag = i >= p.sep;
-        __nv_bfloat16* grow = p.dqkv + att_tok(i, b, p.T, p.B, p.batch_major) * p.ld_dqkv + h * ATT_DH;
+        __nv_bfloat16* grow = p.dqkv + att_tok(i, unit.b, p.T, p.B, p.batch_major) * p.ld_dqkv + unit.h * ATT_DH;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           float x = nblk > 0 ? dq[4 * j + 2 * r] : 0.f, y = nblk > 0 ? dq[4 * j + 2 * r + 1] : 0.f;
@@ -414,7 +345,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           v += __shfl_xor_sync(0xffffffffu, v, 4);
           v += __shfl_xor_sync(0xffffffffu, v, 8);
           v += __shfl_xor_sync(0xffffffffu, v, 16);
-          if (lane < 4) atomicAdd(p.dq_colsum + h * ATT_DH + 8 * j + 2 * lane + e, v);
+          if (lane < 4) atomicAdd(p.dq_colsum + unit.h * ATT_DH + 8 * j + 2 * lane + e, v);
         }
     }
   }
@@ -428,7 +359,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                     const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = att_smem_base(smem_raw);
   uint8_t* sK = smem;                                     // warpgroup g's 64 keys at + g * 16 KB
   uint8_t* sV = smem + 2 * AB_TILE;
   uint8_t* sRing = smem + AB_DKV_OFF_RING;                // stage s: Q at + 2 s * 16 KB, dO at + (2 s + 1) * 16 KB
@@ -437,9 +368,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   uint64_t* empty = full + AB_DKV_STAGES;
   uint64_t* kv_bar = empty + AB_DKV_STAGES;               // K, V of the tile have landed
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kt = static_cast<int>(blockIdx.x) % p.n_tiles;
-  const int bh = static_cast<int>(blockIdx.x) / p.n_tiles;
-  const int h = bh % p.H, b = bh / p.H;
+  const AttUnit unit = att_unit(blockIdx.x, p.n_tiles, p.H);
   const int E = p.H * ATT_DH;
   const int nqb = (p.T + AB_ROWS - 1) / AB_ROWS;
   if (threadIdx.x == 0) {
@@ -456,38 +385,37 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     // ------------------------------------------------------------------ producer: TMA (warp 8), lse2 / delta (warps 10, 11)
     tc::setmaxnreg_dec<40>();
     const int pt = threadIdx.x - 256;
-    int stage = 0;
-    uint32_t phase = 0;
+    AttRing<AB_DKV_STAGES> ring;
     if (pt == 0) {
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
       tc::tma_prefetch_desc(&tmDO);
       tc::mbar_expect_tx(kv_bar, 4 * AB_TILE);
       for (int g = 0; g < 2; ++g) {
-        const int j0 = kt * 128 + 64 * g;
-        att_load_tile(sK + g * AB_TILE, &tmKV, kv_bar, E + h * ATT_DH, b, j0);
-        att_load_tile(sV + g * AB_TILE, &tmKV, kv_bar, 2 * E + h * ATT_DH, b, j0);
+        const int j0 = unit.tile * 128 + 64 * g;
+        att_load_tile(sK + g * AB_TILE, &tmKV, kv_bar, E + unit.h * ATT_DH, unit.b, j0);
+        att_load_tile(sV + g * AB_TILE, &tmKV, kv_bar, 2 * E + unit.h * ATT_DH, unit.b, j0);
       }
       for (int qb = 0; qb < nqb; ++qb) {
-        tc::mbar_wait_suspend(&empty[stage], phase ^ 1);
-        uint8_t* dst = sRing + stage * 2 * AB_TILE;
-        tc::mbar_expect_tx(&full[stage], 2 * AB_TILE);
-        att_load_tile(dst, &tmQ, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
-        att_load_tile(dst + AB_TILE, &tmDO, &full[stage], h * ATT_DH, b, qb * AB_ROWS);
-        if (++stage == AB_DKV_STAGES) { stage = 0; phase ^= 1; }
+        tc::mbar_wait_suspend(&empty[ring.stage], ring.phase ^ 1);
+        uint8_t* dst = sRing + ring.stage * 2 * AB_TILE;
+        tc::mbar_expect_tx(&full[ring.stage], 2 * AB_TILE);
+        att_load_tile(dst, &tmQ, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
+        att_load_tile(dst + AB_TILE, &tmDO, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
+        ring.advance();
       }
     } else if (pt >= 64) {
       const int r = pt - 64;
       for (int qb = 0; qb < nqb; ++qb) {
         const int i = qb * AB_ROWS + r;
         const bool valid = i < p.T;
-        const float l2 = valid ? p.lse[static_cast<size_t>(bh) * p.T + i] * 1.4426950408889634f : INFINITY;
-        const float dl = valid ? ab_delta(p, b, h, i) : 0.f;
-        tc::mbar_wait_suspend(&empty[stage], phase ^ 1);
-        sStat[stage * 2 * AB_ROWS + r] = l2;
-        sStat[stage * 2 * AB_ROWS + AB_ROWS + r] = dl;
-        tc::mbar_arrive(&full[stage]);
-        if (++stage == AB_DKV_STAGES) { stage = 0; phase ^= 1; }
+        const float l2 = valid ? p.lse[static_cast<size_t>(unit.bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+        const float dl = valid ? ab_delta(p, unit.b, unit.h, i) : 0.f;
+        tc::mbar_wait_suspend(&empty[ring.stage], ring.phase ^ 1);
+        sStat[ring.stage * 2 * AB_ROWS + r] = l2;
+        sStat[ring.stage * 2 * AB_ROWS + AB_ROWS + r] = dl;
+        tc::mbar_arrive(&full[ring.stage]);
+        ring.advance();
       }
     }
     return;
@@ -499,21 +427,20 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int tid = threadIdx.x & 127;
   const uint32_t k_tile = tc::smem_u32(sK + g * AB_TILE), v_tile = tc::smem_u32(sV + g * AB_TILE);
   const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
-  const int key_a = kt * 128 + 64 * g + 16 * wq + (lane >> 2);   // this lane's keys: key_a, key_a + 8
-  const uint32_t drow_base = static_cast<uint32_t>(bh) * p.T;
+  const int key_a = unit.tile * 128 + 64 * g + 16 * wq + (lane >> 2);   // this lane's keys: key_a, key_a + 8
+  const uint32_t drow_base = static_cast<uint32_t>(unit.bh) * p.T;
   tc::mbar_wait(kv_bar, 0);
 
   // The first MMAs write dk / dv (scale-d = 0), so nothing but wgmma defines them until the loop has drained.
   float dk[64], dv[64];
-  int stage = 0;
-  uint32_t phase = 0;
+  AttRing<AB_DKV_STAGES> ring;
   bool timed_out = false;
   for (int qb = 0; qb < nqb; ++qb) {
-    if (!tc::mbar_wait_bounded(&full[stage], phase)) { timed_out = true; break; }
-    const uint32_t q_s = tc::smem_u32(sRing + stage * 2 * AB_TILE);
+    if (!tc::mbar_wait_bounded(&full[ring.stage], ring.phase)) { timed_out = true; break; }
+    const uint32_t q_s = tc::smem_u32(sRing + ring.stage * 2 * AB_TILE);
     const uint32_t d_s = q_s + AB_TILE;
     const uint32_t k_s = att_opaque(k_tile), v_s = att_opaque(v_tile);
-    const float* st_lse = sStat + stage * 2 * AB_ROWS;
+    const float* st_lse = sStat + ring.stage * 2 * AB_ROWS;
     const float* st_dl = st_lse + AB_ROWS;
     float s[32], dp[32];
     tc::wgmma_fence();
@@ -556,8 +483,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     }
     tc::wgmma_commit();
     tc::wgmma_wait<0>();
-    if (tid == 0) tc::mbar_arrive(&empty[stage]);
-    if (++stage == AB_DKV_STAGES) { stage = 0; phase ^= 1; }
+    if (tid == 0) tc::mbar_arrive(&empty[ring.stage]);
+    ring.advance();
   }
   tc::wgmma_fence_regs(dk);
   tc::wgmma_fence_regs(dv);
@@ -567,7 +494,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   for (int r = 0; r < 2; ++r) {
     const int key = key_a + 8 * r;
     if (key < p.sep) {
-      __nv_bfloat16* grow = p.dqkv + att_tok(key, b, p.T, p.B, p.batch_major) * p.ld_dqkv + h * ATT_DH;
+      __nv_bfloat16* grow = p.dqkv + att_tok(key, unit.b, p.T, p.B, p.batch_major) * p.ld_dqkv + unit.h * ATT_DH;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         att_st2(grow + E, j, lane, dk[4 * j + 2 * r], dk[4 * j + 2 * r + 1]);
@@ -599,10 +526,8 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
   if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
   if (int rc = att_tensor_map(&tmDO, d->dout, E, d->ld_dout, d->T, d->B, d->T, d->batch_major)) return rc;
   static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_DQ_SMEM));
+  if (first_use_on_device(attr_set))
     PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_DKV_SMEM));
-  }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!d->delta_token_major) {
     const long long rows = static_cast<long long>(d->T) * d->B;
@@ -613,11 +538,9 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
     PFN_LAUNCH_OK();
   }
   p.n_tiles = (d->T + 127) / 128;
-  const long long units = static_cast<long long>(p.n_tiles) * d->B * d->H;
-  PFN_CHECK_ARG(units < (1LL << 31), "attention_bwd_tc: too many tiles");
-  const int grid_dq = units < num_sms() ? static_cast<int>(units) : num_sms();
-  attn_bwd_dq_kernel<<<static_cast<unsigned>(grid_dq), AB_THREADS, AB_DQ_SMEM, s>>>(tmQ, tmKV, tmDO, p);
-  PFN_LAUNCH_OK();
+  if (int rc = att_launch_persistent<attn_bwd_dq_kernel>("attention_bwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                         AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, p))
+    return rc;
   if (d->sep > 0) {
     p.n_tiles = (d->sep + 127) / 128;
     const long long grid = static_cast<long long>(p.n_tiles) * d->B * d->H;

@@ -50,6 +50,137 @@ __device__ __forceinline__ void att_load_tile(uint8_t* dst, const CUtensorMap* m
   tc::tma_load_3d(dst + 8192, m, bar, col0 + 64, b, t0);
 }
 
+// A work unit: one 128-row tile of one (batch, head).  Unit u is tile u % n_tiles of (batch, head) bh = u / n_tiles, so
+// the tiles of one (batch, head) are neighbours and the CTAs that run them at the same time share its K/V in L2.
+struct AttUnit {
+  int tile;   // 128-row tile: of the query rows, or of the train keys in the dK/dV kernel
+  int bh, h, b;
+};
+__device__ __forceinline__ AttUnit att_unit(int u, int n_tiles, int H) {
+  const int bh = u / n_tiles;
+  return {u % n_tiles, bh, bh % H, bh / H};
+}
+
+// Position in a ring of STAGES buffers: the stage and the parity of the barrier phase that completes it
+template <int STAGES>
+struct AttRing {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance() { if (++stage == STAGES) { stage = 0; phase ^= 1; } }
+};
+
+// the dynamic shared memory from its first 1 KB boundary, as the 128-byte swizzle needs (the sizes include the slack)
+__device__ __forceinline__ uint8_t* att_smem_base(uint8_t* raw) {
+  return raw + ((1024u - (tc::smem_u32(raw) & 1023u)) & 1023u);
+}
+
+// The K/V pipeline of the persistent kernels (forward, dQ backward): one TMA thread streams the 64-key blocks of the
+// train keys through a ring of STAGES (K, V) stages to two consumer warpgroups, and hands them the query operands of the
+// CTA's current tile (Q, and dO in the backward) through q_full / q_empty.  Its barriers are 2 STAGES + 2 words.
+template <int STAGES>
+struct AttPipe {
+  uint8_t* ring;        // stage s: K at + 2 s * 16 KB, V at + (2 s + 1) * 16 KB
+  uint64_t* kv_full;    // [STAGES] the stage's K and V have landed
+  uint64_t* kv_empty;   // [STAGES] both warpgroups' MMAs that read the stage have completed
+  uint64_t* q_full;     // the query operands of the CTA's current tile have landed
+  uint64_t* q_empty;    // both warpgroups' last MMAs that read them have completed
+  __device__ __forceinline__ AttPipe(uint8_t* ring_smem, uint64_t* bars)
+      : ring(ring_smem), kv_full(bars), kv_empty(bars + STAGES), q_full(bars + 2 * STAGES), q_empty(bars + 2 * STAGES + 1) {}
+  // by one thread, before tc::mbar_fence_init() and the block barrier
+  __device__ __forceinline__ void init() const {
+    for (int s = 0; s < STAGES; ++s) {
+      tc::mbar_init(&kv_full[s], 1);
+      tc::mbar_init(&kv_empty[s], 2);
+    }
+    tc::mbar_init(q_full, 1);
+    tc::mbar_init(q_empty, 2);
+  }
+};
+
+// The producer of the pipeline (one thread): for each of the CTA's units, the nblk key blocks of its (batch, head).  The
+// next tile's query operands go in once the consumers are done with the current ones, which is before its last key
+// block is (so the first key blocks of the next tile are already in flight by then): load_q(unit) issues q_bytes of
+// TMA loads on q_full.
+template <int STAGES, class LoadQ>
+__device__ __forceinline__ void att_kv_producer(const AttPipe<STAGES>& pp, const CUtensorMap* tmKV, int n_units, int n_tiles,
+                                                int H, int nblk, uint32_t q_bytes, LoadQ&& load_q) {
+  const int E = H * ATT_DH;
+  AttRing<STAGES> ring;
+  for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
+    const AttUnit unit = att_unit(u, n_tiles, H);
+    auto claim_q = [&]() {
+      if (it > 0) tc::mbar_wait_suspend(pp.q_empty, (it - 1) & 1);
+      tc::mbar_expect_tx(pp.q_full, q_bytes);
+      load_q(unit);
+    };
+    const int claim_at = min(STAGES - 1, nblk - 1);
+    if (nblk == 0) claim_q();
+    for (int kb = 0; kb < nblk; ++kb) {
+      if (kb == claim_at) claim_q();
+      tc::mbar_wait_suspend(&pp.kv_empty[ring.stage], ring.phase ^ 1);
+      uint8_t* dst = pp.ring + ring.stage * 2 * ATT_TILE;
+      tc::mbar_expect_tx(&pp.kv_full[ring.stage], 2 * ATT_TILE);
+      att_load_tile(dst, tmKV, &pp.kv_full[ring.stage], E + unit.h * ATT_DH, unit.b, kb * ATT_TILE_ROWS);
+      att_load_tile(dst + ATT_TILE, tmKV, &pp.kv_full[ring.stage], 2 * E + unit.h * ATT_DH, unit.b, kb * ATT_TILE_ROWS);
+      ring.advance();
+    }
+  }
+}
+
+// One consumer warpgroup's key loop over the nblk key blocks of the CTA's it-th tile.  Block kb issues its first MMA
+// group (issue_a: S, or S and dP) and the second group of block kb - 1 (issue_b: O += P V, or dQ += dS K; the flag is
+// false for the tile's first) back to back, waits for the first only and runs math(kb) (softmax, or dS) under the
+// second, then waits for it, releases its stage and runs pack() (the next A fragments).  before_tail() is issued under
+// the tile's last MMAs, or at once when there are none; fence_a / fence_b fence the two groups' accumulators.
+// The accumulators are written only when no MMA that owns them is in flight: otherwise ptxas serialises the whole wgmma
+// pipeline.  For the same reason a timed-out wait inside the loop is recorded and the block runs on; the tile is
+// abandoned once the pipeline has drained.  Returns true when a wait timed out: the caller leaves its tile loop and
+// traps after it, so that ptxas keeps the register budget setmaxnreg raised (tc::mbar_wait_bounded).
+template <int STAGES, class IssueA, class IssueB, class FenceA, class FenceB, class Math, class Pack, class BeforeTail>
+__device__ __forceinline__ bool att_key_loop(const AttPipe<STAGES>& pp, AttRing<STAGES>& ring, int it, int nblk,
+                                             IssueA&& issue_a, IssueB&& issue_b, FenceA&& fence_a, FenceB&& fence_b,
+                                             Math&& math, Pack&& pack, BeforeTail&& before_tail) {
+  const bool leader = (threadIdx.x & 127) == 0;
+  if (!tc::mbar_wait_bounded(pp.q_full, it & 1)) return true;
+  if (nblk > 0) {
+    if (!tc::mbar_wait_bounded(&pp.kv_full[ring.stage], ring.phase)) return true;
+    issue_a(ring.stage);
+    tc::wgmma_wait<0>();
+    fence_a();
+    if (nblk == 1 && leader) tc::mbar_arrive(pp.q_empty);
+    math(0);
+    pack();
+    int cur = ring.stage;                   // ring stage of the block whose second group is next
+    ring.advance();
+    bool timed_out = false;
+    for (int kb = 1; kb < nblk; ++kb) {
+      if (!timed_out && !tc::mbar_wait_bounded(&pp.kv_full[ring.stage], ring.phase)) timed_out = true;
+      issue_a(ring.stage);
+      issue_b(cur, kb > 1);
+      tc::wgmma_wait<1>();
+      fence_a();
+      if (kb == nblk - 1 && leader) tc::mbar_arrive(pp.q_empty);
+      math(kb);
+      tc::wgmma_wait<0>();
+      fence_b();
+      if (leader) tc::mbar_arrive(&pp.kv_empty[cur]);
+      cur = ring.stage;
+      ring.advance();
+      pack();
+    }
+    issue_b(cur, nblk > 1);
+    before_tail();
+    tc::wgmma_wait<0>();
+    fence_b();
+    if (timed_out) return true;
+    if (leader) tc::mbar_arrive(&pp.kv_empty[cur]);
+  } else {
+    if (leader) tc::mbar_arrive(pp.q_empty);
+    before_tail();
+  }
+  return false;
+}
+
 // the 32 columns of a 128-wide head row that lane `lane` owns in an m16n8 accumulator row: 8 j + 2 (lane & 3) + {0, 1}
 __device__ __forceinline__ float2 att_ld2(const __nv_bfloat16* row, int j, int lane) {
   return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + 8 * j + 2 * (lane & 3)));
@@ -78,6 +209,20 @@ static inline int check_tc_attn(const pfn_attn_desc* d, bool bwd, const char* wh
     PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->dout) | reinterpret_cast<uintptr_t>(d->dqkv)) & 15) == 0,
                   "%s: dout/dqkv must be 16-byte aligned", who);
   }
+  return 0;
+}
+
+// Launch of a persistent kernel over `units` work units: one CTA per SM, or one per unit when there are fewer.  The
+// kernel's dynamic shared-memory limit is raised on its first launch on each device.
+template <auto Kernel, class... Args>
+static inline int att_launch_persistent(const char* who, long long units, int threads, int smem, cudaStream_t s,
+                                        const Args&... args) {
+  PFN_CHECK_ARG(units < (1LL << 31), "%s: too many tiles", who);
+  static bool attr_set[64] = {};
+  if (first_use_on_device(attr_set)) PFN_CUDA_OK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const int grid = units < num_sms() ? static_cast<int>(units) : num_sms();
+  Kernel<<<static_cast<unsigned>(grid), threads, smem, s>>>(args...);
+  PFN_LAUNCH_OK();
   return 0;
 }
 

@@ -6,10 +6,10 @@
 // diagonal key of a query row is a 128-wide dot product done by the four lanes that own the row.  Q/K/V rows are read
 // straight out of the packed [T*B, 3E] in-projection output, so there is no head-split / transpose kernel.
 //
-// attn_fwd_kernel is persistent: one CTA per SM walks the (batch, head, 128-row query tile) units, query tile fastest,
-// so the tiles of one (batch, head) run at the same time and share its K/V in L2.  It is warp-specialised like the dQ
-// backward kernel: warpgroup 2 (producer, 40 registers) TMA-loads the tile's Q and a 4-stage ring of (K, V) 64-key blocks;
-// warpgroups 0 and 1 (consumers, 232 registers) each own 64 query rows and run, per key block j,
+// attn_fwd_kernel is persistent: one CTA per SM walks the (batch, head, 128-row query tile) units on the K/V pipeline it
+// shares with the dQ backward kernel (AttPipe, attention_common.cuh).  Warpgroup 2 (producer, 40 registers) TMA-loads
+// the tile's Q and a 4-stage ring of (K, V) 64-key blocks; warpgroups 0 and 1 (consumers, 232 registers) each own 64
+// query rows and run, per key block j,
 //   S_j = Q K_j^T (wgmma m64n64k16, fp32)  ->  online softmax in the log2 domain  ->  P_j as bf16 A fragments (registers)
 //   ->  O += P_j V_j (wgmma m64n128k16, A from registers, V read MN-major)
 // with S_j and the PV MMAs of block j-1 issued together, so the softmax of block j runs under the previous P V.  A row's
@@ -43,25 +43,16 @@ __global__ void __launch_bounds__(AF_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                 const __grid_constant__ CUtensorMap tmO, const AttnFwdParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = att_smem_base(smem_raw);
   uint8_t* sQ = smem;                                     // warpgroup g's 64 rows at + g * 16 KB
   uint8_t* sStg = smem + AF_OFF_STG;                      // warpgroup g's output staging at + g * 16 KB
-  uint8_t* sRing = smem + AF_OFF_RING;                    // stage s: K at + 2 s * 16 KB, V at + (2 s + 1) * 16 KB
-  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + AF_OFF_BAR);
-  uint64_t* kv_empty = kv_full + AF_STAGES;
-  uint64_t* q_full = kv_empty + AF_STAGES;                // Q of the CTA's current tile has landed
-  uint64_t* q_empty = q_full + 1;                         // both warpgroups have finished their last S MMAs of it
+  const AttPipe<AF_STAGES> pp(smem + AF_OFF_RING, reinterpret_cast<uint64_t*>(smem + AF_OFF_BAR));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int E = p.H * ATT_DH;
   const int nblk = (p.sep + ATT_TILE_ROWS - 1) / ATT_TILE_ROWS;
   const int n_units = p.n_tiles * p.B * p.H;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < AF_STAGES; ++s) {
-      tc::mbar_init(&kv_full[s], 1);
-      tc::mbar_init(&kv_empty[s], 2);
-    }
-    tc::mbar_init(q_full, 1);
-    tc::mbar_init(q_empty, 2);
+    pp.init();
     tc::mbar_fence_init();
   }
   __syncthreads();
@@ -72,30 +63,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if (threadIdx.x == 256) {
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
-        const int qt = u % p.n_tiles, bh = u / p.n_tiles;
-        const int h = bh % p.H, b = bh / p.H;
-        // The next tile's Q goes in once the consumers are done with the current one, which is before its last key
-        // block is (so the first key blocks of the next tile are already in flight by then).
-        auto load_q = [&]() {
-          if (it > 0) tc::mbar_wait_suspend(q_empty, (it - 1) & 1);
-          tc::mbar_expect_tx(q_full, 2 * ATT_TILE);
-          for (int g = 0; g < 2; ++g) att_load_tile(sQ + g * ATT_TILE, &tmQ, q_full, h * ATT_DH, b, qt * 128 + 64 * g);
-        };
-        const int claim_at = min(AF_STAGES - 1, nblk - 1);
-        if (nblk == 0) load_q();
-        for (int kb = 0; kb < nblk; ++kb) {
-          if (kb == claim_at) load_q();
-          tc::mbar_wait_suspend(&kv_empty[stage], phase ^ 1);
-          uint8_t* dst = sRing + stage * 2 * ATT_TILE;
-          tc::mbar_expect_tx(&kv_full[stage], 2 * ATT_TILE);
-          att_load_tile(dst, &tmKV, &kv_full[stage], E + h * ATT_DH, b, kb * ATT_TILE_ROWS);
-          att_load_tile(dst + ATT_TILE, &tmKV, &kv_full[stage], 2 * E + h * ATT_DH, b, kb * ATT_TILE_ROWS);
-          if (++stage == AF_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
+      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk, 2 * ATT_TILE, [&](const AttUnit& unit) {
+        for (int g = 0; g < 2; ++g)
+          att_load_tile(sQ + g * ATT_TILE, &tmQ, pp.q_full, unit.h * ATT_DH, unit.b, unit.tile * 128 + 64 * g);
+      });
     }
     return;
   }
@@ -107,13 +78,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const uint32_t q_tile = tc::smem_u32(sQ + g * ATT_TILE);
   uint8_t* stg = sStg + g * ATT_TILE;
   const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
-  int stage = 0;
-  uint32_t phase = 0;
+  AttRing<AF_STAGES> ring;
   bool timed_out = false;
   for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
-    const int qt = u % p.n_tiles, bh = u / p.n_tiles;
-    const int h = bh % p.H, b = bh / p.H;
-    const int t0 = qt * 128 + 64 * g;
+    const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+    const int t0 = unit.tile * 128 + 64 * g;
     const int i0 = t0 + 16 * wq + (lane >> 2);            // this lane's rows: i0, i0 + 8
 
     // Diagonal key first: o[4 j + 2 r + c] is row i0 + 8 r, column 8 j + 2 (lane & 3) + c.  A row i >= sep starts from
@@ -125,8 +94,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     for (int r = 0; r < 2; ++r) {
       const int i = i0 + 8 * r;
       const bool diag = i < p.T && i >= p.sep;
-      drow[r] = static_cast<uint32_t>(bh) * p.T + i;
-      const __nv_bfloat16* qrow = p.qkv + att_tok(diag ? i : 0, b, p.T, p.B, p.batch_major) * p.ld_qkv + h * ATT_DH;
+      drow[r] = static_cast<uint32_t>(unit.bh) * p.T + i;
+      const __nv_bfloat16* qrow = p.qkv + att_tok(diag ? i : 0, unit.b, p.T, p.B, p.batch_major) * p.ld_qkv + unit.h * ATT_DH;
       float sd = 0.f;
       if (diag) {
 #pragma unroll
@@ -146,26 +115,22 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         o[4 * j + 2 * r + 1] = v.y;
       }
     }
-    if (!tc::mbar_wait_bounded(q_full, it & 1)) { timed_out = true; break; }
 
-    // Key loop.  Block kb issues S_kb = Q K_kb^T and PV_{kb-1} (O += P_{kb-1} V_{kb-1}) back to back, waits for S_kb
-    // only and runs its softmax while PV_{kb-1} is on the tensor pipe, then waits for PV_{kb-1}, rescales O and packs
-    // P_kb.  O and the S accumulator are written only when no MMA that owns them is in flight: otherwise ptxas
-    // serialises the whole wgmma pipeline.  For the same reason a timed-out wait inside the loop is recorded and the
-    // block runs on; the tile is abandoned once the pipeline has drained.
+    // Key loop (att_key_loop): S_kb = Q K_kb^T, its online softmax while PV_{kb-1} (O += P_{kb-1} V_{kb-1}) runs, then
+    // O rescaled and P_kb packed.
     float s[32];
     uint32_t ap[16];
     float corr[2];
     auto issue_s = [&](int st) {
-      const uint32_t k_s = tc::smem_u32(sRing + st * 2 * ATT_TILE);
+      const uint32_t k_s = tc::smem_u32(pp.ring + st * 2 * ATT_TILE);
       const uint32_t q_s = att_opaque(q_tile);
       tc::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) att_mma_n64(s, att_desc_k(q_s, kk), att_desc_k(k_s, kk), kk);
       tc::wgmma_commit();
     };
-    auto issue_pv = [&](int st) {
-      const uint32_t v_s = tc::smem_u32(sRing + st * 2 * ATT_TILE) + ATT_TILE;
+    auto issue_pv = [&](int st, bool) {                  // always accumulates: O starts from the diagonal key
+      const uint32_t v_s = tc::smem_u32(pp.ring + st * 2 * ATT_TILE) + ATT_TILE;
       tc::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) tc::wgmma_m64n128k16_rs(o, ap + 4 * kk, att_desc_mn(v_s, kk), 1);
@@ -206,38 +171,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
       for (int e = 0; e < 16; ++e) ap[e] = tc::pack_bf16x2(s[2 * e], s[2 * e + 1]);
     };
-    if (nblk > 0) {
-      if (!tc::mbar_wait_bounded(&kv_full[stage], phase)) { timed_out = true; break; }
-      issue_s(stage);
-      tc::wgmma_wait<0>();
-      tc::wgmma_fence_regs(s);
-      if (nblk == 1 && tid == 0) tc::mbar_arrive(q_empty);
-      softmax(0);
-      rescale_pack();
-      int cur = stage;                      // ring stage of the block whose PV is next
-      if (++stage == AF_STAGES) { stage = 0; phase ^= 1; }
-      for (int kb = 1; kb < nblk; ++kb) {
-        if (!timed_out && !tc::mbar_wait_bounded(&kv_full[stage], phase)) timed_out = true;
-        issue_s(stage);
-        issue_pv(cur);
-        tc::wgmma_wait<1>();
-        tc::wgmma_fence_regs(s);
-        if (kb == nblk - 1 && tid == 0) tc::mbar_arrive(q_empty);
-        softmax(kb);
-        tc::wgmma_wait<0>();
-        tc::wgmma_fence_regs(o);
-        if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
-        cur = stage;
-        if (++stage == AF_STAGES) { stage = 0; phase ^= 1; }
-        rescale_pack();
-      }
-      issue_pv(cur);
-      tc::wgmma_wait<0>();
-      tc::wgmma_fence_regs(o);
-      if (timed_out) break;
-      if (tid == 0) tc::mbar_arrive(&kv_empty[cur]);
-    } else if (tid == 0) {
-      tc::mbar_arrive(q_empty);
+    if (att_key_loop(pp, ring, it, nblk, issue_s, issue_pv, [&] { tc::wgmma_fence_regs(s); },
+                     [&] { tc::wgmma_fence_regs(o); }, softmax, rescale_pack, [] {})) {
+      timed_out = true;
+      break;
     }
 
     // epilogue: O / l -> bf16 into the staging tile (two 64-column boxes, 128-byte swizzle: 16-byte chunk c of row rr at
@@ -255,13 +192,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const uint32_t off = (j >> 3) * 8192 + rr * 128 + (((j & 7) ^ (rr & 7)) << 4) + (lane & 3) * 4;
         *reinterpret_cast<uint32_t*>(stg + off) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
       }
-      if (i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+      if (i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
     }
     tc::fence_proxy_async_smem();
     tc::named_bar_sync(1 + g, 128);
     if (tid == 0 && t0 < p.T) {
-      tc::tma_store_3d(&tmO, stg, h * ATT_DH, b, t0);
-      tc::tma_store_3d(&tmO, stg + 8192, h * ATT_DH + 64, b, t0);
+      tc::tma_store_3d(&tmO, stg, unit.h * ATT_DH, unit.b, t0);
+      tc::tma_store_3d(&tmO, stg + 8192, unit.h * ATT_DH + 64, unit.b, t0);
       tc::bulk_commit();
     }
   }
@@ -288,14 +225,6 @@ extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
   if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
   // out: rows past T are not written
   if (int rc = att_tensor_map(&tmO, d->out, E, d->ld_out, d->T, d->B, d->T, d->batch_major)) return rc;
-  const long long units = static_cast<long long>(p.n_tiles) * d->B * d->H;
-  PFN_CHECK_ARG(units < (1LL << 31), "attention_fwd_tc: too many tiles");
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    PFN_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AF_SMEM));
-  }
-  const int grid = units < num_sms() ? static_cast<int>(units) : num_sms();
-  attn_fwd_kernel<<<static_cast<unsigned>(grid), AF_THREADS, AF_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(tmQ, tmKV, tmO, p);
-  PFN_LAUNCH_OK();
-  return 0;
+  return att_launch_persistent<attn_fwd_kernel>("attention_fwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                AF_THREADS, AF_SMEM, reinterpret_cast<cudaStream_t>(stream), tmQ, tmKV, tmO, p);
 }
