@@ -9,7 +9,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from transformerscandobayesianinference_b200 import _lib as L, bar_distribution, encoders, priors, transformer
-from oracle import pfn_oracle as O
+from oracle import error_budget as EB, pfn_oracle as O
 
 T, B, F, E, H, NHID, NL, NB, SEP = 1000, 512, 1, 512, 4, 1024, 6, 100, 500
 DH = E // H
@@ -29,16 +29,13 @@ def test_attention_fullsize_slices_match_oracle(cuda_device):
     assert torch.isfinite(out.float()).all() and torch.isfinite(dqkv.float()).all()
     q3 = qkv.view(T, B, 3, H, DH)
     for (b, h) in [(0, 0), (257, 2), (511, 3)]:
-        sl = q3[:, b, :, h, :].float().cpu().double()                        # [T, 3, dh]
-        one = sl.permute(0, 1, 2).reshape(T, 3 * DH).clone().requires_grad_(True)   # a 1-batch 1-head problem
-        ref, ref_lse = O.attention_ref(one, T, 1, 1, DH, SEP)
-        got = out.view(T, B, H, DH)[:, b, h, :].float().cpu().double()
-        assert (got - ref).abs().max().item() <= 2e-2 * ref.abs().max().item()
-        assert (lse[b * H + h].cpu().double() - ref_lse[0]).abs().max().item() <= 1e-3 * (ref_lse.abs().max().item() + 1)
-        do = dout.view(T, B, H, DH)[:, b, h, :].float().cpu().double()
-        (ref * do).sum().backward()
-        gd = dqkv.view(T, B, 3, H, DH)[:, b, :, h, :].float().cpu().double().reshape(T, 3 * DH)
-        assert (gd - one.grad).abs().max().item() <= 5e-2 * (one.grad.abs().max().item() + 1e-9)
+        one = q3[:, b, :, h, :].reshape(T, 3 * DH)                                 # a 1-batch 1-head problem
+        f = EB.attention_fwd(one, T, 1, 1, DH, SEP, EB.U)
+        got = out.view(T, B, H, DH)[:, b, h, :]
+        EB.check_attention_fwd(got, lse[b * H + h].view(1, T), f, EB.C_ATT_OUT, EB.C_ATT_LSE)
+        do = dout.view(T, B, H, DH)[:, b, h, :]
+        gd = dqkv.view(T, B, 3, H, DH)[:, b, :, h, :].reshape(T, 3 * DH)
+        EB.check_attention_bwd(gd, EB.attention_bwd(f, do, got), EB.C_ATT_GRAD)
 
 
 def test_gemm_fullsize_rows_match_reference(cuda_device):
@@ -51,8 +48,8 @@ def test_gemm_fullsize_rows_match_reference(cuda_device):
     y = torch.empty(N, 3 * E, device=cuda_device, dtype=torch.bfloat16)
     L.gemm(x, w, y, bias=bias, use_tc=True)
     rows = torch.tensor([0, 1, 127, 128, 255, 256, 65537, 300001, N - 129, N - 1], device=cuda_device)
-    ref = x[rows].double() @ w.double().t() + bias.double()
-    assert (y[rows].double() - ref).abs().max().item() <= 1.5e-2 * ref.abs().max().item()
+    ref, bound, _ = EB.gemm(x[rows], w, EB.U, EB.C_ACC_TC, bias=bias)
+    EB.check("gemm fullsize rows", y[rows], ref, bound, EB.C_GEMM)
     # linearity in the rows: the GEMM of a row-permuted input is the row-permuted output, bit for bit
     perm = torch.randperm(N, device=cuda_device)
     y2 = torch.empty_like(y)
