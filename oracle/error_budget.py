@@ -37,18 +37,30 @@ C_GEMM = 2.0          # GEMM results and epilogues (worst 0.99)
 # SIMT GEMM 0.17 (K = 17..300, three k-splits reduced by fp32 atomics)
 C_ACC_TC = 0.03
 C_ACC_SIMT = 0.35
+# Row kernels (rowwise.cu, bar_nll.cu, optimizer.cu).  Their fp32 sums are bounded by the depth of the kernel's reduction
+# tree (a sum whose longest path adds d terms is within U32 d sum|x| of the exact sum): a worst case that random data
+# reaches a small fraction of, so C_ROWSUM is well below 1.  Where a result is stored in bf16 its rounding alone reaches
+# a ratio of 1.
+C_LN = 2.0            # LayerNorm h, mean, rstd (worst 0.996, bf16 h; fp32: h 0.40, mean 0.14, rstd 0.13)
+C_LN_GRAD = 2.0       # LayerNorm dz, dgamma, dbeta, colsum_out (worst 0.996, bf16 dz; column sums 0.28)
+C_ROWSUM = 0.3        # colsum and the embedding backward's column sums (worst 0.147)
+C_EMBED = 2.0         # embedding forward (worst 0.996, bf16 out)
+C_BAR = 1.1           # bar-NLL lse and nll (worst 0.521, nll; lse 0.330)
+C_BAR_GRAD = 2.0      # bar-NLL dlogits (worst 0.996, bf16 dlogits; 0.487 fp32)
+C_ADAM = 2.0          # Adam p, m, v and the squared gradient norm (worst 0.998, p; m 0.40, v 0.52, norm 0.040)
 
 
-def check(name, got, exact, bound, c):
-    """Assert |got - exact| <= c * bound elementwise; print and return the worst ratio.  Where the bound is 0 the
-    kernel must be exact."""
+def check(name, got, exact, bound, c, verbose=True):
+    """Assert |got - exact| <= c * bound elementwise; print (verbose) and return the worst ratio.  Where the bound is 0
+    the kernel must be exact."""
     err = (got.double() - exact.double()).abs()
     bound = bound.double().expand_as(err)
     if (err[bound == 0] > 0).any():
         raise AssertionError(f"{name}: nonzero error where the bound is 0")
     ratio = (err / bound.clamp_min(1e-300)).masked_fill(bound == 0, 0.0)
     worst = ratio.max().item() if ratio.numel() else 0.0
-    print(f"[error-budget] {name}: worst err/bound = {worst:.4g} (c = {c})")
+    if verbose:
+        print(f"[error-budget] {name}: worst err/bound = {worst:.4g} (c = {c})")
     if not math.isfinite(worst) or worst > c:
         idx = int(ratio.flatten().argmax())
         raise AssertionError(f"{name}: err/bound {worst:.4g} > {c} at flat index {idx} "
@@ -214,3 +226,271 @@ def gemm(A, B, u_out, c_acc, bias=None, aux=None, epilogue="none", fast_gelu=Tru
 
 def gelu_grad(x):
     return 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Row kernels: LayerNorm, embedding, column sums (csrc/rowwise.cu), bar NLL (csrc/bar_nll.cu), Adam (csrc/optimizer.cu).
+# Their fp32 sums are bounded by the depth of the kernel's reduction tree: a sum formed as a tree whose longest
+# root-to-leaf path has d additions is within U32 d sum|x| of the exact sum, whatever the order.  The launch geometry
+# that sets the depth is passed in (num_sms), so that the host test evaluates the same bounds without a device.
+# ------------------------------------------------------------------------------------------------------------------
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def ln_lane_depth(E):
+    """Additions on the longest path of a LayerNorm row sum: a lane's serial sum (8 elements per 256-column chunk on
+    the vector path, ceil(E / 32) on the generic one), the 5-level warp butterfly and the scaling by 1 / E."""
+    return max(8 * _cdiv(E, 256), _cdiv(E, 32)) + 5 + 2
+
+
+def ln_vec(E, ld_list, ptrs_aligned=True):
+    """Whether the LayerNorm launch takes the vector kernel (rowwise.cu layernorm_*_dispatch)."""
+    return E % 8 == 0 and E <= 1024 and all(ld % 8 == 0 for ld in ld_list) and ptrs_aligned
+
+
+def ln_bwd_colsum_depth(rows, E, elem_size, vec, num_sms):
+    """Depth of the backward's column sums (dgamma, dbeta, colsum_out) over rows, plus the initial value of the output.
+    Vector kernel: a lane's serial sum over the rows its warp owns, 8 warps into shared memory, one global atomic per
+    CTA.  Generic kernel: one global atomic per row."""
+    if not vec:
+        return rows + 1
+    row_bytes = 256 * _cdiv(E, 256) * elem_size
+    ctas = 2 if row_bytes <= 512 else 1
+    grid = min(ctas * num_sms, _cdiv(rows, 8))
+    return _cdiv(rows, grid * 8) + 8 + grid + 1
+
+
+def layernorm_fwd(z, gamma, beta, u, eps=1e-5):
+    """Exact h, mean, rstd of LayerNorm over the last dim, and their bounds.
+
+    mean: U32 a_mu mean|z| with a_mu the row sum's depth.  The variance is summed about the kernel's mean: each term
+    rounds twice (z - mu, the fma), the sum has the same depth, and the mean's error adds (mu^ - mu)^2; rsqrtf and
+    the + eps add a few more, so rstd is within U32 (a_r + 4) + (mu^ - mu)^2 / (2 (var + eps)) of r relatively.
+    h: u |h| + U32 (|gamma| r (|z - mu| a_r + a_mu mean|z|) + |beta|)."""
+    zd, gd, bd = z.double(), gamma.double(), beta.double()
+    E = zd.shape[-1]
+    mu = zd.mean(-1, keepdim=True)
+    var = ((zd - mu) ** 2).mean(-1, keepdim=True)
+    r = 1.0 / torch.sqrt(var + eps)
+    h = (zd - mu) * r * gd + bd
+    a = ln_lane_depth(E)
+    mabs = zd.abs().mean(-1, keepdim=True)
+    mu_b = U32 * a * mabs
+    r_rel = U32 * (a + 4) + 0.5 * mu_b ** 2 / (var + eps)
+    h_b = u * h.abs() + U32 * (gd.abs() * r * ((zd - mu).abs() * (a + 4) + a * mabs) + bd.abs()) + gd.abs() * (zd - mu).abs() * r * r_rel
+    return {"h": h, "h_bound": h_b, "mean": mu.squeeze(-1), "mean_bound": mu_b.squeeze(-1),
+            "rstd": r.squeeze(-1), "rstd_bound": (r * r_rel).squeeze(-1)}
+
+
+def layernorm_bwd(dh, z, gamma, mean_k, rstd_k, u, colsum_depth, init=None, eps=1e-5):
+    """Exact dz, dgamma, dbeta, colsum_out = sum_rows dz of LayerNorm for the upstream dh, and their bounds.
+
+    The exact values use fp64 statistics of z.  The kernel reads the mean and rstd the forward stored (mean_k, rstd_k);
+    their actual deviation from the exact ones moves x^ = (z - mu) r by e_x = r |mu^ - mu| + |x^| |r^ / r - 1|, an
+    inherited term E.  dz = r (g - mean g - x^ mean(g x^)), g = dh gamma: the three terms cancel, so its rounding is
+    bounded by their magnitudes, U32 (a + 4) r (|g| + mean|g| + |x^| mean|g x^|) with a the row sum's depth, plus
+    u |dz| for the store.  The column sums over rows: U32 colsum_depth times the sum of the terms' magnitudes.
+    init: the values the column outputs held before the call (accumulated into); eps: the forward's."""
+    zd, dd, gd = z.double(), dh.double(), gamma.double()
+    E = zd.shape[-1]
+    mu = zd.mean(-1, keepdim=True)
+    r = 1.0 / torch.sqrt(((zd - mu) ** 2).mean(-1, keepdim=True) + eps)
+    xh = (zd - mu) * r
+    g = dd * gd
+    s1, s2 = g.mean(-1, keepdim=True), (g * xh).mean(-1, keepdim=True)
+    dz = r * (g - s1 - xh * s2)
+    a = ln_lane_depth(E)
+    eps_r = (rstd_k.double().view_as(r) / r - 1.0).abs()
+    e_x = (r * (mean_k.double().view_as(mu) - mu).abs() + xh.abs() * eps_r) * (1.0 + 4 * U32)   # (z - mu^) r^ rounds too
+    dz_mag = r * (g.abs() + g.abs().mean(-1, keepdim=True) + xh.abs() * (g * xh).abs().mean(-1, keepdim=True))
+    dz_inh = eps_r * dz.abs() + r * (e_x * s2.abs() + xh.abs() * (g.abs() * e_x).mean(-1, keepdim=True))
+    dz_b = u * dz.abs() + U32 * (a + 4) * dz_mag + dz_inh
+    if init is None:
+        init = torch.zeros(3, E, dtype=torch.float64, device=zd.device)
+    init = [t.double() for t in init]
+    d_col = U32 * (colsum_depth + 3)
+    out = {"dz": dz, "dz_bound": dz_b,
+           "dgamma": init[0] + (dd * xh).sum(0),
+           "dgamma_bound": d_col * ((dd * xh).abs().sum(0) + init[0].abs()) + (dd.abs() * e_x).sum(0),
+           "dbeta": init[1] + dd.sum(0),
+           "dbeta_bound": d_col * (dd.abs().sum(0) + init[1].abs()),
+           "colsum": init[2] + dz.sum(0),
+           # colsum_out sums the kernel's fp32 dz before it is stored: its terms carry dz's fp32 error, not the store's
+           "colsum_bound": d_col * (dz.abs().sum(0) + init[2].abs()) + (dz_b - u * dz.abs() + U32 * dz.abs()).sum(0)}
+    return out
+
+
+def colsum_depth(rows, N, ld, elem_size, num_sms, aligned=True):
+    """Depth of pfn_colsum's column sums (rowwise.cu colsum_dispatch), plus the initial value of out."""
+    if N % 8 == 0 and ld % 8 == 0 and aligned:
+        gx = min(num_sms * 4, _cdiv(rows, 8))
+        if N <= 512:
+            grid = gx
+        else:
+            groups = _cdiv(N, 1024)
+            grid = min((gx * 2) // groups if gx // groups > 0 else 1, _cdiv(rows, 8))
+        return _cdiv(rows, grid * 8) + 8 + grid + 1
+    rows_per_cta = max(64, _cdiv(rows, num_sms * 2))
+    return rows_per_cta + _cdiv(rows, rows_per_cta) + 1
+
+
+def colsum(X, init, depth, block_rows=1 << 16):
+    """Exact init + X.sum(0) and its bound U32 depth (sum|X| + |init|).  The fp64 sums run over blocks of rows, so that
+    a full-size X needs no fp64 copy of itself."""
+    s, a = init.double().clone(), init.double().abs()
+    for r0 in range(0, X.shape[0], block_rows):
+        Xd = X[r0:r0 + block_rows].double()
+        s += Xd.sum(0)
+        a += Xd.abs().sum(0)
+    return s, U32 * depth * a
+
+
+def embed_fwd(x, y, Wx, bx, wy, by, sep, u):
+    """Exact embedding x Wx^T + bx (+ y wy + by on the first sep*B rows), x [rows, F], and its bound
+    u |out| + U32 (F + 2) (|x||Wx|^T + |bx| + |y wy| + |by|)."""
+    xd, yd = x.double(), y.double().reshape(-1, 1)
+    W, b, w, bb = Wx.double(), bx.double(), wy.double().reshape(1, -1), by.double()
+    train = (torch.arange(xd.shape[0], device=xd.device) < sep).double().unsqueeze(1)
+    out = xd @ W.t() + b + train * (yd * w + bb)
+    mag = xd.abs() @ W.abs().t() + b.abs() + train * ((yd * w).abs() + bb.abs())
+    return out, u * out.abs() + U32 * (W.shape[1] + 2) * mag
+
+
+def embed_bwd_depth(rows):
+    """embed_bwd: a thread sums its column over a CTA's 512 rows, then one global atomic per CTA, plus the initial value."""
+    return min(rows, 512) + _cdiv(rows, 512) + 1
+
+
+def embed_bwd(dout, x, y, sep, depth):
+    """Exact dWx, dbx, dwy, dby of the embedding for dout [rows, E] (train rows: the first sep*B), and their bounds."""
+    dd, xd, yd = dout.double(), x.double(), y.double().reshape(-1)
+    t = (torch.arange(dd.shape[0], device=dd.device) < sep).double()
+    d_col = U32 * (depth + 1)
+    return {"dWx": (dd.t() @ xd, d_col * (dd.abs().t() @ xd.abs())),
+            "dbx": (dd.sum(0), d_col * dd.abs().sum(0)),
+            "dwy": ((t * yd) @ dd, d_col * ((t * yd).abs() @ dd.abs())),
+            "dby": (t @ dd, d_col * (t @ dd.abs()))}
+
+
+# bar NLL -----------------------------------------------------------------------------------------------------------
+ICDF_HALF = 0.6744897501960817
+HALF_LOG_2PI = 0.5 * math.log(2.0 * math.pi)
+
+
+def bucket_index(y, borders):
+    """searchsorted-left minus one with the edge fix-ups (bar_distribution.py:19-23), on the inputs' device."""
+    b = borders.double()
+    yd = y.double()
+    idx = torch.searchsorted(b, yd) - 1
+    idx = torch.where(yd == b[0], torch.zeros_like(idx), idx)
+    return torch.where(yd == b[-1], torch.full_like(idx, b.numel() - 2), idx)
+
+
+def bar_nll_fwd(logits, y, borders, full_support):
+    """Exact lse and nll of the bar distribution (log_softmax over the bars, so -inf logits add nothing), and bounds.
+
+    lse: U32 (|lse| + A + ceil(n / 32) + 12), A the row's largest |z - lse| over finite logits: each exp term carries
+    U32 |z - m| from its rounded argument, a lane sums ceil(n / 32) terms, the warp combine and logf a few more.
+    nll: U32 (|z_k| + |lse| + 2 |log w| + 4) plus the lse bound.  The width w = b[k+1] - b[k] and the tails' distance
+    v = b[1] - y / y - b[n-1] are differences of the kernel's fp32 inputs, so fp32 rounds each to within U32 of itself
+    (e_w = e_v = U32) however narrow the bucket is next to its borders.  The tails add U32 (|log s| + 2 + 6 t) +
+    2 t (e_v + e_w) with t = v^2 / (2 s^2) the half-normal's quadratic term."""
+    z = logits.double()
+    n = z.shape[-1]
+    b = borders.double()
+    yd = y.double()
+    lse = torch.logsumexp(z, -1)
+    fin = torch.isfinite(z)
+    A = torch.where(fin, (z - lse.unsqueeze(-1)).abs(), torch.zeros_like(z)).amax(-1)
+    lse_b = U32 * (lse.abs() + A + _cdiv(n, 32) + 12)
+    idx = bucket_index(y, borders)
+    if full_support:
+        idx = idx.clamp(0, n - 1)
+    k = idx.clamp(0, n - 1)
+    w = (b[1:] - b[:-1])[k]
+    e_w = U32
+    zk = z.gather(-1, k.unsqueeze(-1)).squeeze(-1)
+    logp = zk - lse - torch.log(w)
+    bound = U32 * (zk.abs() + lse.abs() + 2.0 * torch.log(w).abs() + 4) + lse_b + e_w
+    if full_support:
+        for side in (0, n - 1):
+            sel = k == side
+            v = (b[1] - yd).clamp_min(1e-8) if side == 0 else yd - b[n - 1]
+            e_v = U32
+            wb = b[side + 1] - b[side]
+            s = wb / ICDF_HALF
+            t = v * v / (2.0 * s * s)
+            hn = math.log(2.0) - torch.log(s) - HALF_LOG_2PI - t
+            logp = torch.where(sel, logp + hn + torch.log(wb), logp)
+            tb = U32 * (torch.log(s).abs() + 2 + 6 * t) + 2 * t * (e_v + e_w) + e_w
+            bound = torch.where(sel, bound + tb, bound)
+    oob = (idx < 0) | (idx >= n)
+    nll = torch.where(oob, torch.full_like(logp, float("nan")), -logp)
+    return {"lse": lse, "lse_bound": lse_b, "nll": nll, "nll_bound": bound, "idx": idx}
+
+
+def bar_nll_bwd(logits, idx, lse, g, u_d):
+    """Exact dlogits = g (exp(x) - onehot(idx)) and its bound, with x = fl32(z - lse) the kernel's own fp32 argument
+    (formed from the lse the forward stored; an IEEE fp32 subtraction, so the device forms the same x).  Taking x as
+    the kernel's input leaves only expf's documented 2 ulp (4 U32 relative), the - 1, the * g and the store:
+    u_d |dl| + U32 |g| (4 p + |p - [c = k]|) + U32 |dl|, relative to each probability, so the small ones are bounded
+    too.  A fast exponential (ex2.approx of x log2 e) adds about U32 |x|, which this bound does not allow."""
+    x = (logits.float() - lse.float().unsqueeze(-1)).double()
+    gd = g.double().unsqueeze(-1)
+    p = torch.exp(x)
+    onehot = torch.zeros_like(p).scatter_(-1, idx.unsqueeze(-1), 1.0)
+    dl = gd * (p - onehot)
+    return dl, (u_d + U32) * dl.abs() + U32 * gd.abs() * (4 * p + (p - onehot).abs())
+
+
+# Adam ---------------------------------------------------------------------------------------------------------------
+def adam_norm_depth(n_chunks):
+    """Depth of the squared-gradient-norm sum: a thread's serial sum over its share of an 8192-element chunk (32 on the
+    scalar path, 8 float4 of four products on the vector one), the warp and CTA butterflies, one atomic per chunk."""
+    return 32 + 4 + 8 + n_chunks + 2
+
+
+def adam_step(p, g, m, v, step, lr, beta1, beta2, eps, weight_decay, clip_norm_sq, max_grad_norm, norm_depth):
+    """Exact fp64 result of one torch.optim.Adam step (after clip_grad_norm_) from the state before it (p, m, v: the
+    kernel's own fp32 values), and bounds.  The hyper-parameters are taken as the kernel's fp32 values.
+
+    clip_norm_sq: exact sum of g^2 over every tensor of the step; the kernel's fp32 norm carries U32 norm_depth
+    relative, so the clip coefficient carries half of it plus a few roundings (e_c).  Within that error of 1 the
+    kernel may clip where the exact coefficient does not, or not clip where it does; e_c covers both.  m: 3 U32 (|b1 m| + |(1-b1) g'|) +
+    (1-b1)|g'| e_c; v likewise.  p: the update's error through m, v and the bias corrections (powf and 1 - b^t:
+    U32 (3 b^t / (1 - b^t) + 2)), then U32 |p_new|."""
+    f = lambda x: float(torch.tensor(x, dtype=torch.float32))
+    lr, beta1, beta2, eps, wd = f(lr), f(beta1), f(beta2), f(eps), f(weight_decay)
+    pd, gd, md, vd = p.double(), g.double(), m.double(), v.double()
+    e_c = 0.0
+    clip = 1.0
+    if max_grad_norm and max_grad_norm > 0:
+        norm = math.sqrt(clip_norm_sq)
+        c = f(max_grad_norm) / (norm + 1e-6)
+        e_norm = U32 * (0.5 * norm_depth + 6)
+        if c < 1.0 + 2 * e_norm:
+            clip = min(c, 1.0)
+            e_c = e_norm
+    gp = gd * clip
+    gp_b = gp.abs() * (e_c + U32)
+    if wd != 0.0:
+        gp = gp + wd * pd
+        gp_b = gp_b + U32 * (wd * pd.abs() + gp.abs())
+    m1 = beta1 * md + (1 - beta1) * gp
+    m_b = 3 * U32 * (beta1 * md.abs() + (1 - beta1) * gp.abs()) + (1 - beta1) * gp_b
+    v1 = beta2 * vd + (1 - beta2) * gp * gp
+    v_b = 4 * U32 * v1 + (1 - beta2) * 2 * gp.abs() * gp_b
+    bc1 = 1 - beta1 ** step
+    bc2s = math.sqrt(1 - beta2 ** step)
+    e_bc1 = U32 * (3 * beta1 ** step / bc1 + 2)
+    e_bc2 = U32 * (3 * beta2 ** step / (1 - beta2 ** step) + 2)
+    sq = torch.sqrt(v1) / bc2s
+    denom = sq + eps
+    step_size = lr / bc1
+    delta = step_size * m1 / denom
+    rel_v = v_b / v1.clamp_min(1e-300)
+    delta_b = step_size / denom * m_b + delta.abs() * (0.5 * (rel_v + e_bc2) * sq / denom + e_bc1 + 6 * U32)
+    p1 = pd - delta
+    return {"p": p1, "p_bound": U32 * p1.abs() + delta_b, "m": m1, "m_bound": m_b + U32 * m1.abs(),
+            "v": v1, "v_bound": v_b}

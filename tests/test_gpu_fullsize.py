@@ -92,7 +92,8 @@ def test_model_fullsize_mask_and_batch_properties(cuda_device):
 
 
 def test_bar_nll_fullsize_matches_oracle(cuda_device):
-    """256000 query rows x 100 bars through pfn_bar_nll_fwd/bwd vs the CPU oracle (which is fast at this size)."""
+    """256000 query rows x 100 bars through pfn_bar_nll_fwd/bwd (the criterion's path) against the fp64 bounds of
+    oracle/error_budget.py, element by element; a slice of rows also against the CPU oracle."""
     torch.manual_seed(14)
     NQ = (T - SEP) * B
     borders = torch.sort(torch.randn(NB + 1)).values
@@ -100,11 +101,20 @@ def test_bar_nll_fullsize_matches_oracle(cuda_device):
     logits = torch.randn(NQ, NB, device=cuda_device, requires_grad=True)
     yq = (torch.randn(NQ, device=cuda_device) * 1.2).clamp(-6, 6)
     nll = crit(logits, yq)
-    ref = O.bar_nll_ref(logits.detach().cpu().double(), yq.cpu().double(), borders.double(), full_support=True)
-    assert (nll.detach().cpu().double() - ref).abs().max().item() <= 1e-4 * (ref.abs().max().item() + 1)
+    bd = crit.borders
+    f = EB.bar_nll_fwd(logits.detach(), yq, bd, True)
+    EB.check("bar_nll nll fullsize", nll.detach(), f["nll"], f["nll_bound"], EB.C_BAR)
+    ref = O.bar_nll_ref(logits.detach()[:4096].cpu().double(), yq[:4096].cpu().double(), borders.double(), full_support=True)
+    assert torch.allclose(f["nll"][:4096].cpu(), ref, rtol=1e-12, atol=1e-12)
+    # the stored lse the backward reads: the same kernel called directly gives the criterion's nll bit for bit
+    nll2, lse = torch.empty(NQ, device=cuda_device), torch.empty(NQ, device=cuda_device)
+    idx = torch.empty(NQ, device=cuda_device, dtype=torch.int64)
+    L.bar_nll_fwd(logits.detach(), yq, bd, NB, True, nll2, idx, lse, torch.zeros(1, device=cuda_device, dtype=torch.int32))
+    assert torch.equal(nll2, nll.detach()) and torch.equal(idx, f["idx"])
+    EB.check("bar_nll lse fullsize", lse, f["lse"], f["lse_bound"], EB.C_BAR)
     nll.mean().backward()
-    # gradient rows sum to zero (softmax minus one-hot, scaled): a size-independent invariant of the backward kernel
-    assert logits.grad.sum(dim=1).abs().max().item() <= 1e-6
+    exact, bound = EB.bar_nll_bwd(logits.detach(), idx, lse, torch.full((NQ,), 1.0 / NQ, device=cuda_device), EB.U32)
+    EB.check("bar_nll dlogits fullsize", logits.grad, exact, bound, EB.C_BAR_GRAD)
 
 
 def test_gp_sampler_fullsize_factor_is_a_cholesky(cuda_device):

@@ -38,12 +38,14 @@ bar_nll_fwd_kernel(const T* __restrict__ logits, int ld, const float* __restrict
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int row = warp; row < rows; row += nwarps) {
     const T* z = logits + static_cast<size_t>(row) * ld;
-    // online log-sum-exp, lanes strided over the bars (coalesced)
+    // online log-sum-exp, lanes strided over the bars (coalesced).  A -inf logit adds nothing (as in log_softmax); it is
+    // skipped so that a lane whose running max is still -inf does not form expf(-inf - -inf) = NaN.  A row of -inf only
+    // gives lse = -inf and a NaN nll, as torch does; a NaN logit still propagates.
     float m = -INFINITY, s = 0.f;
     for (int c = lane; c < n_bars; c += 32) {
       const float v = to_f32<T>(z[c]);
       if (v > m) { s = s * expf(m - v) + 1.0f; m = v; }
-      else s += expf(v - m);
+      else if (v != -INFINITY) s += expf(v - m);
     }
     const float mall = warp_max(m);
     s = (m == -INFINITY) ? 0.f : s * expf(m - mall);
