@@ -271,6 +271,38 @@ int pfn_stroke_render(const pfn_stroke_desc* d, uint32_t seed, const int* cls, c
 int pfn_stroke_raster(const int* segs, const int* nseg, const int* widths, const uint8_t* fill, uint8_t* mask,
                       uint8_t* blurred, int N, int K, int S, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Omniglot few-shot episodes (reference priors/omniglot.py:36-72, datasets/omniglotNshot.py:16-77,172-230).
+ * bank [n_classes, PFN_OMNIGLOT_IMAGES, S, S] uint8 holds the resized grey-level images (Pillow 'L', 255 = background);
+ * pixel value v becomes (float)(1.0 - v / 255.0), the reference's float64 inversion cast to float32.
+ * One CTA per episode b writes x [T, B, S*S] fp32, y [T, B] int64 (label of every position, the query's included) and
+ * target_y [T, B] int64 (-100 except the last row, which equals y), T = n_way * k_shot + 1; the support rows come first
+ * and the query is the last row.
+ *   jonas = 0 (OmniglotNShot) : n_way distinct classes of pool_lo .. pool_lo + pool_n - 1, class j gets label j; per class
+ *     k_shot + 1 distinct images (the last is the query image) and one rot90 turn shared by its images; support rows in a
+ *     uniformly random order; the query is the image of a uniformly chosen class.
+ *   jonas = 1 (OmniglotNShotJonas) : a uniform alphabet a < n_alpha; the classes are characters alpha_start[a] + 0..n_way-1
+ *     in a random order, label = position; support class-major, no rotation.  train = 1: k_shot + 1 distinct images per
+ *     class; train = 0: the support is images 0..k_shot-1 in a random order, the query image is uniform on k_shot..19.
+ *     alpha_start (DEVICE, n_alpha ints) holds the first class of every alphabet of the split; every alphabet has at least
+ *     alpha_min >= n_way characters.
+ *   translate = 1 : every image is shifted by integer (tx, ty), uniform over the shifts that keep its ink (pixels != 255)
+ *     inside the image, with NEAREST sampling and fill 0 (out[r][c] = in[r - ty][c - tx]); an image without ink is not shifted.
+ * Random numbers are counter-based hashes of `seed`.  n_way <= PFN_OMNIGLOT_MAX_WAY, S <= PFN_OMNIGLOT_MAX_SIDE.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_OMNIGLOT_IMAGES = 20, PFN_OMNIGLOT_MAX_WAY = 64, PFN_OMNIGLOT_MAX_SIDE = 105 };
+typedef struct pfn_omniglot_desc {
+  int S;                           /* image side */
+  int n_classes;                   /* classes in the bank */
+  int B;                           /* episodes */
+  int n_way, k_shot, T;            /* T = n_way * k_shot + 1 */
+  int jonas, train, translate;
+  int pool_lo, pool_n;             /* jonas = 0: the class pool */
+  int n_alpha, alpha_min;          /* jonas = 1: alphabets of the split and the size of the smallest */
+} pfn_omniglot_desc;
+int pfn_omniglot_episodes(const pfn_omniglot_desc* d, uint32_t seed, const uint8_t* bank, const int* alpha_start, float* x,
+                          int64_t* y, int64_t* target_y, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -25,5 +25,6 @@ def install_dropin():
     sys.modules["priors.fast_gp_mix"] = importlib.import_module(f"{__name__}.priors.fast_gp_mix")
     sys.modules["priors.mlp"] = importlib.import_module(f"{__name__}.priors.mlp")
     sys.modules["priors.stroke"] = importlib.import_module(f"{__name__}.priors.stroke")
+    sys.modules["priors.omniglot"] = importlib.import_module(f"{__name__}.priors.omniglot")
     sys.modules["priors.utils"] = importlib.import_module(f"{__name__}.priors.utils")
     return {name: sys.modules[name] for name in _DROPIN_MODULES}

@@ -42,6 +42,14 @@ class StrokeDesc(ctypes.Structure):
 STROKE_MAX_STROKES, STROKE_MAX_SIDE = 16, 112
 
 
+class OmniglotDesc(ctypes.Structure):
+    _fields_ = [(n, c_int) for n in ("S", "n_classes", "B", "n_way", "k_shot", "T", "jonas", "train", "translate", "pool_lo",
+                                     "pool_n", "n_alpha", "alpha_min")]
+
+
+OMNIGLOT_IMAGES, OMNIGLOT_MAX_WAY, OMNIGLOT_MAX_SIDE = 20, 64, 105
+
+
 c_double = ctypes.c_double
 
 
@@ -92,6 +100,7 @@ EXPORTED_SYMBOLS = [
     "pfn_dropout", "pfn_dropout_keep_mask",
     "pfn_adam_step", "pfn_adam_chunk_elems",
     "pfn_stroke_geometry", "pfn_stroke_render", "pfn_stroke_raster",
+    "pfn_omniglot_episodes",
 ]
 
 _lib = None
@@ -168,6 +177,7 @@ def load():
     lib.pfn_stroke_render.argtypes = [ctypes.POINTER(StrokeDesc), ctypes.c_uint32, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_int, c_int, c_int, c_void_p]
     lib.pfn_stroke_raster.argtypes = [c_void_p] * 6 + [c_int, c_int, c_int, c_void_p]
+    lib.pfn_omniglot_episodes.argtypes = [ctypes.POINTER(OmniglotDesc), ctypes.c_uint32] + [c_void_p] * 6
     _lib = lib
     return lib
 
@@ -549,3 +559,13 @@ def stroke_raster(segs, nseg, widths, fill, mask, blurred, S):
     N, K, _ = segs.shape
     check(load().pfn_stroke_raster(ptr(segs), ptr(nseg), ptr(widths), ptr(fill), ptr(mask), ptr(blurred), N, K, S,
                                    stream_ptr()), "pfn_stroke_raster")
+
+
+@_guarded
+def omniglot_episodes(desc, seed, bank, alpha_start, x, y, target_y):
+    """x [T, B, S*S] fp32, y / target_y [T, B] int64 <- desc.B episodes drawn from bank [n_classes, 20, S, S] uint8
+    (alpha_start [n_alpha] int32: first class of every alphabet of the split, Jonas mode only)."""
+    _count(1)
+    require_cuda(bank, alpha_start, x, y, target_y)
+    check(load().pfn_omniglot_episodes(ctypes.byref(desc), int(seed) & 0xFFFFFFFF, ptr(bank), ptr(alpha_start), ptr(x), ptr(y),
+                                       ptr(target_y), stream_ptr()), "pfn_omniglot_episodes")

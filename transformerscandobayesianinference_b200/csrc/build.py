@@ -30,6 +30,7 @@ SOURCES = [
     "gp_fit.cu",
     "dropout.cu",
     "stroke_prior.cu",
+    "omniglot_prior.cu",
 ]
 
 NVCC_FLAGS = [
