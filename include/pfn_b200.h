@@ -237,6 +237,64 @@ typedef struct pfn_gp_fit_desc {
 int pfn_gp_fit(const pfn_gp_fit_desc* d, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Fully Bayesian GP baseline (reference priors/fast_gp_mix.py:171-268 get_mcmc_model / evaluate_: pyro NUTS over the Gamma
+ * hyperpriors of the same SingleTaskGP, one chain per prefix).  Problem p = i * B + b samples the posterior of
+ * u = log theta, theta = (ls_1..F, s, noise), given rows < ts[i] of dataset b, with the constant mean fixed at 0:
+ *   U(u) = -log N(y | 0, s k_nu(x, x; ls) + noise I) - sum_k log Gamma(theta_k; a_k, b_k) - sum_k u_k
+ * by NUTS with pyro 1.7's defaults (multinomial sampling, generalised no-U-turn criterion, divergence at an energy error
+ * above 1000, step size found by doubling / halving and adapted by dual averaging to acceptance 0.8, diagonal mass matrix
+ * adapted in Stan's windows, init u ~ U(-2, 2)).  A trial point whose K is not PD has U = +inf (a divergence).
+ * Random numbers are counter-based hashes of (seed, b, ts[i], iteration, draw), never of the CTA index, so a chain is a
+ * pure function of its inputs.  After sampling, the latent predictive of rows ts[i] .. ts[i] + n_pred - 1 (those < T) under
+ * every sample, one factorisation per sample.
+ * One CTA per problem, the limits of pfn_gp_fit: t <= T <= PFN_GP_FIT_MAX_T, F <= PFN_GP_FIT_MAX_F.
+ * warmup_steps = num_samples = 0 with init given only evaluates U and its gradient at init (and the predictive there).
+ * A chain without a finite starting point (init given with U = +inf, or none among 100 uniform draws) is not run: its
+ * samples, predictive, step size, acceptance and gradient are NaN and its potential is +inf.
+ * x [B, T, F], y [B, T] fp32 (DEVICE); ts (HOST) [n_ts]; init (DEVICE, optional) [P, F + 2] values of u.
+ * Outputs (DEVICE), S' = max(num_samples, 1): samples [P, S', F + 2] natural values theta; log_samples (optional) the same
+ * samples as u, exactly as sampled (an evaluate-only call at these u reproduces the predictive bit for bit); mean / var
+ * [P, S', n_pred] (optional, NaN for rows >= T); potential [P] and grad [P, F + 2] (optional) U and dU/du at the chain's last state; step_size [P] (the
+ * step size of the sampling phase); accept [P] mean acceptance statistic of the sampling phase; diag [P, PFN_GP_MCMC_NDIAG];
+ * trace (optional) [P, warmup_steps + num_samples, F + 4]: per iteration, u after it, the step size it used and its tree depth.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_GP_MCMC_MAX_DEPTH = 10 };
+enum {
+  PFN_GP_MCMC_LEAPFROG = 0,        /* leapfrog steps of the NUTS trees (warmup and sampling) */
+  PFN_GP_MCMC_EVALS = 1,           /* potential evaluations of all kinds (trees, step-size searches, init, predictive) */
+  PFN_GP_MCMC_DIV_WARMUP = 2,      /* iterations ended by a divergence, warmup */
+  PFN_GP_MCMC_DIV_SAMPLING = 3,    /* iterations ended by a divergence, sampling */
+  PFN_GP_MCMC_MAX_DEPTH_HITS = 4,  /* iterations that reached max_tree_depth */
+  PFN_GP_MCMC_NOT_PD = 5,          /* evaluations whose K was not positive definite */
+  PFN_GP_MCMC_NDIAG = 6
+};
+typedef struct pfn_gp_mcmc_desc {
+  int B, T, F;
+  const float* x;
+  const float* y;
+  int n_ts;
+  const int* ts;
+  int kernel_type;                       /* PFN_KERNEL_MATERN12 / 32 / 52 */
+  double ls_conc, ls_rate, os_conc, os_rate, noise_conc, noise_rate;
+  int num_samples, warmup_steps;
+  int max_tree_depth;                    /* 1 .. PFN_GP_MCMC_MAX_DEPTH */
+  int n_pred;                            /* predictive rows after the prefix, 1 .. PFN_GP_FIT_MAX_T */
+  uint32_t seed;
+  const double* init;                    /* NULL: u ~ U(-2, 2) */
+  double* samples;
+  double* log_samples;
+  double* mean;
+  double* var;
+  double* potential;
+  double* grad;
+  double* step_size;
+  double* accept;
+  int* diag;
+  double* trace;
+} pfn_gp_mcmc_desc;
+int pfn_gp_mcmc(const pfn_gp_mcmc_desc* d, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Stroke prior (reference priors/stroke.py:9-116): per dataset, C classes of 1..3 random strokes; per image, the strokes of
  * its class drawn with a random width, offset and end-point jitter like PIL's ImageDraw.line, ink filled with U{200..254},
  * ImageFilter.GaussianBlur(0.2), ToTensor (k / 255) and optionally per-image standardisation.

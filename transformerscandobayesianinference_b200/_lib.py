@@ -74,6 +74,26 @@ GP_FIT_MAX_T, GP_FIT_MAX_F = 128, 32
 GP_FIT_CONVERGED, GP_FIT_MAX_ITER, GP_FIT_LINE_SEARCH, GP_FIT_NOT_PD = 0, 1, 2, 3
 
 
+class GpMcmcDesc(ctypes.Structure):
+    _fields_ = [
+        ("B", c_int), ("T", c_int), ("F", c_int),
+        ("x", c_void_p), ("y", c_void_p),
+        ("n_ts", c_int), ("ts", ctypes.POINTER(c_int)),
+        ("kernel_type", c_int),
+        ("ls_conc", c_double), ("ls_rate", c_double), ("os_conc", c_double), ("os_rate", c_double),
+        ("noise_conc", c_double), ("noise_rate", c_double),
+        ("num_samples", c_int), ("warmup_steps", c_int), ("max_tree_depth", c_int), ("n_pred", c_int),
+        ("seed", ctypes.c_uint32),
+        ("init", c_void_p),
+        ("samples", c_void_p), ("log_samples", c_void_p), ("mean", c_void_p), ("var", c_void_p), ("potential", c_void_p), ("grad", c_void_p),
+        ("step_size", c_void_p), ("accept", c_void_p), ("diag", c_void_p), ("trace", c_void_p),
+    ]
+
+
+GP_MCMC_MAX_DEPTH = 10
+GP_MCMC_DIAG_NAMES = ("leapfrog", "evals", "div_warmup", "div_sampling", "max_depth_hits", "not_pd")   # diag columns
+
+
 class AttnDesc(ctypes.Structure):
     _fields_ = [
         ("T", c_int), ("B", c_int), ("H", c_int), ("dh", c_int), ("sep", c_int),
@@ -96,7 +116,7 @@ EXPORTED_SYMBOLS = [
     "pfn_embed_fwd", "pfn_embed_bwd",
     "pfn_layernorm_fwd", "pfn_layernorm_bwd", "pfn_colsum",
     "pfn_bar_nll_fwd", "pfn_bar_nll_bwd", "pfn_bar_bucket_idx",
-    "pfn_gp_sample", "pfn_gp_fit",
+    "pfn_gp_sample", "pfn_gp_fit", "pfn_gp_mcmc",
     "pfn_dropout", "pfn_dropout_keep_mask",
     "pfn_adam_step", "pfn_adam_chunk_elems",
     "pfn_stroke_geometry", "pfn_stroke_render", "pfn_stroke_raster",
@@ -169,6 +189,7 @@ def load():
     lib.pfn_gp_sample.argtypes = [c_void_p] * 5 + [c_float, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                   c_void_p]
     lib.pfn_gp_fit.argtypes = [ctypes.POINTER(GpFitDesc), c_void_p]
+    lib.pfn_gp_mcmc.argtypes = [ctypes.POINTER(GpMcmcDesc), c_void_p]
     lib.pfn_dropout.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_uint32, c_int,
                                 c_void_p]
     lib.pfn_dropout_keep_mask.argtypes = [c_void_p, c_int, c_int, ctypes.c_uint32, c_int, c_void_p]
@@ -528,6 +549,43 @@ def gp_fit(x, y, desc, theta, f, iters, nevals, status, theta0=None, grad=None, 
     desc.var = None if var is None else var.data_ptr()
     desc.iters, desc.nevals, desc.status = iters.data_ptr(), nevals.data_ptr(), status.data_ptr()
     check(load().pfn_gp_fit(ctypes.byref(desc), stream_ptr()), "pfn_gp_fit")
+
+
+def gp_mcmc_desc(B, T, F, ts, kernel_type, hyper, num_samples, warmup_steps, seed, max_tree_depth=GP_MCMC_MAX_DEPTH,
+                 n_pred=1):
+    """Descriptor of a pfn_gp_mcmc call without its device pointers.  hyper = (ls_conc, ls_rate, os_conc, os_rate,
+    noise_conc, noise_rate).  The prefix list is kept alive on the descriptor (it is read on the host)."""
+    d = GpMcmcDesc()
+    d.B, d.T, d.F = int(B), int(T), int(F)
+    d._ts = (c_int * max(len(ts), 1))(*[int(t) for t in ts])
+    d.n_ts, d.ts = len(ts), d._ts
+    d.kernel_type = int(kernel_type)
+    d.ls_conc, d.ls_rate, d.os_conc, d.os_rate, d.noise_conc, d.noise_rate = (float(v) for v in hyper)
+    d.num_samples, d.warmup_steps, d.max_tree_depth = int(num_samples), int(warmup_steps), int(max_tree_depth)
+    d.n_pred = int(n_pred)
+    d.seed = int(seed) & 0xFFFFFFFF
+    return d
+
+
+@_guarded
+def gp_mcmc(x, y, desc, samples, step_size, accept, diag, init=None, log_samples=None, mean=None, var=None, potential=None,
+            grad=None, trace=None):
+    """One launch runs a NUTS chain for every (prefix in desc.ts, dataset) problem.  x [B,T,F], y [B,T] fp32; outputs
+    indexed by problem p = i * B + b: samples / log_samples [P, S', F+2], mean / var [P, S', n_pred], potential [P], grad [P, F+2],
+    step_size / accept [P] fp64, diag [P, 6] int32 (GP_MCMC_DIAG_NAMES), trace [P, W + S, F+4]; S' = max(num_samples, 1)."""
+    _count(1)
+    require_cuda(x, y, samples, step_size, accept, diag, init, log_samples, mean, var, potential, grad, trace)
+    desc.x, desc.y = x.data_ptr(), y.data_ptr()
+    desc.init = None if init is None else init.data_ptr()
+    desc.samples, desc.step_size, desc.accept, desc.diag = (samples.data_ptr(), step_size.data_ptr(), accept.data_ptr(),
+                                                            diag.data_ptr())
+    desc.log_samples = None if log_samples is None else log_samples.data_ptr()
+    desc.mean = None if mean is None else mean.data_ptr()
+    desc.var = None if var is None else var.data_ptr()
+    desc.potential = None if potential is None else potential.data_ptr()
+    desc.grad = None if grad is None else grad.data_ptr()
+    desc.trace = None if trace is None else trace.data_ptr()
+    check(load().pfn_gp_mcmc(ctypes.byref(desc), stream_ptr()), "pfn_gp_mcmc")
 
 
 @_guarded

@@ -28,6 +28,7 @@ SOURCES = [
     "attention_bwd_tc.cu",
     "gp_sampler.cu",
     "gp_fit.cu",
+    "gp_mcmc.cu",
     "dropout.cu",
     "stroke_prior.cu",
     "omniglot_prior.cu",
@@ -40,6 +41,9 @@ NVCC_FLAGS = [
     "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
+
+# per-source additions: the NUTS sampler's arithmetic must be the plain IEEE sequence its CPU restatement performs
+EXTRA_FLAGS = {"gp_mcmc.cu": ["-fmad=false"]}
 
 
 def _nvcc():
@@ -63,7 +67,7 @@ def _stale(src, obj, headers):
 
 
 def _compile(nvcc, src, obj, log_dir):
-    cmd = [nvcc] + NVCC_FLAGS + ["-c", src, "-o", obj]
+    cmd = [nvcc] + NVCC_FLAGS + EXTRA_FLAGS.get(os.path.basename(src), []) + ["-c", src, "-o", obj]
     proc = subprocess.run(cmd, capture_output=True, text=True)
     with open(os.path.join(log_dir, os.path.basename(src) + ".ptxas.log"), "w") as fh:
         fh.write(" ".join(cmd) + "\n" + proc.stdout + proc.stderr)

@@ -9,23 +9,26 @@
 //   ->  K^-1 = L^-T L^-1 into the strict lower triangle + dg  ->  alpha = K^-1 (y - mean)
 //   ->  df = -(1/t) [ 1/2 sum_ij (alpha alpha^T - K^-1)_ij dK_ij + dlog-priors ],  dK recomputed from x (not stored).
 // Every reduction has a fixed order, so a problem's result depends on its own inputs only (bitwise repeatable).
+// The factorisation and the trace terms live in gp_posterior.cuh, shared with the NUTS sampler (gp_mcmc.cu); this file
+// adds the softplus / raw-noise parameterisation, the 1/t scaling and the optimiser.
 #include <math_constants.h>
 
-#include "common.cuh"
-#include "../../include/pfn_b200.h"
+#include "gp_posterior.cuh"
 
 namespace pfn {
 namespace {
 
-constexpr int FT = 256;                        // threads per CTA: a 16 x 16 grid for the triangular sweeps
-constexpr int FW = FT / 32;
+using gp::FT;
+using gp::FW;
+using gp::LOG_2PI;
+using gp::Problem;
+using gp::log_gamma_pdf;
 constexpr int FM = 10;                         // L-BFGS memory (scipy's maxcor default)
 constexpr int FN = PFN_GP_FIT_MAX_F + 3;       // parameters: rho_1..F, rho_s, noise, mean
 constexpr int LS_MAX = 20;                     // evaluations per line search (scipy's maxls)
 constexpr double LS_FTOL = 1e-3, LS_GTOL = 0.9, LS_XTOL = 0.1;   // L-BFGS-B's dcsrch constants
 constexpr double XTRAPL = 1.1, XTRAPU = 4.0, STP_BIG = 1e10;
 constexpr double EPSMCH = 2.220446049250313e-16;
-constexpr double LOG_2PI = 1.8378770664093453;
 
 struct LineSearch {                            // More-Thuente (MINPACK-2 dcsrch) state
   double stp, stpmin, stpmax, finit, ginit, gtest, width, width1;
@@ -54,60 +57,10 @@ enum { LS_FG = 0, LS_CONV = 1, LS_WARN = 2 };
 __device__ __forceinline__ double softplus(double r) { return r > 20.0 ? r : log1p(exp(r)); }       // torch threshold 20
 __device__ __forceinline__ double softplus_grad(double r) { return r > 20.0 ? 1.0 : 1.0 / (1.0 + exp(-r)); }
 
-// k(r) and g(r) = -k'(r) / r of the Matern kernels, from r^2 (g is the factor of dk/dls_d = g Delta_d^2 / ls_d^3)
-__device__ __forceinline__ void matern(double r2, int kt, double& k, double& g) {
-  const double r = sqrt(r2);
-  if (kt == PFN_KERNEL_MATERN12) {
-    const double e = exp(-r);
-    k = e;
-    g = r > 0.0 ? e / r : 0.0;                 // r -> 0 pairs (duplicate rows): the derivative term vanishes
-  } else if (kt == PFN_KERNEL_MATERN32) {
-    const double a = 1.7320508075688772 * r, e = exp(-a);
-    k = (1.0 + a) * e;
-    g = 3.0 * e;
-  } else {
-    const double a = 2.23606797749979 * r, e = exp(-a);
-    k = (1.0 + a + (5.0 / 3.0) * r2) * e;
-    g = (5.0 / 3.0) * (1.0 + a) * e;
-  }
-}
-
-// Fixed-order block sum of K values (every thread receives the same sums).
-template <int K>
-__device__ __forceinline__ void block_sum(double (&v)[K], double* red) {
-#pragma unroll
-  for (int q = 0; q < K; ++q)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0)
-#pragma unroll
-    for (int q = 0; q < K; ++q) red[q * FW + (threadIdx.x >> 5)] = v[q];
-  __syncthreads();
-#pragma unroll
-  for (int q = 0; q < K; ++q) {
-    double s = 0.0;
-#pragma unroll
-    for (int w = 0; w < FW; ++w) s += red[q * FW + w];
-    v[q] = s;
-  }
-}
-
-__device__ __forceinline__ double log_gamma_pdf(double v, double a, double b) {
-  return a * log(b) - lgamma(a) + (a - 1.0) * log(v) - b * v;
-}
-
-struct Problem {
-  const double* xs;                            // [t, F] rows of the dataset
-  const double* ys;                            // [t]
-  int t, F, ld, kt;
-  double ls_a, ls_b, os_a, os_b, nz_a, nz_b;
-};
-
 // f and grad at th (all threads).  Leaves alpha in al and K^-1 in (strict lower of A, dg) when the matrix is PD.
 __device__ void evaluate(const Problem& P, const double* th, double* A, double* dg, double* yc, double* al, Eval& E) {
-  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int t = P.t, F = P.F, ld = P.ld;
+  const int tid = threadIdx.x;
+  const int t = P.t, F = P.F;
   for (int d = tid; d < F; d += FT) {
     const double l = softplus(th[d]);
     E.ls[d] = l;
@@ -121,124 +74,20 @@ __device__ void evaluate(const Problem& P, const double* th, double* A, double* 
     E.c = th[F + 2];
   }
   __syncthreads();
-  const double s = E.s, noise = E.noise, c = E.c;
-  // ---- K, lower triangle
-  for (int r = ty; r < t; r += 16)
-    for (int q = tx; q <= r; q += 16) {
-      double v = s + noise;                    // k(x, x) = 1
-      if (q != r) {
-        double r2 = 0.0;
-        for (int d = 0; d < F; ++d) {
-          const double df = (P.xs[r * F + d] - P.xs[q * F + d]) * E.inv_ls[d];
-          r2 = fma(df, df, r2);
-        }
-        double k, g;
-        matern(r2, P.kt, k, g);
-        v = s * k;
-      }
-      A[r * ld + q] = v;
+  const double s = E.s, noise = E.noise;
+  double sums[6];                              // logdet/2, quad, sum alpha, sum W k, sum W_ii, -
+  const int pd = gp::lml_terms(P, E.inv_ls, s, noise, E.c, A, dg, yc, al, E.red, sums, [&](int d, double v) {
+    if (tid == 0) {
+      const double il = E.inv_ls[d];
+      const double dlogn = 0.5 * s * il * il * il * v;
+      const double dprior = (P.ls_a - 1.0) * il - P.ls_b;
+      E.g[d] = -(dlogn + dprior) * E.dls[d] / t;
     }
-  for (int i = tid; i < t; i += FT) yc[i] = P.ys[i] - c;
-  __syncthreads();
-  // ---- Cholesky, right-looking, one barrier per column: phase j updates the trailing block with the unscaled column j
-  // and scales column j-1 (nobody reads it in phase j)
-  int pd = 1;
-  for (int j = 0; j < t; ++j) {
-    const double dj = A[j * ld + j];
-    if (!(dj > 0.0) || !isfinite(dj)) { pd = 0; break; }        // uniform: every thread read the same pivot
-    const double inv_d = 1.0 / dj;
-    if (tid == 0) dg[j] = sqrt(dj);
-    if (j > 0)
-      for (int r = j + tid; r < t; r += FT) A[r * ld + j - 1] /= dg[j - 1];
-    for (int r = j + 1 + ty; r < t; r += 16) {
-      const double arj = A[r * ld + j] * inv_d;
-      for (int q = j + 1 + tx; q <= r; q += 16) A[r * ld + q] = fma(-arj, A[q * ld + j], A[r * ld + q]);
-    }
-    __syncthreads();
-  }
+  });
   if (!pd) {
     if (tid == 0) { E.f = CUDART_INF; E.pd = 0; }
     __syncthreads();
     return;
-  }
-  double acc0[1] = {tid < t ? log(dg[tid]) : 0.0};   // t <= FT
-  // ---- L^-1 into the upper triangle, transposed: U[j][i] = X[i][j] (i >= j), row k of X final after phase k-1.
-  for (int j = ty; j < t; j += 16)
-    for (int i = j + tx; i < t; i += 16) A[j * ld + i] = (i == j) ? 1.0 : 0.0;
-  __syncthreads();
-  for (int k = 0; k < t; ++k) {
-    const double inv_lkk = 1.0 / dg[k];
-    if (k > 0) {
-      const double inv_prev = 1.0 / dg[k - 1];
-      for (int j = tid; j < k; j += FT) A[j * ld + k - 1] *= inv_prev;
-    }
-    for (int i = k + 1 + tx; i < t; i += 16) {
-      const double lik = A[i * ld + k] * inv_lkk;
-      for (int j = ty; j <= k; j += 16) A[j * ld + i] = fma(-lik, A[j * ld + k], A[j * ld + i]);
-    }
-    __syncthreads();
-  }
-  {
-    const double inv_last = 1.0 / dg[t - 1];
-    for (int j = tid; j < t; j += FT) A[j * ld + t - 1] *= inv_last;
-  }
-  __syncthreads();
-  // ---- K^-1 = X^T X: (r, q), q <= r, = sum_{k >= r} U[r][k] U[q][k]; strict lower -> A, diagonal -> dg
-  for (int r = ty; r < t; r += 16)
-    for (int q = tx; q <= r; q += 16) {
-      double v = 0.0;
-      for (int k = r; k < t; ++k) v = fma(A[r * ld + k], A[q * ld + k], v);
-      if (q == r) dg[r] = v; else A[r * ld + q] = v;
-    }
-  __syncthreads();
-  // ---- alpha = K^-1 (y - c)
-  for (int i = tid; i < t; i += FT) {
-    double v = 0.0;
-    for (int j = 0; j < t; ++j) {
-      const double kij = j < i ? A[i * ld + j] : (j > i ? A[j * ld + i] : dg[i]);
-      v = fma(kij, yc[j], v);
-    }
-    al[i] = v;
-  }
-  __syncthreads();
-  // ---- gradient, pass 1: W = alpha alpha^T - K^-1; sum W k (outputscale), sum_i W_ii (noise); P = 2 W g -> upper triangle
-  double sums[6] = {acc0[0], 0.0, 0.0, 0.0, 0.0, 0.0};    // logdet/2, quad, sum alpha, sum W k, sum W_ii, -
-  for (int i = tid; i < t; i += FT) {
-    sums[1] = fma(yc[i], al[i], sums[1]);
-    sums[2] += al[i];
-    const double wii = fma(al[i], al[i], -dg[i]);
-    sums[3] += wii;
-    sums[4] += wii;
-  }
-  for (int r = ty; r < t; r += 16)
-    for (int q = tx; q < r; q += 16) {
-      double r2 = 0.0;
-      for (int d = 0; d < F; ++d) {
-        const double df = (P.xs[r * F + d] - P.xs[q * F + d]) * E.inv_ls[d];
-        r2 = fma(df, df, r2);
-      }
-      double k, g;
-      matern(r2, P.kt, k, g);
-      const double w = fma(al[r], al[q], -A[r * ld + q]);
-      sums[3] = fma(2.0 * w, k, sums[3]);
-      A[q * ld + r] = 2.0 * w * g;
-    }
-  block_sum(sums, E.red);
-  // ---- pass 2: per input dimension, sum P Delta_d^2
-  for (int d = 0; d < F; ++d) {
-    double v[1] = {0.0};
-    for (int r = ty; r < t; r += 16)
-      for (int q = tx; q < r; q += 16) {
-        const double df = P.xs[r * F + d] - P.xs[q * F + d];
-        v[0] = fma(A[q * ld + r], df * df, v[0]);
-      }
-    block_sum(v, E.red);
-    if (tid == 0) {
-      const double il = E.inv_ls[d];
-      const double dlogn = 0.5 * s * il * il * il * v[0];
-      const double dprior = (P.ls_a - 1.0) * il - P.ls_b;
-      E.g[d] = -(dlogn + dprior) * E.dls[d] / t;
-    }
   }
   if (tid == 0) {
     double logn = -0.5 * sums[1] - sums[0] - 0.5 * t * LOG_2PI;
@@ -251,36 +100,6 @@ __device__ void evaluate(const Problem& P, const double* th, double* A, double* 
     E.pd = 1;
   }
   __syncthreads();
-}
-
-// Latent predictive at xstar after an evaluation (all threads): mean = c + k*^T alpha, var = s - k*^T K^-1 k*.
-__device__ void predict(const Problem& P, const double* xstar, const double* A, const double* dg, const double* al,
-                        double* ks, Eval& E, double& mean, double& var) {
-  const int tid = threadIdx.x, t = P.t, F = P.F, ld = P.ld;
-  for (int i = tid; i < t; i += FT) {
-    double r2 = 0.0;
-    for (int d = 0; d < F; ++d) {
-      const double df = (P.xs[i * F + d] - xstar[d]) * E.inv_ls[d];
-      r2 = fma(df, df, r2);
-    }
-    double k, g;
-    matern(r2, P.kt, k, g);
-    ks[i] = E.s * k;
-  }
-  __syncthreads();
-  double v[2] = {0.0, 0.0};
-  for (int i = tid; i < t; i += FT) {
-    double u = 0.0;
-    for (int j = 0; j < t; ++j) {
-      const double kij = j < i ? A[i * ld + j] : (j > i ? A[j * ld + i] : dg[i]);
-      u = fma(kij, ks[j], u);
-    }
-    v[0] = fma(ks[i], al[i], v[0]);
-    v[1] = fma(ks[i], u, v[1]);
-  }
-  block_sum(v, E.red);
-  mean = E.c + v[0];
-  var = E.s - v[1];
 }
 
 // ------------------------------------------------------------------------------------------------ line search
@@ -589,7 +408,7 @@ __global__ void __launch_bounds__(FT, 1) gp_fit_kernel(const FitArgs args) {
     evaluate(P, S.x, A, dg, yc, al, E);       // alpha and K^-1 of the returned point (also its f and gradient)
   }
   double mean = CUDART_NAN, var = CUDART_NAN;
-  if (predict_row && E.pd) predict(P, xstar, A, dg, al, ks, E, mean, var);
+  if (predict_row && E.pd) gp::predict(P, E.inv_ls, E.s, E.c, xstar, A, dg, al, ks, E.red, mean, var);
   if (tid == 0) {
     for (int i = 0; i < n; ++i) {
       D.theta[p * n + i] = S.x[i];
@@ -602,10 +421,6 @@ __global__ void __launch_bounds__(FT, 1) gp_fit_kernel(const FitArgs args) {
     D.nevals[p] = S.nfev;
     D.status[p] = S.status;
   }
-}
-
-size_t fit_smem(int tmax, int F) {
-  return (static_cast<size_t>(tmax) * (tmax | 1) + static_cast<size_t>(tmax) * F + 6 * tmax + F) * sizeof(double);
 }
 
 }  // namespace
@@ -644,11 +459,11 @@ extern "C" int pfn_gp_fit(const pfn_gp_fit_desc* d, void* stream) {
       const int tt = a.slot_t[j]; a.slot_t[j] = a.slot_t[j - 1]; a.slot_t[j - 1] = tt;
       const int ii = a.slot_i[j]; a.slot_i[j] = a.slot_i[j - 1]; a.slot_i[j - 1] = ii;
     }
-  const size_t smem = fit_smem(a.slot_t[0], d->F);
+  const size_t smem = gp::problem_smem(a.slot_t[0], d->F);
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))
     PFN_CUDA_OK(cudaFuncSetAttribute(gp_fit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     static_cast<int>(fit_smem(PFN_GP_FIT_MAX_T, PFN_GP_FIT_MAX_F))));
+                                     static_cast<int>(gp::problem_smem(PFN_GP_FIT_MAX_T, PFN_GP_FIT_MAX_F))));
   gp_fit_kernel<<<d->B * d->n_ts, FT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
   PFN_LAUNCH_OK();
   return 0;

@@ -10,6 +10,11 @@ the hyper-prior restatement is validated distributionally — parity unpinned, s
 The fitted-hyperparameter baseline (`get_model`, `get_fitted_model`, `evaluate`; reference :24-55, :156-169) restates
 botorch's MAP fit (SingleTaskGP + Gamma priors + fit_gpytorch_model) as csrc/gp_fit.cu: one CTA per (dataset, prefix)
 problem runs the whole L-BFGS fit in fp64 and forms the predictive, all problems of a call in one launch (t <= 128).
+
+The fully Bayesian baseline (`get_mcmc_model`, `get_mean_logdensity`, `evaluate_`; reference :171-302) integrates the
+same hyperparameters out by NUTS: csrc/gp_mcmc.cu runs one chain per (dataset, prefix) problem with pyro 1.7's NUTS
+defaults, on the posterior given the prefix (the reference's pyro model registers no observation site; see DESIGN §4),
+and forms the predictive of row t under every sample, all chains of a call in one launch (t <= 128).
 """
 import math
 import random
@@ -333,3 +338,225 @@ def evaluate(x, y, y_non_noisy, use_mse=False, hyperparameters={}, get_model_on_
         losses = -pred.log_prob(y_t.unsqueeze(-1))
     means_list += losses.mean(1).tolist()
     return losses.float().to('cpu'), torch.tensor(means_list).to('cpu'), time.time() - start
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# fully Bayesian GP baseline (reference :171-268 get_mcmc_model / get_mean_logdensity / evaluate_, :274-302 __main__)
+# ----------------------------------------------------------------------------------------------------------------------
+MCMC_NUM_SAMPLES, MCMC_WARMUP_STEPS, MCMC_MAX_TREE_DEPTH = 100, 300, L.GP_MCMC_MAX_DEPTH
+
+
+def _mcmc_seed(seed):
+    """The chains' counter-RNG seed: the caller's, or one draw of torch's CPU generator (reproducible under
+    torch.manual_seed, no device sync)."""
+    return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if seed is None else int(seed)
+
+
+@torch.no_grad()
+def sample_posterior(x, y, ts, hyperparameters=None, num_samples=MCMC_NUM_SAMPLES, warmup_steps=MCMC_WARMUP_STEPS,
+                     seed=None, init=None, max_tree_depth=MCMC_MAX_TREE_DEPTH, trace=False, n_pred=1):
+    """One pfn_gp_mcmc launch: a NUTS chain for every (prefix t in ts, dataset b), x [B,T,F], y [B,T] on a CUDA device.
+    Returns a dict of tensors with leading dims [len(ts), B]: samples [.., S', F+2] (lengthscales, outputscale, noise),
+    log_samples (the same as u = log theta), mean / var [.., S'] (latent predictive of row t per sample, NaN where
+    t == T; [.., S', n_pred] for rows t .. t + n_pred - 1 when n_pred > 1), potential and grad [.., F+2] (U and dU/du at the last state), step_size, accept (mean acceptance statistic
+    of the sampling phase), diag [.., 6] int32 (columns L.GP_MCMC_DIAG_NAMES), and "seed".  S' = max(num_samples, 1).
+    init [len(ts), B, F+2] gives the starting u; num_samples = warmup_steps = 0 then only evaluates U, its gradient and
+    the predictive at init.  A chain without a finite starting point is not run: its samples and predictive are NaN.
+    trace=True adds "trace" [.., W+S, F+4]: per iteration u, the step size used and the tree
+    depth."""
+    Bn, T, F = x.shape
+    if T > MAX_FIT_T:
+        raise ValueError(f"the GP sampler keeps the t x t matrix in shared memory: T={T} exceeds the limit of {MAX_FIT_T}")
+    dev = _fit_device(x.device)
+    kt, prior, _ = _fit_settings(hyperparameters)
+    seed = _mcmc_seed(seed)
+    P, So = len(ts) * Bn, max(int(num_samples), 1)
+    f64 = dict(dtype=torch.float64, device=dev)
+    out = {"samples": torch.empty(P, So, F + 2, **f64), "log_samples": torch.empty(P, So, F + 2, **f64),
+           "mean": torch.empty(P, So, n_pred, **f64), "var": torch.empty(P, So, n_pred, **f64),
+           "potential": torch.empty(P, **f64),
+           "grad": torch.empty(P, F + 2, **f64), "step_size": torch.empty(P, **f64), "accept": torch.empty(P, **f64),
+           "diag": torch.empty(P, len(L.GP_MCMC_DIAG_NAMES), dtype=torch.int32, device=dev)}
+    if trace:
+        out["trace"] = torch.empty(P, int(warmup_steps) + int(num_samples), F + 4, **f64)
+    desc = L.gp_mcmc_desc(Bn, T, F, ts, kt, prior, num_samples, warmup_steps, seed, max_tree_depth, n_pred)
+    u0 = None if init is None else init.to(dev, torch.float64).reshape(P, F + 2).contiguous()
+    L.gp_mcmc(x.to(dev, torch.float32).contiguous(), y.to(dev, torch.float32).contiguous(), desc, out["samples"],
+              out["step_size"], out["accept"], out["diag"], init=u0, log_samples=out["log_samples"], mean=out["mean"],
+              var=out["var"], potential=out["potential"], grad=out["grad"], trace=out.get("trace"))
+    if n_pred == 1:
+        out["mean"], out["var"] = out["mean"][..., 0], out["var"][..., 0]
+    r = {k: v.view(len(ts), Bn, *v.shape[1:]) for k, v in out.items()}
+    r["seed"] = seed
+    return r
+
+
+class _SampleNoiseLikelihood:
+    """likelihood(f) of a sample-batched predictive: adds every sample's own noise (gpytorch GaussianLikelihood on the
+    batch of GPs pyro_load_from_samples builds).  noise [..., S] against mean / variance [..., S, m]."""
+
+    def __init__(self, noise):
+        self.noise = noise
+
+    def eval(self):
+        return self
+
+    def __call__(self, f):
+        return fast_gp._Predictive(f.mean, f.variance + self.noise.to(f.variance.dtype).unsqueeze(-1))
+
+
+class MCMCGP:
+    """The batch of S GPs the reference loads from the NUTS samples (pyro_load_from_samples), on train_x [B,t,F],
+    train_y [B,t].  Calling it on test inputs [m,F] (or [B,m,F]) returns the latent predictive of every sample,
+    mean / variance [S,m] (or [B,S,m]), formed by the sampling kernel in evaluate-only mode at the exact sampled u (one
+    launch, one factorisation per sample for all m points), so it agrees bitwise with the predictive `evaluate_` forms."""
+
+    def __init__(self, train_x, train_y, r, hyperparameters, batched):
+        self.train_x, self.train_y, self.hyperparameters, self.batched = train_x, train_y, hyperparameters, batched
+        F = train_x.shape[-1]
+        self.samples, self.log_samples = r["samples"], r["log_samples"]          # [B, S, F+2]
+        self.lengthscale = self.samples[..., :F]
+        self.outputscale = self.samples[..., F]
+        self.noise = self.samples[..., F + 1]
+        self.step_size, self.accept, self.diag, self.seed = r["step_size"], r["accept"], r["diag"], r["seed"]
+
+    def eval(self):
+        return self
+
+    def train(self, mode=True):
+        return self
+
+    @torch.no_grad()
+    def __call__(self, x):
+        Bn, t, F = self.train_x.shape
+        S = self.samples.shape[1]
+        xs = x.to(self.train_x.device, torch.float32).reshape(Bn, -1, F)
+        m = xs.shape[1]
+        if t + m > MAX_FIT_T:
+            raise ValueError(f"the GP sampler keeps the data and the test points in shared memory: t + m = {t + m} "
+                             f"exceeds the limit of {MAX_FIT_T}")
+        xcat = torch.cat([self.train_x.to(torch.float32), xs], 1).repeat_interleave(S, 0).contiguous()   # q = b * S + s
+        ycat = torch.cat([self.train_y.to(torch.float32), torch.zeros(Bn, m, device=xs.device)], 1)
+        init = self.log_samples.reshape(1, Bn * S, F + 2)
+        r = sample_posterior(xcat, ycat.repeat_interleave(S, 0).contiguous(), [t], self.hyperparameters, 0, 0, seed=0,
+                             init=init, n_pred=m)
+        mean, var = r["mean"][0, :, 0].reshape(Bn, S, m), r["var"][0, :, 0].reshape(Bn, S, m)
+        if not self.batched:
+            mean, var = mean[0], var[0]
+        return fast_gp._Predictive(mean, var)
+
+
+@torch.no_grad()
+def get_mcmc_model(x, y, hyperparameters, device, num_samples, warmup_steps, seed=None):
+    """(model, likelihood) after one NUTS chain per dataset (reference :171-196): x [t,F] and y [t] as the reference
+    passes them, or a batch x [B,t,F], y [B,t].  The model is the batch of GPs at the S samples (MCMCGP), the
+    likelihood adds each sample's noise."""
+    _check_fit_args(hyperparameters)
+    dev = _fit_device(device)
+    batched = x.dim() == 3
+    xb = (x if batched else x.unsqueeze(0)).to(dev, torch.float32).contiguous()
+    yb = (y if batched else y.unsqueeze(0)).to(dev, torch.float32).reshape(xb.shape[0], xb.shape[1]).contiguous()
+    r = sample_posterior(xb, yb, [xb.shape[1]], hyperparameters, num_samples, warmup_steps, seed=seed)
+    r = {k: (v[0] if torch.is_tensor(v) else v) for k, v in r.items()}
+    model = MCMCGP(xb, yb, r, hyperparameters, batched)
+    noise = model.noise if batched else model.noise[0]
+    return model, _SampleNoiseLikelihood(noise)
+
+
+def _mixture_logdensity(mean, var, y, full_range=None):
+    """log of the equal-weight Gaussian mixture over the last dim of mean / var at y (broadcast over the rest), each
+    component renormalised to full_range when given (reference :203-217)."""
+    dist = torch.distributions.Normal(mean, var.sqrt())
+    logprobs = dist.log_prob(y.unsqueeze(-1))
+    if full_range is not None:
+        used_weight = 1. - (dist.cdf(torch.tensor(full_range[0])) + (1. - dist.cdf(torch.tensor(full_range[1]))))
+        if torch.isinf(-torch.log(used_weight)).any() or torch.isinf(torch.log(used_weight)).any():
+            print('factor is inf', -torch.log(used_weight))
+        logprobs = logprobs - torch.log(used_weight)
+    return torch.logsumexp(logprobs, -1) - math.log(logprobs.shape[-1])
+
+
+def get_mean_logdensity(dists, x, full_range=None):
+    """Log density at x of the equal-weight mixture of the predictives in `dists` (reference :203-217)."""
+    means = torch.cat([d.mean.squeeze() for d in dists], 0)
+    vars = torch.cat([d.variance.squeeze() for d in dists], 0)
+    assert len(means.shape) == 1 and len(vars.shape) == 1
+    return _mixture_logdensity(means, vars, torch.as_tensor(x, dtype=means.dtype, device=means.device), full_range)
+
+
+def _report_mcmc(diag, samples):
+    n_dead = int(torch.isnan(samples[..., 0, 0]).sum())
+    if n_dead:
+        print(f"fast_gp_mix.evaluate_: {n_dead} chains found no finite starting point and were not run (NaN losses)")
+    n_div = int(diag[..., L.GP_MCMC_DIAG_NAMES.index("div_sampling")].sum())
+    n_depth = int(diag[..., L.GP_MCMC_DIAG_NAMES.index("max_depth_hits")].sum())
+    if n_div or n_depth:
+        print(f"fast_gp_mix.evaluate_: {diag.shape[0] * diag.shape[1]} chains: {n_div} sampling iterations diverged, "
+              f"{n_depth} iterations (warmup included) hit the tree-depth cap")
+
+
+@torch.no_grad()
+def evaluate_(x, y, y_non_noisy, hyperparameters=None, device=default_device, num_samples=MCMC_NUM_SAMPLES,
+              warmup_steps=MCMC_WARMUP_STEPS, full_range=None, min_seq_len=0, use_likelihood=False, seed=None):
+    """Fully Bayesian GP baseline (reference :220-268): for each t >= max(min_seq_len, 1) and dataset b, NUTS on rows < t
+    of x [T,B,F], y [T,B], then minus the log density of y[t, b] under the mixture of the S sample predictives (with each
+    sample's noise when use_likelihood).  Returns (losses_after_t [n_t (+1)], seconds, all_losses) like the reference:
+    the per-t mean losses with a leading 0 when min_seq_len == 0, and the per-(t, b) losses as lists.
+
+    Every (t, b) chain runs in ONE launch; `seed` (default: drawn from torch's CPU generator) fixes all chains, so the
+    result equals a per-t loop over `get_mcmc_model(x[:t].transpose(0, 1), ...)` with the same seed."""
+    start_time = time.time()
+    hps = hyperparameters or {}
+    _check_fit_args(hps)
+    T = len(x)
+    if T > MAX_FIT_T:
+        raise ValueError(f"fast_gp_mix.evaluate_ keeps the t x t matrix of every chain in shared memory: T={T} exceeds "
+                         f"the limit of {MAX_FIT_T}")
+    dev = _fit_device(device)
+    losses_after_t = [.0] if min_seq_len == 0 else []
+    ts = list(range(max(min_seq_len, 1), T))
+    if not ts:
+        return torch.tensor(losses_after_t), time.time() - start_time, []
+    xb = x.to(dev, torch.float32).transpose(0, 1).contiguous()
+    yb = y.to(dev, torch.float32).transpose(0, 1).contiguous()
+    r = sample_posterior(xb, yb, ts, hps, num_samples, warmup_steps, seed=seed)
+    _report_mcmc(r["diag"], r["samples"])
+    F = xb.shape[-1]
+    var = r["var"] + r["samples"][..., F + 1] if use_likelihood else r["var"]
+    losses = -_mixture_logdensity(r["mean"], var, y[ts].to(dev, torch.float64), full_range)     # [n_t, B]
+    all_losses = losses.tolist()
+    losses_after_t += losses.mean(1).tolist()
+    return torch.tensor(losses_after_t), time.time() - start_time, all_losses
+
+
+if __name__ == '__main__':
+    import argparse
+
+    parser = argparse.ArgumentParser()
+    parser.add_argument('--batch_size', type=int)
+    parser.add_argument('--seq_len', type=int)
+    parser.add_argument('--min_seq_len', type=int, default=0)
+    parser.add_argument('--warmup_steps', type=int)
+    parser.add_argument('--num_samples', type=int)
+    parser.add_argument('--min_y', type=int)
+    parser.add_argument('--max_y', type=int)
+    parser.add_argument('--dim', type=int, default=1)
+    parser.add_argument('--use_likelihood', default=True, type=bool)
+    parser.add_argument('--device', default='cuda')
+    parser.add_argument('--outputscale_concentraion', default=2., type=float)
+    parser.add_argument('--noise_concentration', default=1.1, type=float)
+    parser.add_argument('--noise_rate', default=.05, type=float)
+
+    args = parser.parse_args()
+
+    print('min_y:', args.min_y)
+    full_range = (None if args.min_y is None else (args.min_y, args.max_y))
+
+    # fast_computations only switches gpytorch's approximate solves, which this exact fp64 path does not have
+    hps = {'outputscale_concentration': args.outputscale_concentraion, 'noise_concentration': args.noise_concentration,
+           'noise_rate': args.noise_rate, 'fast_computations': (False, False, False)}
+    x, y, _ = get_batch(args.batch_size, args.seq_len, args.dim, device=args.device, fix_to_range=full_range,
+                        hyperparameters=hps)
+    print('RESULT:', evaluate_(x, y, y, device=args.device, warmup_steps=args.warmup_steps,
+                               num_samples=args.num_samples, full_range=full_range, min_seq_len=args.min_seq_len,
+                               hyperparameters=hps, use_likelihood=args.use_likelihood))
