@@ -48,6 +48,11 @@ C_EMBED = 2.0         # embedding forward (worst 0.996, bf16 out)
 C_BAR = 1.1           # bar-NLL lse and nll (worst 0.521, nll; lse 0.330)
 C_BAR_GRAD = 2.0      # bar-NLL dlogits (worst 0.996, bf16 dlogits; 0.487 fp32)
 C_ADAM = 2.0          # Adam p, m, v and the squared gradient norm (worst 0.998, p; m 0.40, v 0.52, norm 0.040)
+# GP sampler (gp_sampler.cu): L L^T - K against U32 (min(i, j) + 3) |L||L|^T + E_K, and y - L z against U32 (33 +
+# ceil((r + 1) / 32)) |L||z| (the kernel's own L).  The factor's first rows meet its bound nearly term for term
+# (L_00^2 = fl(os + fl(noise + jitter)) through one sqrtf), so its ratio approaches 1; the draw's long sums stay well below.
+C_GP_FACTOR = 1.8     # worst 0.850 (T = 1000, F = 128, Matern-5/2, TR = 128)
+C_GP_Y = 0.6          # worst 0.259 (cfg 2 at full size)
 
 
 def check(name, got, exact, bound, c, verbose=True):
@@ -494,3 +499,149 @@ def adam_step(p, g, m, v, step, lr, beta1, beta2, eps, weight_decay, clip_norm_s
     p1 = pd - delta
     return {"p": p1, "p_bound": U32 * p1.abs() + delta_b, "m": m1, "m_bound": m_b + U32 * m1.abs(),
             "v": v1, "v_bound": v_b}
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# GP prior sampler (csrc/gp_sampler.cu): K = os k(x, x; ls) + (noise + jitter) I evaluated in fp32, its left-looking
+# blocked fp32 Cholesky L (panel width 32) and y = L z.  Kernel types as in _lib.KERNEL_*.
+# ------------------------------------------------------------------------------------------------------------------
+GP_RBF, GP_MATERN12, GP_MATERN32, GP_MATERN52 = 0, 1, 2, 3
+GP_PANEL = 32
+
+
+def _f32(v):
+    return float(torch.tensor(v, dtype=torch.float32))
+
+
+def _is_f32(t):
+    return t.float().double() == t
+
+
+def _exact_add(a, b):
+    """The fp64 sum or difference of two fp32 values is exact when their magnitudes lie within 2^28 of each other."""
+    aa, bb = a.abs(), b.abs()
+    return (aa == 0) | (bb == 0) | ((aa <= bb * 2.0 ** 28) & (bb <= aa * 2.0 ** 28))
+
+
+def gp_kernel(x, ls, os_, noise, jitter, kernel_type):
+    """Exact K + jitter I [B, T, T] from the kernel's fp32 inputs (x [B, T, F], ls [B, F], os_ [B], noise [B], jitter as
+    the fp32 value the kernel receives), and an elementwise bound E_K on the kernel's fp32 evaluation of it.
+
+    gp_kernel_value and its caller round il = 1/ls, x il (each relative U32), their difference, and d2 through an F-term
+    fmaf chain.  Per feature s = (x_r - x_c) il is formed with error U32 (2|s| + a), a = (|x_r| + |x_c|) il: where the two
+    products nearly cancel it is relative to a, not to s.  So d2 is within
+        E_d2 = U32 ((F + 4) d2 + 2 sum_f |s_f| a_f) + U32^2 sum_f (2|s_f| + a_f)^2.
+    The Matern kernels take r = sqrtf(d2): r moves by at most min(sqrt(E_d2), E_d2 / (sqrt(d2) + sqrt(d2 - E_d2))) plus
+    sqrtf's own U32 r.  The rounded constants (sqrt 3, sqrt 5, 5/3 in fp32) move a = c r and the polynomial; each
+    is carried into k by k's derivative.  expf is good to 2 ulp (4 U32 relative), and the products with os and the
+    polynomial round once each.  Where expf's result is subnormal its error is absolute: (2 os p + 1/2) 2^-149.
+    The diagonal is fl(os + fl(noise + jitter))."""
+    xd, ld = x.double(), ls.double()
+    B, T, F = xd.shape
+    jit = _f32(jitter)
+    d2 = torch.zeros(B, T, T, dtype=torch.float64, device=xd.device)
+    s1 = torch.zeros_like(d2)
+    s2 = torch.zeros_like(d2)
+    # Where every intermediate of d2 (il, x il, the difference, its square, each partial sum) is an fp32 value and each
+    # fp64 step forming it is exact, every fp32 rounding of the kernel is exact too, in whatever order or fusion: d2 has
+    # no error there (dyadic x and lengthscales), which leaves expf and the constants alone in the bound
+    exact = torch.ones(B, T, T, dtype=torch.bool, device=xd.device)
+    acc = torch.zeros_like(d2)
+    for f in range(F):
+        il = (1.0 / ld[:, f]).view(B, 1, 1)
+        ilf = (1.0 / ls[:, f].float()).double()
+        xf = xd[:, :, f]
+        s = (xf.unsqueeze(2) - xf.unsqueeze(1)) * il
+        a = (xf.abs().unsqueeze(2) + xf.abs().unsqueeze(1)) * il
+        d2 += s * s
+        s1 += s.abs() * a
+        s2 += (2.0 * s.abs() + a) ** 2
+        xi = xf * ilf.view(B, 1)
+        ok = (ilf * ld[:, f] == 1.0).view(B, 1) & _is_f32(xi)
+        sf = xi.unsqueeze(2) - xi.unsqueeze(1)
+        sq = sf * sf
+        nxt = acc + sq
+        exact &= (ok.unsqueeze(2) & ok.unsqueeze(1) & _exact_add(xi.unsqueeze(2), xi.unsqueeze(1)) & _is_f32(sf)
+                  & _is_f32(sq) & _exact_add(acc, sq) & _is_f32(nxt))
+        acc = nxt
+    e_d2 = (U32 * ((F + 4) * d2 + 2.0 * s1) + U32 * U32 * s2).masked_fill(exact, 0.0)
+    del s1, s2, acc, exact
+    osv = os_.double().view(B, 1, 1)
+    if kernel_type == GP_RBF:
+        k = torch.exp(-0.5 * d2)
+        poly = torch.ones_like(d2)
+        e_k = k * (torch.expm1(0.5 * e_d2) + 5 * U32)
+    else:
+        r = torch.sqrt(d2)
+        far = d2 > e_d2
+        e_r = torch.where(far, e_d2 / (r + (d2 - e_d2).clamp_min(0.0).sqrt()).masked_fill(~far, 1.0), e_d2.sqrt()) + U32 * r
+        if kernel_type == GP_MATERN12:
+            k = torch.exp(-r)
+            poly = torch.ones_like(d2)
+            e_k = k * (torch.expm1(e_r) + 5 * U32)
+        else:
+            c = math.sqrt(3.0) if kernel_type == GP_MATERN32 else math.sqrt(5.0)
+            cf = _f32(c)
+            a = c * r
+            e_a = abs(cf - c) * r + cf * e_r + U32 * cf * (r + e_r)
+            ea = torch.exp(-a)
+            if kernel_type == GP_MATERN32:
+                poly = 1.0 + a
+                k = poly * ea
+                # (1 + a) e^-a: derivative a e^-a; 1 + a, os *, * expf round once each, expf 4 U32
+                e_k = ea * torch.exp(e_a) * a * e_a + 7 * U32 * k
+            else:
+                b = 5.0 / 3.0 * d2
+                poly = 1.0 + a + b
+                k = poly * ea
+                # (1 + a + b) e^-a moves with d2 through a and b at once: dk/dd2 = -e^-a (5/6 + 5 sqrt5 r / 6), finite at
+                # r = 0.  The rounded constants and sqrtf move a (derivative (a + b) e^-a) and b (e^-a) on their own; the
+                # polynomial rounds at most 2 U32 p
+                e_a0 = abs(cf - c) * r + U32 * cf * 2.0 * r
+                e_b0 = abs(_f32(5.0 / 3.0) - 5.0 / 3.0) * d2
+                dk = 5.0 / 6.0 + 5.0 * c / 6.0 * (r + e_r)
+                e_k = ea * torch.exp(e_a) * (dk * e_d2 + (a + b) * e_a0 + e_b0) + 8 * U32 * k
+    K = osv * k
+    E_K = osv * e_k + (2.0 * osv * poly + 0.5) * 2.0 ** -149
+    eye = torch.eye(T, dtype=torch.bool, device=xd.device)
+    nj = noise.double().view(B, 1, 1) + jit
+    diag = osv + nj
+    K = torch.where(eye, diag, K)
+    E_K = torch.where(eye, U32 * (nj.abs() + diag.abs()), E_K)
+    return K, E_K
+
+
+def gp_factor(work, T):
+    """The factor L [B, T, T] from the kernel's work buffer (work[b][c][r] = L[r][c], rows padded to ldw).  Entries above
+    the diagonal outside the 32 x 32 diagonal blocks are never written: tril."""
+    return torch.tril(work[:, :, :T].transpose(1, 2))
+
+
+def gp_factor_residual(Lf, E_K):
+    """L L^T in fp64 and its bound about the exact K + jitter I: |L L^T - K|_ij <= U32 d_ij (|L||L|^T)_ij + E_K,ij with
+    d_ij = min(i, j) + 3.  For j = min(i, j), L_ij comes out of one sequential fp32 sum of K^_ij and j products: the c0
+    products of the finished panels in the update's fmaf chain (c0 roundings), K^ - acc (one), the j - c0 products of
+    the panel in the warp Cholesky or the row solve (one fmaf each); then L_ij = s * fl(1 / L_jj) (two roundings), s / L_jj
+    (one) or sqrtf(s) (two on L_jj^2).  Pushing every rounding onto the products and L_ij L_jj (Higham, Lemma 8.4) leaves
+    K^_ij exact and at most j + 3 relative errors on each term of sum_k<=j L_ik L_jk.  K^ itself is within E_K of K.
+    A product or quotient that lands among the subnormals carries an absolute error of up to 2^-150 instead, once per
+    rounding and scaled by L_jj where it is pushed onto L_ij L_jj: 2^-149 d_ij (1 + max(L_ii, L_jj))."""
+    Ld = Lf.double()
+    T = Ld.shape[-1]
+    i = torch.arange(T, device=Ld.device)
+    d = (torch.minimum(i.unsqueeze(1), i.unsqueeze(0)) + 3).double()
+    La = Ld.abs()
+    dg = torch.diagonal(La, dim1=-2, dim2=-1)
+    floor = 2.0 ** -149 * d * (1.0 + torch.maximum(dg.unsqueeze(-1), dg.unsqueeze(-2)))
+    return Ld @ Ld.transpose(-1, -2), U32 * d * (La @ La.transpose(-1, -2)) + E_K + floor
+
+
+def gp_draw(Lf, z):
+    """Exact y = L z from the kernel's own factor L [B, T, T] and z [B, T], and its bound
+    U32 (32 + ceil((r + 1) / 32) + 1) sum_c |L_rc||z_c|: row r is one 32-term fmaf dot per panel it meets
+    (ceil((r + 1) / 32) of them) added into y[r] in panel order."""
+    Ld, zd = Lf.double(), z.double().unsqueeze(-1)
+    T = Ld.shape[-1]
+    r = torch.arange(T, device=Ld.device)
+    d = (GP_PANEL + (r + GP_PANEL) // GP_PANEL + 1).double()
+    return (Ld @ zd).squeeze(-1), U32 * d * (Ld.abs() @ zd.abs()).squeeze(-1)

@@ -384,12 +384,18 @@ def test_gp_sample_matches_lapack(cuda_device, kernel, code, Bn, T, F, noise):
     work = torch.empty(Bn, T, ldw, device=dev)
     info = torch.full((Bn,), -1, device=dev, dtype=torch.int32)
     L.gp_sample(x, z, ls, os_, nz, 0.0, code, y, work, info)
-    yr, Lr = O.gp_sample_ref(x.cpu().double(), z.cpu().double(), ls.cpu().double(), os_.cpu().double(), nz.cpu().double(), kernel)
     assert info.tolist() == [0] * Bn
-    Lg = torch.tril(work[:, :, :T].transpose(1, 2).cpu().double())     # the kernel keeps the factor transposed
-    K = O.gp_kernel_ref(x.cpu().double(), ls.cpu().double(), os_.cpu().double(), nz.cpu().double(), kernel)
-    resid = (Lg @ Lg.transpose(-1, -2) - K).abs().max().item()
-    assert resid <= 2e-5 * K.abs().max().item(), f"L L^T residual {resid}"
+    Lg = EB.gp_factor(work, T)                  # the kernel keeps the factor transposed
+    assert (torch.diagonal(Lg, dim1=1, dim2=2) > 0).all()
+    K, E_K = EB.gp_kernel(x, ls, os_, nz, 0.0, code)
+    LLt, bound = EB.gp_factor_residual(Lg, E_K)
+    EB.check(f"gp factor {kernel} T={T}", LLt, K, bound, EB.C_GP_FACTOR)
+    ye, yb = EB.gp_draw(Lg, z)
+    EB.check(f"gp y {kernel} T={T}", y, ye, yb, EB.C_GP_Y)
+    # the oracle's kernel matrix and LAPACK's draw (well conditioned here: noise >= 0.05)
+    Kr = O.gp_kernel_ref(x.cpu().double(), ls.cpu().double(), os_.cpu().double(), nz.cpu().double(), kernel)
+    assert torch.allclose(K.cpu(), Kr, rtol=1e-12, atol=1e-15)
+    yr, Lr = O.gp_sample_ref(x.cpu().double(), z.cpu().double(), ls.cpu().double(), os_.cpu().double(), nz.cpu().double(), kernel)
     assert (y.cpu().double() - yr).abs().max().item() <= 5e-3 * yr.abs().max().item()
 
 

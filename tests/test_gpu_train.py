@@ -7,7 +7,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from transformerscandobayesianinference_b200 import bar_distribution, encoders, priors, train as train_mod, utils
-from oracle import pfn_oracle as O
+from oracle import error_budget as EB, pfn_oracle as O
 
 
 def test_fast_gp_get_batch_contract_and_covariance(cuda_device):
@@ -49,11 +49,13 @@ def test_gp_sampler_factorises_the_cfg2_kernel_without_jitter(cuda_device, Bn):
         L.gp_sample(x, z, ls, os_, nz, 0.0, 0, y, work, info)
         assert int((info != 0).sum()) == 0, f"seed {seed}: failing pivots {info[info != 0][:8].tolist()}"
         assert torch.isfinite(y).all()
-        if seed == 0:        # L L^T reproduces the kernel matrix (work holds the factor transposed: work[b][c][r] = L[r][c])
-            Lf = work[:4].transpose(1, 2).tril().double()
-            d = (x[:4, :, None, 0] - x[:4, None, :, 0]).double() / 0.6
-            K = torch.exp(-0.5 * d * d) + 1e-4 * torch.eye(T, device=cuda_device, dtype=torch.float64)
-            assert (Lf @ Lf.transpose(1, 2) - K).abs().max().item() < 2e-5
+        if seed == 0:        # L L^T reproduces the kernel matrix element by element (oracle/error_budget.py)
+            Lf = EB.gp_factor(work[:4], T)
+            K, E_K = EB.gp_kernel(x[:4], ls[:4], os_[:4], nz[:4], 0.0, L.KERNEL_RBF)
+            LLt, bound = EB.gp_factor_residual(Lf, E_K)
+            EB.check(f"gp factor cfg2 Bn={Bn}", LLt, K, bound, EB.C_GP_FACTOR)
+            ye, yb = EB.gp_draw(Lf, z[:4])
+            EB.check(f"gp y cfg2 Bn={Bn}", y[:4], ye, yb, EB.C_GP_Y)
 
 
 def test_fast_gp_notebook_hyperparameters_are_factorisable(cuda_device):
