@@ -361,6 +361,69 @@ typedef struct pfn_omniglot_desc {
 int pfn_omniglot_episodes(const pfn_omniglot_desc* d, uint32_t seed, const uint8_t* bank, const int* alpha_start, float* x,
                           int64_t* y, int64_t* target_y, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Bayesian-NN prior (reference priors/pyro.py:10-34 over mcmc_svi_transformer_on_bayesian.py:28-67 BayesianModel): per
+ * dataset b, theta = (W1 [E, F], b1 [E], W2 [2, E], b2 [2]) ~ N(0, 1) (d = E F + 3 E + 2 values in that order), x [T, F] ~
+ * N(0, 1), logits = W2 (W1 x + b1) + b2 (no nonlinearity between the layers, as in the reference), class ~ softmax(logits)
+ * (class 0 when u < p_0 for u ~ U[0, 1)), then x standardised over the sequence axis per dataset and feature
+ * ((x - mean) / (unbiased std + 1e-6)).  One CTA per dataset.  The normals are fp32 values; logits, softmax and the
+ * statistics of the standardisation are formed from them in fp64.  Random numbers are counter-based hashes of
+ * (seed, dataset_offset + b, counters): dataset b of a batch equals a one-dataset call with dataset_offset = b bit for bit.
+ * x [T, B, F] fp32, y [T, B] fp32 (0. / 1.).  The oracle hook, all optional (NULL on the product path): weights [B, d] fp32,
+ * x_raw [T, B, F] fp32 (x before the standardisation), u [T, B] fp64 (the uniform of every class draw).
+ * d <= PFN_BNN_MAX_D; T * F fp32 values must fit in shared memory beside theta (an error otherwise).
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_BNN_MAX_D = 1024 };
+int pfn_bnn_prior(uint32_t seed, int dataset_offset, int B, int T, int F, int E, float* x, float* y, float* weights,
+                  float* x_raw, double* u, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * NUTS baseline of the Bayesian NN (reference mcmc_svi_transformer_on_bayesian.py:249-267 eval_mcmc: one pyro NUTS chain per
+ * dataset).  Chain b samples the posterior of theta (layout above, all sites N(0, 1), so unconstrained) given the n training
+ * rows of dataset b:
+ *   U(theta) = 1/2 |theta|^2 + d/2 log 2 pi - sum_r log softmax(W2 (W1 x_r + b1) + b2)[y_r]
+ * with the algorithm, constants and random-number keys of pfn_gp_mcmc (keys (seed, b, n, iteration, draw)).  One CTA per
+ * chain; every d-vector of the sampler (79 of them, the trial point always in shared memory: chain state, trajectory ends, the per-level stack of complete subtrees,
+ * the mass-matrix accumulators) lives in dynamic shared memory when it fits and otherwise in `workspace`, which the caller
+ * allocates: pfn_bnn_mcmc_workspace returns the doubles needed PER CHAIN (0 when shared memory holds the state, -1 for an
+ * invalid descriptor); workspace then has N times that many doubles and need not be initialised.  All arithmetic is fp64.
+ * After sampling, the class-1 probability of each of the n_test rows under every kept sample.
+ * warmup_steps = num_samples = 0 with init given only evaluates U and its gradient (and the probabilities) at init.
+ * num_samples = 0 with warmup_steps > 0 runs the warmup only: the one output row of samples (and of probs / obs) is the
+ * state the warmup ended in, and accept is NaN.
+ * A chain whose starting point has no finite potential is not run: its outputs are NaN and its potential +inf.
+ * x_train [N, n, F], y_train [N, n] (0. / 1.), x_test [N, n_test, F] fp32 (DEVICE; x_test may be NULL when n_test = 0);
+ * init (DEVICE, optional) [N, d].  Outputs (DEVICE), S' = max(num_samples, 1): samples [N, S', d]; probs (optional)
+ * [N, S', n_test]; obs (optional) [N, S', n_test] fp32: one class (0. / 1.) drawn per sample and row from probs, with the
+ * chain's keys at iteration warmup_steps + num_samples + 1 (what pyro's predictive returns as 'obs'); potential [N] and grad [N, d] (optional) at the chain's last state; step_size, accept [N];
+ * diag [N, PFN_GP_MCMC_NDIAG] (the counters of pfn_gp_mcmc; NOT_PD counts evaluations whose U was not finite);
+ * trace (optional) [N, warmup_steps + num_samples, d + 2]: per iteration theta after it, the step size used, the tree depth.
+ * d <= PFN_BNN_MAX_D, n <= PFN_BNN_MAX_N.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_BNN_MAX_N = 1024, PFN_BNN_MCMC_VECTORS = 79 };
+typedef struct pfn_bnn_mcmc_desc {
+  int N, n, n_test, F, E;
+  const float* x_train;
+  const float* y_train;
+  const float* x_test;
+  int num_samples, warmup_steps;
+  int max_tree_depth;                    /* 1 .. PFN_GP_MCMC_MAX_DEPTH */
+  uint32_t seed;
+  const double* init;                    /* NULL: theta ~ U(-2, 2) */
+  double* samples;
+  double* probs;
+  float* obs;
+  double* potential;
+  double* grad;
+  double* step_size;
+  double* accept;
+  int* diag;
+  double* trace;
+  double* workspace;                     /* [N, pfn_bnn_mcmc_workspace(d)] doubles; NULL when that is 0 */
+} pfn_bnn_mcmc_desc;
+int pfn_bnn_mcmc_workspace(const pfn_bnn_mcmc_desc* d);
+int pfn_bnn_mcmc(const pfn_bnn_mcmc_desc* d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

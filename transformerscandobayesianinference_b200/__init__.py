@@ -27,4 +27,6 @@ def install_dropin():
     sys.modules["priors.stroke"] = importlib.import_module(f"{__name__}.priors.stroke")
     sys.modules["priors.omniglot"] = importlib.import_module(f"{__name__}.priors.omniglot")
     sys.modules["priors.utils"] = importlib.import_module(f"{__name__}.priors.utils")
+    sys.modules["priors.pyro"] = importlib.import_module(f"{__name__}.priors.pyro")
+    sys.modules["mcmc_svi_transformer_on_bayesian"] = importlib.import_module(f"{__name__}.mcmc_svi_transformer_on_bayesian")
     return {name: sys.modules[name] for name in _DROPIN_MODULES}

@@ -94,6 +94,21 @@ GP_MCMC_MAX_DEPTH = 10
 GP_MCMC_DIAG_NAMES = ("leapfrog", "evals", "div_warmup", "div_sampling", "max_depth_hits", "not_pd")   # diag columns
 
 
+class BnnMcmcDesc(ctypes.Structure):
+    _fields_ = [
+        ("N", c_int), ("n", c_int), ("n_test", c_int), ("F", c_int), ("E", c_int),
+        ("x_train", c_void_p), ("y_train", c_void_p), ("x_test", c_void_p),
+        ("num_samples", c_int), ("warmup_steps", c_int), ("max_tree_depth", c_int),
+        ("seed", ctypes.c_uint32),
+        ("init", c_void_p),
+        ("samples", c_void_p), ("probs", c_void_p), ("obs", c_void_p), ("potential", c_void_p), ("grad", c_void_p),
+        ("step_size", c_void_p), ("accept", c_void_p), ("diag", c_void_p), ("trace", c_void_p), ("workspace", c_void_p),
+    ]
+
+
+BNN_MAX_D, BNN_MAX_N = 1024, 1024
+
+
 class AttnDesc(ctypes.Structure):
     _fields_ = [
         ("T", c_int), ("B", c_int), ("H", c_int), ("dh", c_int), ("sep", c_int),
@@ -121,6 +136,7 @@ EXPORTED_SYMBOLS = [
     "pfn_adam_step", "pfn_adam_chunk_elems",
     "pfn_stroke_geometry", "pfn_stroke_render", "pfn_stroke_raster",
     "pfn_omniglot_episodes",
+    "pfn_bnn_prior", "pfn_bnn_mcmc_workspace", "pfn_bnn_mcmc",
 ]
 
 _lib = None
@@ -199,6 +215,9 @@ def load():
                                       c_int, c_int, c_int, c_void_p]
     lib.pfn_stroke_raster.argtypes = [c_void_p] * 6 + [c_int, c_int, c_int, c_void_p]
     lib.pfn_omniglot_episodes.argtypes = [ctypes.POINTER(OmniglotDesc), ctypes.c_uint32] + [c_void_p] * 6
+    lib.pfn_bnn_prior.argtypes = [ctypes.c_uint32] + [c_int] * 5 + [c_void_p] * 6
+    lib.pfn_bnn_mcmc_workspace.argtypes = [ctypes.POINTER(BnnMcmcDesc)]
+    lib.pfn_bnn_mcmc.argtypes = [ctypes.POINTER(BnnMcmcDesc), c_void_p]
     _lib = lib
     return lib
 
@@ -627,3 +646,48 @@ def omniglot_episodes(desc, seed, bank, alpha_start, x, y, target_y):
     require_cuda(bank, alpha_start, x, y, target_y)
     check(load().pfn_omniglot_episodes(ctypes.byref(desc), int(seed) & 0xFFFFFFFF, ptr(bank), ptr(alpha_start), ptr(x), ptr(y),
                                        ptr(target_y), stream_ptr()), "pfn_omniglot_episodes")
+
+
+@_guarded
+def bnn_prior(x, y, seed, E, dataset_offset=0, weights=None, x_raw=None, u=None):
+    """x [T, B, F] fp32, y [T, B] fp32 <- B datasets of the Bayesian-NN prior with E hidden units.  The oracle hook:
+    weights [B, E F + 3 E + 2] fp32, x_raw [T, B, F] fp32 (before the standardisation), u [T, B] fp64 (class uniforms)."""
+    _count(1)
+    require_cuda(x, y, weights, x_raw, u)
+    T, B, F = x.shape
+    check(load().pfn_bnn_prior(int(seed) & 0xFFFFFFFF, int(dataset_offset), B, T, F, int(E), ptr(x), ptr(y), ptr(weights),
+                               ptr(x_raw), ptr(u), stream_ptr()), "pfn_bnn_prior")
+
+
+def bnn_mcmc_desc(N, n, n_test, F, E, num_samples, warmup_steps, seed, max_tree_depth=GP_MCMC_MAX_DEPTH):
+    """Descriptor of a pfn_bnn_mcmc call without its device pointers."""
+    d = BnnMcmcDesc()
+    d.N, d.n, d.n_test, d.F, d.E = int(N), int(n), int(n_test), int(F), int(E)
+    d.num_samples, d.warmup_steps, d.max_tree_depth = int(num_samples), int(warmup_steps), int(max_tree_depth)
+    d.seed = int(seed) & 0xFFFFFFFF
+    return d
+
+
+def bnn_mcmc_workspace(desc):
+    """Doubles of global workspace every chain of `desc` needs (0: the sampler state fits in shared memory)."""
+    w = int(load().pfn_bnn_mcmc_workspace(ctypes.byref(desc)))
+    if w < 0:
+        check(1, "pfn_bnn_mcmc_workspace")
+    return w
+
+
+@_guarded
+def bnn_mcmc(x_train, y_train, x_test, desc, samples, step_size, accept, diag, init=None, probs=None, obs=None,
+             potential=None, grad=None, trace=None, workspace=None):
+    """One launch runs a NUTS chain for every dataset.  x_train [N,n,F], y_train [N,n], x_test [N,n_test,F] fp32; outputs
+    indexed by dataset: samples [N, S', d], probs [N, S', n_test] fp64, obs [N, S', n_test] fp32 (classes drawn from probs), potential [N], grad [N, d], step_size / accept [N] fp64,
+    diag [N, 6] int32 (GP_MCMC_DIAG_NAMES), trace [N, W + S, d + 2]; workspace [N, bnn_mcmc_workspace(desc)] fp64."""
+    _count(1)
+    require_cuda(x_train, y_train, x_test, samples, step_size, accept, diag, init, probs, obs, potential, grad, trace, workspace)
+    desc.x_train, desc.y_train, desc.x_test = x_train.data_ptr(), y_train.data_ptr(), ptr(x_test)
+    desc.init = ptr(init)
+    desc.samples, desc.step_size, desc.accept, desc.diag = (samples.data_ptr(), step_size.data_ptr(), accept.data_ptr(),
+                                                            diag.data_ptr())
+    desc.probs, desc.obs, desc.potential, desc.grad = ptr(probs), ptr(obs), ptr(potential), ptr(grad)
+    desc.trace, desc.workspace = ptr(trace), ptr(workspace)
+    check(load().pfn_bnn_mcmc(ctypes.byref(desc), stream_ptr()), "pfn_bnn_mcmc")

@@ -32,6 +32,8 @@ SOURCES = [
     "dropout.cu",
     "stroke_prior.cu",
     "omniglot_prior.cu",
+    "bnn_prior.cu",
+    "bnn_mcmc.cu",
 ]
 
 NVCC_FLAGS = [
@@ -42,8 +44,8 @@ NVCC_FLAGS = [
     "-Xptxas", "-v",
 ]
 
-# per-source additions: the NUTS sampler's arithmetic must be the plain IEEE sequence its CPU restatement performs
-EXTRA_FLAGS = {"gp_mcmc.cu": ["-fmad=false"]}
+# per-source additions: the NUTS samplers' arithmetic must be the plain IEEE sequence their CPU restatement performs
+EXTRA_FLAGS = {"gp_mcmc.cu": ["-fmad=false"], "bnn_mcmc.cu": ["-fmad=false"]}
 
 
 def _nvcc():
