@@ -36,6 +36,10 @@ C_GEMM = 2.0          # GEMM results and epilogues (worst 0.99)
 # The wgmma GEMMs reach 0.014 of it (fp32 output, K = 192; 0.008 at K = 512, 5e-4 at K = 2560, 8e-5 at K = 12800); the
 # SIMT GEMM 0.17 (K = 17..300, three k-splits reduced by fp32 atomics)
 C_ACC_TC = 0.03
+# The engine's wgmma weight gradients sum over tokens whose products share a sign, so their partial sums grow with K and
+# the accumulator's rounding errors, which have one sign (as from truncation), do not cancel: they reach 0.066 of
+# U32 K |A||B| (in-projection wgrad, K = 640 tokens), against 0.014 for zero-mean random operands
+C_ACC_WGRAD = 0.15
 C_ACC_SIMT = 0.35
 # Row kernels (rowwise.cu, bar_nll.cu, optimizer.cu).  Their fp32 sums are bounded by the depth of the kernel's reduction
 # tree (a sum whose longest path adds d terms is within U32 d sum|x| of the exact sum): a worst case that random data
@@ -53,6 +57,12 @@ C_ADAM = 2.0          # Adam p, m, v and the squared gradient norm (worst 0.998,
 # (L_00^2 = fl(os + fl(noise + jitter)) through one sqrtf), so its ratio approaches 1; the draw's long sums stay well below.
 C_GP_FACTOR = 1.8     # worst 0.850 (T = 1000, F = 128, Matern-5/2, TR = 128)
 C_GP_Y = 0.6          # worst 0.259 (cfg 2 at full size)
+# Engine stages (tests/test_gpu_engine_stages.py).  The elementwise dropout stores in the activation dtype, so its
+# rounding alone reaches 1; the ROWDOT sums and the fused v-third bias gradient are worst cases random data reach a
+# small fraction of.
+C_DROPOUT = 2.0       # dropout (+ residual), forward and backward masking (worst 0.996, bf16 out; fp32 0.968)
+C_ROWDOT = 0.07       # GEMM ROWDOT epilogue, the attention backward's delta (worst 0.031, kernel test; engine 0.027)
+C_BIAS_FUSED = 0.05   # in-projection bias gradient, v third formed as colsum(dz1) W_out (worst 0.024, cfg 3)
 
 
 def check(name, got, exact, bound, c, verbose=True):
@@ -131,7 +141,7 @@ def rising_max_qkv(T, B, H, dh, generator=None, device=None):
     return x.reshape(T * B, 3 * E).to(device=device, dtype=torch.bfloat16)
 
 
-def attention_bwd(f, dout, out_kernel):
+def attention_bwd(f, dout, out_kernel, delta_kernel=None):
     """Exact dQ, dK, dV (token-major [T*B, E] each) of the forward `f` for the upstream gradient dout, and their bounds.
 
     dS = P (dP - delta) with dP = keep drop_scale dO V^T and delta_i = dO_i . out_i.  The kernel rounds P and dS to the
@@ -140,7 +150,9 @@ def attention_bwd(f, dout, out_kernel):
       dQ: scale (unit |dS|~ |K| + e_delta P |K|)
       dK: scale (|dS|~^T (unit |Q|) + P^T (e_delta |Q|))
     where e_delta,i = |dO_i . (out_kernel - out_exact)_i| is the error the kernel inherits by forming delta from the
-    output it stored (not a rounding of its own, so it is not scaled by u)."""
+    output it stored (not a rounding of its own, so it is not scaled by u).  delta_kernel: a token-major [T*B, H] delta
+    handed to the kernel precomputed (the GEMM ROWDOT epilogue); its own deviation |delta_kernel - dO . out_kernel| from
+    the delta of the stored output adds to e_delta."""
     T, B, H, dh = f["T"], f["B"], f["H"], f["dh"]
     scale, P, Ph, q, k, v = f["scale"], f["P"], f["Ph"], f["q"], f["k"], f["v"]
     unit = f["unit"].unsqueeze(-1)
@@ -151,7 +163,11 @@ def attention_bwd(f, dout, out_kernel):
     delta = (do * out).sum(-1, keepdim=True)
     dS = P * (dP - delta)
     dS_mag = P * (dP.abs() + delta.abs())
-    e_delta = (do * (_heads(out_kernel.double(), T, B, H, dh) - out)).sum(-1, keepdim=True).abs()
+    out_k = _heads(out_kernel.double(), T, B, H, dh)
+    e_delta = (do * (out_k - out)).sum(-1, keepdim=True).abs()
+    if delta_kernel is not None:
+        dk_ = delta_kernel.double().reshape(T, B, H).permute(1, 2, 0).unsqueeze(-1)
+        e_delta = e_delta + (dk_ - (do * out_k).sum(-1, keepdim=True)).abs()
     dq = scale * (dS @ k)
     dk = scale * (dS.transpose(-1, -2) @ q)
     dv = Ph.transpose(-1, -2) @ do
@@ -349,6 +365,61 @@ def colsum(X, init, depth, block_rows=1 << 16):
         s += Xd.sum(0)
         a += Xd.abs().sum(0)
     return s, U32 * depth * a
+
+
+def dropout(x, keep, thr, residual=None, u_out=U):
+    """Exact x keep s (+ residual) of the elementwise dropout kernel (dropout.cu), s = 256 / (256 - thr) in fp64: the
+    kernel's contract is probability thr / 256 at that scale (not the reference's p).  The kernel multiplies by
+    fl32(s) and rounds in fp32, adds the residual in fp32 and stores: |fl32(s) - s| |x| keep + U32 (|x| s keep + |val|)
+    + u_out |val|."""
+    xd, kd = x.double(), keep.double()
+    s = 256.0 / (256.0 - thr)
+    s32 = _f32(s)
+    kept = xd.abs() * kd
+    val = xd * kd * s
+    if residual is not None:
+        val = val + residual.double()
+    return val, u_out * val.abs() + U32 * (kept * s + val.abs()) + abs(s32 - s) * kept
+
+
+def rowdot_depth(width, block_n=128):
+    """Longest addition chain of a ROWDOT sum (gemm_tc.cu epi_pair / the epilogue's quad shuffles): a lane's fmaf chain
+    over its block_n / 4 columns of one tile, two shuffles, one atomic per tile of the group, the zeroed initial value."""
+    return block_n // 4 + 2 + _cdiv(width, block_n) + 1
+
+
+def rowdot(C, aux, width):
+    """Exact sum over each group of `width` columns of C aux, with C the GEMM's stored (bf16) output, and its bound
+    U32 depth sum |C aux| (the products of two bf16 values are exact in fp32; only the additions round).  A last
+    group narrower than width sums the columns that exist."""
+    M, N = C.shape
+    prod = C.double() * aux.double()
+    groups = _cdiv(N, width)
+    pad = groups * width - N
+    if pad:
+        prod = torch.nn.functional.pad(prod, (0, pad))
+    prod = prod.view(M, groups, width)
+    return prod.sum(-1), U32 * rowdot_depth(width) * prod.abs().sum(-1)
+
+
+def bias_v_fused(dattn, da, out_w, colsum_out, ln_b, c_acc):
+    """Bound of the in-projection bias gradient's v third when it is formed as colsum_out W_out (fp32) instead of the
+    column sums of dV.  The exact value is sum_i dO_i over the stored dO = dattn (the rows of P sum to 1), so the bound
+    collects how far colsum_out W_out may be from it:
+      U sum_i |dattn_i| + c_acc U32 E sum_i |da_i| |W_bf16|   the bf16 rounding and fp32 accumulation of the dgrad
+      U |colsum_out| |W|                                      the dgrad read bf16(W), the product reads the fp32 master
+      (colsum_bound + sum_i dz_bound_i) |W|                   colsum_out (the LayerNorm backward's fp32 sums of dz)
+                                                              against the column sums of the stored dz = da
+      U32 E |colsum_out| |W|                                  the fp32 matrix-vector product
+    with W = out_w [E_out, E_in] (fp32 master) and ln_b the layernorm_bwd bounds of that LayerNorm."""
+    W = out_w.double()
+    Wa = W.abs()
+    Wb = out_w.to(torch.bfloat16).double().abs()
+    E = W.shape[0]
+    cs = colsum_out.double().abs()
+    inh = ln_b["colsum_bound"] + ln_b["dz_bound"].sum(0)
+    return (U * dattn.double().abs().sum(0) + c_acc * U32 * E * (da.double().abs().sum(0) @ Wb)
+            + (U * cs + inh + U32 * E * cs) @ Wa)
 
 
 def embed_fwd(x, y, Wx, bx, wy, by, sep, u):

@@ -26,13 +26,15 @@ def test_keep_mask_statistics_and_elementwise_kernel(cuda_device):
         for dt in (torch.float32, torch.bfloat16):
             x = torch.randn(4096, 512, device=dev).to(dt)
             r = torch.randn(4096, 512, device=dev).to(dt)
+            u = EB.U32 if dt == torch.float32 else EB.U
             out = torch.empty_like(x)
             L.dropout(x, out, 1234, thr, residual=r)
-            want = (x.float() * keep * (256.0 / (256 - thr)) + r.float()).to(dt)
-            assert torch.equal(out, want) or (out.float() - want.float()).abs().max().item() <= 1e-2 * want.float().abs().max().item()
+            exact, bound = EB.dropout(x, m, thr, r, u)
+            EB.check(f"dropout + residual p={p} {dt}", out, exact, bound, EB.C_DROPOUT)
             y = x.clone()
             L.dropout(y, y, 1234, thr)                                                                  # in place, no residual
-            assert torch.allclose(y.float(), (x.float() * keep * (256.0 / (256 - thr))).to(dt).float(), rtol=1e-2, atol=1e-3)
+            exact, bound = EB.dropout(x, m, thr, None, u)
+            EB.check(f"dropout in place p={p} {dt}", y, exact, bound, EB.C_DROPOUT)
 
 
 @pytest.mark.parametrize("p", [0.2, 0.5])

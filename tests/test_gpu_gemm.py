@@ -99,8 +99,8 @@ def test_gemm_tc_rowdot(cuda_device, M, N, K, b_mn):
     rd = torch.zeros(M, N // width, device=cuda_device, dtype=torch.float32)
     L.gemm(A, B, C, b_mn_major=b_mn, aux=aux, epilogue=L.EPI_ROWDOT, rowdot=(rd, width), M=M, N=N, K=K, use_tc=True)
     _check("gemm rowdot C", C, A, B, b_mn=b_mn)                                           # aux is NOT added to C
-    want = (C.float() * aux.float()).view(M, N // width, width).sum(-1)                  # exact w.r.t. the stored C
-    assert (rd - want).abs().max().item() <= 1e-4 * want.abs().max().item() + 1e-4
+    exact, bound = EB.rowdot(C, aux, width)                                              # exact w.r.t. the stored C
+    EB.check("gemm rowdot", rd, exact, bound, EB.C_ROWDOT)
     with pytest.raises(Exception):                                                       # group width must be a multiple of 128
         L.gemm(A, B, C, b_mn_major=b_mn, aux=aux, epilogue=L.EPI_ROWDOT, rowdot=(rd, 64), M=M, N=N, K=K, use_tc=True)
 
