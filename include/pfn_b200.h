@@ -249,6 +249,8 @@ int pfn_gp_fit(const pfn_gp_fit_desc* d, void* stream);
  * every sample, one factorisation per sample.
  * One CTA per problem, the limits of pfn_gp_fit: t <= T <= PFN_GP_FIT_MAX_T, F <= PFN_GP_FIT_MAX_F.
  * warmup_steps = num_samples = 0 with init given only evaluates U and its gradient at init (and the predictive there).
+ * num_samples = 0 with warmup_steps > 0 runs the warmup only: the one output row is the state the warmup ended in
+ * (samples = exp(u), log_samples = u), the predictive is formed at that state, and accept is NaN.
  * A chain without a finite starting point (init given with U = +inf, or none among 100 uniform draws) is not run: its
  * samples, predictive, step size, acceptance and gradient are NaN and its potential is +inf.
  * x [B, T, F], y [B, T] fp32 (DEVICE); ts (HOST) [n_ts]; init (DEVICE, optional) [P, F + 2] values of u.

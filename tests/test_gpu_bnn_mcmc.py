@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from oracle import bnn_oracle as O
+from oracle.gp_mcmc_oracle import nuts_chain
 from transformerscandobayesianinference_b200 import _lib as L
 from transformerscandobayesianinference_b200 import mcmc_svi_transformer_on_bayesian as M
 from transformerscandobayesianinference_b200.priors import pyro as P
@@ -53,8 +54,11 @@ def test_potential_and_gradient_match_the_oracle(cuda_device, FE, n):
         assert (r["probs"][b, 0] - p1).abs().max().item() <= 1e-12
 
 
-@pytest.mark.parametrize("FE,n,depth,chains", [(SMALL, 10, 10, 6), (SMALL, 10, 2, 6), (BIG, 20, 4, 4), (BIG, 20, 2, 4)])
-def test_trajectories_follow_the_cpu_restatement(cuda_device, FE, n, depth, chains):
+@pytest.mark.parametrize("FE,n,depth,chains,from_init", [
+    pytest.param(SMALL, 10, 10, 6, False, id="FE0-10-10-6"), pytest.param(SMALL, 10, 2, 6, False, id="FE1-10-2-6"),
+    pytest.param(BIG, 20, 4, 4, False, id="FE2-20-4-4"), pytest.param(BIG, 20, 2, 4, False, id="FE3-20-2-4"),
+    pytest.param(SMALL, 10, 2, 6, True, id="small-10-2-6-init")])
+def test_trajectories_follow_the_cpu_restatement(cuda_device, FE, n, depth, chains, from_init):
     """40 iterations (warmup 30 with windows ending at 3, 26, 29, so one mass-matrix update and three step-size searches,
     then 10 samples) against oracle nuts_chain on the numpy potential: theta to 1e-6, the step size to 1e-6 relative and
     every tree depth.  The two differ in the order of their sums (the device adds per-thread partials), i.e. in the last
@@ -64,17 +68,23 @@ def test_trajectories_follow_the_cpu_restatement(cuda_device, FE, n, depth, chai
     to 32, after which the two are different valid chains.  Every chain must agree through the first step-size search
     and 10 iterations; with the trees capped at depth 2 the amplification is small and at least half of the chains must
     agree through all 40 iterations, mass-matrix update included, with the state in shared memory (`small`) and in the
-    global workspace (`big`)."""
+    global workspace (`big`).  A chain started from a caller's init draws its first momenta at the same keys as one that
+    draws its initial point (the initial point takes no draws then)."""
     F, E = FE
     W, S, seed, d = 30, 10, 4321, O.dim(*FE)
     X, y = _toy(FE, chains, n, cuda_device, seed=17)
     assert _uses_workspace(FE, n) == (FE != SMALL)
-    r = M.sample_bnn_posterior(X, y, None, _spec(FE), S, W, seed=seed, max_tree_depth=depth, trace=True)
+    th0 = torch.randn(chains, d, generator=torch.Generator().manual_seed(9), dtype=torch.float64) if from_init else None
+    r = M.sample_bnn_posterior(X, y, None, _spec(FE), S, W, seed=seed, max_tree_depth=depth, init=th0, trace=True)
     tr = r["trace"].cpu().numpy()
     Xd, yd = X.double().cpu().numpy(), y.cpu().numpy()
     agree, parted, at10 = 0, [], []
     for b in range(chains):
-        c = O.bnn_chain_job((Xd[b], yd[b], F, E, S, W, seed, b, depth))
+        if from_init:
+            c = nuts_chain(O.potential_and_grad_np(Xd[b], yd[b], F, E), d, S, W, seed, b=b, t=n, init=th0[b].tolist(),
+                           max_tree_depth=depth)
+        else:
+            c = O.bnn_chain_job((Xd[b], yd[b], F, E, S, W, seed, b, depth))
         dth = np.abs(c["trace"][:, :d] - tr[b, :, :d]).max(1)
         at10.append(float(dth[10]))
         bad = np.nonzero((dth > 1e-6) | (c["trace"][:, d + 1] != tr[b, :, d + 1]) |

@@ -186,6 +186,42 @@ def test_model_predicts_many_points_in_one_launch(cuda_device):
         model(torch.rand(B, 128 - t + 1, 2, device=cuda_device))
 
 
+def test_warmup_only_returns_the_last_state(cuda_device):
+    """num_samples = 0 with warmup: the single output row is the state after the last warmup iteration, whatever the
+    output buffers held, and the predictive is formed at it, bit for bit as an evaluate-only call there forms it."""
+    torch.manual_seed(12)
+    B, T, F, W, ts = 3, 12, 2, 25, [4, 9]
+    x, y, _ = fast_gp_mix.get_batch(B, T, F, device=cuda_device)
+    xb, yb = x.transpose(0, 1).contiguous(), y.transpose(0, 1).contiguous()
+    r = fast_gp_mix.sample_posterior(xb, yb, ts, {}, 0, W, seed=6, max_tree_depth=4, trace=True, n_pred=2)
+    assert r["samples"].shape == (len(ts), B, 1, F + 2) and r["trace"].shape == (len(ts), B, W, F + 4)
+    assert torch.equal(r["log_samples"][:, :, 0], r["trace"][:, :, -1, :F + 2]) and torch.isnan(r["accept"]).all()
+    e = fast_gp_mix.sample_posterior(xb, yb, ts, {}, 0, 0, init=r["log_samples"][:, :, 0], n_pred=2)
+    for k in ("samples", "log_samples", "mean", "var"):
+        assert torch.equal(e[k], r[k]), k
+    assert torch.isfinite(r["mean"][:, :, 0]).all()
+
+    kt, prior, _ = fast_gp_mix._fit_settings({})
+    P, f64 = len(ts) * B, dict(dtype=torch.float64, device=cuda_device)
+
+    def launch(fill):
+        desc = L.gp_mcmc_desc(B, T, F, ts, kt, prior, 0, W, 6, 4, 2)
+        out = {k: torch.full(shape, fill, **f64) for k, shape in
+               (("samples", (P, 1, F + 2)), ("log_samples", (P, 1, F + 2)), ("mean", (P, 1, 2)), ("var", (P, 1, 2)),
+                ("potential", (P,)), ("grad", (P, F + 2)), ("step_size", (P,)), ("accept", (P,)),
+                ("trace", (P, W, F + 4)))}
+        out["diag"] = torch.full((P, 6), -7, dtype=torch.int32, device=cuda_device)
+        L.gp_mcmc(xb.float(), yb.float(), desc, out["samples"], out["step_size"], out["accept"], out["diag"],
+                  **{k: v for k, v in out.items() if k not in ("samples", "step_size", "accept", "diag")})
+        return out
+
+    a, b = launch(float("nan")), launch(0.0)
+    for k in a:
+        assert torch.equal(a[k].isnan(), b[k].isnan()) and torch.equal(a[k].nan_to_num(0.0), b[k].nan_to_num(0.0)), k
+        assert k == "accept" or not a[k].isnan().any(), k
+    assert torch.equal(a["log_samples"].view(len(ts), B, 1, F + 2), r["log_samples"])
+
+
 def test_a_chain_without_a_finite_start_is_not_run(cuda_device):
     B, T, F = 2, 8, 1
     x = torch.full((B, T, F), 0.5, device=cuda_device)              # identical rows: K = s 11^T + noise I

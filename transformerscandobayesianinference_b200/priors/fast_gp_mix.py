@@ -361,7 +361,9 @@ def sample_posterior(x, y, ts, hyperparameters=None, num_samples=MCMC_NUM_SAMPLE
     t == T; [.., S', n_pred] for rows t .. t + n_pred - 1 when n_pred > 1), potential and grad [.., F+2] (U and dU/du at the last state), step_size, accept (mean acceptance statistic
     of the sampling phase), diag [.., 6] int32 (columns L.GP_MCMC_DIAG_NAMES), and "seed".  S' = max(num_samples, 1).
     init [len(ts), B, F+2] gives the starting u; num_samples = warmup_steps = 0 then only evaluates U, its gradient and
-    the predictive at init.  A chain without a finite starting point is not run: its samples and predictive are NaN.
+    the predictive at init.  num_samples = 0 with warmup_steps > 0 runs the warmup only: the one sample is the state the
+    warmup ended in (samples = exp(u), log_samples = u), the predictive is formed at it and accept is NaN.  A chain
+    without a finite starting point is not run: its samples and predictive are NaN.
     trace=True adds "trace" [.., W+S, F+4]: per iteration u, the step size used and the tree
     depth."""
     Bn, T, F = x.shape
