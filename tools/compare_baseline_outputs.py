@@ -13,7 +13,10 @@ e.g. to compare the tree against its parent commit on a GPU:
 `run` imports the package (and its library) from --tree (default: this checkout) and saves every output tensor of seeded
 calls: the fit at four shapes (theta, f, grad, mean, var, iters, nevals, status); the GP sampler at the sizes
 tools/time_gp_mcmc.py times plus one run capped at tree depth 2; the Bayesian-NN sampler on the `small` and `big`
-models at 64 warmup / 64 samples (samples, probs, obs, potential, grad, step size, acceptance, diag and trace throughout).
+models at 64 warmup / 64 samples (samples, probs, obs, potential, grad, step size, acceptance, diag and trace throughout);
+and the edge paths of both samplers' outputs and of the fit: evaluate-only calls (W = S = 0) at an init whose potential is
+finite for some chains and not for others, warmup-only calls (S = 0), chains started at a non-finite init with W + S > 0,
+and the fit with max_iter = 0.
 `compare` exits non-zero unless every tensor is bitwise equal (NaNs in the same places count as equal).
 """
 import argparse
@@ -26,6 +29,8 @@ FIT_SHAPES = [(32, 40, 1), (16, 64, 3), (8, 128, 5), (100, 50, 1)]  # B, T, F; e
 GP_MCMC = [(100, 50, 1, 1, 300, 100, 10, 1), (100, 128, 5, 10, 300, 100, 10, 3), (32, 40, 2, 3, 100, 50, 2, 1)]
 BNN_MODELS = [("small", 3, 5), ("big", 8, 64)]                      # name, F, E; 100 datasets, 100 training rows
 BNN_STEPS = 64
+# name, samples, warmup, whether every third chain starts at NaN and the others at 0 (otherwise the uniform draws)
+EDGE_PATHS = [("evaluate_only", 0, 0, True), ("warmup_only", 0, 50, False), ("nonfinite_init", 20, 20, True)]
 
 
 def run(out, tree):
@@ -57,6 +62,28 @@ def run(out, tree):
         spec = {"num_features": F, "embed": E}
         r = M.sample_bnn_posterior(X[:, :100], Y[:, :100], X[:, 100:], spec, BNN_STEPS, BNN_STEPS, seed=1, trace=True)
         keep(f"bnn_mcmc/{name}", r)
+
+    def mixed_init(n, d):
+        init = torch.zeros(n, d, dtype=torch.float64)
+        init[::3] = float("nan")
+        return init
+
+    torch.manual_seed(300)
+    B, T, F = FIT_SHAPES[0]
+    x, y, _ = fast_gp_mix.get_batch(B, T, F, device="cuda", batch_size_per_gp_sample=4)
+    xb, yb = x.transpose(0, 1).contiguous(), y.transpose(0, 1).contiguous()
+    keep(f"fit/{B}x{T}x{F}/max_iter0", fast_gp_mix.fit_map(xb, yb, list(range(1, T + 1)), {}, max_iter=0, grad=True))
+    ts = [5, 20, T]                                                    # t = T: no predictive row
+    for name, S, W, nan_init in EDGE_PATHS:
+        init = mixed_init(len(ts) * B, F + 2).view(len(ts), B, F + 2) if nan_init else None
+        keep(f"gp_mcmc/{name}", fast_gp_mix.sample_posterior(xb, yb, ts, {}, S, W, seed=2, init=init, trace=True,
+                                                             n_pred=2))
+    x, y = P.sample_bnn_prior(30, 150, 3, 5, "cuda", seed=8)
+    X, Y = x.transpose(0, 1).contiguous(), y.transpose(0, 1).contiguous()
+    for name, S, W, nan_init in EDGE_PATHS:
+        init = mixed_init(30, 3 * 5 + 3 * 5 + 2) if nan_init else None
+        keep(f"bnn_mcmc/{name}", M.sample_bnn_posterior(X[:, :100], Y[:, :100], X[:, 100:], {"num_features": 3, "embed": 5},
+                                                         S, W, seed=2, init=init, trace=True))
     torch.save(res, out)
     print(f"saved {len(res)} tensors from {tree} to {out}")
 

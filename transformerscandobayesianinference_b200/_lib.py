@@ -540,15 +540,20 @@ def gp_sample(x, z, ls, os_, noise, jitter, kernel_type, y, work, info):
                                ptr(work), ptr(info), Bn, T, F, stream_ptr()), "pfn_gp_sample")
 
 
-def gp_fit_desc(B, T, F, ts, kernel_type, hyper, noise_lb, noise_init, max_iter, max_eval, ftol, gtol):
-    """Descriptor of a pfn_gp_fit call without its device pointers.  hyper = (ls_conc, ls_rate, os_conc, os_rate,
-    noise_conc, noise_rate).  The prefix list is kept alive on the descriptor (it is read on the host)."""
-    d = GpFitDesc()
+def _gp_problems(d, B, T, F, ts, kernel_type, hyper):
+    """Fills the fields GpFitDesc and GpMcmcDesc share.  hyper = (ls_conc, ls_rate, os_conc, os_rate, noise_conc,
+    noise_rate).  The prefix list is kept alive on the descriptor (it is read on the host)."""
     d.B, d.T, d.F = int(B), int(T), int(F)
     d._ts = (c_int * max(len(ts), 1))(*[int(t) for t in ts])
     d.n_ts, d.ts = len(ts), d._ts
     d.kernel_type = int(kernel_type)
     d.ls_conc, d.ls_rate, d.os_conc, d.os_rate, d.noise_conc, d.noise_rate = (float(v) for v in hyper)
+    return d
+
+
+def gp_fit_desc(B, T, F, ts, kernel_type, hyper, noise_lb, noise_init, max_iter, max_eval, ftol, gtol):
+    """Descriptor of a pfn_gp_fit call without its device pointers (hyper and ts: see _gp_problems)."""
+    d = _gp_problems(GpFitDesc(), B, T, F, ts, kernel_type, hyper)
     d.noise_lb, d.noise_init = float(noise_lb), float(noise_init)
     d.max_iter, d.max_eval, d.ftol, d.gtol = int(max_iter), int(max_eval), float(ftol), float(gtol)
     return d
@@ -561,25 +566,16 @@ def gp_fit(x, y, desc, theta, f, iters, nevals, status, theta0=None, grad=None, 
     _count(1)
     require_cuda(x, y, theta, f, iters, nevals, status, theta0, grad, mean, var)
     desc.x, desc.y = x.data_ptr(), y.data_ptr()
-    desc.theta0 = None if theta0 is None else theta0.data_ptr()
     desc.theta, desc.f = theta.data_ptr(), f.data_ptr()
-    desc.grad = None if grad is None else grad.data_ptr()
-    desc.mean = None if mean is None else mean.data_ptr()
-    desc.var = None if var is None else var.data_ptr()
     desc.iters, desc.nevals, desc.status = iters.data_ptr(), nevals.data_ptr(), status.data_ptr()
+    desc.theta0, desc.grad, desc.mean, desc.var = ptr(theta0), ptr(grad), ptr(mean), ptr(var)
     check(load().pfn_gp_fit(ctypes.byref(desc), stream_ptr()), "pfn_gp_fit")
 
 
 def gp_mcmc_desc(B, T, F, ts, kernel_type, hyper, num_samples, warmup_steps, seed, max_tree_depth=GP_MCMC_MAX_DEPTH,
                  n_pred=1):
-    """Descriptor of a pfn_gp_mcmc call without its device pointers.  hyper = (ls_conc, ls_rate, os_conc, os_rate,
-    noise_conc, noise_rate).  The prefix list is kept alive on the descriptor (it is read on the host)."""
-    d = GpMcmcDesc()
-    d.B, d.T, d.F = int(B), int(T), int(F)
-    d._ts = (c_int * max(len(ts), 1))(*[int(t) for t in ts])
-    d.n_ts, d.ts = len(ts), d._ts
-    d.kernel_type = int(kernel_type)
-    d.ls_conc, d.ls_rate, d.os_conc, d.os_rate, d.noise_conc, d.noise_rate = (float(v) for v in hyper)
+    """Descriptor of a pfn_gp_mcmc call without its device pointers (hyper and ts: see _gp_problems)."""
+    d = _gp_problems(GpMcmcDesc(), B, T, F, ts, kernel_type, hyper)
     d.num_samples, d.warmup_steps, d.max_tree_depth = int(num_samples), int(warmup_steps), int(max_tree_depth)
     d.n_pred = int(n_pred)
     d.seed = int(seed) & 0xFFFFFFFF
@@ -595,15 +591,10 @@ def gp_mcmc(x, y, desc, samples, step_size, accept, diag, init=None, log_samples
     _count(1)
     require_cuda(x, y, samples, step_size, accept, diag, init, log_samples, mean, var, potential, grad, trace)
     desc.x, desc.y = x.data_ptr(), y.data_ptr()
-    desc.init = None if init is None else init.data_ptr()
     desc.samples, desc.step_size, desc.accept, desc.diag = (samples.data_ptr(), step_size.data_ptr(), accept.data_ptr(),
                                                             diag.data_ptr())
-    desc.log_samples = None if log_samples is None else log_samples.data_ptr()
-    desc.mean = None if mean is None else mean.data_ptr()
-    desc.var = None if var is None else var.data_ptr()
-    desc.potential = None if potential is None else potential.data_ptr()
-    desc.grad = None if grad is None else grad.data_ptr()
-    desc.trace = None if trace is None else trace.data_ptr()
+    desc.init, desc.log_samples, desc.mean, desc.var = ptr(init), ptr(log_samples), ptr(mean), ptr(var)
+    desc.potential, desc.grad, desc.trace = ptr(potential), ptr(grad), ptr(trace)
     check(load().pfn_gp_mcmc(ctypes.byref(desc), stream_ptr()), "pfn_gp_mcmc")
 
 
@@ -691,3 +682,30 @@ def bnn_mcmc(x_train, y_train, x_test, desc, samples, step_size, accept, diag, i
     desc.probs, desc.obs, desc.potential, desc.grad = ptr(probs), ptr(obs), ptr(potential), ptr(grad)
     desc.trace, desc.workspace = ptr(trace), ptr(workspace)
     check(load().pfn_bnn_mcmc(ctypes.byref(desc), stream_ptr()), "pfn_bnn_mcmc")
+
+
+# ------------------------------------------------------------------------------------------------
+# what the two NUTS samplers (gp_mcmc, bnn_mcmc) share on the host
+# ------------------------------------------------------------------------------------------------
+def mcmc_seed(seed):
+    """The chains' counter-RNG seed: the caller's, or one draw of torch's CPU generator (reproducible under
+    torch.manual_seed, no device sync)."""
+    return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if seed is None else int(seed)
+
+
+def mcmc_outputs(n, d, num_samples, warmup_steps, trace, device):
+    """The per-chain outputs of n chains over d coordinates: samples [n, S', d], potential [n], grad [n, d], step_size /
+    accept [n] fp64, diag [n, 6] int32 and, when `trace`, trace [n, W + S, d + 2]; S' = max(num_samples, 1)."""
+    f64 = dict(dtype=torch.float64, device=device)
+    out = {"samples": torch.empty(n, max(int(num_samples), 1), d, **f64), "potential": torch.empty(n, **f64),
+           "grad": torch.empty(n, d, **f64), "step_size": torch.empty(n, **f64), "accept": torch.empty(n, **f64),
+           "diag": torch.empty(n, len(GP_MCMC_DIAG_NAMES), dtype=torch.int32, device=device)}
+    if trace:
+        out["trace"] = torch.empty(n, int(warmup_steps) + int(num_samples), d + 2, **f64)
+    return out
+
+
+def mcmc_trouble(diag):
+    """(divergent sampling iterations, iterations that hit the tree-depth cap) summed over the chains of diag [..., 6]."""
+    col = GP_MCMC_DIAG_NAMES.index
+    return int(diag[..., col("div_sampling")].sum()), int(diag[..., col("max_depth_hits")].sum())

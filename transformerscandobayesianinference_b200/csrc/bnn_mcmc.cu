@@ -138,22 +138,7 @@ __global__ void __launch_bounds__(NT, 1) bnn_mcmc_kernel(const pfn_bnn_mcmc_desc
   double* trace = D.trace ? D.trace + static_cast<size_t>(b) * (W + S) * (d + 2) : nullptr;
   const bool finite = nuts::run(c, m, D.init ? D.init + static_cast<size_t>(b) * d : nullptr, W, S, D.max_tree_depth, out,
                                 trace);
-  const bool ran = finite && W + S > 0;
-  if (!ran) {
-    // evaluate-only (W = S = 0): the point itself; no finite starting point: the chain is not run and says so with NaN
-    const double* z = c.vec(nuts::V_Z);
-    for (int k = 0; k < So; ++k)
-      for (int i = tid; i < d; i += NT) out[static_cast<size_t>(k) * d + i] = finite || W + S == 0 ? z[i] : CUDART_NAN;
-  }
-  if (tid == 0) {
-    D.step_size[b] = ran ? c.eps : finite ? 0.0 : CUDART_NAN;
-    D.accept[b] = c.accept;
-    if (D.potential) D.potential[b] = c.pe;
-  }
-  if (D.grad) {
-    const double* g = c.vec(nuts::V_G);
-    for (int i = tid; i < d; i += NT) D.grad[static_cast<size_t>(b) * d + i] = finite ? g[i] : CUDART_NAN;
-  }
+  nuts::store_outputs(c, finite, W, S, b, out, D.potential, D.grad, D.step_size, D.accept);
   // ---- class-1 probability of every test row under every kept sample
   if (D.probs || D.obs) {
     c.key_it = static_cast<uint32_t>(W + S) + 1u;
@@ -178,8 +163,7 @@ __global__ void __launch_bounds__(NT, 1) bnn_mcmc_kernel(const pfn_bnn_mcmc_desc
       }
     }
   }
-  if (tid == 0)
-    for (int k = 0; k < PFN_GP_MCMC_NDIAG; ++k) D.diag[b * PFN_GP_MCMC_NDIAG + k] = c.diag[k];
+  nuts::store_diag(c, D.diag + b * PFN_GP_MCMC_NDIAG);
 }
 
 // 0 on success with *in_smem set; the descriptor's sizes only (no pointers)
@@ -211,17 +195,9 @@ extern "C" int pfn_bnn_mcmc_workspace(const pfn_bnn_mcmc_desc* d) {
 extern "C" int pfn_bnn_mcmc(const pfn_bnn_mcmc_desc* d, void* stream) {
   int in_smem = 0;
   if (const int rc = check_sizes(d, "bnn_mcmc", &in_smem)) return rc;
-  PFN_CHECK_ARG(d->x_train && d->y_train && d->samples && d->step_size && d->accept && d->diag,
-                "bnn_mcmc: null input or output pointer");
+  if (const int rc = nuts::check_chain(d, "bnn_mcmc", d->x_train && d->y_train)) return rc;
   PFN_CHECK_ARG(d->n_test == 0 || (d->probs == nullptr && d->obs == nullptr) || d->x_test != nullptr,
                 "bnn_mcmc: probs or obs wanted but x_test is null");
-  PFN_CHECK_ARG(d->num_samples >= 0 && d->warmup_steps >= 0, "bnn_mcmc: negative num_samples=%d or warmup_steps=%d",
-                d->num_samples, d->warmup_steps);
-  PFN_CHECK_ARG(static_cast<long long>(d->num_samples) + d->warmup_steps <= 0x7fffffffLL, "bnn_mcmc: too many iterations");
-  PFN_CHECK_ARG(d->num_samples + d->warmup_steps > 0 || d->init != nullptr,
-                "bnn_mcmc: warmup_steps = num_samples = 0 evaluates at init, which is null");
-  PFN_CHECK_ARG(d->max_tree_depth >= 1 && d->max_tree_depth <= PFN_GP_MCMC_MAX_DEPTH,
-                "bnn_mcmc: max_tree_depth=%d outside [1, %d]", d->max_tree_depth, PFN_GP_MCMC_MAX_DEPTH);
   PFN_CHECK_ARG(in_smem || d->workspace != nullptr,
                 "bnn_mcmc: the sampler state of d=%d does not fit in shared memory and workspace is null", bnn_dim(d->F, d->E));
   const int dim = bnn_dim(d->F, d->E);

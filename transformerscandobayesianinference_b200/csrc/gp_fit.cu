@@ -342,13 +342,7 @@ __device__ int opt_step(const Opt& O, FitState& S, const Eval& E) {
   return 1;
 }
 
-struct FitArgs {
-  pfn_gp_fit_desc d;
-  int slot_t[PFN_GP_FIT_MAX_T];                // prefix lengths, largest first
-  int slot_i[PFN_GP_FIT_MAX_T];                // their index in d.ts
-};
-
-__global__ void __launch_bounds__(FT, 1) gp_fit_kernel(const FitArgs args) {
+__global__ void __launch_bounds__(FT, 1) gp_fit_kernel(const gp::PrefixArgs<pfn_gp_fit_desc> args) {
   const pfn_gp_fit_desc& D = args.d;
   extern __shared__ __align__(16) double fit_dyn[];
   __shared__ FitState S;
@@ -429,36 +423,12 @@ __global__ void __launch_bounds__(FT, 1) gp_fit_kernel(const FitArgs args) {
 using namespace pfn;
 
 extern "C" int pfn_gp_fit(const pfn_gp_fit_desc* d, void* stream) {
-  PFN_CHECK_ARG(d != nullptr, "gp_fit: null descriptor");
-  PFN_CHECK_ARG(d->B > 0 && d->T > 0 && d->F > 0 && d->n_ts > 0, "gp_fit: empty problem B=%d T=%d F=%d n_ts=%d", d->B, d->T,
-                d->F, d->n_ts);
-  PFN_CHECK_ARG(d->T <= PFN_GP_FIT_MAX_T, "gp_fit: T=%d exceeds %d (the t x t fp64 matrix lives in shared memory)", d->T,
-                PFN_GP_FIT_MAX_T);
-  PFN_CHECK_ARG(d->F <= PFN_GP_FIT_MAX_F, "gp_fit: F=%d exceeds %d", d->F, PFN_GP_FIT_MAX_F);
-  PFN_CHECK_ARG(d->n_ts <= PFN_GP_FIT_MAX_T, "gp_fit: n_ts=%d exceeds %d", d->n_ts, PFN_GP_FIT_MAX_T);
-  PFN_CHECK_ARG(d->ts != nullptr, "gp_fit: ts is null");
-  PFN_CHECK_ARG(d->kernel_type >= PFN_KERNEL_MATERN12 && d->kernel_type <= PFN_KERNEL_MATERN52,
-                "gp_fit: kernel type %d is not a Matern kernel", d->kernel_type);
+  gp::PrefixArgs<pfn_gp_fit_desc> a;
+  if (const int rc = gp::check_prefix_problems(d, "gp_fit", a)) return rc;
   PFN_CHECK_ARG(d->x && d->y && d->theta && d->f && d->iters && d->nevals && d->status, "gp_fit: null input or output pointer");
   PFN_CHECK_ARG(d->noise_lb > 0.0, "gp_fit: noise_lb must be positive");
   PFN_CHECK_ARG(d->theta0 != nullptr || d->noise_init >= d->noise_lb, "gp_fit: noise_init %g below the bound %g",
                 d->noise_init, d->noise_lb);
-  PFN_CHECK_ARG(d->ls_rate > 0.0 && d->os_rate > 0.0 && d->noise_rate > 0.0 && d->ls_conc > 0.0 && d->os_conc > 0.0 &&
-                d->noise_conc > 0.0, "gp_fit: Gamma prior parameters must be positive");
-  PFN_CHECK_ARG(static_cast<long long>(d->B) * d->n_ts <= 0x7fffffffLL, "gp_fit: too many problems");
-  FitArgs a;
-  a.d = *d;
-  for (int i = 0; i < d->n_ts; ++i) {
-    PFN_CHECK_ARG(d->ts[i] >= 1 && d->ts[i] <= d->T, "gp_fit: ts[%d]=%d outside [1, T=%d]", i, d->ts[i], d->T);
-    a.slot_t[i] = d->ts[i];
-    a.slot_i[i] = i;
-  }
-  // largest t first, so the longest CTAs start in the first wave instead of forming its tail
-  for (int i = 1; i < d->n_ts; ++i)
-    for (int j = i; j > 0 && a.slot_t[j] > a.slot_t[j - 1]; --j) {
-      const int tt = a.slot_t[j]; a.slot_t[j] = a.slot_t[j - 1]; a.slot_t[j - 1] = tt;
-      const int ii = a.slot_i[j]; a.slot_i[j] = a.slot_i[j - 1]; a.slot_i[j - 1] = ii;
-    }
   const size_t smem = gp::problem_smem(a.slot_t[0], d->F);
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))

@@ -100,13 +100,7 @@ inline size_t mcmc_smem(int tmax, int T, int F, int n_pred) {
          sizeof(double);
 }
 
-struct McmcArgs {
-  pfn_gp_mcmc_desc d;
-  int slot_t[PFN_GP_FIT_MAX_T];                // prefix lengths, largest first
-  int slot_i[PFN_GP_FIT_MAX_T];                // their index in d.ts
-};
-
-__global__ void __launch_bounds__(FT, 1) gp_mcmc_kernel(const McmcArgs args) {
+__global__ void __launch_bounds__(FT, 1) gp_mcmc_kernel(const gp::PrefixArgs<pfn_gp_mcmc_desc> args) {
   const pfn_gp_mcmc_desc& D = args.d;
   extern __shared__ __align__(16) double mcmc_dyn[];
   __shared__ nuts::Shared<Sum> sh;
@@ -140,36 +134,27 @@ __global__ void __launch_bounds__(FT, 1) gp_mcmc_kernel(const McmcArgs args) {
   double* trace = D.trace ? D.trace + p * (W + S) * (d + 2) : nullptr;
   const bool finite = nuts::run(c, m, D.init ? D.init + p * d : nullptr, W, S, D.max_tree_depth, out_u, trace);
   const bool ran = W + S > 0;                  // otherwise evaluate-only: U, grad and the predictive at init
+  nuts::store_outputs(c, finite, W, S, p, out_u, D.potential, D.grad, D.step_size, D.accept);
+  if (!finite && !ran) {
+    // evaluate-only at an init whose U is not finite: step size 0 and the gradient found there, as for a finite U
+    if (tid == 0) D.step_size[p] = 0.0;
+    if (D.grad) nuts::copy(D.grad + p * d, c.vec(nuts::V_G), d);
+  }
   if (!finite && ran) {
-    // no finite starting point (the caller's, or none among INIT_TRIES uniform draws): the chain is not run and says so
-    // with NaN results
-    if (tid == 0) {
+    // no finite starting point (the caller's, or none among INIT_TRIES uniform draws): the chain is not run and its
+    // predictive is NaN
+    if (tid == 0)
       for (int k = 0; k < So; ++k) {
-        for (int i = 0; i < d; ++i) {
-          out_u[static_cast<size_t>(k) * d + i] = CUDART_NAN;
+        for (int i = 0; i < d; ++i)
           if (D.log_samples) D.log_samples[(p * So + k) * d + i] = CUDART_NAN;
-        }
         for (int j = 0; j < D.n_pred; ++j) {
           if (D.mean) D.mean[(p * So + k) * D.n_pred + j] = CUDART_NAN;
           if (D.var) D.var[(p * So + k) * D.n_pred + j] = CUDART_NAN;
         }
       }
-      if (D.potential) D.potential[p] = CUDART_INF;
-      if (D.grad)
-        for (int i = 0; i < d; ++i) D.grad[p * d + i] = CUDART_NAN;
-      D.step_size[p] = CUDART_NAN;
-      D.accept[p] = CUDART_NAN;
-      for (int k = 0; k < PFN_GP_MCMC_NDIAG; ++k) D.diag[p * PFN_GP_MCMC_NDIAG + k] = c.diag[k];
-    }
+    nuts::store_diag(c, D.diag + p * PFN_GP_MCMC_NDIAG);
     return;
   }
-  if (!ran) nuts::copy(out_u, c.vec(nuts::V_Z), d);
-  if (tid == 0) {
-    if (D.potential) D.potential[p] = c.pe;
-    D.step_size[p] = ran ? c.eps : 0.0;
-    D.accept[p] = c.accept;
-  }
-  if (D.grad) nuts::copy(D.grad + p * d, c.vec(nuts::V_G), d);
   // ---- predictive of rows t .. t + n_pred - 1 under every kept sample (warmup only: the state the warmup ended in): one
   // factorisation per sample, no gradient (evaluate-only: at init, whose factorisation is still in A)
   const int want = t < D.T && D.mean != nullptr;
@@ -198,8 +183,7 @@ __global__ void __launch_bounds__(FT, 1) gp_mcmc_kernel(const McmcArgs args) {
     }
     __syncthreads();
   }
-  if (tid == 0)
-    for (int k = 0; k < PFN_GP_MCMC_NDIAG; ++k) D.diag[p * PFN_GP_MCMC_NDIAG + k] = c.diag[k];
+  nuts::store_diag(c, D.diag + p * PFN_GP_MCMC_NDIAG);
 }
 
 }  // namespace
@@ -208,42 +192,11 @@ __global__ void __launch_bounds__(FT, 1) gp_mcmc_kernel(const McmcArgs args) {
 using namespace pfn;
 
 extern "C" int pfn_gp_mcmc(const pfn_gp_mcmc_desc* d, void* stream) {
-  PFN_CHECK_ARG(d != nullptr, "gp_mcmc: null descriptor");
-  PFN_CHECK_ARG(d->B > 0 && d->T > 0 && d->F > 0 && d->n_ts > 0, "gp_mcmc: empty problem B=%d T=%d F=%d n_ts=%d", d->B,
-                d->T, d->F, d->n_ts);
-  PFN_CHECK_ARG(d->T <= PFN_GP_FIT_MAX_T, "gp_mcmc: T=%d exceeds %d (the t x t fp64 matrix lives in shared memory)", d->T,
-                PFN_GP_FIT_MAX_T);
-  PFN_CHECK_ARG(d->F <= PFN_GP_FIT_MAX_F, "gp_mcmc: F=%d exceeds %d", d->F, PFN_GP_FIT_MAX_F);
-  PFN_CHECK_ARG(d->n_ts <= PFN_GP_FIT_MAX_T, "gp_mcmc: n_ts=%d exceeds %d", d->n_ts, PFN_GP_FIT_MAX_T);
-  PFN_CHECK_ARG(d->ts != nullptr, "gp_mcmc: ts is null");
-  PFN_CHECK_ARG(d->kernel_type >= PFN_KERNEL_MATERN12 && d->kernel_type <= PFN_KERNEL_MATERN52,
-                "gp_mcmc: kernel type %d is not a Matern kernel", d->kernel_type);
-  PFN_CHECK_ARG(d->x && d->y && d->samples && d->step_size && d->accept && d->diag,
-                "gp_mcmc: null input or output pointer");
-  PFN_CHECK_ARG(d->ls_rate > 0.0 && d->os_rate > 0.0 && d->noise_rate > 0.0 && d->ls_conc > 0.0 && d->os_conc > 0.0 &&
-                d->noise_conc > 0.0, "gp_mcmc: Gamma prior parameters must be positive");
-  PFN_CHECK_ARG(d->num_samples >= 0 && d->warmup_steps >= 0, "gp_mcmc: negative num_samples=%d or warmup_steps=%d",
-                d->num_samples, d->warmup_steps);
-  PFN_CHECK_ARG(static_cast<long long>(d->num_samples) + d->warmup_steps <= 0x7fffffffLL, "gp_mcmc: too many iterations");
-  PFN_CHECK_ARG(d->num_samples + d->warmup_steps > 0 || d->init != nullptr,
-                "gp_mcmc: warmup_steps = num_samples = 0 evaluates at init, which is null");
+  gp::PrefixArgs<pfn_gp_mcmc_desc> a;
+  if (const int rc = gp::check_prefix_problems(d, "gp_mcmc", a)) return rc;
+  if (const int rc = nuts::check_chain(d, "gp_mcmc", d->x && d->y)) return rc;
   PFN_CHECK_ARG(d->n_pred >= 1 && d->n_pred <= PFN_GP_FIT_MAX_T, "gp_mcmc: n_pred=%d outside [1, %d]", d->n_pred,
                 PFN_GP_FIT_MAX_T);
-  PFN_CHECK_ARG(d->max_tree_depth >= 1 && d->max_tree_depth <= PFN_GP_MCMC_MAX_DEPTH,
-                "gp_mcmc: max_tree_depth=%d outside [1, %d]", d->max_tree_depth, PFN_GP_MCMC_MAX_DEPTH);
-  PFN_CHECK_ARG(static_cast<long long>(d->B) * d->n_ts <= 0x7fffffffLL, "gp_mcmc: too many problems");
-  McmcArgs a;
-  a.d = *d;
-  for (int i = 0; i < d->n_ts; ++i) {
-    PFN_CHECK_ARG(d->ts[i] >= 1 && d->ts[i] <= d->T, "gp_mcmc: ts[%d]=%d outside [1, T=%d]", i, d->ts[i], d->T);
-    a.slot_t[i] = d->ts[i];
-    a.slot_i[i] = i;
-  }
-  for (int i = 1; i < d->n_ts; ++i)            // largest t first
-    for (int j = i; j > 0 && a.slot_t[j] > a.slot_t[j - 1]; --j) {
-      const int tt = a.slot_t[j]; a.slot_t[j] = a.slot_t[j - 1]; a.slot_t[j - 1] = tt;
-      const int ii = a.slot_i[j]; a.slot_i[j] = a.slot_i[j - 1]; a.slot_i[j - 1] = ii;
-    }
   const size_t smem = mcmc_smem(a.slot_t[0], d->T, d->F, d->n_pred);
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))

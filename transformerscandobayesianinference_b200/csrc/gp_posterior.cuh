@@ -4,7 +4,8 @@
 //   ->  K^-1 = L^-T L^-1 into the strict lower triangle + dg  ->  alpha = K^-1 (y - c)
 //   ->  the trace terms of d log N / d theta (W = alpha alpha^T - K^-1), with dK recomputed from x (not stored).
 // Each kernel composes its own parameterisation and priors from these terms.  Every reduction has a fixed order, so a
-// problem's result depends on its own inputs only (bitwise repeatable).
+// problem's result depends on its own inputs only (bitwise repeatable).  On the host: the launch arguments of both
+// kernels and the check of the descriptor fields they share.
 #pragma once
 #include <math_constants.h>
 
@@ -237,6 +238,48 @@ __device__ __forceinline__ void predict(const Problem& P, const double* inv_ls, 
 // x* [F].
 inline size_t problem_smem(int tmax, int F) {
   return (static_cast<size_t>(tmax) * (tmax | 1) + static_cast<size_t>(tmax) * F + 6 * tmax + F) * sizeof(double);
+}
+
+// ------------------------------------------------------------------------------------------------ host
+// Launch arguments of a kernel over the (prefix, dataset) problems of a descriptor (pfn_gp_fit_desc, pfn_gp_mcmc_desc):
+// CTA slot * B + b solves prefix slot_t[slot] of dataset b.
+template <class Desc>
+struct PrefixArgs {
+  Desc d;
+  int slot_t[PFN_GP_FIT_MAX_T];                // prefix lengths, largest first
+  int slot_i[PFN_GP_FIT_MAX_T];                // their index in d.ts
+};
+
+// Checks the fields the two descriptors share, with `who` (the entry point's name) heading every message, and fills a.
+// Returns 0 on success.
+template <class Desc>
+inline int check_prefix_problems(const Desc* d, const char* who, PrefixArgs<Desc>& a) {
+  PFN_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
+  PFN_CHECK_ARG(d->B > 0 && d->T > 0 && d->F > 0 && d->n_ts > 0, "%s: empty problem B=%d T=%d F=%d n_ts=%d", who, d->B,
+                d->T, d->F, d->n_ts);
+  PFN_CHECK_ARG(d->T <= PFN_GP_FIT_MAX_T, "%s: T=%d exceeds %d (the t x t fp64 matrix lives in shared memory)", who, d->T,
+                PFN_GP_FIT_MAX_T);
+  PFN_CHECK_ARG(d->F <= PFN_GP_FIT_MAX_F, "%s: F=%d exceeds %d", who, d->F, PFN_GP_FIT_MAX_F);
+  PFN_CHECK_ARG(d->n_ts <= PFN_GP_FIT_MAX_T, "%s: n_ts=%d exceeds %d", who, d->n_ts, PFN_GP_FIT_MAX_T);
+  PFN_CHECK_ARG(d->ts != nullptr, "%s: ts is null", who);
+  PFN_CHECK_ARG(d->kernel_type >= PFN_KERNEL_MATERN12 && d->kernel_type <= PFN_KERNEL_MATERN52,
+                "%s: kernel type %d is not a Matern kernel", who, d->kernel_type);
+  PFN_CHECK_ARG(d->ls_rate > 0.0 && d->os_rate > 0.0 && d->noise_rate > 0.0 && d->ls_conc > 0.0 && d->os_conc > 0.0 &&
+                d->noise_conc > 0.0, "%s: Gamma prior parameters must be positive", who);
+  PFN_CHECK_ARG(static_cast<long long>(d->B) * d->n_ts <= 0x7fffffffLL, "%s: too many problems", who);
+  a.d = *d;
+  for (int i = 0; i < d->n_ts; ++i) {
+    PFN_CHECK_ARG(d->ts[i] >= 1 && d->ts[i] <= d->T, "%s: ts[%d]=%d outside [1, T=%d]", who, i, d->ts[i], d->T);
+    a.slot_t[i] = d->ts[i];
+    a.slot_i[i] = i;
+  }
+  // largest t first, so the longest CTAs start in the first wave instead of forming its tail
+  for (int i = 1; i < d->n_ts; ++i)
+    for (int j = i; j > 0 && a.slot_t[j] > a.slot_t[j - 1]; --j) {
+      const int tt = a.slot_t[j]; a.slot_t[j] = a.slot_t[j - 1]; a.slot_t[j - 1] = tt;
+      const int ii = a.slot_i[j]; a.slot_i[j] = a.slot_i[j - 1]; a.slot_i[j - 1] = ii;
+    }
+  return 0;
 }
 
 }  // namespace gp

@@ -18,6 +18,7 @@
 // which evaluates U at c.trial (every thread may read it on entry; +inf when U is not finite), writes dU/dtheta into
 // vector V_GE, calls per_elem(i, g_i) on the owner of element i once g_i is known and returns the c.sum of its results in
 // `third` (the fused second leapfrog half returns w_i^2), and counts PFN_GP_MCMC_EVALS and PFN_GP_MCMC_NOT_PD itself.
+// After run, store_outputs and store_diag write the outputs every chain has; check_chain checks their descriptor fields.
 //
 // Random draw k of iteration key `it` is uniform_double(hash5(seed, key_b, key_t, it, 2k), hash5(.., 2k + 1)); the initial
 // point and the first step-size search use key 0, iteration it and the searches after it key it + 1.  Compile with
@@ -25,6 +26,7 @@
 #pragma once
 #include <math_constants.h>
 
+#include "common.cuh"
 #include "counter_rng.cuh"
 #include "../../include/pfn_b200.h"
 
@@ -512,6 +514,54 @@ __device__ bool run(Chain<Sum>& c, Model& m, const double* init, int W, int S, i
   if (S == 0) copy(out, c.vec(V_Z), d);        // warmup only: the one output row is the state the warmup ended in
   else c.accept = acc_sampling / S;
   return true;
+}
+
+// The outputs of chain p after run (finite: what it returned; W, S and out as passed to it): step_size, accept and the
+// optional potential [p] and grad [p, d].  An evaluate-only call (W = S = 0) stores its point as the one row of out.  A
+// chain without a finite starting point is not run: out, its step size and gradient are NaN, its potential +inf (c.pe)
+// and its acceptance NaN (c.accept).  The counters follow with store_diag once the kernel's own work is counted.
+template <class Sum>
+__device__ void store_outputs(const Chain<Sum>& c, bool finite, int W, int S, size_t p, double* out, double* potential,
+                              double* grad, double* step_size, double* accept) {
+  const int tid = threadIdx.x, d = c.d;
+  const bool ran = finite && W + S > 0;
+  if (!ran) {
+    const double* z = c.vec(V_Z);
+    for (int k = 0; k < (S > 0 ? S : 1); ++k)
+      for (int i = tid; i < d; i += NT) out[static_cast<size_t>(k) * d + i] = finite || W + S == 0 ? z[i] : CUDART_NAN;
+  }
+  if (tid == 0) {
+    step_size[p] = ran ? c.eps : finite ? 0.0 : CUDART_NAN;
+    accept[p] = c.accept;
+    if (potential) potential[p] = c.pe;
+  }
+  if (grad) {
+    const double* g = c.vec(V_G);
+    for (int i = tid; i < d; i += NT) grad[p * d + i] = finite ? g[i] : CUDART_NAN;
+  }
+}
+
+// diag [PFN_GP_MCMC_NDIAG]: the chain's counters
+template <class Sum>
+__device__ void store_diag(const Chain<Sum>& c, int* diag) {
+  if (threadIdx.x == 0)
+    for (int k = 0; k < PFN_GP_MCMC_NDIAG; ++k) diag[k] = c.diag[k];
+}
+
+// ------------------------------------------------------------------------------------------------ host
+// The chain fields of a sampler's descriptor (pfn_gp_mcmc_desc, pfn_bnn_mcmc_desc), with `who` (the entry point's name)
+// heading every message; inputs: whether the caller's input pointers are set.  Returns 0 on success.
+template <class Desc>
+inline int check_chain(const Desc* d, const char* who, bool inputs) {
+  PFN_CHECK_ARG(inputs && d->samples && d->step_size && d->accept && d->diag, "%s: null input or output pointer", who);
+  PFN_CHECK_ARG(d->num_samples >= 0 && d->warmup_steps >= 0, "%s: negative num_samples=%d or warmup_steps=%d", who,
+                d->num_samples, d->warmup_steps);
+  PFN_CHECK_ARG(static_cast<long long>(d->num_samples) + d->warmup_steps <= 0x7fffffffLL, "%s: too many iterations", who);
+  PFN_CHECK_ARG(d->num_samples + d->warmup_steps > 0 || d->init != nullptr,
+                "%s: warmup_steps = num_samples = 0 evaluates at init, which is null", who);
+  PFN_CHECK_ARG(d->max_tree_depth >= 1 && d->max_tree_depth <= PFN_GP_MCMC_MAX_DEPTH,
+                "%s: max_tree_depth=%d outside [1, %d]", who, d->max_tree_depth, PFN_GP_MCMC_MAX_DEPTH);
+  return 0;
 }
 
 }  // namespace nuts

@@ -140,12 +140,6 @@ def generate_toy_data(model, bptt, device='cpu'):
     return torch.stack(xs).to(device), torch.stack(ys).to(device)
 
 
-def _seed(seed):
-    """The chains' counter-RNG seed: the caller's, or one draw of torch's CPU generator (reproducible under
-    torch.manual_seed, no device sync)."""
-    return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if seed is None else int(seed)
-
-
 def _mcmc_device(device):
     dev = torch.device(device)
     if dev.type == 'cuda':
@@ -181,17 +175,13 @@ def sample_bnn_posterior(x_train, y_train, x_test, spec, num_samples, warmup_ste
     if not 1 <= max_tree_depth <= L.GP_MCMC_MAX_DEPTH:
         raise ValueError(f"max_tree_depth={max_tree_depth} outside [1, {L.GP_MCMC_MAX_DEPTH}]")
     dev = _mcmc_device(x_train.device)
-    seed = _seed(seed)
+    seed = L.mcmc_seed(seed)
     n_test = 0 if x_test is None else x_test.shape[1]
-    So, WS = max(int(num_samples), 1), int(warmup_steps) + int(num_samples)
+    So = max(int(num_samples), 1)
     f64 = dict(dtype=torch.float64, device=dev)
     with L.on_device(dev):
-        out = {"samples": torch.empty(N, So, d, **f64), "probs": torch.empty(N, So, n_test, **f64),
-               "obs": torch.empty(N, So, n_test, dtype=torch.float32, device=dev),
-               "potential": torch.empty(N, **f64), "grad": torch.empty(N, d, **f64), "step_size": torch.empty(N, **f64),
-               "accept": torch.empty(N, **f64), "diag": torch.empty(N, len(L.GP_MCMC_DIAG_NAMES), dtype=torch.int32, device=dev)}
-        if trace:
-            out["trace"] = torch.empty(N, WS, d + 2, **f64)
+        out = L.mcmc_outputs(N, d, num_samples, warmup_steps, trace, dev)
+        out.update(probs=torch.empty(N, So, n_test, **f64), obs=torch.empty(N, So, n_test, dtype=torch.float32, device=dev))
         desc = L.bnn_mcmc_desc(N, n, n_test, F, E, num_samples, warmup_steps, seed, max_tree_depth)
         per_chain = L.bnn_mcmc_workspace(desc)
         workspace = torch.empty(N, per_chain, **f64) if per_chain else None
@@ -205,8 +195,7 @@ def sample_bnn_posterior(x_train, y_train, x_test, spec, num_samples, warmup_ste
 
 
 def _report_mcmc(diag):
-    col = L.GP_MCMC_DIAG_NAMES.index
-    n_div, n_depth = int(diag[:, col("div_sampling")].sum()), int(diag[:, col("max_depth_hits")].sum())
+    n_div, n_depth = L.mcmc_trouble(diag)
     if n_div or n_depth:
         print(f"eval_mcmc: {diag.shape[0]} chains: {n_div} sampling iterations diverged, {n_depth} iterations (warmup "
               f"included) hit the tree-depth cap")
@@ -224,7 +213,7 @@ def eval_mcmc(X, y, device, model_sampler, training_samples_n, warmup_steps, num
     model = model_sampler()
     spec = {'num_features': model.num_features, 'embed': model.embed}
     dev = _mcmc_device(device)
-    seed = _seed(seed)
+    seed = L.mcmc_seed(seed)
     X, y = X.to(dev), y.to(dev)
     k = training_samples_n
     r = sample_bnn_posterior(X[:, :k], y[:, :k], X[:, k:], spec, num_pred_samples, warmup_steps, seed)

@@ -346,12 +346,6 @@ def evaluate(x, y, y_non_noisy, use_mse=False, hyperparameters={}, get_model_on_
 MCMC_NUM_SAMPLES, MCMC_WARMUP_STEPS, MCMC_MAX_TREE_DEPTH = 100, 300, L.GP_MCMC_MAX_DEPTH
 
 
-def _mcmc_seed(seed):
-    """The chains' counter-RNG seed: the caller's, or one draw of torch's CPU generator (reproducible under
-    torch.manual_seed, no device sync)."""
-    return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if seed is None else int(seed)
-
-
 @torch.no_grad()
 def sample_posterior(x, y, ts, hyperparameters=None, num_samples=MCMC_NUM_SAMPLES, warmup_steps=MCMC_WARMUP_STEPS,
                      seed=None, init=None, max_tree_depth=MCMC_MAX_TREE_DEPTH, trace=False, n_pred=1):
@@ -371,16 +365,12 @@ def sample_posterior(x, y, ts, hyperparameters=None, num_samples=MCMC_NUM_SAMPLE
         raise ValueError(f"the GP sampler keeps the t x t matrix in shared memory: T={T} exceeds the limit of {MAX_FIT_T}")
     dev = _fit_device(x.device)
     kt, prior, _ = _fit_settings(hyperparameters)
-    seed = _mcmc_seed(seed)
+    seed = L.mcmc_seed(seed)
     P, So = len(ts) * Bn, max(int(num_samples), 1)
     f64 = dict(dtype=torch.float64, device=dev)
-    out = {"samples": torch.empty(P, So, F + 2, **f64), "log_samples": torch.empty(P, So, F + 2, **f64),
-           "mean": torch.empty(P, So, n_pred, **f64), "var": torch.empty(P, So, n_pred, **f64),
-           "potential": torch.empty(P, **f64),
-           "grad": torch.empty(P, F + 2, **f64), "step_size": torch.empty(P, **f64), "accept": torch.empty(P, **f64),
-           "diag": torch.empty(P, len(L.GP_MCMC_DIAG_NAMES), dtype=torch.int32, device=dev)}
-    if trace:
-        out["trace"] = torch.empty(P, int(warmup_steps) + int(num_samples), F + 4, **f64)
+    out = L.mcmc_outputs(P, F + 2, num_samples, warmup_steps, trace, dev)
+    out.update(log_samples=torch.empty(P, So, F + 2, **f64), mean=torch.empty(P, So, n_pred, **f64),
+               var=torch.empty(P, So, n_pred, **f64))
     desc = L.gp_mcmc_desc(Bn, T, F, ts, kt, prior, num_samples, warmup_steps, seed, max_tree_depth, n_pred)
     u0 = None if init is None else init.to(dev, torch.float64).reshape(P, F + 2).contiguous()
     L.gp_mcmc(x.to(dev, torch.float32).contiguous(), y.to(dev, torch.float32).contiguous(), desc, out["samples"],
@@ -490,8 +480,7 @@ def _report_mcmc(diag, samples):
     n_dead = int(torch.isnan(samples[..., 0, 0]).sum())
     if n_dead:
         print(f"fast_gp_mix.evaluate_: {n_dead} chains found no finite starting point and were not run (NaN losses)")
-    n_div = int(diag[..., L.GP_MCMC_DIAG_NAMES.index("div_sampling")].sum())
-    n_depth = int(diag[..., L.GP_MCMC_DIAG_NAMES.index("max_depth_hits")].sum())
+    n_div, n_depth = L.mcmc_trouble(diag)
     if n_div or n_depth:
         print(f"fast_gp_mix.evaluate_: {diag.shape[0] * diag.shape[1]} chains: {n_div} sampling iterations diverged, "
               f"{n_depth} iterations (warmup included) hit the tree-depth cap")
