@@ -284,6 +284,30 @@ def require_cuda(*tensors):
     return dev
 
 
+def cuda_device(device, what):
+    """`device` with its index filled in; raises on a non-CUDA device.  `what` names the caller and its kernel."""
+    dev = torch.device(device)
+    if dev.type != 'cuda':
+        raise RuntimeError(f"{what}; device {dev} is not a CUDA device (there is no CPU fallback)")
+    return dev if dev.index is not None else torch.device('cuda', torch.cuda.current_device())
+
+
+def compute_device(device, what):
+    """Where a sampler runs: `device` when it is a CUDA device (index filled in), otherwise (a CPU device, or None) the
+    current CUDA device, whose results the caller may copy to `device`.  Raises when there is no CUDA device."""
+    if device is not None and torch.device(device).type == 'cuda':
+        return cuda_device(device, what)
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"{what}; no CUDA device is available (there is no CPU fallback)")
+    return torch.device('cuda', torch.cuda.current_device())
+
+
+def draw_seed(seed=None):
+    """`seed`, or when None one draw of torch's CPU generator: reproducible under torch.manual_seed, no device sync.
+    Seeds the counter-based random numbers of the samplers, the NUTS chains and dropout."""
+    return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if seed is None else int(seed)
+
+
 def _guarded(fn):
     """Run the wrapped library call with the device of its first tensor argument as the current device (so that
     `stream_ptr()`, `num_sms()` and the launch itself all refer to the device that owns the data)."""
@@ -687,12 +711,6 @@ def bnn_mcmc(x_train, y_train, x_test, desc, samples, step_size, accept, diag, i
 # ------------------------------------------------------------------------------------------------
 # what the two NUTS samplers (gp_mcmc, bnn_mcmc) share on the host
 # ------------------------------------------------------------------------------------------------
-def mcmc_seed(seed):
-    """The chains' counter-RNG seed: the caller's, or one draw of torch's CPU generator (reproducible under
-    torch.manual_seed, no device sync)."""
-    return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if seed is None else int(seed)
-
-
 def mcmc_outputs(n, d, num_samples, warmup_steps, trace, device):
     """The per-chain outputs of n chains over d coordinates: samples [n, S', d], potential [n], grad [n, d], step_size /
     accept [n] fp64, diag [n, 6] int32 and, when `trace`, trace [n, W + S, d + 2]; S' = max(num_samples, 1)."""

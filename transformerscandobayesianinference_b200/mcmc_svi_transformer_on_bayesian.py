@@ -140,14 +140,7 @@ def generate_toy_data(model, bptt, device='cpu'):
     return torch.stack(xs).to(device), torch.stack(ys).to(device)
 
 
-def _mcmc_device(device):
-    dev = torch.device(device)
-    if dev.type == 'cuda':
-        return dev if dev.index is not None else torch.device('cuda', torch.cuda.current_device())
-    if not torch.cuda.is_available():
-        raise RuntimeError("the Bayesian-NN NUTS baseline runs on the sm_90a kernel of csrc/bnn_mcmc.cu; no CUDA device is "
-                           "available (there is no CPU fallback)")
-    return torch.device('cuda', torch.cuda.current_device())
+_KERNEL = "the Bayesian-NN NUTS baseline runs on the sm_90a kernel of csrc/bnn_mcmc.cu"
 
 
 @torch.no_grad()
@@ -174,8 +167,8 @@ def sample_bnn_posterior(x_train, y_train, x_test, spec, num_samples, warmup_ste
         raise ValueError(f"the sampler keeps the training rows in shared memory: n={n} outside [1, {L.BNN_MAX_N}]")
     if not 1 <= max_tree_depth <= L.GP_MCMC_MAX_DEPTH:
         raise ValueError(f"max_tree_depth={max_tree_depth} outside [1, {L.GP_MCMC_MAX_DEPTH}]")
-    dev = _mcmc_device(x_train.device)
-    seed = L.mcmc_seed(seed)
+    dev = L.compute_device(x_train.device, _KERNEL)
+    seed = L.draw_seed(seed)
     n_test = 0 if x_test is None else x_test.shape[1]
     So = max(int(num_samples), 1)
     f64 = dict(dtype=torch.float64, device=dev)
@@ -212,8 +205,8 @@ def eval_mcmc(X, y, device, model_sampler, training_samples_n, warmup_steps, num
     the reference, which runs pyro there) selects the current CUDA device, and raises when there is none."""
     model = model_sampler()
     spec = {'num_features': model.num_features, 'embed': model.embed}
-    dev = _mcmc_device(device)
-    seed = L.mcmc_seed(seed)
+    dev = L.compute_device(device, _KERNEL)
+    seed = L.draw_seed(seed)
     X, y = X.to(dev), y.to(dev)
     k = training_samples_n
     r = sample_bnn_posterior(X[:, :k], y[:, :k], X[:, k:], spec, num_pred_samples, warmup_steps, seed)

@@ -14,73 +14,45 @@ import torch
 
 from .. import _lib as L
 from ..utils import default_device
-from .utils import get_batch_to_dataloader, _Deferred
+from .utils import check_flag, get_batch_to_dataloader, on_requested_device
 
 _JITTERS = (0.0, 1e-6, 1e-5, 1e-4)
+_KERNEL = "priors.fast_gp samples with the sm_90a GP kernel"
 
 
 class NotPSDError(RuntimeError):
     pass
 
 
-def _compute_device(device):
-    dev = torch.device(device)
-    if dev.type == 'cuda':
-        return dev
-    if not torch.cuda.is_available():
-        raise RuntimeError("priors.fast_gp samples with the sm_90a GP kernel; no CUDA device is available "
-                           "(there is no CPU fallback)")
-    return torch.device('cuda', torch.cuda.current_device())
+def sample_gp(x, z, lengthscale, outputscale, noise, kernel_type=L.KERNEL_RBF, return_factor=False, may_defer=True):
+    """x [B,T,F], z [B,T] on a CUDA device; lengthscale [B,F], outputscale [B], noise [B] -> y [B,T].
 
-
-def sample_gp(x, z, lengthscale, outputscale, noise, kernel_type=L.KERNEL_RBF, return_factor=False):
-    """x [B,T,F], z [B,T] on a CUDA device; lengthscale [B,F], outputscale [B], noise [B] -> y [B,T]."""
+    The pivot flags of the jitter-0 factorisation go through `check_flag`: while a loader defers (and `may_defer`), they
+    are looked at when the batch is handed to the consumer, a step later, with no host sync here.  Only if a pivot failed
+    is the whole batch re-factored with gpytorch's jitter escalation, overwriting y in place (every view handed out stays
+    valid).  With `return_factor` the check is immediate and the factor of the jitter that succeeded is returned too."""
     Bn, T, F = x.shape
     dev = x.device
     ldw = (T + 3) // 4 * 4
     y = torch.empty(Bn, T, device=dev, dtype=torch.float32)
     work = torch.empty(Bn, T, ldw, device=dev, dtype=torch.float32)
     info = torch.empty(Bn, device=dev, dtype=torch.int32)
+    L.gp_sample(x, z, lengthscale, outputscale, noise, _JITTERS[0], kernel_type, y, work, info)
 
-    def attempt(jitters):
-        for jitter in jitters:
+    def escalate():
+        nonlocal work
+        if work is None:
+            work = torch.empty(Bn, T, ldw, device=dev, dtype=torch.float32)
+        for jitter in _JITTERS[1:]:
             L.gp_sample(x, z, lengthscale, outputscale, noise, jitter, kernel_type, y, work, info)
             if not bool(info.any().item()):
                 return
         raise NotPSDError(f"kernel matrix not positive definite even with jitter {_JITTERS[-1]:g} "
                           f"(first failing pivots: {info[info > 0][:8].tolist()})")
 
-    if _Deferred.active and not return_factor:
-        # No host sync here: the pivot flags travel to pinned host memory behind the kernel and are looked at when the
-        # batch is handed to the consumer (a step later).  Only then -- and only if a pivot failed -- is the whole batch
-        # re-factored with gpytorch's jitter escalation, overwriting y in place (every view handed out stays valid).
-        L.gp_sample(x, z, lengthscale, outputscale, noise, _JITTERS[0], kernel_type, y, work, info)
-        bad = info.max().reshape(1)
-        bad_host = torch.empty(1, dtype=torch.int32, pin_memory=True)
-        bad_host.copy_(bad, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(dev))
-        del work
-
-        def resolve():
-            ev.synchronize()
-            if int(bad_host[0]) != 0:
-                nonlocal_work = torch.empty(Bn, T, ldw, device=dev, dtype=torch.float32)
-                _retry(x, z, lengthscale, outputscale, noise, kernel_type, y, nonlocal_work, info)
-        _Deferred.pending.append(resolve)
-        return y
-    attempt(_JITTERS)
+    if check_flag(info.max().reshape(1), escalate, may_defer and not return_factor):
+        work = None             # B T^2 floats not held through the step before the check; escalate allocates them again
     return (y, torch.tril(work[:, :, :T].transpose(1, 2))) if return_factor else y
-
-
-def _retry(x, z, lengthscale, outputscale, noise, kernel_type, y, work, info):
-    with torch.cuda.device(x.device):
-        for jitter in _JITTERS[1:]:
-            L.gp_sample(x, z, lengthscale, outputscale, noise, jitter, kernel_type, y, work, info)
-            if not bool(info.any().item()):
-                return
-    raise NotPSDError(f"kernel matrix not positive definite even with jitter {_JITTERS[-1]:g} "
-                      f"(first failing pivots: {info[info > 0][:8].tolist()})")
 
 
 def _hps_to_dict(hyperparameters):
@@ -100,7 +72,7 @@ def get_batch(batch_size, seq_len, num_features, device=default_device, hyperpar
     the caller — e.g. drawn on the host and kept in pinned memory — instead of being drawn on the device; they are
     copied to the device asynchronously."""
     hps = _hps_to_dict(hyperparameters)
-    dev = _compute_device(device)
+    dev = L.compute_device(device, _KERNEL)
     if x is not None:
         assert x.shape == (batch_size, seq_len, num_features)
         x = x.to(dev, torch.float32, non_blocking=True).contiguous()
@@ -118,10 +90,7 @@ def get_batch(batch_size, seq_len, num_features, device=default_device, hyperpar
     os_ = torch.full((batch_size,), float(hps["outputscale"]), device=dev)
     noise = torch.full((batch_size,), float(hps["noise"]), device=dev)
     y = sample_gp(x, z, ls, os_, noise, L.KERNEL_RBF)
-    x_t, y_t = x.transpose(0, 1), y.transpose(0, 1)
-    out_dev = torch.device(device)
-    if out_dev.type != 'cuda':
-        x_t, y_t = x_t.to(out_dev), y_t.to(out_dev)
+    x_t, y_t = on_requested_device(device, x.transpose(0, 1), y.transpose(0, 1))
     return x_t, y_t, y_t
 
 
@@ -224,7 +193,7 @@ def evaluate(x, y, y_non_noisy, use_mse=False, hyperparameters={}, get_model_on_
     hps = _hps_to_dict(hyperparameters if hyperparameters else None)
     if get_model_on_device is not None:
         return _evaluate_per_t(x, y, use_mse, hps, get_model_on_device, device, step_size, start_pos, start)
-    dev = _compute_device(device)
+    dev = L.compute_device(device, _KERNEL)
     xb = x.to(dev, torch.float32).transpose(0, 1).contiguous()            # [B,T,F]
     yb = y.to(dev, torch.float32).transpose(0, 1).contiguous()            # [B,T]
     Bn, T, F = xb.shape

@@ -27,8 +27,8 @@ from .. import _lib as L
 from ..bar_distribution import BarDistribution
 from ..utils import default_device
 from . import fast_gp
-from .fast_gp import _compute_device, sample_gp
-from .utils import get_batch_to_dataloader, _Deferred
+from .fast_gp import sample_gp
+from .utils import get_batch_to_dataloader, on_requested_device
 
 MIN_INFERRED_NOISE_LEVEL = 1e-4  # botorch.models.gp_regression.MIN_INFERRED_NOISE_LEVEL (noise constraint lower bound)
 
@@ -53,7 +53,7 @@ def get_batch(batch_size, seq_len, num_features, device=default_device, hyperpar
     [B,T,F] and normal draws [B,T] (e.g. pinned host memory), see priors.fast_gp.get_batch; only without fix_to_range."""
     assert num_outputs == 1
     hps = hyperparameters or {}
-    dev = _compute_device(device)
+    dev = L.compute_device(device, fast_gp._KERNEL)
     batch_size_per_gp_sample = (batch_size_per_gp_sample or max(batch_size // 10, 1))
     assert batch_size % batch_size_per_gp_sample == 0
     kernel_type = _NU_TO_KERNEL[float(hps.get('nu', 2.5))]
@@ -78,16 +78,10 @@ def get_batch(batch_size, seq_len, num_features, device=default_device, hyperpar
     plain = fix_to_range is None and not hps.get('y_minmax_norm') and not hps.get('sigmoid')
 
     def draw(xs):
-        if not plain and _Deferred.active:
-            _Deferred.active = False
-            try:
-                return draw(xs)
-            finally:
-                _Deferred.active = True
         n = xs.shape[0]
         ls, os_, noise = sample_hyperparameters(n, num_features, hps, dev)
         z = given_z if given_z is not None else torch.randn(n, seq_len, device=dev)
-        s = sample_gp(xs.contiguous(), z, ls, os_, noise, kernel_type)   # [n, T]
+        s = sample_gp(xs.contiguous(), z, ls, os_, noise, kernel_type, may_defer=plain)   # [n, T]
         if hps.get('y_minmax_norm'):
             lo, hi = s.min(1, keepdim=True)[0], s.max(1, keepdim=True)[0]
             s = (s - lo) / (hi - lo)
@@ -120,9 +114,7 @@ def get_batch(batch_size, seq_len, num_features, device=default_device, hyperpar
         x = x.view(-1, batch_size, seq_len, num_features)[0]
     x_t, y_t = x.transpose(0, 1), sample.transpose(0, 1)
     assert x_t.shape[:2] == y_t.shape[:2]
-    out_dev = torch.device(device)
-    if out_dev.type != 'cuda':
-        x_t, y_t = x_t.to(out_dev), y_t.to(out_dev)
+    x_t, y_t = on_requested_device(device, x_t, y_t)
     return x_t, y_t, y_t
 
 
@@ -174,12 +166,7 @@ def _check_fit_args(hyperparameters):
         "Sigmoid and y_minmax_norm can only be used to sample models..."
 
 
-def _fit_device(device):
-    dev = torch.device(device)
-    if dev.type != 'cuda':
-        raise RuntimeError(f"priors.fast_gp_mix fits with the sm_90a GP-fit kernel; device {dev} is not a CUDA device "
-                           "(there is no CPU fallback)")
-    return dev
+_FIT_KERNEL = "priors.fast_gp_mix fits with the sm_90a GP-fit kernel"
 
 
 def default_theta(n, num_features, hyperparameters, device):
@@ -281,7 +268,7 @@ def get_fitted_model(x, y, hyperparameters, device):
     """MAP-fitted (model, likelihood) on x [B,t,F], y [B,t] (reference :156-166): one pfn_gp_fit launch for all B.
     The model exposes the fitted lengthscale / outputscale / noise / mean_constant and f / status / iters per dataset."""
     _check_fit_args(hyperparameters)
-    dev = _fit_device(device)
+    dev = L.cuda_device(device, _FIT_KERNEL)
     xb, yb = x.to(dev, torch.float32).contiguous(), y.to(dev, torch.float32).contiguous()
     r = fit_map(xb, yb, [xb.shape[1]], hyperparameters)
     r = {k: v[0] for k, v in r.items()}
@@ -319,7 +306,7 @@ def evaluate(x, y, y_non_noisy, use_mse=False, hyperparameters={}, get_model_on_
     if T > MAX_FIT_T:
         raise ValueError(f"fast_gp_mix.evaluate keeps the t x t matrix of every fit in shared memory: T={T} exceeds "
                          f"the limit of {MAX_FIT_T}")
-    dev = _fit_device(device)
+    dev = L.cuda_device(device, _FIT_KERNEL)
     ts = list(range(max(start_pos, 1), T, step_size))
     means_list = [.0] if start_pos == 0 else []
     if not ts:
@@ -363,9 +350,9 @@ def sample_posterior(x, y, ts, hyperparameters=None, num_samples=MCMC_NUM_SAMPLE
     Bn, T, F = x.shape
     if T > MAX_FIT_T:
         raise ValueError(f"the GP sampler keeps the t x t matrix in shared memory: T={T} exceeds the limit of {MAX_FIT_T}")
-    dev = _fit_device(x.device)
+    dev = L.cuda_device(x.device, _FIT_KERNEL)
     kt, prior, _ = _fit_settings(hyperparameters)
-    seed = L.mcmc_seed(seed)
+    seed = L.draw_seed(seed)
     P, So = len(ts) * Bn, max(int(num_samples), 1)
     f64 = dict(dtype=torch.float64, device=dev)
     out = L.mcmc_outputs(P, F + 2, num_samples, warmup_steps, trace, dev)
@@ -444,7 +431,7 @@ def get_mcmc_model(x, y, hyperparameters, device, num_samples, warmup_steps, see
     passes them, or a batch x [B,t,F], y [B,t].  The model is the batch of GPs at the S samples (MCMCGP), the
     likelihood adds each sample's noise."""
     _check_fit_args(hyperparameters)
-    dev = _fit_device(device)
+    dev = L.cuda_device(device, _FIT_KERNEL)
     batched = x.dim() == 3
     xb = (x if batched else x.unsqueeze(0)).to(dev, torch.float32).contiguous()
     yb = (y if batched else y.unsqueeze(0)).to(dev, torch.float32).reshape(xb.shape[0], xb.shape[1]).contiguous()
@@ -503,7 +490,7 @@ def evaluate_(x, y, y_non_noisy, hyperparameters=None, device=default_device, nu
     if T > MAX_FIT_T:
         raise ValueError(f"fast_gp_mix.evaluate_ keeps the t x t matrix of every chain in shared memory: T={T} exceeds "
                          f"the limit of {MAX_FIT_T}")
-    dev = _fit_device(device)
+    dev = L.cuda_device(device, _FIT_KERNEL)
     losses_after_t = [.0] if min_seq_len == 0 else []
     ts = list(range(max(min_seq_len, 1), T))
     if not ts:

@@ -165,19 +165,14 @@ def episode_desc(bank, batch_size, n_way, k_shot, train=True, jonas_style=False,
     return d
 
 
-def _compute_device():
-    if not torch.cuda.is_available():
-        raise RuntimeError("priors.omniglot draws its episodes with the sm_90a Omniglot kernel; no CUDA device is available "
-                           "(there is no CPU fallback)")
-    return torch.device('cuda', torch.cuda.current_device())
+_KERNEL = "priors.omniglot draws its episodes with the sm_90a Omniglot kernel"
 
 
 @torch.no_grad()
 def sample_episodes(bank, desc, seed=None, device=None):
     """-> x [T, B, S²] fp32, y [T, B] int64, target_y [T, B] int64 on `device` (default: the current CUDA device)."""
-    dev = _compute_device() if device is None else torch.device(device)
-    if seed is None:
-        seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item())       # torch's CPU generator: no device sync
+    dev = L.compute_device(None, _KERNEL) if device is None else torch.device(device)
+    seed = L.draw_seed(seed)
     with L.on_device(dev):
         bank_t, alpha_start = bank.on_device(dev, desc.train)
         x = torch.empty(desc.T, desc.B, desc.S * desc.S, dtype=torch.float32, device=dev)
@@ -204,7 +199,7 @@ class DataLoader(PriorDataLoader):
         return self.num_steps
 
     def __iter__(self):
-        _compute_device()
+        L.compute_device(None, _KERNEL)
         return (self._batch() for _ in range(self.num_steps))
 
     def _batch(self):

@@ -19,26 +19,14 @@ from ..utils import default_device
 from .utils import get_batch_to_dataloader, normalize_data
 
 
-def _draw_seed():
-    return int(torch.randint(0, 2 ** 31 - 1, (1,)).item())       # torch's CPU generator: no device sync
-
-
-def _cuda_device(device):
-    dev = torch.device(device)
-    if dev.type != 'cuda':
-        raise RuntimeError(f"priors.pyro draws BayesianModel datasets with the sm_90a kernel of csrc/bnn_prior.cu; got "
-                           f"device {dev} (there is no CPU fallback)")
-    return dev if dev.index is not None else torch.device('cuda', torch.cuda.current_device())
-
-
 def sample_bnn_prior(batch_size, seq_len, num_features, embed, device, seed=None, dataset_offset=0, return_draws=False):
     """x [seq_len, B, F] fp32 (standardised), y [seq_len, B] fp32 from one kernel launch.  With return_draws also the
     oracle hook (weights [B, d] fp32, x_raw [seq_len, B, F] fp32, u [seq_len, B] fp64)."""
     d = embed * num_features + 3 * embed + 2
     if d > L.BNN_MAX_D:
         raise ValueError(f"priors.pyro: the network has d = E F + 3 E + 2 = {d} weights, above the limit of {L.BNN_MAX_D}")
-    dev = _cuda_device(device)
-    seed = _draw_seed() if seed is None else int(seed)
+    dev = L.cuda_device(device, "priors.pyro draws BayesianModel datasets with the sm_90a kernel of csrc/bnn_prior.cu")
+    seed = L.draw_seed(seed)
     with L.on_device(dev):
         x = torch.empty(seq_len, batch_size, num_features, dtype=torch.float32, device=dev)
         y = torch.empty(seq_len, batch_size, dtype=torch.float32, device=dev)

@@ -21,7 +21,7 @@ import torch
 
 from .. import _lib as L
 from ..utils import default_device
-from .utils import get_batch_to_dataloader, _Deferred
+from .utils import check_flag, get_batch_to_dataloader, on_requested_device
 
 # mnist_prior's keyword defaults (reference :9-10), as fractions of the image side
 PRIOR_DEFAULTS = dict(min_max_strokes=(1, 3), min_max_len=(5 / 28, 20 / 28), min_max_start=(2 / 28, 25 / 28),
@@ -68,21 +68,12 @@ def stroke_desc(size, num_outputs, max_iters=MAX_ITERS, **kwargs):
     return d
 
 
-def _rejection_message(d, kw):
+def _reject(d, kw):
     kw = dict(PRIOR_DEFAULTS, **kw)
-    return (f"priors.stroke: a class stroke found no end point inside [0, {d.S - 1}]^2 in {d.max_iters} rejection draws; "
-            f"min_max_len={kw['min_max_len']!r} (lengths {d.len_min}..{d.len_max}) is too long for "
-            f"min_max_start={kw['min_max_start']!r} (starts {d.start_min}..{d.start_max}) at size {d.S}")
-
-
-def _compute_device(device):
-    dev = torch.device(device)
-    if dev.type == 'cuda':
-        return dev
-    if not torch.cuda.is_available():
-        raise RuntimeError("priors.stroke draws its images with the sm_90a stroke kernels; no CUDA device is available "
-                           "(there is no CPU fallback)")
-    return torch.device('cuda', torch.cuda.current_device())
+    raise StrokeRejectionError(
+        f"priors.stroke: a class stroke found no end point inside [0, {d.S - 1}]^2 in {d.max_iters} rejection draws; "
+        f"min_max_len={kw['min_max_len']!r} (lengths {d.len_min}..{d.len_max}) is too long for "
+        f"min_max_start={kw['min_max_start']!r} (starts {d.start_min}..{d.start_max}) at size {d.S}")
 
 
 def class_table(batch_size, seq_len, num_outputs, only_train_for_last_idx, device):
@@ -108,23 +99,6 @@ def sample_geometry(batch_size, desc, seed, device):
     return geom, turns, flag
 
 
-def _check_flag(flag, desc, kw, dev):
-    if _Deferred.active:
-        # no host sync: the flag travels to pinned memory behind the kernels and is looked at when the batch is handed over
-        flag_host = torch.empty(1, dtype=torch.int32, pin_memory=True)
-        flag_host.copy_(flag, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(dev))
-
-        def resolve():
-            ev.synchronize()
-            if int(flag_host[0]) != 0:
-                raise StrokeRejectionError(_rejection_message(desc, kw))
-        _Deferred.pending.append(resolve)
-    elif int(flag.item()) != 0:
-        raise StrokeRejectionError(_rejection_message(desc, kw))
-
-
 @torch.no_grad()
 def get_batch(batch_size, seq_len, num_features=None, noisy_std=None, only_train_for_last_idx=False, normalize_x=False,
               num_outputs=2, use_saved_from=None, device=default_device, **kwargs):
@@ -141,8 +115,8 @@ def get_batch(batch_size, seq_len, num_features=None, noisy_std=None, only_train
     if only_train_for_last_idx:
         assert (seq_len - 1) % num_outputs == 0
     desc = stroke_desc(size, num_outputs, **kwargs)
-    dev = _compute_device(device)
-    seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item())       # torch's CPU generator: no device sync
+    dev = L.compute_device(device, "priors.stroke draws its images with the sm_90a stroke kernels")
+    seed = L.draw_seed()
 
     with L.on_device(dev):
         y = class_table(batch_size, seq_len, num_outputs, only_train_for_last_idx, dev)
@@ -154,11 +128,8 @@ def get_batch(batch_size, seq_len, num_features=None, noisy_std=None, only_train
             target_y[-1] = y[-1]
         else:
             target_y = y
-        _check_flag(flag, desc, kwargs, dev)
-    out_dev = torch.device(device)
-    if out_dev.type != 'cuda':
-        x, y, target_y = x.to(out_dev), y.to(out_dev), target_y.to(out_dev)
-    return x, y, target_y
+        check_flag(flag, lambda: _reject(desc, kwargs))
+    return on_requested_device(device, x, y, target_y)
 
 
 DataLoader = get_batch_to_dataloader(get_batch)

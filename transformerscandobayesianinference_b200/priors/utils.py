@@ -7,13 +7,14 @@ import scipy.stats as stats
 import torch
 from torch import nn
 
+from .. import _lib as L
 from ..utils import set_locals_in_self
 from .prior import PriorDataLoader
 
 
 class _Deferred:
     """Registry of device-side validity checks that a sampler could not finish without a host sync (e.g. the Cholesky
-    pivot flags of priors.fast_gp).  While `active`, samplers append a zero-argument callable instead of syncing; the
+    pivot flags of priors.fast_gp).  While `active`, `check_flag` appends a zero-argument callable instead of syncing; the
     prefetching loader runs them when the batch is handed to the consumer — a full step later, when the flags have long
     been copied to pinned host memory, so nothing stalls."""
     active = False
@@ -25,7 +26,34 @@ class _Deferred:
         return out
 
 
-def prefetch_enabled(device_hint=None):
+def check_flag(flag, on_set, may_defer=True):
+    """Calls `on_set()` when the int32 device tensor `flag` [1] is non-zero.  While a loader defers (and `may_defer`), the
+    flag travels to pinned host memory behind the work on the current stream and is looked at when the batch is handed
+    over; otherwise it is read at once (a host sync).  Returns whether the check was deferred."""
+    if not (may_defer and _Deferred.active):
+        if int(flag.item()) != 0:
+            on_set()
+        return False
+    flag_host = torch.empty(1, dtype=torch.int32, pin_memory=True)
+    flag_host.copy_(flag, non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(flag.device))
+
+    def resolve():
+        ev.synchronize()
+        if int(flag_host[0]) != 0:
+            on_set()
+    _Deferred.pending.append(resolve)
+    return True
+
+
+def on_requested_device(device, *tensors):
+    """A sampler's outputs, copied to `device` when the caller asked for a non-CUDA one (the sampler ran on CUDA)."""
+    dev = torch.device(device)
+    return tensors if dev.type == 'cuda' else tuple(t.to(dev) for t in tensors)
+
+
+def prefetch_enabled():
     import os
     return os.environ.get("PFN_B200_PREFETCH", "1") != "0" and torch.cuda.is_available()
 
@@ -77,8 +105,7 @@ def get_batch_to_dataloader(get_batch_method_):
         def _iter_prefetch(self):
             side = getattr(self, '_side_stream', None)
             if side is None:
-                dev = self.get_batch_kwargs.get('device', None)
-                dev = torch.device(dev) if dev is not None and torch.device(dev).type == 'cuda' else torch.device('cuda', torch.cuda.current_device())
+                dev = L.compute_device(self.get_batch_kwargs.get('device'), "the prefetching loader samples on a side stream")
                 side = self._side_stream = torch.cuda.Stream(device=dev, priority=0)
                 self._side_device = dev
 

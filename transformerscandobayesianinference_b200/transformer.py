@@ -10,7 +10,7 @@ import torch.nn as nn
 from torch.nn import TransformerEncoder, TransformerEncoderLayer
 
 from . import engine
-from ._lib import drop_threshold as L_drop_threshold
+from ._lib import draw_seed, drop_threshold as L_drop_threshold
 from .positional_encodings import NoPositionalEncoding
 from .utils import SeqBN
 
@@ -122,7 +122,7 @@ class TransformerModel(nn.Module):
         if self.training and self.dropout > 0:
             # one seed per forward from torch's CPU generator (reproducible under torch.manual_seed, no device sync); the
             # kernels derive per-layer / per-site counter-based masks from it
-            drop = (int(torch.randint(0, 2 ** 31 - 1, (1,)).item()), L_drop_threshold(self.dropout))
+            drop = (draw_seed(), L_drop_threshold(self.dropout))
         h = engine.EncoderStackFn.apply(h, T, B, sep, self.nhead, precision, torch.is_grad_enabled(), drop, *params)
 
         hq = h[sep * B:]
