@@ -66,9 +66,14 @@ class Call:
 
     @property
     def sig(self):
-        if self.fn != "gemm":
-            return self.fn
-        return "gemm/" + EPI_NAMES[int(self.a["epilogue"])] + ("/acc" if self.a["accumulate"] else "")
+        return call_sig(self.fn, self.a)
+
+
+def call_sig(fn, a):
+    """A call's entry in a call plan: the function, and for a GEMM its epilogue and whether it accumulates."""
+    if fn != "gemm":
+        return fn
+    return "gemm/" + EPI_NAMES[int(a["epilogue"])] + ("/acc" if a["accumulate"] else "")
 
 
 class Recorder:
@@ -115,6 +120,16 @@ def layer_plan(drop, u_is_grad, rowdot, fused_bias):
            + ["gemm/none/acc", "gemm/rowdot" if rowdot else "gemm/none", "attention_bwd"]
            + ([] if fused_bias else ["colsum"]) + ["gemm/none/acc", "gemm/none"])
     return fwd, bwd
+
+
+def step_plan(n_layers, drop, paths, bar):
+    """Call signatures of one training step: embedding, the stack's forward, the decoder head (and the bar loss), the
+    decoder's backward, the stack's backward (last layer first), the embedding's backward."""
+    pf, pb = layer_plan(drop, paths["u_is_grad"], paths["rowdot"], paths["fused_bias"])
+    head = ["gemm/gelu", "gemm/none"] + (["bar_nll_fwd", "bar_nll_bwd"] if bar else [])
+    dec_b = ["colsum", "gemm/none/acc", "gemm/mul" if paths["u_is_grad"] else "gemm/gelu_bwd", "colsum", "gemm/none/acc",
+             "gemm/none"]
+    return ["embed_fwd"] + pf * n_layers + head + dec_b + pb * n_layers + ["embed_bwd"]
 
 
 def _u(t):
@@ -290,7 +305,8 @@ class StageCheck:
                 gb = grads["in_b"]
                 self.bitwise("din_b q final", torch.equal(gb[:E], dq_sum))
                 self.bitwise("din_b k", bool((gb[E:2 * E] == 0).all()))
-                bound = EB.bias_v_fused(dattn, da, p["out_w"], c_ln1.out["colsum_out"], lb1, EB.C_ACC_TC)
+                bound = EB.bias_v_fused(dattn.double().abs().sum(0), da.double().abs().sum(0), p["out_w"],
+                                        c_ln1.out["colsum_out"], lb1, EB.C_ACC_TC)
                 self.chk("din_b v", gb[2 * E:], bb["dv"].sum(0), bound, EB.C_BIAS_FUSED)
         else:
             self.colsum("din_b", next(b), dqkv)
@@ -328,13 +344,10 @@ class StageCheck:
         N, nq = T * B, (T - sep) * B
         dt = torch.bfloat16 if precision == "bf16" else torch.float32
         n = len(layers)
-        pf, pb = layer_plan(bool(self.thr), self.paths["u_is_grad"], self.paths["rowdot"], self.paths["fused_bias"])
+        pf, _ = layer_plan(bool(self.thr), self.paths["u_is_grad"], self.paths["rowdot"], self.paths["fused_bias"])
         bar = borders is not None
-        dg = "gemm/mul" if self.paths["u_is_grad"] else "gemm/gelu_bwd"
-        head = ["gemm/gelu", "gemm/none"] + (["bar_nll_fwd", "bar_nll_bwd"] if bar else [])
-        dec_b = ["colsum", "gemm/none/acc", dg, "colsum", "gemm/none/acc", "gemm/none"]
         sig = [c.sig for c in calls]
-        want = ["embed_fwd"] + pf * n + head + dec_b + pb * n + ["embed_bwd"]
+        want = step_plan(n, bool(self.thr), self.paths, bar)
         assert sig == want, f"step: call plan {sig} != expected {want}"
         Wx, bx, wy, by = emb
         W0, b0, W2, b2 = dec
@@ -403,3 +416,190 @@ class StageCheck:
     def report(self, what):
         for stage, r in self.worst.items():
             print(f"[engine-stages] {what} {stage}: worst err/bound = {r:.4g}")
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Full-size steps: the reductions over the token axis checked as they happen
+# ----------------------------------------------------------------------------------------------------------------------
+# Stage names of the reduction calls in one layer's backward, in call order, per signature
+_LAYER_REDUCTIONS = {"gemm/none/acc": ("dw2", "dw1", "dw_out", "dw_in"),
+                     "layernorm_bwd": (("dg2", "dbe2", "db2"), ("dg1", "dbe1", "dout_b")),
+                     "attention_bwd": ("din_b q",)}
+_DEC_REDUCTIONS = {"gemm/none/acc": ("dec dW2", "dec dW0"), "colsum": ("dec db2", "dec db0")}
+
+
+def _colsums(X, block):
+    """sum_i X_i and sum_i |X_i| over the rows in fp64, `block` rows at a time."""
+    s = a = 0.0
+    for r0 in range(0, X.shape[0], block):
+        Xd = X[r0:r0 + block].double()
+        s, a = s + Xd.sum(0), a + Xd.abs().sum(0)
+    return s, a
+
+
+def _name_calls(plan, names):
+    """Stage names of the calls of `plan` whose signature `names` lists (in order of appearance), None for the others."""
+    left = {k: list(v) for k, v in names.items()}
+    return [left[s].pop(0) if left.get(s) else None for s in plan]
+
+
+class ReductionCheck:
+    """Checks every reduction over the token axis of one training step while the step runs, for steps too large to
+    record (`Recorder` keeps tens of GB at the benchmark's batch).  `install` wraps the OUTPUTS entry points of `lib`;
+    every call's signature is asserted against the step's plan as it is made, and the calls that reduce over tokens
+    are checked right after they return, from their own operands (still alive then) and a copy of the small accumulated
+    output taken before the call:
+      wgrad GEMMs (accumulate)    against EB.gemm at C_ACC_WGRAD; the requested k_splits against splits(K, M, N) (the
+                                  engine's policy), and `k_splits[stage]` collects the split count that request
+                                  launches (EB.splitk_launch restates the kernel's rule; the library does not report it)
+      colsum                      against EB.colsum at C_ROWSUM
+      layernorm_bwd               dgamma, dbeta, colsum_out against EB.layernorm_bwd at C_LN_GRAD
+      attention_bwd's dq_colsum   against the column sums of the dQ third it stored (it sums the stored bf16 values)
+      embed_bwd                   against EB.embed_bwd at C_ROWSUM
+    The fp64 work takes `block` tokens at a time.  The fused in-projection bias keeps a few column sums per layer, and
+    `finish` checks its k and v thirds once the backward is complete.
+
+    n_layers, drop, paths as for StageCheck; head: "bar" or "bce" for a whole step (embedding and decoder included),
+    None for the encoder stack alone."""
+
+    def __init__(self, lib, *, n_layers, drop, paths, head, num_sms, splits, block=1 << 16, c=None, tag=""):
+        self.lib, self.num_sms, self.splits, self.block, self.c, self.tag = lib, num_sms, splits, block, c, tag
+        self.paths = paths
+        pf, pb = layer_plan(drop, paths["u_is_grad"], paths["rowdot"], paths["fused_bias"])
+        col = ("db2", "db1", "dout_b", "din_b") if drop else ("db1",) + (() if paths["fused_bias"] else ("din_b",))
+        layer_names = _name_calls(pb, dict(_LAYER_REDUCTIONS, colsum=col))
+        if not paths["fused_bias"]:
+            layer_names = [None if s == "attention_bwd" else n for s, n in zip(pb, layer_names)]
+        if head is None:
+            self.plan = pf * n_layers + pb * n_layers
+            pre = [None] * (len(pf) * n_layers)
+        else:
+            self.plan = step_plan(n_layers, drop, paths, head == "bar")
+            n_pre = 1 + len(pf) * n_layers + (4 if head == "bar" else 2)
+            pre = [None] * n_pre + _name_calls(self.plan[n_pre:n_pre + 6], _DEC_REDUCTIONS)
+        self.names = pre + layer_names * n_layers + ([] if head is None else ["embed"])
+        self.layer_of = [None] * len(pre) + [li for li in reversed(range(n_layers)) for _ in pb] + [None] * (head is not None)
+        self.sigs = []
+        self.worst = {}
+        self.k_splits = {}
+        self.fused = {}
+        self._orig = {}
+
+    def install(self):
+        for name in OUTPUTS:
+            real = getattr(self.lib, name)
+            self._orig[name] = real
+            setattr(self.lib, name, self._wrap(name, real))
+        return self
+
+    def remove(self):
+        for name, real in self._orig.items():
+            setattr(self.lib, name, real)
+        self._orig = {}
+
+    def _wrap(self, name, real):
+        sig = inspect.signature(real)
+        outs = OUTPUTS[name]
+
+        def wrapper(*args, **kwargs):
+            b = sig.bind(*args, **kwargs)
+            b.apply_defaults()
+            a = b.arguments
+            i, s = len(self.sigs), call_sig(name, a)
+            want = self.plan[i] if i < len(self.plan) else "the end of the step"
+            assert s == want, f"{self.tag}call {i} is {s} where the plan has {want} (after {self.sigs[-3:]})"
+            self.sigs.append(s)
+            stage = self.names[i]
+            if stage is None:
+                return real(*args, **kwargs)
+            before = {k: a[k].clone() for k in outs if a.get(k) is not None and k not in ("dz", "dqkv", "delta")}
+            # the engine zeroes every gradient it accumulates into: a second sum into one would pass its own bound
+            assert all(bool((t == 0).all()) for t in before.values()), f"{self.tag}{stage}: accumulates into a nonzero gradient"
+            r = real(*args, **kwargs)
+            if a[outs[0]].is_cuda:
+                torch.cuda.synchronize()
+            getattr(self, "_" + name)(stage, self.layer_of[i], a, before)
+            return r
+        return wrapper
+
+    # ---------------------------------------------------------------- checks
+    def chk(self, stage, got, exact, bound, c):
+        r = EB.check(f"{self.tag}{stage}", got, exact, bound, self.c if self.c is not None else c, verbose=False)
+        self.worst[stage] = max(self.worst.get(stage, 0.0), r)
+
+    def bitwise(self, stage, ok):
+        assert bool(ok), f"{self.tag}{stage}: not bitwise equal to its exact value"
+        self.worst.setdefault(stage, 0.0)
+
+    def _gemm(self, stage, li, a, before):
+        M, N, K = a["M"], a["N"], a["K"]
+        A = a["A"].t() if a["a_mn_major"] else a["A"]
+        Bm = a["B"].t() if a["b_mn_major"] else a["B"]
+        assert A.shape == (M, K) and Bm.shape == (N, K) and a["C"].shape == (M, N), f"{self.tag}{stage}: operand shapes"
+        want = self.splits(K, M, N)
+        assert a["k_splits"] == want, f"{self.tag}{stage}: k_splits {a['k_splits']}, expected {want}"
+        self.k_splits.setdefault(stage, set()).add(EB.splitk_launch(K, a["k_splits"])[0])
+        c_acc = EB.C_ACC_WGRAD if A.dtype == torch.bfloat16 else EB.C_ACC_SIMT
+        ex, bd, _ = EB.gemm(A, Bm, _u(a["C"]), c_acc, aux=before["C"], block_k=self.block)
+        self.chk(stage, a["C"], ex, bd, EB.C_GEMM)
+
+    def _colsum(self, stage, li, a, before):
+        X = a["X"] if a["N"] is None else a["X"][:, :a["N"]]
+        depth = EB.colsum_depth(X.shape[0], X.shape[1], X.stride(0), X.element_size(), self.num_sms)
+        ex, bd = EB.colsum(X, before["out"], depth, self.block)
+        self.chk(stage, a["out"], ex, bd, EB.C_ROWSUM)
+
+    def _layernorm_bwd(self, names, li, a, before):
+        z, cs = a["z"], a["colsum_out"]
+        rows, E = z.shape
+        vec = EB.ln_vec(E, [a["dh"].stride(0), z.stride(0), a["dz"].stride(0)])
+        depth = EB.ln_bwd_colsum_depth(rows, E, z.element_size(), vec, self.num_sms)
+        init = (before["dgamma"], before["dbeta"], before["colsum_out"] if cs is not None else torch.zeros_like(a["dbeta"]))
+        b = EB.layernorm_bwd(a["dh"], z, a["gamma"], a["mean"], a["rstd"], _u(z), depth, init, block_rows=self.block)
+        self.chk(names[0], a["dgamma"], b["dgamma"], b["dgamma_bound"], EB.C_LN_GRAD)
+        self.chk(names[1], a["dbeta"], b["dbeta"], b["dbeta_bound"], EB.C_LN_GRAD)
+        if cs is not None:
+            self.chk(names[2], cs, b["colsum"], b["colsum_bound"], EB.C_LN_GRAD)
+        if names[2] == "dout_b" and self.paths["fused_bias"]:
+            # the LN1 backward's dz is the out-projection's upstream gradient da: what the fused v third is formed from
+            self.fused[li] = {"colsum_out": cs.clone(), "ln_b": b, "da_abs": _colsums(a["dz"], self.block)[1]}
+
+    def _attention_bwd(self, stage, li, a, before):
+        E = a["dout"].shape[1]
+        T, B = a["T"], a["B"]
+        dq = a["dqkv"][:, :E]
+        ex, bd = EB.colsum(dq, before["dq_colsum"], EB.dq_colsum_depth(T, B), self.block)
+        self.chk(stage, a["dq_colsum"], ex, bd, EB.C_ROWSUM)
+        f = self.fused[li]
+        f["dq_colsum"] = a["dq_colsum"].clone()
+        f["dattn"], f["dattn_abs"] = _colsums(a["dout"], self.block)
+
+    def _embed_bwd(self, stage, li, a, before):
+        T, B, F, sep = a["T"], a["B"], a["F"], a["sep"]
+        eb = EB.embed_bwd(a["dout"], a["x"].reshape(T * B, F), a["y"].reshape(T * B), sep * B, EB.embed_bwd_depth(T * B),
+                          block_rows=self.block)
+        for name in ("dWx", "dbx", "dwy", "dby"):
+            got = a[name]
+            self.chk("embed " + name, got, eb[name][0].reshape(got.shape), eb[name][1].reshape(got.shape), EB.C_ROWSUM)
+
+    def finish(self, layers, grads):
+        """After the backward: the whole plan ran, and the fused in-projection bias of every layer (layers / grads: the
+        layers' fp32 parameters / final gradients by LAYER_PARAM_NAMES) has its q third from the dQ kernel, a zero k
+        third and a v third colsum(dz1) W_out within EB.bias_v_fused of the column sums of the stored dO."""
+        assert self.sigs == self.plan, f"{self.tag}the step made {len(self.sigs)} of the plan's {len(self.plan)} calls"
+        if not self.paths["fused_bias"]:
+            return
+        assert sorted(self.fused) == list(range(len(layers))), f"{self.tag}fused bias summaries {sorted(self.fused)}"
+        for li, f in self.fused.items():
+            gb = grads[li]["in_b"]
+            E = gb.shape[0] // 3
+            self.bitwise("din_b q final", torch.equal(gb[:E], f["dq_colsum"]))
+            self.bitwise("din_b k", bool((gb[E:2 * E] == 0).all()))
+            bound = EB.bias_v_fused(f["dattn_abs"], f["da_abs"], layers[li]["out_w"], f["colsum_out"], f["ln_b"],
+                                    EB.C_ACC_TC)
+            self.chk("din_b v", gb[2 * E:], f["dattn"], bound, EB.C_BIAS_FUSED)
+
+    def report(self, what):
+        for stage, r in self.worst.items():
+            print(f"[error-budget] {what} {stage}: worst err/bound = {r:.4g}")
+        print(f"[k-splits launched] {what} " + ", ".join(f"{s} {sorted(v)}" for s, v in self.k_splits.items()))

@@ -195,7 +195,18 @@ def check_attention_bwd(dqkv, b, c, tag=""):
 # ------------------------------------------------------------------------------------------------------------------
 # GEMM  C = epi(A B^T + bias) (+ aux), A [M, K], B [N, K] as logical (already transposed) operands
 # ------------------------------------------------------------------------------------------------------------------
-def gemm(A, B, u_out, c_acc, bias=None, aux=None, epilogue="none", fast_gelu=True):
+def _products(A, B, block_k):
+    """A B^T and |A||B|^T in fp64, summed over blocks of block_k columns of the contraction: an fp64 copy of one block of
+    each operand at a time, never of a whole operand (a weight gradient contracts over every token of the step)."""
+    acc = mag = 0.0
+    for k0 in range(0, A.shape[1], block_k):
+        Ad, Bd = A[:, k0:k0 + block_k].double(), B[:, k0:k0 + block_k].double()
+        acc = acc + Ad @ Bd.t()
+        mag = mag + Ad.abs() @ Bd.abs().t()
+    return acc, mag
+
+
+def gemm(A, B, u_out, c_acc, bias=None, aux=None, epilogue="none", fast_gelu=True, block_k=None):
     """Exact result and bound of one GEMM launch.  A, B: the logical [M, K] / [N, K] operands (bf16 or fp32 values).
 
     The fp32 accumulation over K contributes c_acc U32 K (|A||B|^T) -- the worst-case model of a K-term sum, scaled by the
@@ -206,11 +217,16 @@ def gemm(A, B, u_out, c_acc, bias=None, aux=None, epilogue="none", fast_gelu=Tru
       "gelu_grad" gelu'(acc + bias), the forward's C2 output (GELU_GRAD_ABS + TANH_REL (1 + |x|))
       "gelu_bwd"  acc * gelu'(aux)
       "mul"       acc * aux
-    fast_gelu=False for the SIMT kernels, which evaluate erff: no approximant term.  Returns (exact, bound, pre) with pre = acc + bias in fp64."""
-    Ad, Bd = A.double(), B.double()
-    K = Ad.shape[1]
-    acc = Ad @ Bd.t()
-    acc_err = c_acc * U32 * K * (Ad.abs() @ Bd.abs().t())
+    fast_gelu=False for the SIMT kernels, which evaluate erff: no approximant term.  block_k: take the contraction that many
+    columns at a time (a weight gradient's K is the step's token count).  Returns (exact, bound, pre) with pre = acc + bias
+    in fp64."""
+    K = A.shape[1]
+    if block_k is None:
+        Ad, Bd = A.double(), B.double()
+        acc, mag = Ad @ Bd.t(), Ad.abs() @ Bd.abs().t()
+    else:
+        acc, mag = _products(A, B, block_k)
+    acc_err = c_acc * U32 * K * mag
     pre = acc if bias is None else acc + bias.double()
     g_abs, g_grad_abs, t_rel = (GELU_ABS, GELU_GRAD_ABS, TANH_REL) if fast_gelu else (0.0, 0.0, 0.0)
     auxd = None if aux is None else aux.double()
@@ -304,7 +320,7 @@ def layernorm_fwd(z, gamma, beta, u, eps=1e-5):
             "rstd": r.squeeze(-1), "rstd_bound": (r * r_rel).squeeze(-1)}
 
 
-def layernorm_bwd(dh, z, gamma, mean_k, rstd_k, u, colsum_depth, init=None, eps=1e-5):
+def layernorm_bwd(dh, z, gamma, mean_k, rstd_k, u, colsum_depth, init=None, eps=1e-5, block_rows=None):
     """Exact dz, dgamma, dbeta, colsum_out = sum_rows dz of LayerNorm for the upstream dh, and their bounds.
 
     The exact values use fp64 statistics of z.  The kernel reads the mean and rstd the forward stored (mean_k, rstd_k);
@@ -312,7 +328,38 @@ def layernorm_bwd(dh, z, gamma, mean_k, rstd_k, u, colsum_depth, init=None, eps=
     inherited term E.  dz = r (g - mean g - x^ mean(g x^)), g = dh gamma: the three terms cancel, so its rounding is
     bounded by their magnitudes, U32 (a + 4) r (|g| + mean|g| + |x^| mean|g x^|) with a the row sum's depth, plus
     u |dz| for the store.  The column sums over rows: U32 colsum_depth times the sum of the terms' magnitudes.
-    init: the values the column outputs held before the call (accumulated into); eps: the forward's."""
+    init: the values the column outputs held before the call (accumulated into); eps: the forward's.
+    block_rows: work through the rows that many at a time and return the column results only (no per-row dz), so that
+    a full-size step needs no fp64 copy of a whole activation.  "dz_bound_sum" (the column sums of dz's bound) is
+    returned either way."""
+    rows, E = z.shape
+    step = block_rows or max(rows, 1)
+    sums = torch.zeros(9, E, dtype=torch.float64, device=z.device)
+    out = {}
+    for r0 in range(0, rows, step):
+        sl = slice(r0, r0 + step)
+        dz, dz_b, parts = _ln_bwd_rows(dh[sl], z[sl], gamma, mean_k[sl], rstd_k[sl], u, eps)
+        sums += parts
+        if block_rows is None:
+            out["dz"], out["dz_bound"] = dz, dz_b
+    if init is None:
+        init = torch.zeros(3, E, dtype=torch.float64, device=z.device)
+    init = [t.double() for t in init]
+    d_col = U32 * (colsum_depth + 3)
+    dxh, dxh_abs, dex, dd, dd_abs, dzs, dz_abs, dz_f32b, dz_bs = sums
+    out.update({"dgamma": init[0] + dxh,
+                "dgamma_bound": d_col * (dxh_abs + init[0].abs()) + dex,
+                "dbeta": init[1] + dd,
+                "dbeta_bound": d_col * (dd_abs + init[1].abs()),
+                "colsum": init[2] + dzs,
+                # colsum_out sums the kernel's fp32 dz before it is stored: its terms carry dz's fp32 error, not the store's
+                "colsum_bound": d_col * (dz_abs + init[2].abs()) + dz_f32b,
+                "dz_bound_sum": dz_bs})
+    return out
+
+
+def _ln_bwd_rows(dh, z, gamma, mean_k, rstd_k, u, eps):
+    """layernorm_bwd on a block of rows: dz, its bound and the column sums [9, E] of the terms the column outputs need."""
     zd, dd, gd = z.double(), dh.double(), gamma.double()
     E = zd.shape[-1]
     mu = zd.mean(-1, keepdim=True)
@@ -327,19 +374,10 @@ def layernorm_bwd(dh, z, gamma, mean_k, rstd_k, u, colsum_depth, init=None, eps=
     dz_mag = r * (g.abs() + g.abs().mean(-1, keepdim=True) + xh.abs() * (g * xh).abs().mean(-1, keepdim=True))
     dz_inh = eps_r * dz.abs() + r * (e_x * s2.abs() + xh.abs() * (g.abs() * e_x).mean(-1, keepdim=True))
     dz_b = u * dz.abs() + U32 * (a + 4) * dz_mag + dz_inh
-    if init is None:
-        init = torch.zeros(3, E, dtype=torch.float64, device=zd.device)
-    init = [t.double() for t in init]
-    d_col = U32 * (colsum_depth + 3)
-    out = {"dz": dz, "dz_bound": dz_b,
-           "dgamma": init[0] + (dd * xh).sum(0),
-           "dgamma_bound": d_col * ((dd * xh).abs().sum(0) + init[0].abs()) + (dd.abs() * e_x).sum(0),
-           "dbeta": init[1] + dd.sum(0),
-           "dbeta_bound": d_col * (dd.abs().sum(0) + init[1].abs()),
-           "colsum": init[2] + dz.sum(0),
-           # colsum_out sums the kernel's fp32 dz before it is stored: its terms carry dz's fp32 error, not the store's
-           "colsum_bound": d_col * (dz.abs().sum(0) + init[2].abs()) + (dz_b - u * dz.abs() + U32 * dz.abs()).sum(0)}
-    return out
+    dxh = dd * xh
+    parts = torch.stack([dxh.sum(0), dxh.abs().sum(0), (dd.abs() * e_x).sum(0), dd.sum(0), dd.abs().sum(0), dz.sum(0),
+                         dz.abs().sum(0), (dz_b - u * dz.abs() + U32 * dz.abs()).sum(0), dz_b.sum(0)])
+    return dz, dz_b, parts
 
 
 def colsum_depth(rows, N, ld, elem_size, num_sms, aligned=True):
@@ -382,6 +420,16 @@ def dropout(x, keep, thr, residual=None, u_out=U):
     return val, u_out * val.abs() + U32 * (kept * s + val.abs()) + abs(s32 - s) * kept
 
 
+def splitk_launch(K, k_splits, block_k=64):
+    """(splits, k-blocks per split) the tensor-core GEMM launches for a requested k_splits (gemm_tc.cu, pfn_gemm_bf16_tc):
+    at most one split per 64-wide k-block, an equal share of ceil(num_kb / splits) k-blocks each, and only as many splits
+    as those shares need, so a request can launch fewer splits than it asked for."""
+    num_kb = _cdiv(K, block_k)
+    splits = min(max(k_splits, 1), num_kb)
+    per = _cdiv(num_kb, splits)
+    return _cdiv(num_kb, per), per
+
+
 def rowdot_depth(width, block_n=128):
     """Longest addition chain of a ROWDOT sum (gemm_tc.cu epi_pair / the epilogue's quad shuffles): a lane's fmaf chain
     over its block_n / 4 columns of one tile, two shuffles, one atomic per tile of the group, the zeroed initial value."""
@@ -402,7 +450,15 @@ def rowdot(C, aux, width):
     return prod.sum(-1), U32 * rowdot_depth(width) * prod.abs().sum(-1)
 
 
-def bias_v_fused(dattn, da, out_w, colsum_out, ln_b, c_acc):
+def dq_colsum_depth(T, B):
+    """Depth of the tensor-core attention backward's dq_colsum (attention_bwd_tc.cu): a lane adds its two rows, three
+    shuffles reduce the warp's 16 rows, then one fp32 atomic per column and warp: 8 warps per 128-row query tile, every
+    tile of every sequence, plus the initial value.  The kernel sums the bf16 values it stores, so the column sums of the
+    stored dQ are the exact value."""
+    return 2 + 3 + 8 * _cdiv(T, 128) * B + 1
+
+
+def bias_v_fused(dattn_abs, da_abs, out_w, colsum_out, ln_b, c_acc):
     """Bound of the in-projection bias gradient's v third when it is formed as colsum_out W_out (fp32) instead of the
     column sums of dV.  The exact value is sum_i dO_i over the stored dO = dattn (the rows of P sum to 1), so the bound
     collects how far colsum_out W_out may be from it:
@@ -411,14 +467,15 @@ def bias_v_fused(dattn, da, out_w, colsum_out, ln_b, c_acc):
       (colsum_bound + sum_i dz_bound_i) |W|                   colsum_out (the LayerNorm backward's fp32 sums of dz)
                                                               against the column sums of the stored dz = da
       U32 E |colsum_out| |W|                                  the fp32 matrix-vector product
-    with W = out_w [E_out, E_in] (fp32 master) and ln_b the layernorm_bwd bounds of that LayerNorm."""
+    with W = out_w [E_out, E_in] (fp32 master), dattn_abs = sum_i |dattn_i| and da_abs = sum_i |da_i| (column sums over
+    the tokens) and ln_b the layernorm_bwd bounds of that LayerNorm."""
     W = out_w.double()
     Wa = W.abs()
     Wb = out_w.to(torch.bfloat16).double().abs()
     E = W.shape[0]
     cs = colsum_out.double().abs()
-    inh = ln_b["colsum_bound"] + ln_b["dz_bound"].sum(0)
-    return (U * dattn.double().abs().sum(0) + c_acc * U32 * E * (da.double().abs().sum(0) @ Wb)
+    inh = ln_b["colsum_bound"] + ln_b["dz_bound_sum"]
+    return (U * dattn_abs.double() + c_acc * U32 * E * (da_abs.double() @ Wb)
             + (U * cs + inh + U32 * E * cs) @ Wa)
 
 
@@ -438,15 +495,22 @@ def embed_bwd_depth(rows):
     return min(rows, 512) + _cdiv(rows, 512) + 1
 
 
-def embed_bwd(dout, x, y, sep, depth):
-    """Exact dWx, dbx, dwy, dby of the embedding for dout [rows, E] (train rows: the first sep*B), and their bounds."""
-    dd, xd, yd = dout.double(), x.double(), y.double().reshape(-1)
-    t = (torch.arange(dd.shape[0], device=dd.device) < sep).double()
+def embed_bwd(dout, x, y, sep, depth, block_rows=None):
+    """Exact dWx, dbx, dwy, dby of the embedding for dout [rows, E] (train rows: the first sep*B), and their bounds.
+    block_rows: sum over that many rows at a time (fp64 copies of one block only)."""
+    rows = dout.shape[0]
+    y = y.reshape(-1)
+    step = block_rows or max(rows, 1)
+    s = [0.0] * 8
+    for r0 in range(0, rows, step):
+        dd, xd, yd = dout[r0:r0 + step].double(), x[r0:r0 + step].double(), y[r0:r0 + step].double()
+        t = (torch.arange(r0, r0 + dd.shape[0], device=dd.device) < sep).double()
+        da, ty = dd.abs(), t * yd
+        parts = (dd.t() @ xd, da.t() @ xd.abs(), dd.sum(0), da.sum(0), ty @ dd, ty.abs() @ da, t @ dd, t @ da)
+        s = [a + b for a, b in zip(s, parts)]
     d_col = U32 * (depth + 1)
-    return {"dWx": (dd.t() @ xd, d_col * (dd.abs().t() @ xd.abs())),
-            "dbx": (dd.sum(0), d_col * dd.abs().sum(0)),
-            "dwy": ((t * yd) @ dd, d_col * ((t * yd).abs() @ dd.abs())),
-            "dby": (t @ dd, d_col * (t @ dd.abs()))}
+    return {"dWx": (s[0], d_col * s[1]), "dbx": (s[2], d_col * s[3]), "dwy": (s[4], d_col * s[5]),
+            "dby": (s[6], d_col * s[7])}
 
 
 # bar NLL -----------------------------------------------------------------------------------------------------------

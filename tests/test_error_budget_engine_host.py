@@ -45,11 +45,14 @@ class FakeLib:
     def __init__(self):
         self.noscale = False             # slip: dropout without 1 / (1 - p)
         self.rowdot_unrounded = False    # slip: ROWDOT from the fp32 accumulator instead of the stored bf16 C
+        self.wgrad_lost_token = False    # slip: a weight gradient without the step's last token
 
     def gemm(self, A, B, C, *, a_mn_major=False, b_mn_major=False, bias=None, aux=None, C2=None, epilogue=0,
              accumulate=False, k_splits=1, M=None, N=None, K=None, use_tc=None, rowdot=None, c2_gelu_grad=False):
         Al = (A.t() if a_mn_major else A).double()
         Bl = (B.t() if b_mn_major else B).double()
+        if accumulate and self.wgrad_lost_token:
+            Al, Bl = Al[:, :-1], Bl[:, :-1]
         y = (Al @ Bl.t()).float()
         if bias is not None:
             y = y + bias.float()
@@ -79,12 +82,12 @@ class FakeLib:
             km = keep_bits(drop[0], B * H * T, T, drop[1]).double().reshape(B, H, T, T) * (256.0 / (256 - drop[1]))
         return q, k, v, s, P, km
 
-    def attention_fwd(self, qkv, out, lse, T_, B_, H_, dh, sep, use_tc=None, batch_major=False, drop=None):
+    def attention_fwd(self, qkv, out, lse, T, B, H, dh, sep, use_tc=None, batch_major=False, drop=None):
         q, k, v, s, P, km = self._probs(qkv, drop)
         out.copy_(_tokens((P * km) @ v).to(out.dtype))
         lse.copy_(torch.logsumexp(s, -1).reshape(B * H, T).float())
 
-    def attention_bwd(self, qkv, out, lse, dout, dqkv, delta, T_, B_, H_, dh, sep, use_tc=None, batch_major=False,
+    def attention_bwd(self, qkv, out, lse, dout, dqkv, delta, T, B, H, dh, sep, use_tc=None, batch_major=False,
                       drop=None, dq_colsum=None, delta_token_major=False):
         q, k, v, s, P, km = self._probs(qkv, drop)
         do = _heads(dout)
@@ -294,3 +297,58 @@ def test_wiring_slip_falls_outside_its_stage(slip, thr, stage):
     assert f"{slip}: {stage}:" in str(e.value), str(e.value)
     print(f"[engine-stages host] {slip}: {str(e.value)[:160]}; old end-to-end tolerances "
           f"{'pass' if _old_tolerances_pass(grads, ref) else 'fail'} it")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ES.ReductionCheck, the inline checker of the full-size steps, on the same restatement: its wrappers assert the call plan
+# as the calls are made and check the token-axis reductions from the calls' own operands, 7 rows at a time (a block that
+# does not divide the 48 tokens)
+# ---------------------------------------------------------------------------------------------------------------------
+def _reductions(thr, slip=None, c=None):
+    layers, src, dout = _params(3)
+    lib = FakeLib()
+    lib.wgrad_lost_token = slip == "wgrad_lost_token"
+    chk = ES.ReductionCheck(lib, n_layers=NLAYERS, drop=bool(thr), head=None, num_sms=NUM_SMS, block=7, c=c,
+                            paths={"u_is_grad": True, "rowdot": True, "fused_bias": not thr},
+                            splits=lambda K, M, N: 1, tag=f"{slip or 'clean'}: ").install()
+    try:
+        _, grads = stack_step(lib, layers, src, dout, thr, slip)
+    finally:
+        chk.remove()
+    chk.finish(layers, grads)
+    return chk
+
+
+@pytest.mark.parametrize("thr", [0, THR])
+def test_reduction_check_restatement_inside_bounds_at_c1(thr):
+    chk = _reductions(thr, c=1.0)
+    chk.report(f"restatement thr={thr}")
+    want = {"dw2", "dw1", "dw_out", "dw_in", "dg2", "dbe2", "db2", "db1", "dg1", "dbe1", "dout_b"}
+    want |= {"din_b"} if thr else {"din_b q", "din_b q final", "din_b k", "din_b v"}
+    assert set(chk.worst) == want
+    assert max(chk.worst.values()) <= 1.0
+    assert chk.k_splits == {s: {1} for s in ("dw2", "dw1", "dw_out", "dw_in")}
+
+
+@pytest.mark.parametrize("slip,thr,stage", [("wgrad_lost_token", 0, "dw2"), ("v_third_no_w", 0, "din_b v"),
+                                            ("b2_colsum_out_with_dropout", THR, "db2")])
+def test_reduction_check_catches_slip(slip, thr, stage):
+    """A weight gradient short of one token, a v third without W_out, and a bias gradient summed twice (the LN2 backward
+    of the dropout path handed the b2 gradient as well as the colsum after the mask)."""
+    with pytest.raises(AssertionError) as e:
+        _reductions(thr, slip)
+    assert f"{slip}: {stage}" in str(e.value), str(e.value)
+
+
+def test_reduction_check_asserts_the_plan_as_it_runs():
+    """A path the step does not take (the delta from a separate pass instead of the out-projection dgrad) fails at the
+    first call that differs, while the step runs."""
+    layers, src, dout = _params(3)
+    lib = FakeLib()
+    chk = ES.ReductionCheck(lib, n_layers=NLAYERS, drop=False, head=None, num_sms=NUM_SMS, splits=lambda K, M, N: 1,
+                            paths={"u_is_grad": True, "rowdot": False, "fused_bias": True}).install()
+    try:
+        with pytest.raises(AssertionError, match="is gemm/rowdot where the plan has gemm/none"):
+            stack_step(lib, layers, src, dout, 0)
+    finally:
+        chk.remove()

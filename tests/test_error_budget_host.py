@@ -169,3 +169,11 @@ def test_exact_attention_matches_autograd(T, B, H, dh, sep, p):
     for n, name in enumerate(("dq", "dk", "dv")):
         assert torch.allclose(b[name], qkv.grad[:, n * E:(n + 1) * E], atol=1e-11), name
         assert (b[name + "_bound"] >= 0).all()
+
+
+@pytest.mark.parametrize("K,req,want", [(640, 4, (4, 3)), (576, 4, (3, 3)), (64, 8, (1, 1)), (131072, 33, (33, 63)),
+                                        (512000, 16, (16, 500)), (512000, 5, (5, 1600)), (256000, 33, (33, 122))])
+def test_splitk_launch_normalises_the_request(K, req, want):
+    """Nine k-blocks asked to split 4 ways take 3 per split and so launch 3 splits; the engine's full-size requests
+    launch as asked."""
+    assert EB.splitk_launch(K, req) == want
