@@ -1,16 +1,16 @@
-"""The engine stage checks (oracle/engine_stages.py) on a CPU restatement of two bf16 encoder layers: the kernels are
-restated in float32 with bf16 rounding where the engine stores, the layers' forward and backward call them the way
-engine.EncoderStackFn does, and the calls are recorded and checked by the same code as the GPU test.  The correct
-restatement stays inside every bound at c = 1; each wiring slip below falls outside its stage's bound at the GPU
-constants.  Each slip also reports whether the end-to-end tolerances of the bf16 engine tests (gradient norms within
-6 %, elements within 8 % of the tensor's largest gradient) pass it."""
+"""The engine stage checks (oracle/engine_stages.py) on the CPU: engine.EncoderStackFn runs two bf16 encoder layers
+forward and backward through a float32 fake of the kernel library (the kernels restated with bf16 rounding where they
+store bf16), and the calls are recorded and checked by the same code as the GPU test.  The engine stays inside every
+bound at c = 1; each wiring slip below, made by the fake at the one library call it concerns, falls outside its stage's
+bound at the GPU constants.  Each slip also reports whether the end-to-end tolerances of the bf16 engine tests
+(gradient norms within 6 %, elements within 8 % of the tensor's largest gradient) pass it."""
 import math
-import types
 
 import pytest
 import torch
 
 from oracle import engine_stages as ES, error_budget as EB
+from transformerscandobayesianinference_b200 import _lib, engine
 
 T, B, H, DH, NHID, SEP, NLAYERS = 24, 2, 2, 128, 512, 10, 2
 E = H * DH
@@ -19,10 +19,7 @@ NUM_SMS = 132
 THR = 51                     # p = 0.2
 SEED = 1234567
 BF = torch.bfloat16
-
-
-def site_seed(seed, layer, site):
-    return (int(seed) + 0x9E3779B9 * (4 * layer + site + 1)) & 0xFFFFFFFF
+SITES = {engine.site_seed(SEED, li, site): (li, site) for li in range(NLAYERS) for site in range(4)}
 
 
 def keep_bits(seed, rows, cols, thr):
@@ -31,41 +28,58 @@ def keep_bits(seed, rows, cols, thr):
     return (torch.randint(0, 256, (rows, cols), generator=g) >= thr).to(torch.uint8)
 
 
-def _heads(t):
-    return t.double().reshape(T, B, H, DH).permute(1, 2, 0, 3)
-
-
-def _tokens(t):
-    return t.permute(2, 0, 1, 3).reshape(N, E)
-
-
 class FakeLib:
-    """The kernels as float32 restatements with the kernels' signatures; bf16 rounding wherever they store bf16."""
+    """What the engine reads of the kernel library: the kernels as float32 restatements with the kernels' signatures and
+    bf16 rounding wherever they store bf16, and the bf16 tensor-core path taken everywhere.  `slip` names one wiring
+    mistake, which the fake makes at the call it concerns."""
+    EPI_NONE, EPI_GELU, EPI_GELU_BWD, EPI_ROWDOT, EPI_MUL = (_lib.EPI_NONE, _lib.EPI_GELU, _lib.EPI_GELU_BWD,
+                                                             _lib.EPI_ROWDOT, _lib.EPI_MUL)
 
-    def __init__(self):
-        self.noscale = False             # slip: dropout without 1 / (1 - p)
-        self.rowdot_unrounded = False    # slip: ROWDOT from the fp32 accumulator instead of the stored bf16 C
-        self.wgrad_lost_token = False    # slip: a weight gradient without the step's last token
+    def __init__(self, slip=None):
+        self.slip = slip
+        self.backward = False     # the stack's backward has begun (its first call is a layernorm_bwd)
+        self.ln_bwd_calls = 0     # the backward of each layer calls layernorm_bwd for LN2, then for LN1
+        self.dz2 = None           # dz of the latest LN2 backward
+        self.b2_extra = None      # LN2's column sum of dz under dropout, for the next colsum
+        self.gelu_grads = []      # C2 of the forward's gemm/gelu calls, one per layer
 
-    def gemm(self, A, B, C, *, a_mn_major=False, b_mn_major=False, bias=None, aux=None, C2=None, epilogue=0,
+    def require_cuda(self, *tensors):
+        pass
+
+    def num_sms(self, device=None):
+        return NUM_SMS
+
+    def tc_gemm_ok(self, *args):
+        return True
+
+    def tc_attention_ok(self, *args):
+        return True
+
+    def gemm(self, A, B, C, *, a_mn_major=False, b_mn_major=False, bias=None, aux=None, C2=None, epilogue=EPI_NONE,
              accumulate=False, k_splits=1, M=None, N=None, K=None, use_tc=None, rowdot=None, c2_gelu_grad=False):
+        if epilogue == self.EPI_GELU:
+            self.gelu_grads.append(C2)
+        elif epilogue == self.EPI_MUL and self.slip == "gelu_grad_other_layer":
+            aux = next(u for u in self.gelu_grads if u is not aux)
+        if self.slip == "dh1_no_aux" and aux is not None and aux is self.dz2:
+            aux = None
         Al = (A.t() if a_mn_major else A).double()
         Bl = (B.t() if b_mn_major else B).double()
-        if accumulate and self.wgrad_lost_token:
+        if accumulate and self.slip == "wgrad_lost_token":
             Al, Bl = Al[:, :-1], Bl[:, :-1]
         y = (Al @ Bl.t()).float()
         if bias is not None:
             y = y + bias.float()
-        if epilogue == 1:
+        if epilogue == self.EPI_GELU:
             if C2 is not None:
                 C2.copy_((EB.gelu_grad(y.double()).float() if c2_gelu_grad else y).to(C2.dtype))
             y = torch.nn.functional.gelu(y)
-        elif epilogue == 2:
+        elif epilogue == self.EPI_GELU_BWD:
             y = y * EB.gelu_grad(aux.double()).float()
-        elif epilogue == 4:
+        elif epilogue == self.EPI_MUL:
             y = y * aux.float()
-        elif epilogue == 3:
-            c = y if self.rowdot_unrounded else y.to(C.dtype).float()
+        elif epilogue == self.EPI_ROWDOT:
+            c = y if self.slip == "delta_unrounded" else y.to(C.dtype).float()
             rd, w = rowdot
             rd += (c.double() * aux.double()).reshape(y.shape[0], -1, w).sum(-1).float()
         elif aux is not None:
@@ -73,7 +87,7 @@ class FakeLib:
         C.copy_((C.float() + y if accumulate else y).to(C.dtype))
 
     def _probs(self, qkv, drop):
-        q, k, v = (_heads(qkv[:, n * E:(n + 1) * E]) for n in range(3))
+        q, k, v = (EB._heads(qkv[:, n * E:(n + 1) * E].double(), T, B, H, DH) for n in range(3))
         ok = EB.allowed_keys(T, SEP, "cpu")
         s = (q @ k.transpose(-1, -2) / math.sqrt(DH)).masked_fill(~ok, float("-inf"))
         P = torch.softmax(s, -1)
@@ -84,22 +98,24 @@ class FakeLib:
 
     def attention_fwd(self, qkv, out, lse, T, B, H, dh, sep, use_tc=None, batch_major=False, drop=None):
         q, k, v, s, P, km = self._probs(qkv, drop)
-        out.copy_(_tokens((P * km) @ v).to(out.dtype))
+        out.copy_(EB._tokens((P * km) @ v, T, B, H, dh).to(out.dtype))
         lse.copy_(torch.logsumexp(s, -1).reshape(B * H, T).float())
 
     def attention_bwd(self, qkv, out, lse, dout, dqkv, delta, T, B, H, dh, sep, use_tc=None, batch_major=False,
                       drop=None, dq_colsum=None, delta_token_major=False):
+        if self.slip == "att_bwd_next_layer_seed" and drop is not None:
+            drop = (engine.site_seed(SEED, SITES[drop[0]][0] + 1, 0), drop[1])
         q, k, v, s, P, km = self._probs(qkv, drop)
-        do = _heads(dout)
+        do = EB._heads(dout.double(), T, B, H, dh)
         if delta_token_major:
             dl = delta.double().reshape(T, B, H).permute(1, 2, 0).unsqueeze(-1)
         else:
-            dl = (do * _heads(out)).sum(-1, keepdim=True)
+            dl = (do * EB._heads(out.double(), T, B, H, dh)).sum(-1, keepdim=True)
             delta.copy_(dl.squeeze(-1).reshape(B * H, T).float())
         dS = P * ((do @ v.transpose(-1, -2)) * km - dl) / math.sqrt(DH)
         grads = (dS @ k, dS.transpose(-1, -2) @ q, (P * km).transpose(-1, -2) @ do)
         for n, g in enumerate(grads):
-            dqkv[:, n * E:(n + 1) * E] = _tokens(g).to(dqkv.dtype)
+            dqkv[:, n * E:(n + 1) * E] = EB._tokens(g, T, B, H, dh).to(dqkv.dtype)
         if dq_colsum is not None:
             dq_colsum += dqkv[:, :E].double().sum(0).float()
 
@@ -112,6 +128,9 @@ class FakeLib:
         h.copy_(((zd - mean.double().unsqueeze(-1)) * rstd.double().unsqueeze(-1) * gamma.double() + beta.double()).to(h.dtype))
 
     def layernorm_bwd(self, dh, z, mean, rstd, gamma, dz, dgamma, dbeta, colsum_out=None):
+        self.backward = True
+        ln2 = self.ln_bwd_calls % 2 == 0
+        self.ln_bwd_calls += 1
         r = rstd.double().unsqueeze(-1)
         xh = (z.double() - mean.double().unsqueeze(-1)) * r
         dd = dh.double()
@@ -122,13 +141,23 @@ class FakeLib:
         dbeta += dd.sum(0).float()
         if colsum_out is not None:
             colsum_out += d.sum(0).float()
+        if ln2:
+            self.dz2 = dz
+            if self.slip == "b2_colsum_out_with_dropout" and colsum_out is None:
+                self.b2_extra = d.sum(0).float()
 
     def colsum(self, X, out, N=None):
         out += X.double().sum(0).float()
+        if self.b2_extra is not None:
+            out += self.b2_extra
+            self.b2_extra = None
 
     def dropout(self, x, out, seed, thr, residual=None):
+        if self.slip == "bwd_mask_site2" and self.backward and SITES[seed][1] == 3:
+            seed = engine.site_seed(SEED, SITES[seed][0], 2)
         keep = keep_bits(seed, x.shape[0], x.shape[1], thr).float()
-        sc = 1.0 if self.noscale else float(torch.tensor(256.0 / (256 - thr), dtype=torch.float32))
+        noscale = self.backward and self.slip == "bwd_mask_no_scale"
+        sc = 1.0 if noscale else float(torch.tensor(256.0 / (256 - thr), dtype=torch.float32))
         y = x.float() * keep * sc
         if residual is not None:
             y = y + residual.float()
@@ -152,107 +181,33 @@ def _params(seed):
     return layers, r(N, E).to(BF), r(N, E).to(BF)
 
 
-def stack_step(L, layers, src, dout, thr, slip=None):
-    """engine.EncoderStackFn's forward and backward on the bf16 head-dim-128 path, with one optional wiring slip."""
-    def lin(x, w, bias=None, aux=None, epi=0, C2=None, c2g=False, out_dtype=None):
-        y = torch.empty(x.shape[0], w.shape[0], dtype=out_dtype or x.dtype)
-        L.gemm(x, w, y, bias=bias, aux=aux, C2=C2, epilogue=epi, c2_gelu_grad=c2g)
-        return y
-
-    def dgrad(dy, w, aux=None, epi=0, rowdot=None):
-        dx = torch.empty(dy.shape[0], w.shape[1], dtype=dy.dtype)
-        L.gemm(dy, w, dx, b_mn_major=True, aux=aux, epilogue=epi, M=dy.shape[0], N=w.shape[1], K=w.shape[0], rowdot=rowdot)
-        return dx
-
-    def wgrad(dy, x, dw):
-        L.gemm(dy, x, dw, a_mn_major=True, b_mn_major=True, accumulate=True, M=dw.shape[0], N=dw.shape[1], K=dy.shape[0])
-
-    saved, h = [], src
-    for li, P in enumerate(layers):
-        wc = {k: P[k].to(BF) for k in ("in_w", "out_w", "w1", "w2")}
-        qkv = lin(h, wc["in_w"], P["in_b"])
-        attn = torch.empty(N, E, dtype=BF)
-        lse = torch.empty(B * H, T)
-        L.attention_fwd(qkv, attn, lse, T, B, H, DH, SEP, drop=(site_seed(SEED, li, 0), thr) if thr else None)
-        if thr:
-            z1 = lin(attn, wc["out_w"], P["out_b"])
-            L.dropout(z1, z1, site_seed(SEED, li, 1), thr, residual=h)
-        else:
-            z1 = lin(attn, wc["out_w"], P["out_b"], aux=h)
-        h1, m1, r1 = torch.empty_like(z1), torch.empty(N), torch.empty(N)
-        L.layernorm_fwd(z1, P["g1"], P["be1"], h1, m1, r1)
-        u = torch.empty(N, NHID, dtype=BF)
-        g = lin(h1, wc["w1"], P["b1"], epi=1, C2=u, c2g=True)
-        if thr:
-            L.dropout(g, g, site_seed(SEED, li, 2), thr)
-            z2 = lin(g, wc["w2"], P["b2"])
-            L.dropout(z2, z2, site_seed(SEED, li, 3), thr, residual=h1)
-        else:
-            z2 = lin(g, wc["w2"], P["b2"], aux=h1)
-        h2, m2, r2 = torch.empty_like(z2), torch.empty(N), torch.empty(N)
-        L.layernorm_fwd(z2, P["g2"], P["be2"], h2, m2, r2)
-        saved.append((h, qkv, attn, lse, z1, m1, r1, h1, u, g, z2, m2, r2, wc))
-        h = h2
-    out = h
-    grads = [{k: torch.zeros_like(v) for k, v in P.items()} for P in layers]
-    dh2 = dout
-    for li in reversed(range(NLAYERS)):
-        P, G = layers[li], grads[li]
-        h, qkv, attn, lse, z1, m1, r1, h1, u, g, z2, m2, r2, wc = saved[li]
-        if slip == "gelu_grad_other_layer":
-            u = saved[1 - li][8]
-        dz2 = torch.empty_like(z2)
-        L.layernorm_bwd(dh2, z2, m2, r2, P["g2"], dz2, G["g2"], G["be2"],
-                        G["b2"] if (not thr or slip == "b2_colsum_out_with_dropout") else None)
-        L.noscale = slip == "bwd_mask_no_scale"
-        dm = dz2
-        if thr:
-            dm = torch.empty_like(dz2)
-            L.dropout(dz2, dm, site_seed(SEED, li, 2 if slip == "bwd_mask_site2" else 3), thr)
-            L.colsum(dm, G["b2"])
-        wgrad(dm, g, G["w2"])
-        du = dgrad(dm, wc["w2"], aux=u, epi=4)
-        if thr:
-            L.dropout(du, du, site_seed(SEED, li, 2), thr)
-        L.colsum(du, G["b1"])
-        wgrad(du, h1, G["w1"])
-        dh1 = dgrad(du, wc["w1"], aux=None if slip == "dh1_no_aux" else dz2)
-        dz1 = torch.empty_like(z1)
-        L.layernorm_bwd(dh1, z1, m1, r1, P["g1"], dz1, G["g1"], G["be1"], None if thr else G["out_b"])
-        da = dz1
-        if thr:
-            da = torch.empty_like(dz1)
-            L.dropout(dz1, da, site_seed(SEED, li, 1), thr)
-            L.colsum(da, G["out_b"])
-        L.noscale = False
-        wgrad(da, attn, G["out_w"])
-        delta = torch.zeros(N, H)
-        dattn = dgrad(da, wc["out_w"], aux=attn, epi=3, rowdot=(delta, DH))
-        dqkv = torch.empty_like(qkv)
-        fused = not thr
-        a_li = li + 1 if slip == "att_bwd_next_layer_seed" else li
-        L.attention_bwd(qkv, attn, lse, dattn, dqkv, delta, T, B, H, DH, SEP,
-                        drop=(site_seed(SEED, a_li, 0), thr) if thr else None,
-                        dq_colsum=G["in_b"][:E] if fused else None, delta_token_major=True)
-        if fused:
-            W = P["out_w"]
-            G["in_b"][2 * E:] += {"v_third_no_w": lambda: G["out_b"],
-                                  "v_third_w_transposed": lambda: G["out_b"] @ W.t()}.get(slip, lambda: G["out_b"] @ W)()
-        else:
-            L.colsum(dqkv, G["in_b"])
-        wgrad(dqkv, h, G["in_w"])
-        dh2 = dgrad(dqkv, wc["in_w"], aux=dz1)
-    return out, grads
+def _step(lib, layers, src, dout, thr, slip=None):
+    """engine.EncoderStackFn's forward and backward on `lib` (delta and GELU' fusions on); the layers' gradients.  The
+    v third of the in-projection bias gradient is formed outside the library, so its slips are made here."""
+    names = engine.LAYER_PARAM_NAMES
+    params = [P[k].detach().requires_grad_() for P in layers for k in names]
+    with pytest.MonkeyPatch.context() as mp:
+        mp.setattr(engine, "L", lib)
+        mp.setattr(engine, "_DELTA_FUSION", True)
+        mp.setattr(engine, "_GELU_GRAD_FWD", True)
+        out = engine.EncoderStackFn.apply(src, T, B, SEP, H, "bf16", True, (SEED, thr) if thr else None, *params)
+        out.backward(dout)
+    grads = [dict(zip(names, (p.grad for p in params[i:i + len(names)]))) for i in range(0, len(params), len(names))]
+    for P, G in zip(layers, grads):
+        if slip == "v_third_no_w":
+            G["in_b"][2 * E:] = G["out_b"]
+        elif slip == "v_third_w_transposed":
+            G["in_b"][2 * E:] = G["out_b"] @ P["out_w"].t()
+    return grads
 
 
 def _run(thr, slip=None, c=None):
     layers, src, dout = _params(3)
-    lib = FakeLib()
-    lib.rowdot_unrounded = slip == "delta_unrounded"
+    lib = FakeLib(slip)
     rec = ES.Recorder(lib).install()
-    _, grads = stack_step(lib, layers, src, dout, thr, slip)
+    grads = _step(lib, layers, src, dout, thr, slip)
     rec.remove()
-    mask = lambda li, site, rows, cols: keep_bits(site_seed(SEED, li, site), rows, cols, thr)
+    mask = lambda li, site, rows, cols: keep_bits(engine.site_seed(SEED, li, site), rows, cols, thr)
     chk = ES.StageCheck(T=T, B=B, H=H, sep=SEP, thr=thr, mask=mask, num_sms=NUM_SMS, c=c,
                         paths={"u_is_grad": True, "rowdot": True, "fused_bias": not thr}, tag=f"{slip or 'clean'}: ")
     return chk, rec.calls, layers, src, dout, grads
@@ -267,7 +222,7 @@ def _check(thr, slip=None, c=None):
 @pytest.mark.parametrize("thr", [0, THR])
 def test_restatement_inside_bounds_at_c1(thr):
     chk, _ = _check(thr, c=1.0)
-    chk.report(f"restatement thr={thr}")
+    chk.report(f"engine thr={thr}")
     assert max(chk.worst.values()) <= 1.0
 
 
@@ -300,19 +255,18 @@ def test_wiring_slip_falls_outside_its_stage(slip, thr, stage):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# ES.ReductionCheck, the inline checker of the full-size steps, on the same restatement: its wrappers assert the call plan
+# ES.ReductionCheck, the inline checker of the full-size steps, on the same engine run: its wrappers assert the call plan
 # as the calls are made and check the token-axis reductions from the calls' own operands, 7 rows at a time (a block that
 # does not divide the 48 tokens)
 # ---------------------------------------------------------------------------------------------------------------------
 def _reductions(thr, slip=None, c=None):
     layers, src, dout = _params(3)
-    lib = FakeLib()
-    lib.wgrad_lost_token = slip == "wgrad_lost_token"
+    lib = FakeLib(slip)
     chk = ES.ReductionCheck(lib, n_layers=NLAYERS, drop=bool(thr), head=None, num_sms=NUM_SMS, block=7, c=c,
                             paths={"u_is_grad": True, "rowdot": True, "fused_bias": not thr},
-                            splits=lambda K, M, N: 1, tag=f"{slip or 'clean'}: ").install()
+                            splits=engine._wgrad_splits, tag=f"{slip or 'clean'}: ").install()
     try:
-        _, grads = stack_step(lib, layers, src, dout, thr, slip)
+        grads = _step(lib, layers, src, dout, thr, slip)
     finally:
         chk.remove()
     chk.finish(layers, grads)
@@ -322,7 +276,7 @@ def _reductions(thr, slip=None, c=None):
 @pytest.mark.parametrize("thr", [0, THR])
 def test_reduction_check_restatement_inside_bounds_at_c1(thr):
     chk = _reductions(thr, c=1.0)
-    chk.report(f"restatement thr={thr}")
+    chk.report(f"engine thr={thr}")
     want = {"dw2", "dw1", "dw_out", "dw_in", "dg2", "dbe2", "db2", "db1", "dg1", "dbe1", "dout_b"}
     want |= {"din_b"} if thr else {"din_b q", "din_b q final", "din_b k", "din_b v"}
     assert set(chk.worst) == want
@@ -333,8 +287,8 @@ def test_reduction_check_restatement_inside_bounds_at_c1(thr):
 @pytest.mark.parametrize("slip,thr,stage", [("wgrad_lost_token", 0, "dw2"), ("v_third_no_w", 0, "din_b v"),
                                             ("b2_colsum_out_with_dropout", THR, "db2")])
 def test_reduction_check_catches_slip(slip, thr, stage):
-    """A weight gradient short of one token, a v third without W_out, and a bias gradient summed twice (the LN2 backward
-    of the dropout path handed the b2 gradient as well as the colsum after the mask)."""
+    """A weight gradient short of one token, a v third without W_out, and a bias gradient summed twice (LN2's column sum
+    of dz under dropout added into the b2 gradient as well as the colsum after the mask)."""
     with pytest.raises(AssertionError) as e:
         _reductions(thr, slip)
     assert f"{slip}: {stage}" in str(e.value), str(e.value)
@@ -345,10 +299,10 @@ def test_reduction_check_asserts_the_plan_as_it_runs():
     first call that differs, while the step runs."""
     layers, src, dout = _params(3)
     lib = FakeLib()
-    chk = ES.ReductionCheck(lib, n_layers=NLAYERS, drop=False, head=None, num_sms=NUM_SMS, splits=lambda K, M, N: 1,
+    chk = ES.ReductionCheck(lib, n_layers=NLAYERS, drop=False, head=None, num_sms=NUM_SMS, splits=engine._wgrad_splits,
                             paths={"u_is_grad": True, "rowdot": False, "fused_bias": True}).install()
     try:
         with pytest.raises(AssertionError, match="is gemm/rowdot where the plan has gemm/none"):
-            stack_step(lib, layers, src, dout, 0)
+            _step(lib, layers, src, dout, 0)
     finally:
         chk.remove()
