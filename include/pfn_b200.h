@@ -426,6 +426,30 @@ typedef struct pfn_bnn_mcmc_desc {
 int pfn_bnn_mcmc_workspace(const pfn_bnn_mcmc_desc* d);
 int pfn_bnn_mcmc(const pfn_bnn_mcmc_desc* d, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * KNN baseline of the tabular evaluation (reference tabular.py:350-369 knn_metric): for each of S problems,
+ * GridSearchCV(KNeighborsClassifier(), {'n_neighbors': 1 .. K}, cv=StratifiedKFold(min(5, n // 2))) on its n training
+ * rows, then the class-1 probability of its m test rows under the refit with the best k.  K = min(5, n - 2).  One CTA per
+ * problem, all problems in one launch.  Neighbours: Euclidean in fp64 from direct differences, ordered by (distance, row);
+ * vote ties predict class 0; the best k is the first maximal mean CV accuracy.
+ * x [n + m, S, F] fp32 (rows 0 .. n-1 train, n .. n+m-1 test), y [n, S] fp32 labels (0. / 1.).  Outputs (DEVICE):
+ * proba [m, S] fp64 (count of class-1 neighbours / k), k_best [S] int32, cv_mean [S, K] fp64 (NaN for a candidate larger
+ * than some fold's training set), status [S] int32 (PFN_KNN_*; a problem that is not OK has NaN outputs and k_best 0).
+ * 4 <= n <= PFN_KNN_MAX_N, F <= PFN_KNN_MAX_F.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_KNN_MAX_N = 1024, PFN_KNN_MAX_F = 1024, PFN_KNN_MAX_K = 5, PFN_KNN_MAX_SPLITS = 5 };
+enum { PFN_KNN_OK = 0, PFN_KNN_BAD_LABEL = 1, PFN_KNN_FEW_MEMBERS = 2, PFN_KNN_ONE_CLASS = 3 };
+typedef struct pfn_knn_cv_desc {
+  int S, n, m, F;
+  const float* x;
+  const float* y;
+  double* proba;
+  int* k_best;
+  double* cv_mean;
+  int* status;
+} pfn_knn_cv_desc;
+int pfn_knn_cv(const pfn_knn_cv_desc* d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

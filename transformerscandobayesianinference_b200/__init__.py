@@ -29,4 +29,5 @@ def install_dropin():
     sys.modules["priors.utils"] = importlib.import_module(f"{__name__}.priors.utils")
     sys.modules["priors.pyro"] = importlib.import_module(f"{__name__}.priors.pyro")
     sys.modules["mcmc_svi_transformer_on_bayesian"] = importlib.import_module(f"{__name__}.mcmc_svi_transformer_on_bayesian")
+    sys.modules["tabular"] = importlib.import_module(f"{__name__}.tabular")
     return {name: sys.modules[name] for name in _DROPIN_MODULES}

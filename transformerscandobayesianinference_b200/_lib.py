@@ -109,6 +109,18 @@ class BnnMcmcDesc(ctypes.Structure):
 BNN_MAX_D, BNN_MAX_N = 1024, 1024
 
 
+class KnnCvDesc(ctypes.Structure):
+    _fields_ = [
+        ("S", c_int), ("n", c_int), ("m", c_int), ("F", c_int),
+        ("x", c_void_p), ("y", c_void_p),
+        ("proba", c_void_p), ("k_best", c_void_p), ("cv_mean", c_void_p), ("status", c_void_p),
+    ]
+
+
+KNN_MAX_N, KNN_MAX_F, KNN_MAX_K = 1024, 1024, 5
+KNN_OK, KNN_BAD_LABEL, KNN_FEW_MEMBERS, KNN_ONE_CLASS = 0, 1, 2, 3
+
+
 class AttnDesc(ctypes.Structure):
     _fields_ = [
         ("T", c_int), ("B", c_int), ("H", c_int), ("dh", c_int), ("sep", c_int),
@@ -137,6 +149,7 @@ EXPORTED_SYMBOLS = [
     "pfn_stroke_geometry", "pfn_stroke_render", "pfn_stroke_raster",
     "pfn_omniglot_episodes",
     "pfn_bnn_prior", "pfn_bnn_mcmc_workspace", "pfn_bnn_mcmc",
+    "pfn_knn_cv",
 ]
 
 _lib = None
@@ -218,6 +231,7 @@ def load():
     lib.pfn_bnn_prior.argtypes = [ctypes.c_uint32] + [c_int] * 5 + [c_void_p] * 6
     lib.pfn_bnn_mcmc_workspace.argtypes = [ctypes.POINTER(BnnMcmcDesc)]
     lib.pfn_bnn_mcmc.argtypes = [ctypes.POINTER(BnnMcmcDesc), c_void_p]
+    lib.pfn_knn_cv.argtypes = [ctypes.POINTER(KnnCvDesc), c_void_p]
     _lib = lib
     return lib
 
@@ -706,6 +720,21 @@ def bnn_mcmc(x_train, y_train, x_test, desc, samples, step_size, accept, diag, i
     desc.probs, desc.obs, desc.potential, desc.grad = ptr(probs), ptr(obs), ptr(potential), ptr(grad)
     desc.trace, desc.workspace = ptr(trace), ptr(workspace)
     check(load().pfn_bnn_mcmc(ctypes.byref(desc), stream_ptr()), "pfn_bnn_mcmc")
+
+
+@_guarded
+def knn_cv(x, y, proba, k_best, cv_mean, status):
+    """One launch runs the KNN grid-search CV and refit of every problem.  x [n+m, S, F], y [n, S] fp32; outputs
+    proba [m, S] fp64, k_best [S] int32, cv_mean [S, min(5, n - 2)] fp64, status [S] int32 (KNN_*)."""
+    _count(1)
+    require_cuda(x, y, proba, k_best, cv_mean, status)
+    d = KnnCvDesc()
+    rows, d.S, d.F = x.shape
+    d.n = y.shape[0]
+    d.m = rows - d.n
+    d.x, d.y = x.data_ptr(), y.data_ptr()
+    d.proba, d.k_best, d.cv_mean, d.status = proba.data_ptr(), k_best.data_ptr(), cv_mean.data_ptr(), status.data_ptr()
+    check(load().pfn_knn_cv(ctypes.byref(d), stream_ptr()), "pfn_knn_cv")
 
 
 # ------------------------------------------------------------------------------------------------

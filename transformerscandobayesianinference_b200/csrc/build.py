@@ -34,6 +34,7 @@ SOURCES = [
     "omniglot_prior.cu",
     "bnn_prior.cu",
     "bnn_mcmc.cu",
+    "knn_cv.cu",
 ]
 
 NVCC_FLAGS = [
