@@ -1,10 +1,11 @@
-"""Op-by-op check of the engine's training step -- TEST INFRASTRUCTURE ONLY.
+"""Op-by-op check of the engine's training step and of its eval-mode forward -- TEST INFRASTRUCTURE ONLY.
 
 `Recorder` replaces the kernel entry points of a library namespace (`transformerscandobayesianinference_b200._lib`, or a
 CPU restatement with the same signatures) with wrappers that keep every argument as it was before the call and every
 buffer the call writes as it is after it.  `StageCheck` then walks the recorded calls of one step, asserts the call plan
 of the engine path (the sequence of functions and the epilogue of every GEMM), and holds each stage to the per-element
-bound of oracle/error_budget.py.
+bound of oracle/error_budget.py (`step`: a training step; `forward`: one inference forward, as the tabular evaluation
+runs it).
 
 Each stage's exact fp64 value is computed from the engine's own stored outputs of earlier stages, chosen by their role
 in the reference layer (torch `TransformerEncoderLayer`, oracle/pfn_oracle.encoder_layer_dropout_ref), never from the
@@ -122,14 +123,21 @@ def layer_plan(drop, u_is_grad, rowdot, fused_bias):
     return fwd, bwd
 
 
+def forward_plan(n_layers, drop=False):
+    """Call signatures of one forward: embedding, the stack's forward, the decoder head (GELU layer, logits).  An eval-mode
+    forward (inference) has no dropout."""
+    pf, _ = layer_plan(drop, False, False, False)
+    return ["embed_fwd"] + pf * n_layers + ["gemm/gelu", "gemm/none"]
+
+
 def step_plan(n_layers, drop, paths, bar):
-    """Call signatures of one training step: embedding, the stack's forward, the decoder head (and the bar loss), the
-    decoder's backward, the stack's backward (last layer first), the embedding's backward."""
-    pf, pb = layer_plan(drop, paths["u_is_grad"], paths["rowdot"], paths["fused_bias"])
-    head = ["gemm/gelu", "gemm/none"] + (["bar_nll_fwd", "bar_nll_bwd"] if bar else [])
+    """Call signatures of one training step: the forward (forward_plan), the bar loss, the decoder's backward, the
+    stack's backward (last layer first), the embedding's backward."""
+    _, pb = layer_plan(drop, paths["u_is_grad"], paths["rowdot"], paths["fused_bias"])
+    loss = ["bar_nll_fwd", "bar_nll_bwd"] if bar else []
     dec_b = ["colsum", "gemm/none/acc", "gemm/mul" if paths["u_is_grad"] else "gemm/gelu_bwd", "colsum", "gemm/none/acc",
              "gemm/none"]
-    return ["embed_fwd"] + pf * n_layers + head + dec_b + pb * n_layers + ["embed_bwd"]
+    return forward_plan(n_layers, drop) + loss + dec_b + pb * n_layers + ["embed_bwd"]
 
 
 def _u(t):
@@ -214,28 +222,24 @@ class StageCheck:
         return self.mask(li, site, rows, cols) if self.thr else None
 
     # ---------------------------------------------------------------- one encoder layer
-    def layer(self, li, fwd, bwd, p, x_in, dh_in, grads=None):
-        """Forward and backward of layer li.  p: its fp32 master parameters by LAYER_PARAM_NAMES; x_in: its input as the
-        engine stored it; dh_in: the gradient of its output as the engine handed it; grads: its final gradients (the
-        in-projection bias is completed outside any kernel on the fused path)."""
+    def layer_fwd(self, li, fwd, p, x_in):
+        """Forward of layer li.  p: its fp32 master parameters by LAYER_PARAM_NAMES; x_in: its input as the engine stored
+        it.  Returns what the backward reads of the forward (its output, the stored h2, under "h2")."""
         T, B, H, sep = self.T, self.B, self.H, self.sep
         drop = bool(self.thr)
         N, E = x_in.shape
         dh = E // H
         nhid = p["w1"].shape[0]
-        pf, pb = layer_plan(drop, self.paths["u_is_grad"], self.paths["rowdot"], self.paths["fused_bias"])
+        pf, _ = layer_plan(drop, self.paths["u_is_grad"], self.paths["rowdot"], self.paths["fused_bias"])
         _expect(fwd, pf, f"layer {li} forward")
-        _expect(bwd, pb, f"layer {li} backward")
-        f, b = iter(fwd), iter(bwd)
-        u_at = _u(x_in)
+        f = iter(fwd)
         k0 = self.keep(li, 0, B * H * T, T)
         k0 = None if k0 is None else k0.reshape(B, H, T, T)
         k1, k2, k3 = self.keep(li, 1, N, E), self.keep(li, 2, N, nhid), self.keep(li, 3, N, E)
-        # ---- forward
         c = next(f)
         qkv = self.gemm("qkv", c, x_in, self.weight("qkv", c, p["in_w"]), bias=p["in_b"])
         c = next(f)
-        fa = EB.attention_fwd(qkv, T, B, H, dh, sep, u_at, k0, self.s)
+        fa = EB.attention_fwd(qkv, T, B, H, dh, sep, _u(x_in), k0, self.s)
         self.chk("attn", c.out["out"], fa["out"], fa["out_bound"], EB.C_ATT_OUT)
         self.chk("lse", c.out["lse"], fa["lse"], fa["lse_bound"], EB.C_ATT_LSE)
         attn = c.out["out"]
@@ -260,8 +264,22 @@ class StageCheck:
         else:
             z2 = self.gemm("z2", c, g, w2, bias=p["b2"], aux=h1)
         h2, mean2, rstd2 = self.ln_fwd("h2", next(f), z2, p["g2"], p["be2"])
-        # ---- backward
-        dz2, _ = self.ln_bwd("dz2", next(b), dh_in, z2, p["g2"], mean2, rstd2, ("dg2", "dbe2", "db2"))
+        return {"x_in": x_in, "fa": fa, "attn": attn, "z1": z1, "h1": h1, "mean1": mean1, "rstd1": rstd1, "g": g, "u": u,
+                "z2": z2, "h2": h2, "mean2": mean2, "rstd2": rstd2, "k1": k1, "k2": k2, "k3": k3}
+
+    def layer_bwd(self, li, bwd, p, st, dh_in, grads=None):
+        """Backward of layer li.  st: what layer_fwd returned for it; dh_in: the gradient of its output as the engine
+        handed it; grads: its final gradients (the in-projection bias is completed outside any kernel on the fused path).
+        Returns the gradient of its input as the engine stored it."""
+        drop = bool(self.thr)
+        x_in, fa, attn, z1, h1, g, u, z2 = (st[k] for k in ("x_in", "fa", "attn", "z1", "h1", "g", "u", "z2"))
+        k1, k2, k3 = st["k1"], st["k2"], st["k3"]
+        E = x_in.shape[1]
+        dh = E // self.H
+        _, pb = layer_plan(drop, self.paths["u_is_grad"], self.paths["rowdot"], self.paths["fused_bias"])
+        _expect(bwd, pb, f"layer {li} backward")
+        b = iter(bwd)
+        dz2, _ = self.ln_bwd("dz2", next(b), dh_in, z2, p["g2"], st["mean2"], st["rstd2"], ("dg2", "dbe2", "db2"))
         dm = dz2
         if drop:
             dm = self.dropout("dm", next(b), dz2, k3)
@@ -277,7 +295,7 @@ class StageCheck:
         c = next(b)
         dh1 = self.gemm("dh1", c, du, self.weight("dh1", c, p["w1"]).t(), aux=dz2)
         c_ln1 = next(b)
-        dz1, lb1 = self.ln_bwd("dz1", c_ln1, dh1, z1, p["g1"], mean1, rstd1, ("dg1", "dbe1", "dout_b"))
+        dz1, lb1 = self.ln_bwd("dz1", c_ln1, dh1, z1, p["g1"], st["mean1"], st["rstd1"], ("dg1", "dbe1", "dout_b"))
         da = dz1
         if drop:
             da = self.dropout("da", next(b), dz1, k1)
@@ -312,10 +330,20 @@ class StageCheck:
             self.colsum("din_b", next(b), dqkv)
         self.gemm("dw_in", next(b), dqkv.t(), x_in.t())
         c = next(b)
-        dh_out = self.gemm("dh", c, dqkv, self.weight("dh", c, p["in_w"]).t(), aux=dz1)
-        return h2, dh_out
+        return self.gemm("dh", c, dqkv, self.weight("dh", c, p["in_w"]).t(), aux=dz1)
 
     # ---------------------------------------------------------------- the encoder stack
+    def stack_fwd(self, calls, layers, x_in):
+        """calls: the stack's forward (layer 0 first); layers: per-layer parameter dicts; x_in: the stack's input as
+        stored.  Returns the stack's output as the engine stored it."""
+        pf, _ = layer_plan(bool(self.thr), self.paths["u_is_grad"], self.paths["rowdot"], self.paths["fused_bias"])
+        nf = len(pf)
+        assert len(calls) == len(layers) * nf, f"stack forward: {len(calls)} calls for {len(layers)} layers of {nf}"
+        h = x_in
+        for li, p in enumerate(layers):
+            h = self.layer_fwd(li, calls[li * nf:(li + 1) * nf], p, h)["h2"]
+        return h
+
     def stack(self, calls, layers, x_in, dh_top, grads=None):
         """calls: the stack's forward (layer 0 first) then its backward (last layer first); layers: per-layer parameter
         dicts; x_in: the stack's input as stored; dh_top: the gradient handed to the stack.  The records of a layer are
@@ -330,11 +358,52 @@ class StageCheck:
         h, dh0 = x_in, None
         for li in range(n):
             dh_in = dh_top if li == n - 1 else bwd[li + 1][-1].out["C"]
-            h, dh = self.layer(li, fwd[li], bwd[li], layers[li], h, dh_in, None if grads is None else grads[li])
+            st = self.layer_fwd(li, fwd[li], layers[li], h)
+            dh = self.layer_bwd(li, bwd[li], layers[li], st, dh_in, None if grads is None else grads[li])
+            h = st["h2"]
             if li == 0:
                 dh0 = dh
-            fwd[li] = bwd[li] = None
+            fwd[li] = bwd[li] = st = None
         return h, dh0
+
+    # ---------------------------------------------------------------- embedding and decoder head
+    def embed(self, c, x, y, emb):
+        """The embedding of x [T, B, F], y [T, B] with emb = (Wx, bx, wy, by) fp32 masters; returns its stored output."""
+        T, B, sep = self.T, self.B, self.sep
+        F = x.shape[-1]
+        Wx, bx, wy, by = emb
+        got = c.out["out"]
+        ex, bd = EB.embed_fwd(x.reshape(T * B, F), y.reshape(T * B), Wx, bx, wy, by, sep * B, _u(got))
+        self.chk("embed", got, ex, bd, EB.C_EMBED)
+        return got
+
+    def decoder(self, calls, hq, dec):
+        """The decoder head GELU(hq W0^T + b0) W2^T + b2 on the query rows hq of the last layer's stored output: calls
+        [gemm/gelu, gemm/none], dec = (W0, b0, W2, b2) fp32 masters.  Returns (g, u, logits) as stored."""
+        W0, b0, W2, b2 = dec
+        c = calls[0]
+        w0 = self.weight("dec g", c, W0)
+        g_dec = self.gemm("dec g", c, hq, w0, bias=b0, epi="gelu")
+        u_dec = self.gemm("dec u", c, hq, w0, bias=b0, epi="gelu_grad" if self.paths["u_is_grad"] else "none", out="C2")
+        c = calls[1]
+        logits = self.gemm("logits", c, g_dec, self.weight("logits", c, W2), bias=b2)
+        return g_dec, u_dec, logits
+
+    # ---------------------------------------------------------------- one forward (inference)
+    def forward(self, calls, *, x, y, emb, layers, dec, precision):
+        """embedding -> layers -> decoder of one eval-mode forward (no dropout: thr must be 0).  x [T, B, F], y [T, B];
+        emb = (Wx, bx, wy, by), dec = (W0, b0, W2, b2) fp32 masters.  Returns the logits [(T - sep) * B, n_out] as the
+        engine stored them."""
+        assert not self.thr, "an eval-mode forward has no dropout"
+        n = len(layers)
+        sig = [c.sig for c in calls]
+        want = forward_plan(n)
+        assert sig == want, f"forward: call plan {sig} != expected {want}"
+        x_in = self.embed(calls[0], x, y, emb)
+        dt = torch.bfloat16 if precision == "bf16" else torch.float32
+        assert x_in.dtype == dt, f"forward: {x_in.dtype} activations for {precision}"
+        h = self.stack_fwd(calls[1:-2], layers, x_in)
+        return self.decoder(calls[-2:], h[self.sep * self.B:], dec)[2]
 
     # ---------------------------------------------------------------- one training step
     def step(self, calls, *, x, y, emb, layers, dec, precision, borders=None, full_support=True, grads=None):
@@ -349,26 +418,15 @@ class StageCheck:
         sig = [c.sig for c in calls]
         want = step_plan(n, bool(self.thr), self.paths, bar)
         assert sig == want, f"step: call plan {sig} != expected {want}"
-        Wx, bx, wy, by = emb
-        W0, b0, W2, b2 = dec
+        W0, _, W2, _ = dec
         F = x.shape[-1]
         x2, y1 = x.reshape(N, F), y.reshape(N)
-        # embedding
-        c_ef = calls[0]
-        ex, bd = EB.embed_fwd(x2, y1, Wx, bx, wy, by, sep * B, _u(c_ef.out["out"]))
-        self.chk("embed", c_ef.out["out"], ex, bd, EB.C_EMBED)
-        x_in = c_ef.out["out"]
+        x_in = self.embed(calls[0], x, y, emb)
         i = 1 + n * len(pf)
         stack_fwd = calls[1:i]
         # decoder on the query rows of the last layer's output (its stored h2)
-        h_last = stack_fwd[-1].out["h"]
-        hq = h_last[sep * B:]
-        c = calls[i]
-        w0 = self.weight("dec g", c, W0)
-        g_dec = self.gemm("dec g", c, hq, w0, bias=b0, epi="gelu")
-        u_dec = self.gemm("dec u", c, hq, w0, bias=b0, epi="gelu_grad" if self.paths["u_is_grad"] else "none", out="C2")
-        c = calls[i + 1]
-        logits = self.gemm("logits", c, g_dec, self.weight("logits", c, W2), bias=b2)
+        hq = stack_fwd[-1].out["h"][sep * B:]
+        g_dec, u_dec, logits = self.decoder(calls[i:i + 2], hq, dec)
         i += 2
         dl = None
         if bar:

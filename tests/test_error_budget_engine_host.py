@@ -2,7 +2,8 @@
 forward and backward through a float32 fake of the kernel library (the kernels restated with bf16 rounding where they
 store bf16), and the calls are recorded and checked by the same code as the GPU test.  The engine stays inside every
 bound at c = 1; each wiring slip below, made by the fake at the one library call it concerns, falls outside its stage's
-bound at the GPU constants.  Each slip also reports whether the end-to-end tolerances of the bf16 engine tests
+bound at the GPU constants.  The forward alone, run under torch.no_grad() as inference runs it, is checked the same way
+with its own slips.  Each slip also reports whether the end-to-end tolerances of the bf16 engine tests
 (gradient norms within 6 %, elements within 8 % of the tensor's largest gradient) pass it."""
 import math
 
@@ -59,6 +60,10 @@ class FakeLib:
              accumulate=False, k_splits=1, M=None, N=None, K=None, use_tc=None, rowdot=None, c2_gelu_grad=False):
         if epilogue == self.EPI_GELU:
             self.gelu_grads.append(C2)
+            if self.slip == "g_stale_weight":
+                # the bf16 copy of W1 from before ten Adam steps of lr 1e-3: every element 1e-2 away from the current one
+                step = torch.randn(B.shape, generator=torch.Generator().manual_seed(5)).sign()
+                B = (B.float() + 1e-2 * step).to(B.dtype)
         elif epilogue == self.EPI_MUL and self.slip == "gelu_grad_other_layer":
             aux = next(u for u in self.gelu_grads if u is not aux)
         if self.slip == "dh1_no_aux" and aux is not None and aux is self.dz2:
@@ -86,9 +91,9 @@ class FakeLib:
             y = y + aux.float()
         C.copy_((C.float() + y if accumulate else y).to(C.dtype))
 
-    def _probs(self, qkv, drop):
+    def _probs(self, qkv, drop, sep=SEP):
         q, k, v = (EB._heads(qkv[:, n * E:(n + 1) * E].double(), T, B, H, DH) for n in range(3))
-        ok = EB.allowed_keys(T, SEP, "cpu")
+        ok = EB.allowed_keys(T, sep, "cpu")
         s = (q @ k.transpose(-1, -2) / math.sqrt(DH)).masked_fill(~ok, float("-inf"))
         P = torch.softmax(s, -1)
         km = torch.ones_like(P)
@@ -97,7 +102,8 @@ class FakeLib:
         return q, k, v, s, P, km
 
     def attention_fwd(self, qkv, out, lse, T, B, H, dh, sep, use_tc=None, batch_major=False, drop=None):
-        q, k, v, s, P, km = self._probs(qkv, drop)
+        # attn_sep_plus_1: the first query row is taken for a train row, so every later query row sees it as a key
+        q, k, v, s, P, km = self._probs(qkv, drop, sep + 1 if self.slip == "attn_sep_plus_1" else sep)
         out.copy_(EB._tokens((P * km) @ v, T, B, H, dh).to(out.dtype))
         lse.copy_(torch.logsumexp(s, -1).reshape(B * H, T).float())
 
@@ -241,6 +247,9 @@ def _old_tolerances_pass(grads, ref):
 SLIPS = [("bwd_mask_site2", THR, "dm"), ("att_bwd_next_layer_seed", THR, "dqkv"), ("bwd_mask_no_scale", THR, "dm"),
          ("b2_colsum_out_with_dropout", THR, "db2"), ("dh1_no_aux", 0, "dh1"), ("gelu_grad_other_layer", 0, "du"),
          ("v_third_no_w", 0, "din_b v"), ("v_third_w_transposed", 0, "din_b v"), ("delta_unrounded", 0, "delta")]
+# slips of the forward alone, caught in the training step as well as in an inference forward
+FWD_SLIPS = [("attn_sep_plus_1", "attn"), ("g_stale_weight", "g")]
+SLIPS += [(slip, 0, stage) for slip, stage in FWD_SLIPS]
 
 
 @pytest.mark.parametrize("slip,thr,stage", SLIPS)
@@ -252,6 +261,47 @@ def test_wiring_slip_falls_outside_its_stage(slip, thr, stage):
     assert f"{slip}: {stage}:" in str(e.value), str(e.value)
     print(f"[engine-stages host] {slip}: {str(e.value)[:160]}; old end-to-end tolerances "
           f"{'pass' if _old_tolerances_pass(grads, ref) else 'fail'} it")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The forward alone, as inference runs it (the tabular evaluation): EncoderStackFn under torch.no_grad() keeps no
+# activation, and StageCheck.stack_fwd checks its calls
+# ---------------------------------------------------------------------------------------------------------------------
+def _forward(slip=None, c=None):
+    layers, src, _ = _params(3)
+    lib = FakeLib(slip)
+    rec = ES.Recorder(lib).install()
+    params = [P[k] for P in layers for k in engine.LAYER_PARAM_NAMES]
+    with pytest.MonkeyPatch.context() as mp, torch.no_grad():
+        mp.setattr(engine, "L", lib)
+        mp.setattr(engine, "_GELU_GRAD_FWD", True)
+        out = engine.EncoderStackFn.apply(src, T, B, SEP, H, "bf16", torch.is_grad_enabled(), None, *params)
+    rec.remove()
+    assert out.grad_fn is None
+    chk = ES.StageCheck(T=T, B=B, H=H, sep=SEP, thr=0, mask=None, num_sms=NUM_SMS, c=c,
+                        paths={"u_is_grad": True, "rowdot": True, "fused_bias": True}, tag=f"{slip or 'clean'}: ")
+    return chk, rec.calls, layers, src, out
+
+
+def test_forward_restatement_inside_bounds_at_c1():
+    chk, calls, layers, src, out = _forward(c=1.0)
+    pf, _ = ES.layer_plan(False, True, True, True)
+    assert [c.sig for c in calls] == pf * NLAYERS
+    h = chk.stack_fwd(calls, layers, src)
+    assert torch.equal(h, out)
+    chk.report("engine forward")
+    assert set(chk.worst) == {"qkv", "qkv weight", "attn", "lse", "z1", "z1 weight", "h1", "h1 mean", "h1 rstd", "g",
+                              "g weight", "u", "z2", "z2 weight", "h2", "h2 mean", "h2 rstd"}
+    assert max(chk.worst.values()) <= 1.0
+
+
+@pytest.mark.parametrize("slip,stage", FWD_SLIPS)
+def test_forward_slip_falls_outside_its_stage(slip, stage):
+    chk, calls, layers, src, _ = _forward(slip)
+    with pytest.raises(AssertionError) as e:
+        chk.stack_fwd(calls, layers, src)
+    assert f"{slip}: {stage}:" in str(e.value), str(e.value)
+    print(f"[engine-stages host] forward {slip}: {str(e.value)[:160]}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -14,7 +14,7 @@ sys.path.insert(0, ROOT)
 
 import transformerscandobayesianinference_b200 as pfn  # noqa: E402
 from transformerscandobayesianinference_b200 import tabular  # noqa: E402
-from oracle import tabular_oracle as T  # noqa: E402
+from oracle import error_budget as EB, tabular_oracle as T  # noqa: E402
 
 GOLDEN = torch.load(os.path.join(ROOT, "tests", "golden", "tabular.pt"), weights_only=False)
 
@@ -148,6 +148,47 @@ def test_dataset_shorter_than_bptt_raises():
     X, y = torch.randn(100, 3), (torch.arange(100) % 2).float()
     with pytest.raises(ValueError):
         tabular.evaluate_position(X, y, [], _fake_metric, 100, 30)
+
+
+def _context_columns(g, bptt, S):
+    """Feature columns where the per-context standardisation goes wrong: standard normal, a constant, integers, large
+    offsets with unit and with tiny spread, a spread of 1e-6 around 1, and integers at 1e6."""
+    x = torch.randn(bptt, S, 7, generator=g, dtype=torch.float64)
+    x[..., 1] = 3.25
+    x[..., 2] = torch.randint(-5, 6, (bptt, S), generator=g)
+    x[..., 3] = 1e4 + torch.randn(bptt, S, generator=g)
+    x[..., 4] = -3e5 + 1e-2 * torch.randn(bptt, S, generator=g)
+    x[..., 5] = 1.0 + 1e-6 * torch.randn(bptt, S, generator=g)
+    x[..., 6] = 1e6 + torch.randint(0, 3, (bptt, S), generator=g)
+    return x.float()
+
+
+@pytest.mark.parametrize("p", [1, 2, 10, 30, 64, 99])
+def test_pfn_contexts_match_the_fp64_oracle_elementwise(p):
+    """tabular.pfn_contexts (incremental fp64 statistics from the train prefix) against tabular_oracle.pfn_contexts_ref
+    (two-pass fp64 statistics of each context), element by element.  The one fp32 rounding is 2^-24 |x|.  Each side's
+    fp64 work rounds ctx - mean and carries its mean's rounding, a few units of 2^-53 (|ctx| + mean |ctx|) before the
+    division by std (a sum's rounding scales with the sum of magnitudes, so an integer column whose mean is 0 still
+    carries one): where the standardised value is near 0 (a large offset, a tiny spread) that term is the larger one,
+    so the bound takes it twice.  A column constant in a context must give exactly 0, and ys must be exact."""
+    g = torch.Generator().manual_seed(p)
+    bptt, S = 100, 20
+    x = _context_columns(g, bptt, S)
+    y = (torch.rand(bptt, S, generator=g) < 0.5).float()
+    Q, F = bptt - p, x.shape[2]
+    for rescale in (1.0, 7 / 60):
+        xs, ys = tabular.pfn_contexts(x, y, p, rescale)
+        rx, ry = T.pfn_contexts_ref(x, y, p, rescale)
+        assert xs.dtype == ys.dtype == torch.float32 and xs.shape == (p + 1, Q * S, F) and ys.shape == (p + 1, Q * S)
+        assert torch.equal(ys[:p], ry.float()) and bool((ys[p] == 0).all())
+        xd = x.double()
+        ctx = torch.cat([xd[:p].unsqueeze(1).expand(p, Q, S, F), xd[p:].unsqueeze(0)], 0).reshape(p + 1, Q * S, F)
+        std = ((ctx - ctx.mean(0)) ** 2).sum(0).div(p).sqrt() + 1e-6
+        bound = 2.0 ** -24 * rx.abs() + 2 * 2.0 ** -53 * (ctx.abs() + ctx.abs().mean(0)) / std / rescale
+        EB.check(f"pfn_contexts p={p} rescale={rescale:.3g}", xs, rx, bound, 1.0)
+        flat = (ctx == ctx[:1]).all(0)                                 # columns constant in their context
+        assert bool(flat[:, 1].all()) and (p > 2 or bool(flat[:, 2].any()))     # the constant column; integer ties
+        assert bool((xs.permute(1, 2, 0)[flat] == 0).all())
 
 
 NOTEBOOK_BNN_CONFIG = {
