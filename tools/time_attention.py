@@ -30,12 +30,7 @@ DH, LAUNCHES, ROUNDS, WARMUP = 128, 30, 3, 3
 
 
 def open_lib(path):
-    lib = ctypes.CDLL(os.path.abspath(path))
-    lib.pfn_last_error.restype = ctypes.c_char_p
-    for fn in (lib.pfn_attention_fwd_tc, lib.pfn_attention_bwd_tc):
-        fn.restype = ctypes.c_int
-        fn.argtypes = [ctypes.POINTER(L.AttnDesc), ctypes.c_void_p]
-    return lib
+    return L.declare(ctypes.CDLL(os.path.abspath(path)))
 
 
 def card():

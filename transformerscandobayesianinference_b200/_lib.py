@@ -2,9 +2,14 @@
 
 There is deliberately no fallback: if the shared object is missing or a call fails, a RuntimeError with the
 library's own message is raised.  Tensors are passed as raw device pointers on torch's current CUDA stream.
+
+The header is restated here once: one ctypes Structure per descriptor, the mirrored enum constants, and one
+`_PROTOTYPES` line per entry point.  tests/test_cabi.py holds all three against the header.
 """
 import ctypes
+import functools
 import os
+from ctypes import POINTER
 
 import torch
 
@@ -16,7 +21,7 @@ F32, BF16 = 0, 1
 EPI_NONE, EPI_GELU, EPI_GELU_BWD, EPI_ROWDOT, EPI_MUL = 0, 1, 2, 3, 4
 KERNEL_RBF, KERNEL_MATERN12, KERNEL_MATERN32, KERNEL_MATERN52 = 0, 1, 2, 3
 
-c_int, c_float, c_void_p = ctypes.c_int, ctypes.c_float, ctypes.c_void_p
+c_int, c_uint32, c_float, c_double, c_void_p = ctypes.c_int, ctypes.c_uint32, ctypes.c_float, ctypes.c_double, ctypes.c_void_p
 
 
 class GemmDesc(ctypes.Structure):
@@ -50,14 +55,16 @@ class OmniglotDesc(ctypes.Structure):
 OMNIGLOT_IMAGES, OMNIGLOT_MAX_WAY, OMNIGLOT_MAX_SIDE = 20, 64, 105
 
 
-c_double = ctypes.c_double
+class AdamTensor(ctypes.Structure):
+    _fields_ = [("p", c_void_p), ("g", c_void_p), ("m", c_void_p), ("v", c_void_p), ("p_bf16", c_void_p),
+                ("n", ctypes.c_longlong)]
 
 
 class GpFitDesc(ctypes.Structure):
     _fields_ = [
         ("B", c_int), ("T", c_int), ("F", c_int),
         ("x", c_void_p), ("y", c_void_p),
-        ("n_ts", c_int), ("ts", ctypes.POINTER(c_int)),
+        ("n_ts", c_int), ("ts", POINTER(c_int)),
         ("kernel_type", c_int),
         ("ls_conc", c_double), ("ls_rate", c_double), ("os_conc", c_double), ("os_rate", c_double),
         ("noise_conc", c_double), ("noise_rate", c_double),
@@ -78,12 +85,12 @@ class GpMcmcDesc(ctypes.Structure):
     _fields_ = [
         ("B", c_int), ("T", c_int), ("F", c_int),
         ("x", c_void_p), ("y", c_void_p),
-        ("n_ts", c_int), ("ts", ctypes.POINTER(c_int)),
+        ("n_ts", c_int), ("ts", POINTER(c_int)),
         ("kernel_type", c_int),
         ("ls_conc", c_double), ("ls_rate", c_double), ("os_conc", c_double), ("os_rate", c_double),
         ("noise_conc", c_double), ("noise_rate", c_double),
         ("num_samples", c_int), ("warmup_steps", c_int), ("max_tree_depth", c_int), ("n_pred", c_int),
-        ("seed", ctypes.c_uint32),
+        ("seed", c_uint32),
         ("init", c_void_p),
         ("samples", c_void_p), ("log_samples", c_void_p), ("mean", c_void_p), ("var", c_void_p), ("potential", c_void_p), ("grad", c_void_p),
         ("step_size", c_void_p), ("accept", c_void_p), ("diag", c_void_p), ("trace", c_void_p),
@@ -99,7 +106,7 @@ class BnnMcmcDesc(ctypes.Structure):
         ("N", c_int), ("n", c_int), ("n_test", c_int), ("F", c_int), ("E", c_int),
         ("x_train", c_void_p), ("y_train", c_void_p), ("x_test", c_void_p),
         ("num_samples", c_int), ("warmup_steps", c_int), ("max_tree_depth", c_int),
-        ("seed", ctypes.c_uint32),
+        ("seed", c_uint32),
         ("init", c_void_p),
         ("samples", c_void_p), ("probs", c_void_p), ("obs", c_void_p), ("potential", c_void_p), ("grad", c_void_p),
         ("step_size", c_void_p), ("accept", c_void_p), ("diag", c_void_p), ("trace", c_void_p), ("workspace", c_void_p),
@@ -131,26 +138,50 @@ class AttnDesc(ctypes.Structure):
         ("dout", c_void_p), ("ld_dout", c_int),
         ("dqkv", c_void_p), ("ld_dqkv", c_int),
         ("delta", c_void_p), ("batch_major", c_int),
-        ("drop_seed", ctypes.c_uint32), ("drop_thr", c_int),
+        ("drop_seed", c_uint32), ("drop_thr", c_int),
         ("dq_colsum", c_void_p), ("delta_token_major", c_int),
     ]
 
 
-EXPORTED_SYMBOLS = [
-    "pfn_last_error", "pfn_version", "pfn_num_sms",
-    "pfn_gemm_bf16_tc", "pfn_gemm_simt",
-    "pfn_attention_fwd_simt", "pfn_attention_bwd_simt", "pfn_attention_fwd_tc", "pfn_attention_bwd_tc",
-    "pfn_embed_fwd", "pfn_embed_bwd",
-    "pfn_layernorm_fwd", "pfn_layernorm_bwd", "pfn_colsum",
-    "pfn_bar_nll_fwd", "pfn_bar_nll_bwd", "pfn_bar_bucket_idx",
-    "pfn_gp_sample", "pfn_gp_fit", "pfn_gp_mcmc",
-    "pfn_dropout", "pfn_dropout_keep_mask",
-    "pfn_adam_step", "pfn_adam_chunk_elems",
-    "pfn_stroke_geometry", "pfn_stroke_render", "pfn_stroke_raster",
-    "pfn_omniglot_episodes",
-    "pfn_bnn_prior", "pfn_bnn_mcmc_workspace", "pfn_bnn_mcmc",
-    "pfn_knn_cv",
-]
+P, I, F, U = c_void_p, c_int, c_float, c_uint32
+
+# argument types of every entry point, in header order, one per C parameter (pointers to descriptors as POINTER(...), every
+# other pointer, the stream included, as P).  Each returns an int status, except pfn_last_error (a string).
+_PROTOTYPES = {
+    "pfn_last_error": [],
+    "pfn_version": [],
+    "pfn_num_sms": [],
+    "pfn_gemm_bf16_tc": [POINTER(GemmDesc), P],
+    "pfn_gemm_simt": [POINTER(GemmDesc), P],
+    "pfn_attention_fwd_simt": [POINTER(AttnDesc), P],
+    "pfn_attention_bwd_simt": [POINTER(AttnDesc), P],
+    "pfn_attention_fwd_tc": [POINTER(AttnDesc), P],
+    "pfn_attention_bwd_tc": [POINTER(AttnDesc), P],
+    "pfn_embed_fwd": [P, P, P, P, P, P, P, I, I, I, I, I, I, P],
+    "pfn_embed_bwd": [P, I, P, P, P, P, P, P, I, I, I, I, I, P],
+    "pfn_layernorm_fwd": [P, I, P, P, P, I, P, P, I, I, F, I, P],
+    "pfn_layernorm_bwd": [P, I, P, I, P, P, P, P, I, P, P, P, I, I, I, P],
+    "pfn_dropout": [P, I, P, I, P, I, I, I, I, U, I, P],
+    "pfn_dropout_keep_mask": [P, I, I, U, I, P],
+    "pfn_adam_chunk_elems": [],
+    "pfn_adam_step": [P, P, I, I, F, F, F, F, F, F, I, P, P],
+    "pfn_colsum": [P, I, I, P, I, I, P],
+    "pfn_bar_nll_fwd": [P, I, I, P, P, I, I, P, P, P, P, I, P],
+    "pfn_bar_nll_bwd": [P, I, I, P, P, P, P, I, I, I, I, I, P],
+    "pfn_bar_bucket_idx": [P, P, I, P, I, P],
+    "pfn_gp_sample": [P, P, P, P, P, F, I, P, P, P, I, I, I, P],
+    "pfn_gp_fit": [POINTER(GpFitDesc), P],
+    "pfn_gp_mcmc": [POINTER(GpMcmcDesc), P],
+    "pfn_stroke_geometry": [POINTER(StrokeDesc), U, I, P, P, P, P],
+    "pfn_stroke_render": [POINTER(StrokeDesc), U, P, P, P, P, I, I, I, P],
+    "pfn_stroke_raster": [P, P, P, P, P, P, I, I, I, P],
+    "pfn_omniglot_episodes": [POINTER(OmniglotDesc), U, P, P, P, P, P, P],
+    "pfn_bnn_prior": [U, I, I, I, I, I, P, P, P, P, P, P],
+    "pfn_bnn_mcmc_workspace": [POINTER(BnnMcmcDesc)],
+    "pfn_bnn_mcmc": [POINTER(BnnMcmcDesc), P],
+    "pfn_knn_cv": [POINTER(KnnCvDesc), P],
+}
+EXPORTED_SYMBOLS = tuple(_PROTOTYPES)
 
 _lib = None
 _launches = 0          # kernel launches issued through this binding (bench.py reports it as gpu_launches)
@@ -183,57 +214,27 @@ def _count(n=1):
     _launches += n
 
 
+def declare(lib):
+    """Check that the ctypes handle `lib` exports every entry point and give each its prototype; returns `lib`."""
+    for name, argtypes in _PROTOTYPES.items():
+        if not hasattr(lib, name):
+            raise RuntimeError(f"libpfn_b200.so does not export {name}")
+        fn = getattr(lib, name)
+        fn.argtypes = argtypes
+        fn.restype = ctypes.c_char_p if name == "pfn_last_error" else c_int
+    return lib
+
+
 def load():
     """Load (once) and return the ctypes handle.  Raises if the library has not been built."""
     global _lib
-    if _lib is not None:
-        return _lib
-    if not os.path.exists(LIB_PATH):
-        raise RuntimeError(
-            f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(there is no CPU / PyTorch fallback for the PFN hot path)")
-    lib = ctypes.CDLL(LIB_PATH)
-    lib.pfn_last_error.restype = ctypes.c_char_p
-    for name in EXPORTED_SYMBOLS:
-        if not hasattr(lib, name):
-            raise RuntimeError(f"libpfn_b200.so does not export {name}")
-        if name != "pfn_last_error":
-            getattr(lib, name).restype = c_int
-    lib.pfn_gemm_bf16_tc.argtypes = [ctypes.POINTER(GemmDesc), c_void_p]
-    lib.pfn_gemm_simt.argtypes = [ctypes.POINTER(GemmDesc), c_void_p]
-    for n in ("pfn_attention_fwd_simt", "pfn_attention_bwd_simt", "pfn_attention_fwd_tc", "pfn_attention_bwd_tc"):
-        getattr(lib, n).argtypes = [ctypes.POINTER(AttnDesc), c_void_p]
-    lib.pfn_embed_fwd.argtypes = [c_void_p] * 7 + [c_int] * 6 + [c_void_p]
-    lib.pfn_embed_bwd.argtypes = [c_void_p, c_int] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p]
-    lib.pfn_layernorm_fwd.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
-                                      c_int, c_int, c_float, c_int, c_void_p]
-    lib.pfn_layernorm_bwd.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                      c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]
-    lib.pfn_colsum.argtypes = [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]
-    lib.pfn_bar_nll_fwd.argtypes = [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
-                                    c_void_p, c_void_p, c_int, c_void_p]
-    lib.pfn_bar_nll_bwd.argtypes = [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                    c_int, c_int, c_int, c_void_p]
-    lib.pfn_bar_bucket_idx.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]
-    lib.pfn_gp_sample.argtypes = [c_void_p] * 5 + [c_float, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                  c_void_p]
-    lib.pfn_gp_fit.argtypes = [ctypes.POINTER(GpFitDesc), c_void_p]
-    lib.pfn_gp_mcmc.argtypes = [ctypes.POINTER(GpMcmcDesc), c_void_p]
-    lib.pfn_dropout.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_uint32, c_int,
-                                c_void_p]
-    lib.pfn_dropout_keep_mask.argtypes = [c_void_p, c_int, c_int, ctypes.c_uint32, c_int, c_void_p]
-    lib.pfn_stroke_geometry.argtypes = [ctypes.POINTER(StrokeDesc), ctypes.c_uint32, c_int, c_void_p, c_void_p, c_void_p,
-                                        c_void_p]
-    lib.pfn_stroke_render.argtypes = [ctypes.POINTER(StrokeDesc), ctypes.c_uint32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                      c_int, c_int, c_int, c_void_p]
-    lib.pfn_stroke_raster.argtypes = [c_void_p] * 6 + [c_int, c_int, c_int, c_void_p]
-    lib.pfn_omniglot_episodes.argtypes = [ctypes.POINTER(OmniglotDesc), ctypes.c_uint32] + [c_void_p] * 6
-    lib.pfn_bnn_prior.argtypes = [ctypes.c_uint32] + [c_int] * 5 + [c_void_p] * 6
-    lib.pfn_bnn_mcmc_workspace.argtypes = [ctypes.POINTER(BnnMcmcDesc)]
-    lib.pfn_bnn_mcmc.argtypes = [ctypes.POINTER(BnnMcmcDesc), c_void_p]
-    lib.pfn_knn_cv.argtypes = [ctypes.POINTER(KnnCvDesc), c_void_p]
-    _lib = lib
-    return lib
+    if _lib is None:
+        if not os.path.exists(LIB_PATH):
+            raise RuntimeError(
+                f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
+                "(there is no CPU / PyTorch fallback for the PFN hot path)")
+        _lib = declare(ctypes.CDLL(LIB_PATH))
+    return _lib
 
 
 def check(rc, what):
@@ -325,8 +326,6 @@ def draw_seed(seed=None):
 def _guarded(fn):
     """Run the wrapped library call with the device of its first tensor argument as the current device (so that
     `stream_ptr()`, `num_sms()` and the launch itself all refer to the device that owns the data)."""
-    import functools
-
     @functools.wraps(fn)
     def wrapper(*args, **kwargs):
         dev = None
@@ -561,12 +560,9 @@ def adam_step(table, chunk_start, n_tensors, n_chunks, lr, beta1, beta2, eps, we
     """Clip (max_grad_norm > 0) + Adam update of every tensor of the device-resident pointer table (optim.FusedClipAdam)."""
     _count(2 if max_grad_norm > 0 else 1)
     require_cuda(table, chunk_start, norm_sq)
-    c_float = ctypes.c_float
-    fn = load().pfn_adam_step
-    fn.argtypes = [c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_int, c_void_p,
-                   c_void_p]
-    check(fn(ptr(table), ptr(chunk_start), int(n_tensors), int(n_chunks), float(lr), float(beta1), float(beta2), float(eps),
-             float(weight_decay), float(max_grad_norm), int(step), ptr(norm_sq), stream_ptr()), "pfn_adam_step")
+    check(load().pfn_adam_step(ptr(table), ptr(chunk_start), int(n_tensors), int(n_chunks), float(lr), float(beta1),
+                               float(beta2), float(eps), float(weight_decay), float(max_grad_norm), int(step), ptr(norm_sq),
+                               stream_ptr()), "pfn_adam_step")
 
 
 @_guarded

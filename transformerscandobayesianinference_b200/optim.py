@@ -9,8 +9,6 @@ before the step).  `step()` hands a device-resident table of (param, grad, exp_a
 `pfn_adam_step` (csrc/optimizer.cu): one launch for the gradient norm, one for clip + update; the update also rewrites the
 bf16 copy of every 2-D weight that the next step's wgmma GEMMs read (engine._cast picks it up), so the per-step cast pass
 disappears.  CUDA only: on other devices build torch.optim.Adam (train.py does)."""
-import ctypes
-
 import torch
 
 from . import _lib as L
@@ -26,7 +24,7 @@ class FusedClipAdam(torch.optim.Optimizer):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.max_grad_norm = float(max_grad_norm) if max_grad_norm else 0.0
         self.bf16_shadows = bool(bf16_shadows)
-        self._tables = {}          # per group: (key of pointers, device table, device chunk_start, n_chunks, keep-alive list)
+        self._tables = {}          # per group: (key of pointers, device table, device chunk_start, n_chunks)
         self._norm_sq = None
         self.last_grad_norm_sq = None
 
@@ -50,7 +48,7 @@ class FusedClipAdam(torch.optim.Optimizer):
 
     def _table(self, gi, plist):
         chunk = L.adam_chunk_elems()
-        entries, keep = [], []
+        entries = []
         for p in plist:
             st = self.state[p]
             sh = self._shadow(p)
@@ -61,11 +59,11 @@ class FusedClipAdam(torch.optim.Optimizer):
         if cached is not None and cached[0] == key:
             return cached
         dev = plist[0].device
-        flat = torch.tensor([x for e in entries for x in e], dtype=torch.int64)
+        host = torch.frombuffer((L.AdamTensor * len(entries))(*entries), dtype=torch.uint8)   # pfn_adam_tensor[n_tensors]
         starts = [0]
         for e in entries:
             starts.append(starts[-1] + (e[5] + chunk - 1) // chunk)
-        table = flat.pin_memory().to(dev, non_blocking=True)
+        table = host.pin_memory().to(dev, non_blocking=True)
         chunk_start = torch.tensor(starts, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
         cached = (key, table, chunk_start, starts[-1])
         self._tables[gi] = cached
