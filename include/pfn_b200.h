@@ -450,6 +450,43 @@ typedef struct pfn_knn_cv_desc {
 } pfn_knn_cv_desc;
 int pfn_knn_cv(const pfn_knn_cv_desc* d, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Convolutional image encoder (encoders.Conv; the reference has no conv encoder).  One call per 3x3 layer and direction:
+ * a valid 3x3 convolution (stride 1, bias) then ReLU, from C_in (1 or 64) to 64 channels, on N square images of side S
+ * (4 <= S <= PFN_CONV_MAX_SIDE) whose activations are NHWC: pixel (n, r, c) of a side-s grid at ((n s + r) s + c) 64.
+ * The images themselves (C_in = 1) are fp32 [N, S, S]; every other activation is in `dtype`.
+ * Gradient grids are zero-padded: the output gradient g of a layer (side S - 2) is stored as [N, S + 2, S + 2, 64] with two
+ * zero pixels on every side, so that the data gradient is the valid convolution of g with the flipped weights.
+ * pfn_conv_fwd   : y [N, S-2, S-2, 64] = relu(conv(x, w) + bias).  w: fp32 [64, C_in, 3, 3] (torch layout) on the direct
+ *                  kernels (C_in = 1, or dtype PFN_F32); bf16 [64, 9, 64] (co, tap, ci) on the wgmma kernel (C_in = 64, bf16).
+ * pfn_conv_dgrad : (C_in = 64) y = g_below, the input gradient times [x > 0] (the ReLU of the layer below), written as a
+ *                  padded [N, S + 4, S + 4, 64] buffer, zero border included (need not be initialised).  w: fp32 torch
+ *                  layout (PFN_F32) or bf16 [64, 9, 64] (ci, tap, co) holding w[co, ci, 2 - dr, 2 - dc] at tap 3 dr + dc.
+ * pfn_conv_wgrad : dw [64, C_in, 3, 3] and db [64] fp32 (overwritten) from g and x, summed over pixel chunks into
+ *                  `workspace` (pfn_conv_wgrad_workspace floats, or -1 for an invalid descriptor) and then reduced over the
+ *                  chunks in a fixed order: two runs give the same bits.  w unused.
+ * pfn_conv_mean_fwd : feat [N, 64] (dtype) = mean of y [N, s, s, 64] over its s^2 pixels, in a fixed order.
+ * pfn_conv_mean_bwd : g [N, s + 4, s + 4, 64] = dfeat [N, 64] / s^2 times [y > 0] inside, zero on the 2-pixel border.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_CONV_MAX_SIDE = 112, PFN_CONV_CH = 64 };
+typedef struct pfn_conv_desc {
+  int N, S, C_in, dtype;
+  const void* x;                         /* layer input: fp32 [N, S, S] (C_in = 1) or [N, S, S, 64] */
+  const void* w;
+  const float* bias;                     /* [64] (fwd) */
+  const void* g;                         /* padded output gradient [N, S + 2, S + 2, 64] (dgrad, wgrad) */
+  void* y;                               /* fwd: [N, S - 2, S - 2, 64]; dgrad: padded [N, S + 4, S + 4, 64] */
+  float* dw;
+  float* db;
+  float* workspace;
+} pfn_conv_desc;
+int pfn_conv_fwd(const pfn_conv_desc* d, void* stream);
+int pfn_conv_dgrad(const pfn_conv_desc* d, void* stream);
+int pfn_conv_wgrad_workspace(const pfn_conv_desc* d);
+int pfn_conv_wgrad(const pfn_conv_desc* d, void* stream);
+int pfn_conv_mean_fwd(const void* y, int N, int s, int dtype, void* feat, void* stream);
+int pfn_conv_mean_bwd(const void* dfeat, const void* y, int N, int s, int dtype, void* g, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

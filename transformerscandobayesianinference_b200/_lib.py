@@ -143,6 +143,17 @@ class AttnDesc(ctypes.Structure):
     ]
 
 
+class ConvDesc(ctypes.Structure):
+    _fields_ = [
+        ("N", c_int), ("S", c_int), ("C_in", c_int), ("dtype", c_int),
+        ("x", c_void_p), ("w", c_void_p), ("bias", c_void_p), ("g", c_void_p), ("y", c_void_p),
+        ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p),
+    ]
+
+
+CONV_MAX_SIDE, CONV_CH = 112, 64
+
+
 P, I, F, U = c_void_p, c_int, c_float, c_uint32
 
 # argument types of every entry point, in header order, one per C parameter (pointers to descriptors as POINTER(...), every
@@ -180,6 +191,12 @@ _PROTOTYPES = {
     "pfn_bnn_mcmc_workspace": [POINTER(BnnMcmcDesc)],
     "pfn_bnn_mcmc": [POINTER(BnnMcmcDesc), P],
     "pfn_knn_cv": [POINTER(KnnCvDesc), P],
+    "pfn_conv_fwd": [POINTER(ConvDesc), P],
+    "pfn_conv_dgrad": [POINTER(ConvDesc), P],
+    "pfn_conv_wgrad_workspace": [POINTER(ConvDesc)],
+    "pfn_conv_wgrad": [POINTER(ConvDesc), P],
+    "pfn_conv_mean_fwd": [P, I, I, I, P, P],
+    "pfn_conv_mean_bwd": [P, P, I, I, I, P, P],
 }
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)
 
@@ -752,3 +769,60 @@ def mcmc_trouble(diag):
     """(divergent sampling iterations, iterations that hit the tree-depth cap) summed over the chains of diag [..., 6]."""
     col = GP_MCMC_DIAG_NAMES.index
     return int(diag[..., col("div_sampling")].sum()), int(diag[..., col("max_depth_hits")].sum())
+
+
+def _conv_desc(N, S, C_in, dtype, x=None, w=None, bias=None, g=None, y=None, dw=None, db=None, workspace=None):
+    """Descriptor of one 3x3 layer of the conv encoder (include/pfn_b200.h, pfn_conv_desc); S is the layer's input side."""
+    require_cuda(x, w, bias, g, y, dw, db, workspace)
+    d = ConvDesc()
+    d.N, d.S, d.C_in, d.dtype = N, S, C_in, dtype_code(dtype) if torch.is_tensor(dtype) else dtype
+    for name, t in (("x", x), ("w", w), ("bias", bias), ("g", g), ("y", y), ("dw", dw), ("db", db),
+                    ("workspace", workspace)):
+        setattr(d, name, None if t is None else t.data_ptr())
+    return d
+
+
+@_guarded
+def conv_fwd(x, w, bias, y, N, S, C_in):
+    """y [N, S-2, S-2, 64] = relu(conv3x3(x) + bias); y's dtype is the activation dtype."""
+    _count()
+    check(load().pfn_conv_fwd(ctypes.byref(_conv_desc(N, S, C_in, y, x=x, w=w, bias=bias, y=y)), stream_ptr()),
+          "pfn_conv_fwd")
+
+
+@_guarded
+def conv_dgrad(g, w, x, out, N, S):
+    """out (padded, side S + 4) interior = (input gradient of the 64 -> 64 layer with input x) * [x > 0]."""
+    _count()
+    check(load().pfn_conv_dgrad(ctypes.byref(_conv_desc(N, S, CONV_CH, out, x=x, w=w, g=g, y=out)), stream_ptr()),
+          "pfn_conv_dgrad")
+
+
+def conv_wgrad_workspace(N, S, C_in):
+    n = load().pfn_conv_wgrad_workspace(ctypes.byref(_conv_desc(N, S, C_in, F32)))
+    if n < 0:
+        check(1, "pfn_conv_wgrad_workspace")
+    return n
+
+
+@_guarded
+def conv_wgrad(g, x, dw, db, N, S, C_in):
+    """dw [64, C_in, 3, 3], db [64] fp32 (overwritten) of the layer with input x and padded output gradient g."""
+    ws = torch.empty(conv_wgrad_workspace(N, S, C_in), device=g.device, dtype=torch.float32)
+    _count(2)
+    check(load().pfn_conv_wgrad(ctypes.byref(_conv_desc(N, S, C_in, g, x=x, g=g, dw=dw, db=db, workspace=ws)),
+                                stream_ptr()), "pfn_conv_wgrad")
+
+
+@_guarded
+def conv_mean_fwd(y, feat, N, s):
+    require_cuda(y, feat)
+    _count()
+    check(load().pfn_conv_mean_fwd(ptr(y), N, s, dtype_code(y), ptr(feat), stream_ptr()), "pfn_conv_mean_fwd")
+
+
+@_guarded
+def conv_mean_bwd(dfeat, y, g, N, s):
+    require_cuda(dfeat, y, g)
+    _count()
+    check(load().pfn_conv_mean_bwd(ptr(dfeat), ptr(y), N, s, dtype_code(y), ptr(g), stream_ptr()), "pfn_conv_mean_bwd")

@@ -35,6 +35,7 @@ SOURCES = [
     "bnn_prior.cu",
     "bnn_mcmc.cu",
     "knn_cv.cu",
+    "conv_encoder.cu",
 ]
 
 NVCC_FLAGS = [

@@ -1,11 +1,52 @@
 """Input encoders with the reference's names (reference encoders.py).  `Linear` feeds the fused embedding kernel;
-anything else runs as a regular PyTorch module in front of the CUDA encoder stack."""
+anything else runs as a regular PyTorch module in front of the CUDA encoder stack.  `Conv` (not in the reference) is
+an image encoder on the library's own convolution kernels."""
 import math
 
 import torch
 import torch.nn as nn
 
+from . import _lib as L
+from . import engine
+
 Linear = nn.Linear
+
+
+class Conv(nn.Module):
+    """Image encoder: x [..., S*S] (pixel k = r S + c) -> [..., emsize].  Up to five valid 3x3 convolutions to 64
+    channels, each followed by ReLU and applied while the current side is at least 4 (n_conv = min(5, (S - 2) // 2)),
+    then the mean over the remaining pixels and Linear(64, emsize).  Runs on the sm_90a kernels of csrc/conv_encoder.cu
+    (bf16 NHWC activations on tensor cores, or fp32 FMA in parity mode); convs that are not applied get no gradient, and
+    the images themselves none at all."""
+
+    def __init__(self, input_size, emsize):
+        super().__init__()
+        S = math.isqrt(input_size)
+        # L.CONV_MAX_SIDE (112) is the larger of the stroke and Omniglot samplers' largest image sides
+        if S * S != input_size or not 4 <= S <= L.CONV_MAX_SIDE:
+            raise ValueError(f"encoders.Conv takes square images of side 4 .. {L.CONV_MAX_SIDE}; "
+                             f"input_size={input_size} is not one")
+        self.convs = nn.ModuleList([nn.Conv2d(1 if i == 0 else 64, 64, 3) for i in range(5)])
+        self.linear = nn.Linear(64, emsize)
+        self.side = S
+        self.n_conv = min(5, (S - 2) // 2)
+        self.precision = engine.default_precision()
+
+    def forward(self, x):
+        if x.requires_grad:
+            raise ValueError("encoders.Conv computes no gradient for its input images; pass a tensor without requires_grad")
+        if not x.is_cuda:
+            raise RuntimeError(
+                "encoders.Conv runs on hand-written sm_90a kernels only; inputs are on "
+                f"{x.device}. Move model and data to a CUDA device (there is no CPU fallback).")
+        S = self.side
+        if x.shape[-1] != S * S:
+            raise ValueError(f"encoders.Conv({S * S}, ...) got inputs of {x.shape[-1]} pixels")
+        lead = x.shape[:-1]
+        params = [p for conv in self.convs[:self.n_conv] for p in (conv.weight, conv.bias)]
+        params += [self.linear.weight, self.linear.bias]
+        out = engine.ConvEncoderFn.apply(x.reshape(-1, S * S), S, self.precision, torch.is_grad_enabled(), *params)
+        return out.reshape(*lead, -1)
 
 
 class Normalize(nn.Module):

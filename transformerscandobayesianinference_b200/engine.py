@@ -343,6 +343,94 @@ class DecoderFn(torch.autograd.Function):
         return dhq, dW0, db0, dW2, db2, None
 
 
+def conv_weight_operand(W, dgrad=False):
+    """bf16 B operand of the 64 -> 64 tensor-core conv kernels: [64, 9, 64] (co, tap, ci) for the forward; for the data
+    gradient (ci, tap, co) holding W[co, ci, 2 - dr, 2 - dc] at tap 3 dr + dc (the flipped kernel)."""
+    W = W.detach()
+    if dgrad:
+        W = W.flip(2, 3).permute(1, 0, 2, 3)
+    return W.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)
+
+
+class ConvEncoderFn(torch.autograd.Function):
+    """x [N, S*S] fp32 images -> [N, E] fp32: the conv stack of encoders.Conv (n_conv valid 3x3 convolutions + ReLU, the
+    spatial mean, Linear(64, E)).  params: (weight, bias) of each applied conv, then the linear's weight and bias.
+    Activations are NHWC in the activation dtype; each conv's post-ReLU output is kept for the backward (its own ReLU mask
+    and the next layer's weight-gradient operand).  Gradient grids are zero-padded by 2 pixels; the kernels that produce
+    them write the border too.  No gradient flows to x.  Every gradient is summed in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, x, S, precision, keep, *params):
+        L.require_cuda(x, *params)
+        dt = act_dtype(precision)
+        N = x.shape[0]
+        convs, (lin_w, lin_b) = [params[i:i + 2] for i in range(0, len(params) - 2, 2)], params[-2:]
+        h, s = x.detach().contiguous().float(), S
+        acts = []
+        for li, (W, b) in enumerate(convs):
+            y = torch.empty(N, s - 2, s - 2, L.CONV_CH, device=x.device, dtype=dt)
+            cin = 1 if li == 0 else L.CONV_CH
+            w_op = conv_weight_operand(W) if (cin == L.CONV_CH and dt == torch.bfloat16) else W.detach().contiguous()
+            L.conv_fwd(h, w_op, b.detach().contiguous(), y, N, s, cin)
+            acts.append(y)
+            h, s = y, s - 2
+        feat = torch.empty(N, L.CONV_CH, device=x.device, dtype=dt)
+        L.conv_mean_fwd(h, feat, N, s)
+        lin_wc = _cast(lin_w, dt)
+        out = _linear_fwd(feat, lin_wc, lin_b.detach().contiguous(), out_dtype=torch.float32)
+        if keep and any(ctx.needs_input_grad):
+            ctx.saved = (x.detach().contiguous().float(), acts, feat, lin_wc)
+        else:
+            ctx.saved = None
+        ctx.meta = (S, precision)
+        ctx.params = params
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        if ctx.saved is None:
+            raise RuntimeError("ConvEncoderFn: no activations were kept (forward under no_grad, or a second backward)")
+        x, acts, feat, lin_wc = ctx.saved
+        ctx.saved = None
+        S, precision = ctx.meta
+        params = ctx.params
+        dt = act_dtype(precision)
+        dev = dout.device
+        N, E = dout.shape
+        dy = dout.contiguous().to(dt)
+        # the projection's weight and bias gradients as ONE GEMM over [feat, 1] without split-K: a single store per
+        # element, so that every gradient of the encoder is reproducible bit for bit (K = N images is short)
+        feat1 = torch.zeros(N, L.CONV_CH + 8, device=dev, dtype=dt)
+        feat1[:, :L.CONV_CH] = feat
+        feat1[:, L.CONV_CH] = 1
+        d_lin = torch.empty(E, L.CONV_CH + 8, device=dev)
+        L.gemm(dy, feat1, d_lin, a_mn_major=True, b_mn_major=True, M=E, N=L.CONV_CH + 8, K=N)
+        d_lin_w, d_lin_b = d_lin[:, :L.CONV_CH], d_lin[:, L.CONV_CH]
+        dfeat = _linear_dgrad(dy, lin_wc)
+        del dy, feat, feat1
+        s = S - 2 * len(acts)
+        g = torch.empty(N, s + 4, s + 4, L.CONV_CH, device=dev, dtype=dt)
+        L.conv_mean_bwd(dfeat, acts[-1], g, N, s)
+        grads = []
+        for li in reversed(range(len(acts))):
+            W = params[2 * li]
+            s_in = s + 2
+            cin = 1 if li == 0 else L.CONV_CH
+            x_in = x if li == 0 else acts[li - 1]
+            dW = torch.empty_like(W, dtype=torch.float32)
+            db = torch.empty(L.CONV_CH, device=dev)
+            L.conv_wgrad(g, x_in, dW, db, N, s_in, cin)
+            grads = [dW, db] + grads
+            if li > 0:
+                g_in = torch.empty(N, s_in + 4, s_in + 4, L.CONV_CH, device=dev, dtype=dt)
+                w_op = conv_weight_operand(W, dgrad=True) if dt == torch.bfloat16 else W.detach().contiguous()
+                L.conv_dgrad(g, w_op, x_in, g_in, N, s_in)
+                g = g_in
+            acts[li] = None
+            s = s_in
+        return (None, None, None, None) + tuple(grads) + (d_lin_w, d_lin_b)
+
+
 def layer_params(layer):
     """The 12 parameter tensors of one nn.TransformerEncoderLayer in LAYER_PARAM_NAMES order."""
     return (layer.self_attn.in_proj_weight, layer.self_attn.in_proj_bias, layer.self_attn.out_proj.weight,
