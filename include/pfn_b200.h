@@ -487,6 +487,64 @@ int pfn_conv_wgrad(const pfn_conv_desc* d, void* stream);
 int pfn_conv_mean_fwd(const void* y, int N, int s, int dtype, void* feat, void* stream);
 int pfn_conv_mean_bwd(const void* dfeat, const void* y, int N, int s, int dtype, void* g, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Ridge baseline of the ridge prior (reference priors/ridge.py:23-34: sklearn Ridge(alpha).fit(x[:t, b], y[:t, b]) and
+ * predict(x[t, b]) for every t and b).  For every dataset b and prefix t = 1 .. T-1, in ONE launch (one CTA per dataset):
+ * centre the rows < t by their means mu_x, mu_y; w = argmin |Xc w - yc|^2 + alpha |w|^2; pred[b, t] = mu_y + (x_t - mu_x) w
+ * and sq_err[b, t] = (target[b, t] - pred[b, t])^2.  Column 0 of both outputs is NaN.
+ * The centred rows are folded into an F x (F + 1) triangular factor [R | Q^T yc] by Givens rotations, one row per t
+ * (R^T R = Xc^T Xc), and every prefix is solved from a one-sided Jacobi SVD of that factor in fp64.  With alpha = 0 the
+ * solution is the minimum-norm least-squares one, singular values of Xc at or below max(t, F) eps s_max (numpy lstsq's
+ * cutoff, eps = 2^-52) counting as zero; with alpha > 0 every singular value is used.
+ * x [B, T, F], y [B, T] (fitted), target [B, T] (scored) fp32; pred, sq_err [B, T] fp64.  alpha >= 0, F <= PFN_RIDGE_MAX_F.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_RIDGE_MAX_F = 64 };
+typedef struct pfn_ridge_prefix_desc {
+  int B, T, F;
+  double alpha;
+  const float* x;
+  const float* y;
+  const float* target;
+  double* pred;
+  double* sq_err;
+} pfn_ridge_prefix_desc;
+int pfn_ridge_prefix(const pfn_ridge_prefix_desc* d, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Fixed-hyperparameter exact GP of the sklearn GP prior (reference priors/gp.py), kernel k(a, b) = exp(-|a - b|^2 / 2 ls^2)
+ * with the differences taken between the quotients x / ls, as sklearn forms them.  One CTA per dataset
+ * holds a T x T fp64 matrix in shared memory (the layout of the GP fits: T <= PFN_GP_FIT_MAX_T).
+ *   PFN_EXACT_GP_EVALUATE (priors/gp.py:41-62, GaussianProcessRegressor(alpha).fit(x[:t], y[:t]).predict(x[t])): one
+ *     Cholesky of K_T + alpha I answers every prefix t = 1 .. T-1 (its leading t x t block is the factor of prefix t):
+ *     mean[b, t] = k*^T (K_t + alpha I)^-1 y_<t and the latent var[b, t] = max(1 - k*^T (K_t + alpha I)^-1 k*, 0).  Column 0 is
+ *     NaN.  status[b] = 0, or s > 0 when the factor of prefix s <= T - 1 fails (pivot s - 1 not positive; sklearn raises
+ *     there): mean and var are then NaN from t = s on.  x [B, T, F], y [B, T] fp32; mean, var [B, T] fp64; status [B] int32.
+ *   PFN_EXACT_GP_SAMPLE (priors/gp.py:19-34, GaussianProcessRegressor.sample_y of the unfitted model: y ~ N(0, K), no noise
+ *     term; alpha unused): a diagonal-pivoted Cholesky of K that stops at the numerical rank r, the first step whose largest
+ *     remaining diagonal is at or below T eps; sample[b] = P L[:, :r] z[b, :r] with P L L^T P^T = K to rounding.
+ *     x [B, T, F], z [B, T] fp32 standard normals; sample [B, T] fp32, rank [B] int32.  Optional (NULL: not written):
+ *     factor [B, T, T] fp64, the factor P L in the rows' own order (factor[b, i, k] = 0 for k >= r), and perm [B, T] int32,
+ *     the pivot order (perm[b, k] is the row of pivot k; the rows never chosen follow in increasing order).
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_EXACT_GP_EVALUATE = 0, PFN_EXACT_GP_SAMPLE = 1 };
+typedef struct pfn_exact_gp_desc {
+  int B, T, F;
+  int mode;                              /* PFN_EXACT_GP_EVALUATE / PFN_EXACT_GP_SAMPLE */
+  double length_scale;                   /* > 0 */
+  double alpha;                          /* evaluate: added to the training diagonal (sklearn's default 1e-10), >= 0 */
+  const float* x;
+  const float* y;                        /* evaluate */
+  const float* z;                        /* sample */
+  double* mean;                          /* evaluate */
+  double* var;
+  int* status;
+  float* sample;                         /* sample */
+  int* rank;
+  double* factor;
+  int* perm;
+} pfn_exact_gp_desc;
+int pfn_exact_gp(const pfn_exact_gp_desc* d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -28,6 +28,9 @@ def install_dropin():
     sys.modules["priors.omniglot"] = importlib.import_module(f"{__name__}.priors.omniglot")
     sys.modules["priors.utils"] = importlib.import_module(f"{__name__}.priors.utils")
     sys.modules["priors.pyro"] = importlib.import_module(f"{__name__}.priors.pyro")
+    sys.modules["priors.gp"] = importlib.import_module(f"{__name__}.priors.gp")
+    sys.modules["priors.ridge"] = importlib.import_module(f"{__name__}.priors.ridge")
+    sys.modules["priors.binarized_regression"] = importlib.import_module(f"{__name__}.priors.binarized_regression")
     sys.modules["mcmc_svi_transformer_on_bayesian"] = importlib.import_module(f"{__name__}.mcmc_svi_transformer_on_bayesian")
     sys.modules["tabular"] = importlib.import_module(f"{__name__}.tabular")
     return {name: sys.modules[name] for name in _DROPIN_MODULES}

@@ -154,6 +154,32 @@ class ConvDesc(ctypes.Structure):
 CONV_MAX_SIDE, CONV_CH = 112, 64
 
 
+class RidgePrefixDesc(ctypes.Structure):
+    _fields_ = [
+        ("B", c_int), ("T", c_int), ("F", c_int),
+        ("alpha", c_double),
+        ("x", c_void_p), ("y", c_void_p), ("target", c_void_p),
+        ("pred", c_void_p), ("sq_err", c_void_p),
+    ]
+
+
+RIDGE_MAX_F = 64
+
+
+class ExactGpDesc(ctypes.Structure):
+    _fields_ = [
+        ("B", c_int), ("T", c_int), ("F", c_int),
+        ("mode", c_int),
+        ("length_scale", c_double), ("alpha", c_double),
+        ("x", c_void_p), ("y", c_void_p), ("z", c_void_p),
+        ("mean", c_void_p), ("var", c_void_p), ("status", c_void_p),
+        ("sample", c_void_p), ("rank", c_void_p), ("factor", c_void_p), ("perm", c_void_p),
+    ]
+
+
+EXACT_GP_EVALUATE, EXACT_GP_SAMPLE = 0, 1
+
+
 P, I, F, U = c_void_p, c_int, c_float, c_uint32
 
 # argument types of every entry point, in header order, one per C parameter (pointers to descriptors as POINTER(...), every
@@ -197,6 +223,8 @@ _PROTOTYPES = {
     "pfn_conv_wgrad": [POINTER(ConvDesc), P],
     "pfn_conv_mean_fwd": [P, I, I, I, P, P],
     "pfn_conv_mean_bwd": [P, P, I, I, I, P, P],
+    "pfn_ridge_prefix": [POINTER(RidgePrefixDesc), P],
+    "pfn_exact_gp": [POINTER(ExactGpDesc), P],
 }
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)
 
@@ -748,6 +776,49 @@ def knn_cv(x, y, proba, k_best, cv_mean, status):
     d.x, d.y = x.data_ptr(), y.data_ptr()
     d.proba, d.k_best, d.cv_mean, d.status = proba.data_ptr(), k_best.data_ptr(), cv_mean.data_ptr(), status.data_ptr()
     check(load().pfn_knn_cv(ctypes.byref(d), stream_ptr()), "pfn_knn_cv")
+
+
+@_guarded
+def ridge_prefix(x, y, target, alpha, pred, sq_err):
+    """One launch fits sklearn's Ridge(alpha) to every prefix t = 1 .. T-1 of every dataset.  x [B,T,F], y / target [B,T]
+    fp32; outputs pred / sq_err [B,T] fp64 (column 0 NaN)."""
+    _count(1)
+    require_cuda(x, y, target, pred, sq_err)
+    d = RidgePrefixDesc()
+    d.B, d.T, d.F = x.shape
+    d.alpha = float(alpha)
+    d.x, d.y, d.target, d.pred, d.sq_err = x.data_ptr(), y.data_ptr(), target.data_ptr(), pred.data_ptr(), sq_err.data_ptr()
+    check(load().pfn_ridge_prefix(ctypes.byref(d), stream_ptr()), "pfn_ridge_prefix")
+
+
+def _exact_gp_desc(x, mode, length_scale, alpha=0.0):
+    d = ExactGpDesc()
+    d.B, d.T, d.F = x.shape
+    d.mode, d.length_scale, d.alpha = mode, float(length_scale), float(alpha)
+    d.x = x.data_ptr()
+    return d
+
+
+@_guarded
+def exact_gp_evaluate(x, y, length_scale, alpha, mean, var, status):
+    """The RBF exact GP's predictive of row t given rows < t, every t = 1 .. T-1 and dataset, from one factor per dataset.
+    x [B,T,F], y [B,T] fp32; outputs mean / var [B,T] fp64 (column 0 NaN), status [B] int32 (0 or the failing prefix)."""
+    _count(1)
+    require_cuda(x, y, mean, var, status)
+    d = _exact_gp_desc(x, EXACT_GP_EVALUATE, length_scale, alpha)
+    d.y, d.mean, d.var, d.status = y.data_ptr(), mean.data_ptr(), var.data_ptr(), status.data_ptr()
+    check(load().pfn_exact_gp(ctypes.byref(d), stream_ptr()), "pfn_exact_gp")
+
+
+@_guarded
+def exact_gp_sample(x, z, length_scale, sample, rank, factor=None, perm=None):
+    """sample [B,T] fp32 = P L z[:, :r] with P L L^T P^T = RBF(x, x) (pivoted Cholesky to the numerical rank r); rank [B]
+    int32; optional factor [B,T,T] fp64 (P L) and perm [B,T] int32 (pivot order)."""
+    _count(1)
+    require_cuda(x, z, sample, rank, factor, perm)
+    d = _exact_gp_desc(x, EXACT_GP_SAMPLE, length_scale)
+    d.z, d.sample, d.rank, d.factor, d.perm = z.data_ptr(), sample.data_ptr(), rank.data_ptr(), ptr(factor), ptr(perm)
+    check(load().pfn_exact_gp(ctypes.byref(d), stream_ptr()), "pfn_exact_gp")
 
 
 # ------------------------------------------------------------------------------------------------

@@ -36,6 +36,7 @@ SOURCES = [
     "bnn_mcmc.cu",
     "knn_cv.cu",
     "conv_encoder.cu",
+    "regression_baselines.cu",
 ]
 
 NVCC_FLAGS = [

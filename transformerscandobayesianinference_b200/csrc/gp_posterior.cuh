@@ -62,6 +62,29 @@ __device__ __forceinline__ double log_gamma_pdf(double v, double a, double b) {
   return a * log(b) - lgamma(a) + (a - 1.0) * log(v) - b * v;
 }
 
+// Cholesky of the t x t lower triangle of A in place (all threads), right-looking, one barrier per column: phase j
+// updates the trailing block with the unscaled column j and scales column j-1 (nobody reads it in phase j).  On success
+// returns t, with L's strict lower triangle in A and its diagonal in dg.  Otherwise returns the first pivot j that is not
+// positive: columns < j - 1 of L and dg[0 .. j-1] are then final, column j - 1 below the diagonal still awaits its
+// division by dg[j-1], and the rest of A is unspecified.
+__device__ __forceinline__ int cholesky_lower(double* A, double* dg, int t, int ld) {
+  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+  for (int j = 0; j < t; ++j) {
+    const double dj = A[j * ld + j];
+    if (!(dj > 0.0) || !isfinite(dj)) return j;                  // uniform: every thread read the same pivot
+    const double inv_d = 1.0 / dj;
+    if (tid == 0) dg[j] = sqrt(dj);
+    if (j > 0)
+      for (int r = j + tid; r < t; r += FT) A[r * ld + j - 1] /= dg[j - 1];
+    for (int r = j + 1 + ty; r < t; r += 16) {
+      const double arj = A[r * ld + j] * inv_d;
+      for (int q = j + 1 + tx; q <= r; q += 16) A[r * ld + q] = fma(-arj, A[q * ld + j], A[r * ld + q]);
+    }
+    __syncthreads();
+  }
+  return t;
+}
+
 struct Problem {
   const double* xs;                            // [t, F] rows of the dataset
   const double* ys;                            // [t]
@@ -94,21 +117,7 @@ __device__ __forceinline__ int factor(const Problem& P, const double* inv_ls, do
     }
   for (int i = tid; i < t; i += FT) yc[i] = P.ys[i] - c;
   __syncthreads();
-  // ---- Cholesky, right-looking, one barrier per column: phase j updates the trailing block with the unscaled column j
-  // and scales column j-1 (nobody reads it in phase j)
-  for (int j = 0; j < t; ++j) {
-    const double dj = A[j * ld + j];
-    if (!(dj > 0.0) || !isfinite(dj)) return 0;                  // uniform: every thread read the same pivot
-    const double inv_d = 1.0 / dj;
-    if (tid == 0) dg[j] = sqrt(dj);
-    if (j > 0)
-      for (int r = j + tid; r < t; r += FT) A[r * ld + j - 1] /= dg[j - 1];
-    for (int r = j + 1 + ty; r < t; r += 16) {
-      const double arj = A[r * ld + j] * inv_d;
-      for (int q = j + 1 + tx; q <= r; q += 16) A[r * ld + q] = fma(-arj, A[q * ld + j], A[r * ld + q]);
-    }
-    __syncthreads();
-  }
+  if (cholesky_lower(A, dg, t, ld) < t) return 0;
   log_dg = tid < t ? log(dg[tid]) : 0.0;       // t <= FT
   // ---- L^-1 into the upper triangle, transposed: U[j][i] = X[i][j] (i >= j), row k of X final after phase k-1.
   for (int j = ty; j < t; j += 16)

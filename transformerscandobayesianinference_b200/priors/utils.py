@@ -47,6 +47,15 @@ def check_flag(flag, on_set, may_defer=True):
     return True
 
 
+def again_after_deferred_checks(fn):
+    """Calls `fn()` at once and, while a loader defers and checks are pending, once more at hand-off after them (a check
+    may rewrite a sampler's output in place, e.g. fast_gp's jitter escalation).  So what `fn` writes is valid at once and
+    final after hand-off; anything derived from it before hand-off (inside the loader's `_produce`) may be stale."""
+    fn()
+    if _Deferred.active and _Deferred.pending:
+        _Deferred.pending.append(fn)
+
+
 def on_requested_device(device, *tensors):
     """A sampler's outputs, copied to `device` when the caller asked for a non-CUDA one (the sampler ran on CUDA)."""
     dev = torch.device(device)
