@@ -113,7 +113,9 @@ def test_attention_tc_slowly_rising_max(cuda_device, T, B, H, sep):
     EB.check_attention_bwd(dqkv, EB.attention_bwd(f, dout, out), EB.C_ATT_GRAD)
 
 
-@pytest.mark.parametrize("T,B,H,sep", TC_CASES + [(1000, 1, 2, 1000), (96, 1, 1, 33)])
+@pytest.mark.parametrize("T,B,H,sep", TC_CASES + [(1000, 1, 2, 1000), (96, 1, 1, 33), (128, 1, 1, 128), (256, 1, 1, 64),
+                                                  (256, 1, 1, 128), (256, 1, 1, 192), (128, 2, 1, 64), (128, 1, 2, 64),
+                                                  (200, 1, 1, 100)])
 def test_attention_tc_bwd(cuda_device, T, B, H, sep):
     torch.manual_seed(T * 3 + sep)
     dh = 128

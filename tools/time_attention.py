@@ -6,7 +6,7 @@ libpfn_b200.so on the same inputs.
 Every library is loaded with ctypes and called with the same seeded qkv and dO at the cfg-2 shape (T = 1000, sep = 500,
 B = 512, H = 4) and the cfg-4 shape (T = 2000, sep = 1000, B = 256, H = 4).  After a warm-up, each round times 30
 launches per library with CUDA events, alternating the libraries, over 3 rounds.  It prints ms per launch and the
-algorithmic TFLOP/s (the pair count of tools/step_breakdown.py: forward S and PV, backward S, dP, dV, dK and dQ over
+algorithmic TFLOP/s (gpu_timing.attention_pairs: forward S and PV, backward S, dP, dV, dK and dQ over
 T * sep + (T - sep) pairs).  The backward is called the way the engine calls it: out and lse from the first library's
 forward, delta precomputed token-major ([T*B, H], delta_token_major = 1) and dq_colsum set.
 
@@ -18,12 +18,12 @@ difference in bf16 ulps of the first library's value, and the max |d dq_colsum|.
 the mean CUDA time of each of its kernels.  The card name, power limit and max SM clock are printed with the numbers."""
 import ctypes
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from transformerscandobayesianinference_b200 import _lib as L
+from gpu_timing import attention_pairs, card, event_times, kernel_seconds
 
 SHAPES = [("cfg2", 1000, 500, 512, 4), ("cfg4", 2000, 1000, 256, 4)]
 DH, LAUNCHES, ROUNDS, WARMUP = 128, 30, 3, 3
@@ -33,31 +33,15 @@ def open_lib(path):
     return L.declare(ctypes.CDLL(os.path.abspath(path)))
 
 
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    except (OSError, subprocess.CalledProcessError, IndexError):
-        q = f"{torch.cuda.get_device_name()}, power limit not read, max SM clock not read"
-    return q
-
-
 def time_rounds(launch, n):
     """ms per launch of launch(k) for each of n libraries, alternated over ROUNDS rounds after a warm-up"""
     for k in range(n):
         for _ in range(WARMUP):
             launch(k)
-    torch.cuda.synchronize()
     times = [[] for _ in range(n)]
     for _ in range(ROUNDS):
         for k in range(n):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(LAUNCHES):
-                launch(k)
-            e1.record()
-            torch.cuda.synchronize()
-            times[k].append(e0.elapsed_time(e1) / LAUNCHES)
+            times[k] += [1e3 * s for s in event_times(lambda: launch(k), 1, warmup=0, calls=LAUNCHES)]
     return times
 
 
@@ -82,17 +66,10 @@ def diff_line(name, a, ref):
 
 
 def profile_bwd(paths, launch):
-    from torch.profiler import ProfilerActivity, profile
     for k, p in enumerate(paths):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(LAUNCHES):
-                launch(k)
-            torch.cuda.synchronize()
-        for ev in prof.key_averages():
-            if ev.device_type == torch.autograd.DeviceType.CUDA and ev.count > 0:
-                us = getattr(ev, "device_time_total", None) or ev.cuda_time_total
-                print(f"  profile {p}: {ev.key[:60]}: {us / ev.count / 1e3:.3f} ms x {ev.count}")
+        kernels = kernel_seconds(lambda: [launch(k) for _ in range(LAUNCHES)])
+        for name, (s, n) in kernels.items():
+            print(f"  profile {p}: {name[:60]}: {s / n * 1e3:.3f} ms x {n}")
 
 
 def main():
@@ -101,10 +78,10 @@ def main():
     paths = [a for a in args if a != "--profile"]
     if not paths:
         sys.exit(__doc__)
+    print(f"card: {card('time_attention')}")
     torch.cuda.init()
     libs = [open_lib(p) for p in paths]
     stream = torch.cuda.current_stream().cuda_stream
-    print(f"card: {card()}")
 
     def call(k, fn, desc):
         rc = getattr(libs[k], fn)(ctypes.byref(desc), ctypes.c_void_p(stream))
@@ -118,7 +95,7 @@ def main():
         outs = [torch.empty(T * B, E, device="cuda", dtype=torch.bfloat16) for _ in libs]
         lses = [torch.empty(B * H, T, device="cuda") for _ in libs]
         descs = [L.attention_desc(qkv, o, s, T, B, H, DH, sep) for o, s in zip(outs, lses)]
-        pairs = T * sep + (T - sep)
+        pairs = attention_pairs(T, sep)
 
         times = time_rounds(lambda k: call(k, "pfn_attention_fwd_tc", descs[k]), len(libs))
         flop = 2 * 2.0 * pairs * DH * B * H

@@ -14,7 +14,6 @@ seconds per chain.  The card's name and power limit are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -26,28 +25,7 @@ import torch  # noqa: E402
 from transformerscandobayesianinference_b200 import _lib as L  # noqa: E402
 from transformerscandobayesianinference_b200 import mcmc_svi_transformer_on_bayesian as M  # noqa: E402
 from transformerscandobayesianinference_b200.priors import pyro as P  # noqa: E402
-
-
-def card():
-    if not torch.cuda.is_available():
-        raise SystemExit("time_bnn_mcmc needs a CUDA device (nothing is timed on the host alone)")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
-
-
-def timed(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        times.append(e0.elapsed_time(e1) / 1e3)
-    return sorted(times)
+from gpu_timing import card, event_times  # noqa: E402
 
 
 def work(X, y, spec, n, steps):
@@ -69,7 +47,7 @@ def main():
     ap.add_argument("--cpu-chains", type=int, default=1)
     ap.add_argument("--no-sweep", action="store_true")
     args = ap.parse_args()
-    print(f"[time_bnn_mcmc] card: {card()}", flush=True)
+    print(f"[time_bnn_mcmc] card: {card('time_bnn_mcmc')}", flush=True)
     dev = torch.device("cuda:0")
     for size in ("small", "big"):
         spec = M.get_default_model_spec(size)
@@ -77,23 +55,17 @@ def main():
         X, y = M.generate_toy_data(sampler(), spec["seq_len"], device=dev)
         d = spec["embed"] * spec["num_features"] + 3 * spec["embed"] + 2
         for steps in (64, 512):
-            t = timed(lambda: M.eval_mcmc(X, y, dev, sampler, 100, steps, steps, seed=1), args.reps)
+            t = event_times(lambda: M.eval_mcmc(X, y, dev, sampler, 100, steps, steps, seed=1), args.reps)
             print(json.dumps(dict({"model": size, "d": d, "chains": 100, "train_rows": 100, "warmup": steps, "samples": steps,
                                    "eval_mcmc_s": t}, **work(X, y, spec, 100, steps))), flush=True)
         if not args.no_sweep:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            points, per_point = M.get_default_evaluation_points(), []
+            points = M.get_default_evaluation_points()
             M.eval_mcmc(X, y, dev, sampler, points[0], 8, 8, seed=1)
-            torch.cuda.synchronize()
-            for n in points:
-                e0.record()
-                M.eval_mcmc(X, y, dev, sampler, n, 512, 512, seed=1)
-                e1.record()
-                torch.cuda.synchronize()
-                per_point.append(round(e0.elapsed_time(e1) / 1e3, 3))
+            per_point = [round(event_times(lambda: M.eval_mcmc(X, y, dev, sampler, n, 512, 512, seed=1), 1, warmup=0)[0], 3)
+                         for n in points]
             print(json.dumps({"model": size, "sweep_train_rows": points, "warmup": 512, "samples": 512,
                               "eval_mcmc_s_per_point": per_point, "sweep_total_s": sum(per_point)}), flush=True)
-        t = timed(lambda: P.get_batch(256, 300, model=sampler, device=dev), max(args.reps, 10))
+        t = event_times(lambda: P.get_batch(256, 300, model=sampler, device=dev), max(args.reps, 10))
         print(json.dumps({"model": size, "get_batch": [256, 300], "get_batch_s": t}), flush=True)
         if args.cpu_chains > 0:
             from oracle import bnn_oracle as O
@@ -103,7 +75,7 @@ def main():
                 O.bnn_chain_job((Xd[b], yd[b], spec["num_features"], spec["embed"], 64, 64, 1, b, 10))
             print(json.dumps({"model": size, "cpu_restatement_warmup_samples": [64, 64],
                               "cpu_restatement_s_per_chain": (time.time() - t0) / args.cpu_chains}), flush=True)
-    print(f"[time_bnn_mcmc] card (again): {card()}", flush=True)
+    print(f"[time_bnn_mcmc] card (again): {card('time_bnn_mcmc')}", flush=True)
 
 
 if __name__ == "__main__":

@@ -11,7 +11,6 @@ Trainer.step with the Omniglot sampler on a synthetic bank.  Prints the GPU name
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -19,6 +18,8 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 import torch.nn as nn  # noqa: E402
+
+from gpu_timing import card, event_times, kernel_seconds  # noqa: E402
 
 PEAK_BF16, PEAK_BW = 989e12, 3.35e12      # H100 SXM data sheet (dense bf16, HBM3)
 
@@ -51,26 +52,8 @@ def act_bytes(N, S, dt_size=2):
     return b
 
 
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        out = ""
-    return out or torch.cuda.get_device_name()
-
-
-def time_ms(fn, iters, warmup=5):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
+def time_ms(fn, iters):
+    return 1e3 * event_times(fn, 1, warmup=5, calls=iters)[0]
 
 
 def time_encoder(T, B, S, E, iters):
@@ -135,19 +118,16 @@ def time_cfg5_step(iters, E=512, B=256):
 
 
 def profile_encoder(T=6, B=256, S=28, E=512):
-    from torch.profiler import ProfilerActivity, profile
     from transformerscandobayesianinference_b200 import encoders
     enc = encoders.Conv(S * S, E).cuda()
     x = torch.rand(T, B, S * S, device="cuda")
     dout = torch.randn(T, B, E, device="cuda")
     for _ in range(3):
         enc(x).backward(dout)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(5):
-            enc(x).backward(dout)
-        torch.cuda.synchronize()
-    print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=20))
+    kernels = kernel_seconds(lambda: [enc(x).backward(dout) for _ in range(5)])
+    print(f"{'kernel':90s} {'total ms':>9s} {'launches':>8s} {'ms each':>8s}")
+    for name, (s, n) in sorted(kernels.items(), key=lambda kv: -kv[1][0])[:20]:
+        print(f"{name[:90]:90s} {s * 1e3:9.3f} {n:8d} {s / n * 1e3:8.3f}")
 
 
 def main():
@@ -155,13 +135,10 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--profile", action="store_true")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_conv_encoder: no CUDA device")
+    print(json.dumps({"gpu": card("time_conv_encoder")}))
     if args.profile:
-        print(json.dumps({"gpu": gpu_info()}))
         profile_encoder()
         return
-    print(json.dumps({"gpu": gpu_info()}))
     print(json.dumps(time_encoder(6, 256, 28, 512, args.iters)))
     print(json.dumps(time_encoder(26, 100, 28, 512, args.iters)))
     print(json.dumps(time_cfg5_step(args.iters)))

@@ -16,7 +16,6 @@ import argparse
 import json
 import multiprocessing as mp
 import os
-import subprocess
 import sys
 import time
 
@@ -26,17 +25,10 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 from transformerscandobayesianinference_b200.priors import fast_gp_mix  # noqa: E402
+from gpu_timing import card, event_times, kernel_seconds  # noqa: E402
 
 SHAPES = [(1000, 100, 1), (1000, 100, 5), (100, 128, 5)]
 FP64_PEAK = 34e12
-
-
-def card():
-    if not torch.cuda.is_available():
-        raise SystemExit("time_gp_fit needs a CUDA device (nothing is timed on the host alone)")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
 def flops(r, ts):
@@ -50,32 +42,21 @@ def main():
     ap.add_argument("--scipy-datasets", type=int, default=2)
     args = ap.parse_args()
     dev = torch.device("cuda:0")
-    print(f"[time_gp_fit] card: {card()}", flush=True)
+    print(f"[time_gp_fit] card: {card('time_gp_fit')}", flush=True)
     results = []
     for B, T, F in SHAPES:
         torch.manual_seed(B + T + F)
         x, y, _ = fast_gp_mix.get_batch(B, T, F, device=dev)
-        fast_gp_mix.evaluate(x, y, y, device=dev)                   # warm-up (module load, first launch)
-        times = []
-        for _ in range(args.reps):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            torch.cuda.synchronize()
-            e0.record()
-            losses, _, _ = fast_gp_mix.evaluate(x, y, y, device=dev)
-            e1.record()
-            torch.cuda.synchronize()
-            times.append(e0.elapsed_time(e1) / 1e3)
+        losses, _, _ = fast_gp_mix.evaluate(x, y, y, device=dev)    # warm-up (module load, first launch)
+        times = event_times(lambda: fast_gp_mix.evaluate(x, y, y, device=dev), args.reps, warmup=0)
         ts = list(range(1, T))
         xb, yb = x.transpose(0, 1).contiguous(), y.transpose(0, 1).contiguous()
         r = fast_gp_mix.fit_map(xb, yb, ts, {})
-        from torch.profiler import ProfilerActivity, profile
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fast_gp_mix.fit_map(xb, yb, ts, {})
-            torch.cuda.synchronize()
-        kern = sum(e.device_time for e in prof.events() if "gp_fit_kernel" in e.name and e.device_time > 0) / 1e6
+        kernels = kernel_seconds(lambda: fast_gp_mix.fit_map(xb, yb, ts, {}))
+        kern = sum(s for name, (s, _) in kernels.items() if "gp_fit_kernel" in name)
         fl = flops(r, ts)
         st = r["status"]
-        res = {"B": B, "T": T, "F": F, "evaluate_s": sorted(times), "kernel_s": kern, "gflop": fl / 1e9,
+        res = {"B": B, "T": T, "F": F, "evaluate_s": times, "kernel_s": kern, "gflop": fl / 1e9,
                "tflops": fl / kern / 1e12 if kern > 0 else None,
                "share_of_fp64_peak": fl / kern / FP64_PEAK if kern > 0 else None,
                "mean_evals": float(r["nevals"].double().mean()), "max_evals": int(r["nevals"].max()),
@@ -97,7 +78,7 @@ def main():
                         "scipy_restatement_s_per_call_extrapolated": per_dataset * B})
         print(json.dumps(res), flush=True)
         results.append(res)
-    print(f"[time_gp_fit] card (again): {card()}", flush=True)
+    print(f"[time_gp_fit] card (again): {card('time_gp_fit')}", flush=True)
 
 
 if __name__ == "__main__":

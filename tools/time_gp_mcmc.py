@@ -16,7 +16,6 @@ The card's name and power limit are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -27,18 +26,11 @@ import torch  # noqa: E402
 
 from transformerscandobayesianinference_b200 import _lib as L  # noqa: E402
 from transformerscandobayesianinference_b200.priors import fast_gp_mix  # noqa: E402
+from gpu_timing import card, event_times, kernel_seconds  # noqa: E402
 
 SHAPES = [(100, 50, 1, 1), (1000, 100, 1, 10), (100, 128, 5, 10)]     # B, T, F, prefix step
 FP64_PEAK = 34e12
 W, S = 300, 100
-
-
-def card():
-    if not torch.cuda.is_available():
-        raise SystemExit("time_gp_mcmc needs a CUDA device (nothing is timed on the host alone)")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
 def main():
@@ -47,7 +39,7 @@ def main():
     ap.add_argument("--cpu-chains", type=int, default=2)
     args = ap.parse_args()
     dev = torch.device("cuda:0")
-    print(f"[time_gp_mcmc] card: {card()}", flush=True)
+    print(f"[time_gp_mcmc] card: {card('time_gp_mcmc')}", flush=True)
     col = {n: i for i, n in enumerate(L.GP_MCMC_DIAG_NAMES)}
     for B, T, F, step in SHAPES:
         torch.manual_seed(B + T + F)
@@ -61,29 +53,19 @@ def main():
                 return fast_gp_mix.evaluate_(xs, ys, ys, {}, device=dev, num_samples=S, warmup_steps=W, seed=1)
             xb, yb = xs.transpose(0, 1).contiguous(), ys.transpose(0, 1).contiguous()
             return fast_gp_mix.sample_posterior(xb, yb, ts, {}, S, W, seed=1)
-        run()
-        torch.cuda.synchronize()
-        times = []
-        for _ in range(args.reps):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            torch.cuda.synchronize()
-            e0.record()
-            run()
-            e1.record()
-            torch.cuda.synchronize()
-            times.append(e0.elapsed_time(e1) / 1e3)
+        times = event_times(run, args.reps)
         xb, yb = xs.transpose(0, 1).contiguous(), ys.transpose(0, 1).contiguous()
-        from torch.profiler import ProfilerActivity, profile
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            r = fast_gp_mix.sample_posterior(xb, yb, ts, {}, S, W, seed=1, trace=True)
-            torch.cuda.synchronize()
-        kern = sum(e.device_time for e in prof.events() if "gp_mcmc_kernel" in e.name and e.device_time > 0) / 1e6
+        traced = []
+        kernels = kernel_seconds(lambda: traced.append(
+            fast_gp_mix.sample_posterior(xb, yb, ts, {}, S, W, seed=1, trace=True)))
+        kern = sum(s for name, (s, _) in kernels.items() if "gp_mcmc_kernel" in name)
+        r = traced[0]
         tt = torch.tensor(ts, dtype=torch.float64, device=dev).view(-1, 1)
         evals = r["diag"][..., col["evals"]].double()
         fl = float((evals * tt ** 3).sum())
         depth = r["trace"][..., F + 3]
         res = {"B": B, "T": T, "F": F, "prefixes": len(ts), "chains": len(ts) * B,
-               "entry": "evaluate_" if step == 1 else "sample_posterior", "call_s": sorted(times), "kernel_s": kern,
+               "entry": "evaluate_" if step == 1 else "sample_posterior", "call_s": times, "kernel_s": kern,
                "mean_leapfrog_per_chain": float(r["diag"][..., col["leapfrog"]].double().mean()),
                "mean_evals_per_chain": float(evals.mean()), "mean_tree_depth": float(depth.mean()),
                "max_depth_hits": int(r["diag"][..., col["max_depth_hits"]].sum()),
@@ -99,7 +81,7 @@ def main():
                 M.nuts_chain(M.potential_and_grad_np(xd[b, :t], yd[b, :t]), F + 2, S, W, 1, b=b, t=t)
             res.update({"cpu_restatement_t": t, "cpu_restatement_s_per_chain": (time.time() - t0) / args.cpu_chains})
         print(json.dumps(res), flush=True)
-    print(f"[time_gp_mcmc] card (again): {card()}", flush=True)
+    print(f"[time_gp_mcmc] card (again): {card('time_gp_mcmc')}", flush=True)
 
 
 if __name__ == "__main__":

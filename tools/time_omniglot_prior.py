@@ -9,7 +9,6 @@ no GPU; PIL and torchvision must import).
 import argparse
 import os
 import statistics
-import subprocess
 import sys
 import tempfile
 import time
@@ -21,6 +20,8 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_timing import card, event_times, kernel_seconds  # noqa: E402
+
 S, N_WAY, K_SHOT = 28, 5, 5
 T = N_WAY * K_SHOT + 1
 
@@ -31,24 +32,13 @@ def written_bytes(B):
 
 def time_device(omniglot, bank, B, jonas, iters):
     desc = omniglot.episode_desc(bank, B, N_WAY, K_SHOT, train=True, jonas_style=jonas, translations=True)
-    for _ in range(5):
-        omniglot.sample_episodes(bank, desc)
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        omniglot.sample_episodes(bank, desc)
-        e1.record()
-        e1.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    from torch.profiler import profile, ProfilerActivity
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    def calls():
         for _ in range(iters):
             omniglot.sample_episodes(bank, desc)
-        torch.cuda.synchronize()
-    kern = [ev for ev in prof.key_averages() if "omniglot_episode_kernel" in ev.key]
-    us = (getattr(kern[0], "device_time_total", None) or kern[0].cuda_time_total) / kern[0].count if kern else float("nan")
+    ms = [1e3 * s for s in event_times(lambda: omniglot.sample_episodes(bank, desc), iters, warmup=5)]
+    kernels = kernel_seconds(calls)
+    kern = [(s, n) for name, (s, n) in kernels.items() if "omniglot_episode_kernel" in name]
+    us = kern[0][0] / kern[0][1] * 1e6 if kern else float("nan")
     return statistics.median(ms), min(ms), us
 
 
@@ -91,13 +81,8 @@ def main():
     tm = _test_module()
     if a.reference_dir:
         time_reference(tm, a.reference_dir, a.reference_batches)
-    if not torch.cuda.is_available():
-        print("no CUDA device: device timings not measured")
-        return
+    print(f"device: {card('time_omniglot_prior')}")
     from transformerscandobayesianinference_b200.priors import omniglot
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    print(f"device: {torch.cuda.get_device_name(0)}; nvidia-smi: {q.stdout.strip() or q.stderr.strip()}")
     bank = omniglot.Bank(*tm.synthetic_bank())
     for B in (1000, 100):
         for jonas in (False, True):

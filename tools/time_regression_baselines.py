@@ -8,7 +8,6 @@ the reference's own sklearn loop on the host cores for the same inputs, on the f
 """
 import argparse
 import os
-import subprocess
 import sys
 import time
 
@@ -18,23 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from transformerscandobayesianinference_b200.priors import gp, ridge  # noqa: E402
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else torch.cuda.get_device_name()
-
-
-def timed(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    out = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        fn()                                    # ends in a copy of the losses to the host
-        out.append(time.perf_counter() - t0)
-    return min(out), sorted(out)[len(out) // 2]
+from gpu_timing import card, event_times  # noqa: E402
 
 
 def main():
@@ -42,15 +25,15 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--ref-datasets", type=int, default=100)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a CUDA device"
+    print(f"card: {card('time_regression_baselines')}")
     torch.manual_seed(0)
     B, T, F = 1000, 10, 10
     rx, ry, ryn = (v.cuda() for v in ridge.get_batch(B, T, F, noisy_std=.01))
     gx, gy, _ = gp.get_batch(B, T, F, noisy_std=.6)
-    print(f"card: {card()}")
     for name, fn in (("ridge.evaluate(alpha=.01)", lambda: ridge.evaluate(rx, ry, ryn, alpha=.01)),
                      ("gp.evaluate(ls=.6, nll)", lambda: gp.evaluate(gx, gy, gy))):
-        best, med = timed(fn, a.reps)
+        t = event_times(fn, a.reps)              # each call ends in a copy of the losses to the host
+        best, med = t[0], t[len(t) // 2]
         print(f"{name:28s} B={B} T={T} F={F}: device {best * 1e3:8.2f} ms best, {med * 1e3:8.2f} ms median")
     if os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "sklearn_priors")):
         import warnings

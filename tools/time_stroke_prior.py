@@ -17,38 +17,24 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+from gpu_timing import card, event_times, kernel_seconds  # noqa: E402
+
 T, C, F = 26, 5, 784
 KW = dict(num_features=F, num_outputs=C, only_train_for_last_idx=True)
 
 
 def time_device(stroke, B, iters):
-    for _ in range(3):
-        stroke.get_batch(B, T, device='cuda:0', **KW)
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        stroke.get_batch(B, T, device='cuda:0', **KW)
-        e1.record()
-        e1.synchronize()
-        ms.append(e0.elapsed_time(e1))
+    ms = [1e3 * s for s in event_times(lambda: stroke.get_batch(B, T, device='cuda:0', **KW), iters, warmup=3)]
     return statistics.median(ms), min(ms)
 
 
 def profile_kernels(stroke, B):
-    from torch.profiler import profile, ProfilerActivity
-    stroke.get_batch(B, T, device='cuda:0', **KW)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    def calls():
         for _ in range(5):
             stroke.get_batch(B, T, device='cuda:0', **KW)
-        torch.cuda.synchronize()
-    rows = []
-    for ev in prof.key_averages():
-        t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
-        if t > 0 and ev.count > 0:
-            rows.append((t / ev.count, ev.count, ev.key))
+    stroke.get_batch(B, T, device='cuda:0', **KW)
+    kernels = kernel_seconds(calls)
+    rows = [(s / n * 1e6, n, name) for name, (s, n) in kernels.items()]
     for us, n, key in sorted(rows, reverse=True)[:10]:
         print(f"    {us:9.1f} us  x{n:<3d} {key[:90]}")
 
@@ -79,25 +65,13 @@ def time_steps(stroke, steps):
                        y_encoder_generator=encoders.get_Canonical(C), extra_prior_kwargs_dict=dict(KW, fuse_x_y=False),
                        single_eval_pos_gen=T - 1, gpu_device='cuda:0')
     (x, y), tgt = next(iter(tr.dl))
-    for _ in range(3):
-        tr.step((x, y), tgt, T - 1)
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        tr.step((x, y), tgt, T - 1)
-    torch.cuda.synchronize()
-    pre = (time.perf_counter() - t0) / steps
+    pre = event_times(lambda: tr.step((x, y), tgt, T - 1), 1, warmup=3, calls=steps)[0]
     it = iter(tr.dl)
-    for _ in range(3):
+
+    def fed_step():
         (x, y), tgt = next(it)
         tr.step((x, y), tgt, T - 1)
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        (x, y), tgt = next(it)
-        tr.step((x, y), tgt, T - 1)
-    torch.cuda.synchronize()
-    fed = (time.perf_counter() - t0) / steps
+    fed = event_times(fed_step, 1, warmup=3, calls=steps)[0]
     print(f"Trainer.step emsize 1024 nhead 4 6 layers B=1000 T=26: pre-drawn batch {pre * 1e3:.2f} ms/step, "
           f"sampled by the prefetching loader {fed * 1e3:.2f} ms/step")
 
@@ -108,14 +82,14 @@ def short_train(steps):
     import priors.stroke  # noqa: F401  (the drop-in module, as the notebook imports it)
     encoders, train_mod = mods["encoders"], mods["train"]
     torch.manual_seed(0)
-    t0 = time.perf_counter()
-    res = train_mod.train(sys.modules["priors.stroke"].DataLoader, train_mod.Losses.ce, encoders.Linear, emsize=1024, nhead=4,
-                          warmup_epochs=5, nhid=2048, y_encoder_generator=encoders.get_Canonical(5), lr=.0001, epochs=1,
-                          single_eval_pos_gen=T - 1, extra_prior_kwargs_dict=dict(KW, fuse_x_y=False), bptt=T, nlayers=6,
-                          dropout=0.0, steps_per_epoch=steps, batch_size=1000)
-    torch.cuda.synchronize()
-    print(f"train(priors.stroke.DataLoader, ...) notebook settings, 1 epoch x {steps} steps: {time.perf_counter() - t0:.1f} s, "
-          f"final loss {res[0]:.4f}")
+    res = []
+    secs = event_times(lambda: res.append(train_mod.train(
+        sys.modules["priors.stroke"].DataLoader, train_mod.Losses.ce, encoders.Linear, emsize=1024, nhead=4, warmup_epochs=5,
+        nhid=2048, y_encoder_generator=encoders.get_Canonical(5), lr=.0001, epochs=1, single_eval_pos_gen=T - 1,
+        extra_prior_kwargs_dict=dict(KW, fuse_x_y=False), bptt=T, nlayers=6, dropout=0.0, steps_per_epoch=steps,
+        batch_size=1000)), 1, warmup=0)[0]
+    print(f"train(priors.stroke.DataLoader, ...) notebook settings, 1 epoch x {steps} steps: {secs:.1f} s, "
+          f"final loss {res[0][0]:.4f}")
 
 
 def main():
@@ -127,11 +101,8 @@ def main():
     a = ap.parse_args()
     if a.reference_dir:
         time_reference(1000, a.reference_dir)
-    if not torch.cuda.is_available():
-        print("no CUDA device: device timings skipped")
-        return
+    print(f"device: {card('time_stroke_prior')}")
     from transformerscandobayesianinference_b200.priors import stroke
-    print(f"device: {torch.cuda.get_device_name(0)}")
     for B in (1000, 512):
         med, best = time_device(stroke, B, a.iters)
         mb = T * B * F * 4 / 1e6

@@ -10,7 +10,6 @@ import argparse
 import contextlib
 import io
 import os
-import subprocess
 import sys
 import time
 
@@ -20,6 +19,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from transformerscandobayesianinference_b200 import encoders, tabular  # noqa: E402
 from transformerscandobayesianinference_b200.transformer import TransformerModel  # noqa: E402
+from gpu_timing import card, event_times  # noqa: E402
 
 
 def synthetic_datasets(n, rows=400, seed=0):
@@ -34,13 +34,9 @@ def synthetic_datasets(n, rows=400, seed=0):
     return out
 
 
-def timed(fn):
-    torch.cuda.synchronize()
-    t0 = time.time()
+def quiet(fn):
     with contextlib.redirect_stdout(io.StringIO()):
-        r = fn()
-    torch.cuda.synchronize()
-    return time.time() - t0, r
+        return fn()
 
 
 def main():
@@ -48,9 +44,7 @@ def main():
     ap.add_argument("--datasets", type=int, default=37)
     ap.add_argument("--no-sklearn", action="store_true")
     args = ap.parse_args()
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                          text=True).stdout.strip()
-    print(f"card: {card}")
+    print(f"card: {card('time_tabular')}")
     ds = synthetic_datasets(args.datasets)
     torch.manual_seed(0)
     model = TransformerModel(encoders.Linear(60, 512), 1, 512, 4, 1024, 5, 0.5, y_encoder=encoders.Linear(1, 512)).cuda()
@@ -58,9 +52,8 @@ def main():
     for label, fn in (("pfn", lambda: tabular.evaluate(ds, model, 'transformer', max_features=60, extend_features=True,
                                                        rescale_features=True, **kw)),
                       ("knn", lambda: tabular.evaluate(ds, tabular.knn_metric, 'knn', **kw))):
-        timed(fn)                                   # warm-up: module loads, allocator
-        secs = [timed(fn)[0] for _ in range(3)]
-        r = timed(fn)[1]
+        secs = event_times(lambda: quiet(fn), 3)    # one warm-up call first: module loads, allocator
+        r = quiet(fn)
         print(f"{label}: evaluate over {len(ds)} datasets: best {min(secs):.3f} s, median {np.median(secs):.3f} s "
               f"(mean AUC {r['mean_metric']:.4f})")
     if not args.no_sklearn:
@@ -79,7 +72,9 @@ def main():
             clf.fit(x.numpy(), y.long().numpy())
             pred = clf.predict_proba(test_x.numpy())[:, 1]
             return tabular.metric_used(test_y.numpy(), pred), pred
-        secs, _ = timed(lambda: tabular.evaluate(ds, host_knn, 'knn_host', **kw))
+        t0 = time.time()
+        quiet(lambda: tabular.evaluate(ds, host_knn, 'knn_host', **kw))
+        secs = time.time() - t0
         print(f"knn (sklearn GridSearchCV per sample on {os.cpu_count()} host cores): {secs:.3f} s")
 
 

@@ -423,13 +423,18 @@ def gemm(A, B, C, *, a_mn_major=False, b_mn_major=False, bias=None, aux=None, C2
             e0.record()
             check(lib.pfn_gemm_bf16_tc(ctypes.byref(d), stream_ptr()), "pfn_gemm_bf16_tc")
             e1.record()
-            esz = 4 if C.dtype == torch.float32 else 2
-            nbytes = 2.0 * (M * K + N * K) + esz * M * N * (2 if C2 is not None else 1) + (2.0 * M * N if aux is not None else 0.0)
-            PROFILE_GEMM.append((2.0 * M * N * K, e0, e1, nbytes))
+            PROFILE_GEMM.append((2.0 * M * N * K, e0, e1, gemm_bytes(d)))
         else:
             check(lib.pfn_gemm_bf16_tc(ctypes.byref(d), stream_ptr()), "pfn_gemm_bf16_tc")
     else:
         check(lib.pfn_gemm_simt(ctypes.byref(d), stream_ptr()), "pfn_gemm_simt")
+
+
+def gemm_bytes(d):
+    """Algorithmic HBM bytes of the wgmma GEMM `d` (a GemmDesc): bf16 A and B read once, C (and C2) written once in C's
+    dtype, bf16 aux read once."""
+    esz = 4 if d.c_dtype == F32 else 2
+    return 2.0 * (d.M * d.K + d.N * d.K) + esz * d.M * d.N * (2 if d.C2 else 1) + (2.0 * d.M * d.N if d.aux else 0.0)
 
 
 def tc_gemm_ok(A, B, C, aux=None, C2=None):
