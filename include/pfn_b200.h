@@ -545,6 +545,33 @@ typedef struct pfn_exact_gp_desc {
 } pfn_exact_gp_desc;
 int pfn_exact_gp(const pfn_exact_gp_desc* d, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Learned-temperature decoder heads (reference decoders.py:6-30): the row work after the head's second GEMM, whose output
+ * zz is fp32.  One warp per row; every sum runs in a fixed order, without atomics.
+ * ScaledDecoder (decoders.py:13-20), zz [rows, ldz] = [z | zt] with z = linear1(x) (n_out columns) and zt = linear2(x):
+ *   pfn_scaled_head_fwd : p = softmax(zt) (max, expf, butterfly sum of depth 5); temp = sum_k p_k c_k (depth 5) with
+ *                         c = {1, 1.4, 1.7, 2, 5, 10, 20, 40, 80, 160} in fp32; out [rows, ldo] = z / temp; temp [rows].
+ *   pfn_scaled_head_bwd : from g [rows, ldg] = dL/dout and the forward's temp: dzz[:, j] = g_j / temp (j < n_out);
+ *                         dzz[:, n_out + k] = p_k (c_k - temp) dtemp with dtemp = -(sum_j g_j z_j) / temp^2 (the sum: fmaf
+ *                         per lane over columns lane, lane + 32, ..., then the butterfly: depth ceil(n_out / 32) + 5);
+ *                         columns [n_out + 10, n_cols_pad) are zero.  dzz in d_dtype (PFN_F32 / PFN_BF16).
+ * FixedScaledDecoder (decoders.py:22-30), z [rows, ldz] = mapper(x), T [n_t] the temperature parameter:
+ *   pfn_fixed_scaled_head_fwd : S = sum(T) (depth ceil(n_t / 256) + 8; formed by every CTA, stored to *S) and
+ *                               out [rows, ldo] = z / S.
+ *   pfn_fixed_scaled_head_bwd : dz = g / S (d_dtype, zero in columns [n_out, n_cols_pad)); row_dot [rows] fp32 workspace
+ *                               = sum_j g_j z_j (depth ceil(n_out / 32) + 5); D = sum of row_dot (one CTA, depth
+ *                               ceil(rows / 1024) + 10); every dT_i = -D / S^2 (overwritten).  S is the forward's.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PFN_HEAD_TEMPS = 10 };
+int pfn_scaled_head_fwd(const float* zz, int ldz, int n_out, float* out, int ldo, float* temp, int rows, void* stream);
+int pfn_scaled_head_bwd(const float* g, int ldg, const float* zz, int ldz, const float* temp, int n_out, void* dzz, int ldd,
+                        int d_dtype, int n_cols_pad, int rows, void* stream);
+int pfn_fixed_scaled_head_fwd(const float* z, int ldz, int n_out, const float* T, int n_t, float* out, int ldo, float* S,
+                              int rows, void* stream);
+int pfn_fixed_scaled_head_bwd(const float* g, int ldg, const float* z, int ldz, const float* S, int n_out, void* dz,
+                              int ldd, int d_dtype, int n_cols_pad, float* row_dot, float* dT, int n_t, int rows,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

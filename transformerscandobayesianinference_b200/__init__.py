@@ -2,8 +2,9 @@
 automl/TransformersCanDoBayesianInference, behind the reference's own Python module API.
 
     from transformerscandobayesianinference_b200 import train, transformer, bar_distribution, priors, encoders, utils
+    from transformerscandobayesianinference_b200 import decoders      # ScaledDecoder, FixedScaledDecoder
 
-or, for unmodified notebooks that do `from train import train; import priors, encoders, ...`:
+or, for unmodified notebooks that do `from train import train; import priors, encoders, decoders, ...`:
 
     import transformerscandobayesianinference_b200 as pfn; pfn.install_dropin()
 """
@@ -17,7 +18,8 @@ _DROPIN_MODULES = ("utils", "encoders", "positional_encodings", "bar_distributio
 
 def install_dropin():
     """Register this package's modules under the reference's top-level module names (train, transformer,
-    bar_distribution, priors, encoders, positional_encodings, utils) so reference notebooks import them unchanged."""
+    bar_distribution, priors, encoders, positional_encodings, utils, and also decoders, tabular and the priors' submodules)
+    so reference notebooks import them unchanged."""
     for name in _DROPIN_MODULES:
         mod = importlib.import_module(f"{__name__}.{name}")
         sys.modules[name] = mod
@@ -33,4 +35,5 @@ def install_dropin():
     sys.modules["priors.binarized_regression"] = importlib.import_module(f"{__name__}.priors.binarized_regression")
     sys.modules["mcmc_svi_transformer_on_bayesian"] = importlib.import_module(f"{__name__}.mcmc_svi_transformer_on_bayesian")
     sys.modules["tabular"] = importlib.import_module(f"{__name__}.tabular")
+    sys.modules["decoders"] = importlib.import_module(f"{__name__}.decoders")
     return {name: sys.modules[name] for name in _DROPIN_MODULES}

@@ -178,6 +178,7 @@ class ExactGpDesc(ctypes.Structure):
 
 
 EXACT_GP_EVALUATE, EXACT_GP_SAMPLE = 0, 1
+HEAD_TEMPS = 10        # temperature logits of decoders.ScaledDecoder
 
 
 P, I, F, U = c_void_p, c_int, c_float, c_uint32
@@ -225,6 +226,10 @@ _PROTOTYPES = {
     "pfn_conv_mean_bwd": [P, P, I, I, I, P, P],
     "pfn_ridge_prefix": [POINTER(RidgePrefixDesc), P],
     "pfn_exact_gp": [POINTER(ExactGpDesc), P],
+    "pfn_scaled_head_fwd": [P, I, I, P, I, P, I, P],
+    "pfn_scaled_head_bwd": [P, I, P, I, P, I, P, I, I, I, I, P],
+    "pfn_fixed_scaled_head_fwd": [P, I, I, P, I, P, I, P, I, P],
+    "pfn_fixed_scaled_head_bwd": [P, I, P, I, P, I, P, I, I, I, P, P, I, I, P],
 }
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)
 
@@ -902,3 +907,49 @@ def conv_mean_bwd(dfeat, y, g, N, s):
     require_cuda(dfeat, y, g)
     _count()
     check(load().pfn_conv_mean_bwd(ptr(dfeat), ptr(y), N, s, dtype_code(y), ptr(g), stream_ptr()), "pfn_conv_mean_bwd")
+
+
+# ------------------------------------------------------------------------------------------------
+# learned-temperature decoder heads (csrc/scaled_head.cu)
+# ------------------------------------------------------------------------------------------------
+@_guarded
+def scaled_head_fwd(zz, n_out, out, temp):
+    """out [rows, n_out] = zz[:, :n_out] / temp, temp [rows] = softmax(zz[:, n_out:n_out + 10]) . c; zz, out, temp fp32."""
+    _count()
+    require_cuda(zz, out, temp)
+    check(load().pfn_scaled_head_fwd(ptr(zz), zz.stride(0), int(n_out), ptr(out), out.stride(0), ptr(temp), zz.shape[0],
+                                     stream_ptr()), "pfn_scaled_head_fwd")
+
+
+@_guarded
+def scaled_head_bwd(g, zz, temp, n_out, dzz, n_cols_pad=None):
+    """dzz [rows, n_cols_pad] (activation dtype) <- g [rows, n_out] fp32, the forward's zz and temp."""
+    _count()
+    require_cuda(g, zz, temp, dzz)
+    n_cols_pad = n_out + HEAD_TEMPS if n_cols_pad is None else n_cols_pad
+    check(load().pfn_scaled_head_bwd(ptr(g), g.stride(0), ptr(zz), zz.stride(0), ptr(temp), int(n_out), ptr(dzz),
+                                     dzz.stride(0), dtype_code(dzz), int(n_cols_pad), g.shape[0], stream_ptr()),
+          "pfn_scaled_head_bwd")
+
+
+@_guarded
+def fixed_scaled_head_fwd(z, n_out, T, out, S):
+    """out [rows, n_out] = z[:, :n_out] / S with S [1] = sum(T), all fp32."""
+    _count()
+    require_cuda(z, T, out, S)
+    check(load().pfn_fixed_scaled_head_fwd(ptr(z), z.stride(0), int(n_out), ptr(T), T.numel(), ptr(out), out.stride(0),
+                                           ptr(S), z.shape[0], stream_ptr()), "pfn_fixed_scaled_head_fwd")
+
+
+@_guarded
+def fixed_scaled_head_bwd(g, z, S, n_out, dz, dT, n_cols_pad=None, row_dot=None):
+    """dz [rows, n_cols_pad] (activation dtype) = g / S; every dT [n_t] = -sum(g z) / S^2 (fp32)."""
+    require_cuda(g, z, S, dz, dT, row_dot)
+    rows = g.shape[0]
+    _count(2 if rows else 1)
+    if row_dot is None:
+        row_dot = torch.empty(rows, device=g.device, dtype=torch.float32)
+    n_cols_pad = n_out if n_cols_pad is None else n_cols_pad
+    check(load().pfn_fixed_scaled_head_bwd(ptr(g), g.stride(0), ptr(z), z.stride(0), ptr(S), int(n_out), ptr(dz),
+                                           dz.stride(0), dtype_code(dz), int(n_cols_pad), ptr(row_dot), ptr(dT), dT.numel(),
+                                           rows, stream_ptr()), "pfn_fixed_scaled_head_bwd")

@@ -37,6 +37,7 @@ SOURCES = [
     "knn_cv.cu",
     "conv_encoder.cu",
     "regression_baselines.cu",
+    "scaled_head.cu",
 ]
 
 NVCC_FLAGS = [

@@ -343,6 +343,124 @@ class DecoderFn(torch.autograd.Function):
         return dhq, dW0, db0, dW2, db2, None
 
 
+def _flat_grads(dev, *shapes):
+    """One zeroed fp32 buffer holding gradients of the given shapes back to back (a single all-reduce under DP), and
+    views of it in that order."""
+    sizes = [torch.Size(s).numel() for s in shapes]
+    flat = torch.zeros(sum(sizes), device=dev, dtype=torch.float32)
+    views, off = [], 0
+    for s, n in zip(shapes, sizes):
+        views.append(flat[off:off + n].view(s))
+        off += n
+    return flat, views
+
+
+def _bucket_ready(flat):
+    if GRAD_BUCKET_HOOK is not None:
+        GRAD_BUCKET_HOOK(flat)
+        GRAD_BUCKET_SYNC()     # a small bucket: wait for it (stream-level) so autograd never touches a buffer NCCL is still writing
+
+
+def _head_grad_rows(dout, n_cols, dt):
+    """The fp32 output gradient with unit column stride, and an uninitialised [Nq, n_cols rounded up to 8] buffer in the
+    activation dtype for the row kernel to fill (the padding keeps the GEMM operands' row pitch a multiple of 16 bytes)."""
+    dout = dout.float()
+    if dout.stride(1) != 1:
+        dout = dout.contiguous()
+    return dout, torch.empty(dout.shape[0], (n_cols + 7) // 8 * 8, device=dout.device, dtype=dt)
+
+
+class ScaledDecoderFn(torch.autograd.Function):
+    """hq [Nq, E] -> (logits [Nq, n_out] fp32, temp [Nq] fp32) of decoders.ScaledDecoder (reference decoders.py:13-20):
+    x = GELU(hq W^T + b); [z | zt] = x [W1; W2]^T + [b1; b2] in one GEMM against the stacked second-layer weights;
+    temp = softmax(zt) . c and logits = z / temp in one row kernel (csrc/scaled_head.cu).  temp is not differentiable."""
+
+    @staticmethod
+    def forward(ctx, hq, W, b, W1, b1, W2, b2, precision):
+        L.require_cuda(hq, W, b, W1, b1, W2, b2)
+        dt = act_dtype(precision)
+        hq = hq.contiguous()
+        Nq, n_out = hq.shape[0], W1.shape[0]
+        nz = n_out + L.HEAD_TEMPS
+        w = _cast(W, dt)
+        w12 = torch.cat([W1.detach(), W2.detach()], 0).to(dt)
+        b12 = torch.cat([b1.detach(), b2.detach()], 0).float()
+        g, u, u_is_grad = _gelu_linear_fwd(hq, w, b)
+        zz = torch.empty(Nq, (nz + 3) // 4 * 4, device=hq.device, dtype=torch.float32)[:, :nz]
+        L.gemm(g, w12, zz, bias=b12)
+        logits = torch.empty(Nq, (n_out + 3) // 4 * 4, device=hq.device, dtype=torch.float32)[:, :n_out]
+        temp = torch.empty(Nq, device=hq.device, dtype=torch.float32)
+        L.scaled_head_fwd(zz, n_out, logits, temp)
+        ctx.save_for_backward(hq, u, g, zz, temp, w, w12)
+        ctx.mark_non_differentiable(temp)
+        ctx.u_is_grad = u_is_grad
+        ctx.meta = (precision, W.shape, W1.shape, W2.shape)
+        return logits, temp
+
+    @staticmethod
+    def backward(ctx, dlogits, _dtemp):
+        hq, u, g, zz, temp, w, w12 = ctx.saved_tensors
+        precision, w_shape, w1_shape, w2_shape = ctx.meta
+        n_out, nhid = w1_shape
+        nz = n_out + L.HEAD_TEMPS
+        dlogits, dzz = _head_grad_rows(dlogits, nz, act_dtype(precision))
+        L.scaled_head_bwd(dlogits, zz, temp, n_out, dzz, dzz.shape[1])
+        dzv = dzz[:, :nz]
+        # [W1; W2] and [b1; b2] are contiguous in the bucket, so the stacked GEMM writes both layers' gradients in place
+        flat, (dW, db, dW12, db12) = _flat_grads(hq.device, w_shape, w_shape[:1], (nz, nhid), (nz,))
+        L.colsum(dzv, db12)
+        _linear_wgrad(dzv, g, dW12)
+        du = _gelu_linear_dgrad(dzv, w12, u, ctx.u_is_grad)
+        L.colsum(du, db)
+        _linear_wgrad(du, hq, dW)
+        dhq = _linear_dgrad(du, w)
+        _bucket_ready(flat)
+        return dhq, dW, db, dW12[:n_out], db12[:n_out], dW12[n_out:], db12[n_out:], None
+
+
+class FixedScaledDecoderFn(torch.autograd.Function):
+    """hq [Nq, E] -> logits [Nq, n_out] fp32 of decoders.FixedScaledDecoder (reference decoders.py:22-30):
+    (GELU(hq W0^T + b0) W2^T + b2) / sum(T).  The sum is formed on the device inside the row kernel; T's gradient is
+    -sum(dlogits * z) / sum(T)^2 in every entry."""
+
+    @staticmethod
+    def forward(ctx, hq, W0, b0, W2, b2, T, precision):
+        L.require_cuda(hq, W0, b0, W2, b2, T)
+        dt = act_dtype(precision)
+        hq = hq.contiguous()
+        Nq, n_out = hq.shape[0], W2.shape[0]
+        w0, w2 = _cast(W0, dt), _cast(W2, dt)
+        g, u, u_is_grad = _gelu_linear_fwd(hq, w0, b0)
+        ld = (n_out + 3) // 4 * 4
+        z = torch.empty(Nq, ld, device=hq.device, dtype=torch.float32)[:, :n_out]
+        L.gemm(g, w2, z, bias=b2.detach().contiguous())
+        logits = torch.empty(Nq, ld, device=hq.device, dtype=torch.float32)[:, :n_out]
+        S = torch.empty(1, device=hq.device, dtype=torch.float32)
+        L.fixed_scaled_head_fwd(z, n_out, T.detach().contiguous().float(), logits, S)
+        ctx.save_for_backward(hq, u, g, z, S, w0, w2)
+        ctx.u_is_grad = u_is_grad
+        ctx.meta = (precision, W0.shape, W2.shape, T.shape)
+        return logits
+
+    @staticmethod
+    def backward(ctx, dlogits):
+        hq, u, g, z, S, w0, w2 = ctx.saved_tensors
+        precision, w0_shape, w2_shape, t_shape = ctx.meta
+        n_out = w2_shape[0]
+        dlogits, dz = _head_grad_rows(dlogits, n_out, act_dtype(precision))
+        flat, (dW0, db0, dW2, db2, dT) = _flat_grads(hq.device, w0_shape, w0_shape[:1], w2_shape, w2_shape[:1], t_shape)
+        L.fixed_scaled_head_bwd(dlogits, z, S, n_out, dz, dT, dz.shape[1])
+        dzv = dz[:, :n_out]
+        L.colsum(dzv, db2)
+        _linear_wgrad(dzv, g, dW2)
+        du = _gelu_linear_dgrad(dzv, w2, u, ctx.u_is_grad)
+        L.colsum(du, db0)
+        _linear_wgrad(du, hq, dW0)
+        dhq = _linear_dgrad(du, w0)
+        _bucket_ready(flat)
+        return dhq, dW0, db0, dW2, db2, dT, None
+
+
 def conv_weight_operand(W, dgrad=False):
     """bf16 B operand of the 64 -> 64 tensor-core conv kernels: [64, 9, 64] (co, tap, ci) for the forward; for the data
     gradient (ci, tap, co) holding W[co, ci, 2 - dr, 2 - dc] at tap 3 dr + dc (the flipped kernel)."""

@@ -9,7 +9,7 @@ import torch
 import torch.nn as nn
 from torch.nn import TransformerEncoder, TransformerEncoderLayer
 
-from . import engine
+from . import decoders, engine
 from ._lib import draw_seed, drop_threshold as L_drop_threshold
 from .positional_encodings import NoPositionalEncoding
 from .utils import SeqBN
@@ -129,6 +129,10 @@ class TransformerModel(nn.Module):
         if self._default_decoder():
             out = engine.DecoderFn.apply(hq, self.decoder[0].weight, self.decoder[0].bias, self.decoder[2].weight,
                                          self.decoder[2].bias, precision)
+        elif isinstance(self.decoder, (decoders.ScaledDecoder, decoders.FixedScaledDecoder)):
+            out = self.decoder.fused(hq, (T - sep, B), precision)
         else:
-            out = self.decoder(hq.float())
+            # any other head runs as its own torch ops on the sequence-first [T - sep, B, E] rows, the shape the reference
+            # hands its decoder (reference transformer.py:85)
+            out = self.decoder(hq.float().view(T - sep, B, -1))
         return out.reshape(T - sep, B, -1)
