@@ -111,6 +111,32 @@ int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream);
 int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Context attention (inference against cached training rows; forward only, no lse):
+ *   keys(i) = the n cached training keys of batch b  U  {query row i itself}
+ *   o_i = softmax([q_i.K_b^T, q_i.k_i] * scale) [V_b; v_i]
+ * which is row n + i of the single_eval_pos attention above on the sequence (training rows, query rows) with sep = n.
+ * qkv : [m*B, 3*H*dh] packed in-projection output of the m query rows (q | k | v), token row i*B + b.
+ * kv  : [n*B, 2*H*dh] the cache: k | v of the n training rows as the training rows' in-projection produced them, token row
+ *       t*B + b; head h = columns h*dh..(h+1)*dh of each half.  On the tensor-core path a 64-key x 64-column block of one
+ *       head is one TMA box (rows t*B + b of one b are ld_kv apart), like the packed qkv of pfn_attn_desc.  Unused (may be
+ *       null) when n == 0: a query then attends only to itself.
+ * out : [m*B, H*dh].
+ * pfn_attention_ctx_fwd_tc   : TMA + wgmma path (bf16, dh = 128; leading dims multiples of 8; 16-byte aligned bases).
+ * pfn_attention_ctx_fwd_simt : fp32-FMA path (fp32 or bf16, dh <= 256).
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct pfn_attn_ctx_desc {
+  int m, n, B, H, dh;      /* query rows, cached training rows (n >= 0), batch, heads, head dim */
+  int dtype;               /* of qkv, kv and out */
+  float scale;
+  const void* qkv; int ld_qkv;
+  const void* kv; int ld_kv;
+  void* out; int ld_out;
+} pfn_attn_ctx_desc;
+
+int pfn_attention_ctx_fwd_simt(const pfn_attn_ctx_desc* d, void* stream);
+int pfn_attention_ctx_fwd_tc(const pfn_attn_ctx_desc* d, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Embedding stage (reference transformer.py:68-74):
  *   out[t,b,:] = x[t,b,:] Wx^T + bx + (t < sep ? y[t,b] wy + by : 0)
  * x [T*B, F] fp32, y [T*B] fp32, Wx [E,F], bx [E], wy [E], by [E] fp32; out [T*B, E] (out_dtype).

@@ -143,6 +143,16 @@ class AttnDesc(ctypes.Structure):
     ]
 
 
+class AttnCtxDesc(ctypes.Structure):
+    _fields_ = [
+        ("m", c_int), ("n", c_int), ("B", c_int), ("H", c_int), ("dh", c_int),
+        ("dtype", c_int), ("scale", c_float),
+        ("qkv", c_void_p), ("ld_qkv", c_int),
+        ("kv", c_void_p), ("ld_kv", c_int),
+        ("out", c_void_p), ("ld_out", c_int),
+    ]
+
+
 class ConvDesc(ctypes.Structure):
     _fields_ = [
         ("N", c_int), ("S", c_int), ("C_in", c_int), ("dtype", c_int),
@@ -195,6 +205,8 @@ _PROTOTYPES = {
     "pfn_attention_bwd_simt": [POINTER(AttnDesc), P],
     "pfn_attention_fwd_tc": [POINTER(AttnDesc), P],
     "pfn_attention_bwd_tc": [POINTER(AttnDesc), P],
+    "pfn_attention_ctx_fwd_simt": [POINTER(AttnCtxDesc), P],
+    "pfn_attention_ctx_fwd_tc": [POINTER(AttnCtxDesc), P],
     "pfn_embed_fwd": [P, P, P, P, P, P, P, I, I, I, I, I, I, P],
     "pfn_embed_bwd": [P, I, P, P, P, P, P, P, I, I, I, I, I, P],
     "pfn_layernorm_fwd": [P, I, P, P, P, I, P, P, I, I, F, I, P],
@@ -511,6 +523,33 @@ def attention_bwd(qkv, out, lse, dout, dqkv, delta, T, B, H, dh, sep, use_tc=Non
         d.delta_token_major = 1
     fn = lib.pfn_attention_bwd_tc if use_tc else lib.pfn_attention_bwd_simt
     check(fn(ctypes.byref(d), stream_ptr()), "pfn_attention_bwd")
+
+
+def attention_ctx_desc(qkv, kv, out, m, n, B, H, dh):
+    d = AttnCtxDesc()
+    d.m, d.n, d.B, d.H, d.dh = m, n, B, H, dh
+    d.dtype = dtype_code(qkv)
+    d.scale = 1.0 / (dh ** 0.5)
+    d.qkv, d.ld_qkv = qkv.data_ptr(), qkv.stride(0)
+    d.kv, d.ld_kv = (kv.data_ptr(), kv.stride(0)) if n > 0 else (None, 0)
+    d.out, d.ld_out = out.data_ptr(), out.stride(0)
+    return d
+
+
+@_guarded
+def attention_ctx_fwd(qkv, kv, out, m, n, B, H, dh, use_tc=None):
+    """out [m*B, H*dh] <- the context attention of the m query rows (packed qkv [m*B, 3*H*dh]) against the n cached training
+    rows of the same batch (kv [n*B, 2*H*dh], k | v; unused when n == 0) plus each row's own key."""
+    _count(1)
+    lib = load()
+    require_cuda(qkv, kv if n > 0 else None, out)
+    if qkv.dtype != out.dtype or (n > 0 and kv.dtype != qkv.dtype):
+        raise TypeError("attention_ctx_fwd: qkv, kv and out must share one dtype")
+    d = attention_ctx_desc(qkv, kv, out, m, n, B, H, dh)
+    if use_tc is None:
+        use_tc = tc_attention_ok(qkv, dh)
+    fn = lib.pfn_attention_ctx_fwd_tc if use_tc else lib.pfn_attention_ctx_fwd_simt
+    check(fn(ctypes.byref(d), stream_ptr()), "pfn_attention_ctx_fwd")
 
 
 @_guarded

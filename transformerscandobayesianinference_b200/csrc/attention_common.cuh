@@ -18,6 +18,7 @@ constexpr int ATT_TILE_ROWS = 64;                             // rows of one TMA
 constexpr int ATT_TILE = ATT_TILE_ROWS * ATT_ROW_BYTES;       // 16 KB
 
 int check_attn_desc_public(const pfn_attn_desc* d, bool bwd, const char* who);
+int check_attn_ctx_desc(const pfn_attn_ctx_desc* d, const char* who);
 
 // token row of (time t, batch b) in the [T*B, cols] activations
 __device__ __forceinline__ size_t att_tok(int t, int b, int T, int B, int batch_major) {
@@ -100,11 +101,10 @@ struct AttPipe {
 // The producer of the pipeline (one thread): for each of the CTA's units, the nblk key blocks of its (batch, head).  The
 // next tile's query operands go in once the consumers are done with the current ones, which is before its last key
 // block is (so the first key blocks of the next tile are already in flight by then): load_q(unit) issues q_bytes of
-// TMA loads on q_full.
+// TMA loads on q_full.  k_col / v_col: the first column of head 0's K and V in the map tmKV.
 template <int STAGES, class LoadQ>
 __device__ __forceinline__ void att_kv_producer(const AttPipe<STAGES>& pp, const CUtensorMap* tmKV, int n_units, int n_tiles,
-                                                int H, int nblk, uint32_t q_bytes, LoadQ&& load_q) {
-  const int E = H * ATT_DH;
+                                                int H, int nblk, int k_col, int v_col, uint32_t q_bytes, LoadQ&& load_q) {
   AttRing<STAGES> ring;
   for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
     const AttUnit unit = att_unit(u, n_tiles, H);
@@ -120,8 +120,8 @@ __device__ __forceinline__ void att_kv_producer(const AttPipe<STAGES>& pp, const
       tc::mbar_wait_suspend(&pp.kv_empty[ring.stage], ring.phase ^ 1);
       uint8_t* dst = pp.ring + ring.stage * 2 * ATT_TILE;
       tc::mbar_expect_tx(&pp.kv_full[ring.stage], 2 * ATT_TILE);
-      att_load_tile(dst, tmKV, &pp.kv_full[ring.stage], E + unit.h * ATT_DH, unit.b, kb * ATT_TILE_ROWS);
-      att_load_tile(dst + ATT_TILE, tmKV, &pp.kv_full[ring.stage], 2 * E + unit.h * ATT_DH, unit.b, kb * ATT_TILE_ROWS);
+      att_load_tile(dst, tmKV, &pp.kv_full[ring.stage], k_col + unit.h * ATT_DH, unit.b, kb * ATT_TILE_ROWS);
+      att_load_tile(dst + ATT_TILE, tmKV, &pp.kv_full[ring.stage], v_col + unit.h * ATT_DH, unit.b, kb * ATT_TILE_ROWS);
       ring.advance();
     }
   }

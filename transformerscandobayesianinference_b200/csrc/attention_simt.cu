@@ -1,7 +1,8 @@
 // fp32-FMA masked attention (forward, dQ, dK/dV) for the fp32 parity mode and for head sizes / dtypes the
 // tensor-core kernels do not take.  One warp per (batch, head, row); the head dimension is spread over the
 // lanes, scores are reduced with warp shuffles, softmax is computed online.  The single_eval_pos mask of
-// reference transformer.py:35-41 is implicit:  keys(i) = [0, sep)  U  {i if i >= sep}.
+// reference transformer.py:35-41 is implicit:  keys(i) = [0, sep)  U  {i if i >= sep}.  The forward also serves the
+// context attention (pfn_attention_ctx_fwd_simt): there the sep keys come from the K/V cache and every row has its own key.
 #include "common.cuh"
 #include "dropout.cuh"
 #include "../../include/pfn_b200.h"
@@ -25,9 +26,16 @@ __device__ __forceinline__ void store_head(T* base, int dh, int lane, const floa
   }
 }
 
+// The sep keys shared by all rows of batch b: K of key j at kv + (j*B + b)*ld + h*dh, V at + v_off (the packed qkv itself for
+// the masked attention, the K/V cache for the context attention).  Rows i >= diag_from also attend to their own key; the key
+// order is the same in both uses, so a query row gets the same bits from either entry point.
+struct SharedKeys {
+  const void* kv; int ld; int v_off; int diag_from;
+};
+
 template <typename T, int DPL>
 __global__ void __launch_bounds__(256)
-attn_fwd_simt_kernel(const pfn_attn_desc d) {
+attn_fwd_simt_kernel(const pfn_attn_desc d, const SharedKeys sk) {
   const int E = d.H * d.dh;
   const long long total = static_cast<long long>(d.B) * d.H * d.T;
   const int lane = threadIdx.x & 31;
@@ -44,13 +52,15 @@ attn_fwd_simt_kernel(const pfn_attn_desc d) {
 #pragma unroll
     for (int c = 0; c < DPL; ++c) { q[c] *= d.scale; o[c] = 0.f; }
     float m = -INFINITY, l = 0.f;
-    const int nkeys = d.sep + (i >= d.sep ? 1 : 0);
+    const int nkeys = d.sep + (i >= sk.diag_from ? 1 : 0);
     for (int jj = 0; jj < nkeys; ++jj) {
       const int j = jj < d.sep ? jj : i;
-      const T* krow = qkv + (static_cast<size_t>(j) * d.B + b) * d.ld_qkv + E + h * d.dh;
+      const T* krow = jj < d.sep ? reinterpret_cast<const T*>(sk.kv) + (static_cast<size_t>(j) * d.B + b) * sk.ld + h * d.dh
+                                 : qkv + (static_cast<size_t>(i) * d.B + b) * d.ld_qkv + E + h * d.dh;
+      const int v_off = jj < d.sep ? sk.v_off : E;
       float k[DPL], v[DPL];
       load_head<T, DPL>(krow, d.dh, lane, k);
-      load_head<T, DPL>(krow + E, d.dh, lane, v);
+      load_head<T, DPL>(krow + v_off, d.dh, lane, v);
       float s = 0.f;
 #pragma unroll
       for (int c = 0; c < DPL; ++c) s = fmaf(q[c], k[c], s);
@@ -68,7 +78,7 @@ attn_fwd_simt_kernel(const pfn_attn_desc d) {
 #pragma unroll
     for (int c = 0; c < DPL; ++c) o[c] *= inv_l;
     store_head<T, DPL>(out + (static_cast<size_t>(i) * d.B + b) * d.ld_out + h * d.dh, d.dh, lane, o);
-    if (lane == 0) d.lse[static_cast<size_t>(bh) * d.T + i] = m + logf(l);
+    if (lane == 0 && d.lse) d.lse[static_cast<size_t>(bh) * d.T + i] = m + logf(l);
   }
 }
 
@@ -189,13 +199,13 @@ static int check_attn_desc(const pfn_attn_desc* d, bool bwd, const char* who) {
 }
 
 template <typename T, int DPL>
-static int launch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s) {
+static int launch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, const SharedKeys& sk) {
   const long long tasks = static_cast<long long>(d->B) * d->H * d->T;
   long long grid = (tasks + 7) / 8;
   const long long max_grid = static_cast<long long>(num_sms()) * 16;
   if (grid > max_grid) grid = max_grid;
   if (!bwd) {
-    attn_fwd_simt_kernel<T, DPL><<<static_cast<int>(grid), 256, 0, s>>>(*d);
+    attn_fwd_simt_kernel<T, DPL><<<static_cast<int>(grid), 256, 0, s>>>(*d, sk);
     PFN_LAUNCH_OK();
     return 0;
   }
@@ -212,15 +222,37 @@ static int launch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s) {
 }
 
 template <typename T>
-static int dispatch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s) {
-  if (d->dh <= 32) return launch_attn_simt<T, 1>(d, bwd, s);
-  if (d->dh <= 64) return launch_attn_simt<T, 2>(d, bwd, s);
-  if (d->dh <= 128) return launch_attn_simt<T, 4>(d, bwd, s);
+static int dispatch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, const SharedKeys& sk) {
+  if (d->dh <= 32) return launch_attn_simt<T, 1>(d, bwd, s, sk);
+  if (d->dh <= 64) return launch_attn_simt<T, 2>(d, bwd, s, sk);
+  if (d->dh <= 128) return launch_attn_simt<T, 4>(d, bwd, s, sk);
   PFN_CHECK_ARG(d->dh <= 256, "attention_simt: head dim %d > 256 unsupported", d->dh);
-  return launch_attn_simt<T, 8>(d, bwd, s);
+  return launch_attn_simt<T, 8>(d, bwd, s, sk);
+}
+
+// the keys of the masked attention: [0, sep) of the packed qkv, and row i's own key for i >= sep
+static SharedKeys masked_keys(const pfn_attn_desc* d) {
+  const size_t esz = d->dtype == PFN_F32 ? 4 : 2;
+  return {static_cast<const char*>(d->qkv) + esz * d->H * d->dh, d->ld_qkv, d->H * d->dh, d->sep};
+}
+
+static int dispatch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, const SharedKeys& sk) {
+  return d->dtype == PFN_F32 ? dispatch_attn_simt<float>(d, bwd, s, sk) : dispatch_attn_simt<__nv_bfloat16>(d, bwd, s, sk);
 }
 
 int check_attn_desc_public(const pfn_attn_desc* d, bool bwd, const char* who) { return check_attn_desc(d, bwd, who); }
+
+int check_attn_ctx_desc(const pfn_attn_ctx_desc* d, const char* who) {
+  PFN_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
+  PFN_CHECK_ARG(d->m > 0 && d->n >= 0 && d->B > 0 && d->H > 0 && d->dh > 0, "%s: bad shape m=%d n=%d B=%d H=%d dh=%d", who,
+                d->m, d->n, d->B, d->H, d->dh);
+  PFN_CHECK_ARG(d->dtype == PFN_F32 || d->dtype == PFN_BF16, "%s: bad dtype %d", who, d->dtype);
+  PFN_CHECK_ARG(d->qkv && d->out && (d->kv || d->n == 0), "%s: null qkv/kv/out", who);
+  PFN_CHECK_ARG(d->ld_qkv >= 3 * d->H * d->dh && d->ld_out >= d->H * d->dh && (d->n == 0 || d->ld_kv >= 2 * d->H * d->dh),
+                "%s: leading dims too small", who);
+  PFN_CHECK_ARG(static_cast<long long>(d->m + d->n) * d->B * d->H < (1LL << 31), "%s: too many rows", who);
+  return 0;
+}
 
 }  // namespace pfn
 
@@ -229,14 +261,23 @@ using namespace pfn;
 extern "C" int pfn_attention_fwd_simt(const pfn_attn_desc* d, void* stream) {
   if (int rc = check_attn_desc(d, false, "attention_fwd_simt")) return rc;
   PFN_CHECK_ARG(d->batch_major == 0, "attention_fwd_simt: batch-major token order is only implemented by the tensor-core kernels");
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  return d->dtype == PFN_F32 ? dispatch_attn_simt<float>(d, false, s) : dispatch_attn_simt<__nv_bfloat16>(d, false, s);
+  return dispatch_attn_simt(d, false, reinterpret_cast<cudaStream_t>(stream), masked_keys(d));
 }
 
 extern "C" int pfn_attention_bwd_simt(const pfn_attn_desc* d, void* stream) {
   if (int rc = check_attn_desc(d, true, "attention_bwd_simt")) return rc;
   PFN_CHECK_ARG(d->batch_major == 0, "attention_bwd_simt: batch-major token order is only implemented by the tensor-core kernels");
   PFN_CHECK_ARG(d->delta_token_major == 0, "attention_bwd_simt: a precomputed token-major delta is only consumed by the tensor-core kernels");
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  return d->dtype == PFN_F32 ? dispatch_attn_simt<float>(d, true, s) : dispatch_attn_simt<__nv_bfloat16>(d, true, s);
+  return dispatch_attn_simt(d, true, reinterpret_cast<cudaStream_t>(stream), masked_keys(d));
+}
+
+extern "C" int pfn_attention_ctx_fwd_simt(const pfn_attn_ctx_desc* d, void* stream) {
+  if (int rc = check_attn_ctx_desc(d, "attention_ctx_fwd_simt")) return rc;
+  // rows of the masked-attention forward with T = m query rows and sep = n shared keys taken from the cache
+  pfn_attn_desc a = {};
+  a.T = d->m; a.B = d->B; a.H = d->H; a.dh = d->dh; a.sep = d->n;
+  a.dtype = d->dtype; a.scale = d->scale;
+  a.qkv = d->qkv; a.ld_qkv = d->ld_qkv;
+  a.out = d->out; a.ld_out = d->ld_out;
+  return dispatch_attn_simt(&a, false, reinterpret_cast<cudaStream_t>(stream), SharedKeys{d->kv, d->ld_kv, d->H * d->dh, 0});
 }

@@ -16,6 +16,10 @@
 // diagonal key is folded in before the loop: m = s_ii, l = 1, O = keep_ii v_i (rows < sep start from -inf, 0, 0).
 // O / l is packed to bf16 into a 128-byte-swizzled staging tile per warpgroup and written with TMA tile stores, which
 // clip rows past T.
+//
+// The context attention (kCtx, pfn_attention_ctx_fwd_tc) is the same kernel on other operands: the query tiles come from
+// the query rows' packed [m*B, 3E] qkv (T = m), the key blocks from the [n*B, 2E] K/V cache (sep = n), and every query row
+// has its diagonal key.  It writes no lse.
 #include "attention_common.cuh"
 
 namespace pfn {
@@ -33,12 +37,14 @@ struct AttnFwdParams {
   int T, B, H, sep;
   float scale_log2;   // scale * log2(e)
   const __nv_bfloat16* qkv; int ld_qkv;
+  int k_col, v_col;   // first column of head 0's K and V in the key map
   float* lse;
   int n_tiles;        // 128-row query tiles per (batch, head)
   int batch_major;
   uint32_t drop_seed; int drop_thr;   // dropout on the probabilities (thr 0 = off), csrc/dropout.cuh
 };
 
+template <bool kCtx>
 __global__ void __launch_bounds__(AF_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                 const __grid_constant__ CUtensorMap tmO, const AttnFwdParams p) {
@@ -63,7 +69,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if (threadIdx.x == 256) {
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
-      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk, 2 * ATT_TILE, [&](const AttUnit& unit) {
+      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk, p.k_col, p.v_col, 2 * ATT_TILE, [&](const AttUnit& unit) {
         for (int g = 0; g < 2; ++g)
           att_load_tile(sQ + g * ATT_TILE, &tmQ, pp.q_full, unit.h * ATT_DH, unit.b, unit.tile * 128 + 64 * g);
       });
@@ -93,7 +99,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int i = i0 + 8 * r;
-      const bool diag = i < p.T && i >= p.sep;
+      const bool diag = i < p.T && (kCtx || i >= p.sep);
       drow[r] = static_cast<uint32_t>(unit.bh) * p.T + i;
       const __nv_bfloat16* qrow = p.qkv + att_tok(diag ? i : 0, unit.b, p.T, p.B, p.batch_major) * p.ld_qkv + unit.h * ATT_DH;
       float sd = 0.f;
@@ -192,7 +198,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const uint32_t off = (j >> 3) * 8192 + rr * 128 + (((j & 7) ^ (rr & 7)) << 4) + (lane & 3) * 4;
         *reinterpret_cast<uint32_t*>(stg + off) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
       }
-      if (i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+      if (!kCtx && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
     }
     tc::fence_proxy_async_smem();
     tc::named_bar_sync(1 + g, 128);
@@ -216,15 +222,45 @@ extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
   p.T = d->T; p.B = d->B; p.H = d->H; p.sep = d->sep;
   p.scale_log2 = d->scale * 1.4426950408889634f;
   p.qkv = reinterpret_cast<const __nv_bfloat16*>(d->qkv); p.ld_qkv = d->ld_qkv;
+  const int E = d->H * ATT_DH;
+  p.k_col = E; p.v_col = 2 * E;
   p.lse = d->lse;
   p.n_tiles = (d->T + 127) / 128;
   p.batch_major = d->batch_major;
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
-  const int E = d->H * ATT_DH;
   CUtensorMap tmQ, tmKV, tmO;
   if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
   // out: rows past T are not written
   if (int rc = att_tensor_map(&tmO, d->out, E, d->ld_out, d->T, d->B, d->T, d->batch_major)) return rc;
-  return att_launch_persistent<attn_fwd_kernel>("attention_fwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
+  return att_launch_persistent<attn_fwd_kernel<false>>("attention_fwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
                                                 AF_THREADS, AF_SMEM, reinterpret_cast<cudaStream_t>(stream), tmQ, tmKV, tmO, p);
+}
+
+extern "C" int pfn_attention_ctx_fwd_tc(const pfn_attn_ctx_desc* d, void* stream) {
+  if (int rc = check_attn_ctx_desc(d, "attention_ctx_fwd_tc")) return rc;
+  PFN_CHECK_ARG(d->dtype == PFN_BF16, "attention_ctx_fwd_tc: bf16 only");
+  PFN_CHECK_ARG(d->dh == ATT_DH, "attention_ctx_fwd_tc: head dim %d unsupported (built for 128)", d->dh);
+  PFN_CHECK_ARG(d->ld_qkv % 8 == 0 && d->ld_kv % 8 == 0 && d->ld_out % 8 == 0,
+                "attention_ctx_fwd_tc: leading dims must be multiples of 8");
+  // with n == 0 no key block is loaded; the key map then only needs a valid base
+  const void* kv = d->n > 0 ? d->kv : d->qkv;
+  PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->qkv) | reinterpret_cast<uintptr_t>(kv) | reinterpret_cast<uintptr_t>(d->out)) &
+                 15) == 0, "attention_ctx_fwd_tc: qkv/kv/out must be 16-byte aligned");
+  AttnFwdParams p;
+  p.T = d->m; p.B = d->B; p.H = d->H; p.sep = d->n;
+  p.scale_log2 = d->scale * 1.4426950408889634f;
+  p.qkv = reinterpret_cast<const __nv_bfloat16*>(d->qkv); p.ld_qkv = d->ld_qkv;
+  const int E = d->H * ATT_DH;
+  p.k_col = 0; p.v_col = E;
+  p.lse = nullptr;
+  p.n_tiles = (d->m + 127) / 128;
+  p.batch_major = 0;
+  p.drop_seed = 0; p.drop_thr = 0;
+  CUtensorMap tmQ, tmKV, tmO;
+  if (int rc = att_tensor_map(&tmQ, d->qkv, 3 * E, d->ld_qkv, d->m, d->B, d->m, 0)) return rc;
+  if (int rc = att_tensor_map(&tmKV, kv, d->n > 0 ? 2 * E : 3 * E, d->n > 0 ? d->ld_kv : d->ld_qkv, d->n, d->B,
+                              d->n > 0 ? d->n : 1, 0)) return rc;
+  if (int rc = att_tensor_map(&tmO, d->out, E, d->ld_out, d->m, d->B, d->m, 0)) return rc;
+  return att_launch_persistent<attn_fwd_kernel<true>>("attention_ctx_fwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                      AF_THREADS, AF_SMEM, reinterpret_cast<cudaStream_t>(stream), tmQ, tmKV, tmO, p);
 }

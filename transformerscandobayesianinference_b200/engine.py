@@ -115,6 +115,41 @@ def _linear_wgrad(dy, x, dw, rows=None, cols=None):
            M=N, N=K, K=n_tok)
 
 
+def _layer_operands(params, li, dt):
+    """Layer li's parameters by name, and its four weight matrices in the activation dtype."""
+    P = dict(zip(LAYER_PARAM_NAMES, params[li * N_LAYER_PARAMS:(li + 1) * N_LAYER_PARAMS]))
+    return P, tuple(_cast(P[k], dt) for k in ("in_w", "out_w", "w1", "w2"))
+
+
+def _layer_tail(h, attn, P, out_w, w1, w2, drop, li):
+    """One encoder layer after its attention: z1 = h + attn W_out^T + b_out, h1 = LN1(z1), g = GELU(h1 W1^T + b1),
+    z2 = h1 + g W2^T + b2, h2 = LN2(z2), with dropout at the last three sites when `drop` is set.  Returns
+    (z1, mean1, rstd1, h1, u, u_is_grad, g, z2, mean2, rstd2, h2)."""
+    N = h.shape[0]
+    thr = drop[1] if drop else 0
+    if thr:
+        z1 = _linear_fwd(attn, out_w, P["out_b"])
+        L.dropout(z1, z1, site_seed(drop[0], li, 1), thr, residual=h)           # h + dropout1(attn block)
+    else:
+        z1 = _linear_fwd(attn, out_w, P["out_b"], aux=h)
+    h1 = torch.empty_like(z1)
+    mean1 = torch.empty(N, device=h.device, dtype=torch.float32)
+    rstd1 = torch.empty_like(mean1)
+    L.layernorm_fwd(z1, P["g1"], P["be1"], h1, mean1, rstd1, LN_EPS)
+    g, u, u_is_grad = _gelu_linear_fwd(h1, w1, P["b1"])
+    if thr:
+        L.dropout(g, g, site_seed(drop[0], li, 2), thr)                           # dropout(GELU(.)), in place
+        z2 = _linear_fwd(g, w2, P["b2"])
+        L.dropout(z2, z2, site_seed(drop[0], li, 3), thr, residual=h1)          # h1 + dropout2(MLP block)
+    else:
+        z2 = _linear_fwd(g, w2, P["b2"], aux=h1)
+    h2 = torch.empty_like(z2)
+    mean2 = torch.empty_like(mean1)
+    rstd2 = torch.empty_like(mean1)
+    L.layernorm_fwd(z2, P["g2"], P["be2"], h2, mean2, rstd2, LN_EPS)
+    return z1, mean1, rstd1, h1, u, u_is_grad, g, z2, mean2, rstd2, h2
+
+
 class EncoderStackFn(torch.autograd.Function):
     """src [T*B, E] (activation dtype) -> output of `nlayers` post-norm encoder layers under the sep mask."""
 
@@ -136,32 +171,12 @@ class EncoderStackFn(torch.autograd.Function):
         h = src.contiguous()
         thr = drop[1] if drop else 0
         for li in range(n_layers):
-            P = dict(zip(LAYER_PARAM_NAMES, params[li * N_LAYER_PARAMS:(li + 1) * N_LAYER_PARAMS]))
-            in_w, out_w, w1, w2 = (_cast(P[k], dt) for k in ("in_w", "out_w", "w1", "w2"))
+            P, (in_w, out_w, w1, w2) = _layer_operands(params, li, dt)
             qkv = _linear_fwd(h, in_w, P["in_b"])
             attn = torch.empty(N, E, device=h.device, dtype=dt)
             lse = torch.empty(B * nhead, T, device=h.device, dtype=torch.float32)
             L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, sep, drop=(site_seed(drop[0], li, 0), thr) if thr else None)
-            if thr:
-                z1 = _linear_fwd(attn, out_w, P["out_b"])
-                L.dropout(z1, z1, site_seed(drop[0], li, 1), thr, residual=h)           # h + dropout1(attn block)
-            else:
-                z1 = _linear_fwd(attn, out_w, P["out_b"], aux=h)
-            h1 = torch.empty_like(z1)
-            mean1 = torch.empty(N, device=h.device, dtype=torch.float32)
-            rstd1 = torch.empty_like(mean1)
-            L.layernorm_fwd(z1, P["g1"], P["be1"], h1, mean1, rstd1, LN_EPS)
-            g, u, u_is_grad = _gelu_linear_fwd(h1, w1, P["b1"])
-            if thr:
-                L.dropout(g, g, site_seed(drop[0], li, 2), thr)                           # dropout(GELU(.)), in place
-                z2 = _linear_fwd(g, w2, P["b2"])
-                L.dropout(z2, z2, site_seed(drop[0], li, 3), thr, residual=h1)          # h1 + dropout2(MLP block)
-            else:
-                z2 = _linear_fwd(g, w2, P["b2"], aux=h1)
-            h2 = torch.empty_like(z2)
-            mean2 = torch.empty_like(mean1)
-            rstd2 = torch.empty_like(mean1)
-            L.layernorm_fwd(z2, P["g2"], P["be2"], h2, mean2, rstd2, LN_EPS)
+            z1, mean1, rstd1, h1, u, u_is_grad, g, z2, mean2, rstd2, h2 = _layer_tail(h, attn, P, out_w, w1, w2, drop, li)
             if keep:
                 # the activation-dtype weight copies are kept for the backward as well (4 small tensors per layer) instead of
                 # being cast a second time there
@@ -262,6 +277,54 @@ class EncoderStackFn(torch.autograd.Function):
             GRAD_BUCKET_SYNC()
         ctx.saved_acts = None
         return (dh2, None, None, None, None, None, None, None) + tuple(grads)
+
+
+@torch.no_grad()
+def encode_context(src, T, B, nhead, precision, *params):
+    """The K/V cache of T training rows: src [T*B, E] (their embedding, activation dtype, T >= 1) runs through the encoder
+    layers with sep = T, and kv [n_layers, T*B, 2E] keeps each layer's K | V of those rows, as the in-projection produced
+    them.  The last layer's attention and MLP are not run: no later layer reads their output."""
+    L.require_cuda(src, *params)
+    dt = act_dtype(precision)
+    assert src.dtype == dt and src.dim() == 2
+    n_layers = len(params) // N_LAYER_PARAMS
+    N, E = src.shape
+    dh = E // nhead
+    kv = torch.empty(n_layers, N, 2 * E, device=src.device, dtype=dt)
+    h = src.contiguous()
+    for li in range(n_layers):
+        P, (in_w, out_w, w1, w2) = _layer_operands(params, li, dt)
+        qkv = _linear_fwd(h, in_w, P["in_b"])
+        kv[li].copy_(qkv[:, E:])
+        if li == n_layers - 1:
+            break
+        attn = torch.empty(N, E, device=h.device, dtype=dt)
+        lse = torch.empty(B * nhead, T, device=h.device, dtype=torch.float32)
+        L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, T)
+        h = _layer_tail(h, attn, P, out_w, w1, w2, None, li)[-1]
+    return kv
+
+
+@torch.no_grad()
+def query_stack(src, kv, n, B, nhead, precision, *params):
+    """src [m*B, E] (the query rows' embedding, activation dtype) -> their output of the encoder layers, each query row
+    attending to the n training rows whose K | V the cache kv [n_layers, n*B, 2E] holds (encode_context) and to itself:
+    rows n .. n + m - 1 of EncoderStackFn on (training rows, query rows) with sep = n.  Per layer: the in-projection GEMM,
+    the context attention, then the same out-projection, LayerNorm and MLP kernels as EncoderStackFn.forward."""
+    L.require_cuda(src, kv, *params)
+    dt = act_dtype(precision)
+    assert src.dtype == dt and kv.dtype == dt and src.dim() == 2
+    n_layers = len(params) // N_LAYER_PARAMS
+    N, E = src.shape
+    dh = E // nhead
+    h = src.contiguous()
+    for li in range(n_layers):
+        P, (in_w, out_w, w1, w2) = _layer_operands(params, li, dt)
+        qkv = _linear_fwd(h, in_w, P["in_b"])
+        attn = torch.empty(N, E, device=h.device, dtype=dt)
+        L.attention_ctx_fwd(qkv, kv[li], attn, N // B, n, B, nhead, dh)
+        h = _layer_tail(h, attn, P, out_w, w1, w2, None, li)[-1]
+    return h
 
 
 class EmbedFn(torch.autograd.Function):

@@ -4,6 +4,11 @@ The module keeps `self.transformer_encoder = nn.TransformerEncoder(...)` purely 
 identical state_dict keys (the five reference checkpoints under results/ load with strict=True), identical
 construction-time RNG consumption and the reference's zero-init of `linear2` / `out_proj` — but its forward is
 never called.  `forward()` routes embedding -> encoder stack -> decoder through `engine.*Fn`.
+
+For inference against one training set, `encode_context(x_train, y_train)` runs the training rows once and keeps every
+layer's K and V of them; `predict(ctx, x_query)` then scores any number of query sets against that context.  Under the
+single_eval_pos mask a training row attends only to training rows and a query row to the training rows and itself, so
+`predict` returns what `forward` returns for the concatenated sequence at single_eval_pos = n.
 """
 import torch
 import torch.nn as nn
@@ -13,6 +18,17 @@ from . import decoders, engine
 from ._lib import draw_seed, drop_threshold as L_drop_threshold
 from .positional_encodings import NoPositionalEncoding
 from .utils import SeqBN
+
+
+class TrainingContext:
+    """What `TransformerModel.encode_context` keeps of n training rows: `kv` [nlayers, n*B, 2*E] holds each layer's K | V
+    of the rows (token row t*B + b, the model's activation dtype), plus the shapes and the precision it was made with.
+    It holds no weights: `predict` uses the model it is called on.  `predict` never writes to it."""
+    __slots__ = ("kv", "n", "B", "E", "nhead", "nlayers", "precision", "device")
+
+    def __init__(self, kv, n, B, E, nhead, nlayers, precision, device):
+        self.kv, self.n, self.B, self.E, self.nhead, self.nlayers = kv, n, B, E, nhead, nlayers
+        self.precision, self.device = precision, torch.device(device)
 
 
 class TransformerModel(nn.Module):
@@ -74,6 +90,43 @@ class TransformerModel(nn.Module):
                 and isinstance(d[1], nn.GELU) and getattr(d[1], 'approximate', 'none') == 'none'
                 and isinstance(d[2], nn.Linear) and d[0].bias is not None and d[2].bias is not None)
 
+    def _embed(self, x_src, y_src, sep):
+        """[T*B, E] activation-dtype input of the encoder stack: the x embedding of every row plus the y embedding of the
+        rows t < sep."""
+        T, B = x_src.shape[0], x_src.shape[1]
+        precision = self.precision
+        if self._fused_embed_ok():
+            return engine.EmbedFn.apply(x_src, y_src, self.encoder.weight, self.encoder.bias, self.y_encoder.weight,
+                                        self.y_encoder.bias, sep, precision)
+        xs = self.encoder(x_src)
+        ys = self.y_encoder(y_src.unsqueeze(-1) if y_src.dim() == 2 else y_src)
+        h = torch.cat([xs[:sep] + ys[:sep], xs[sep:]], 0)
+        if self.input_ln is not None:
+            h = self.input_ln(h)
+        if self.pos_encoder is not None:
+            h = self.pos_encoder(h)
+        return h.reshape(T * B, self.ninp).to(engine.act_dtype(precision))
+
+    def _layer_params(self):
+        params = []
+        for layer in self.transformer_encoder.layers:
+            params.extend(engine.layer_params(layer))
+        return params
+
+    def _decode(self, hq, rows, B):
+        """Logits [rows, B, n_out] of the decoder on the output hq [rows*B, E] of the query rows."""
+        precision = self.precision
+        if self._default_decoder():
+            out = engine.DecoderFn.apply(hq, self.decoder[0].weight, self.decoder[0].bias, self.decoder[2].weight,
+                                         self.decoder[2].bias, precision)
+        elif isinstance(self.decoder, (decoders.ScaledDecoder, decoders.FixedScaledDecoder)):
+            out = self.decoder.fused(hq, (rows, B), precision)
+        else:
+            # any other head runs as its own torch ops on the sequence-first [T - sep, B, E] rows, the shape the reference
+            # hands its decoder (reference transformer.py:85)
+            out = self.decoder(hq.float().view(rows, B, -1))
+        return out.reshape(rows, B, -1)
+
     def forward(self, src, src_mask=None, single_eval_pos=None):
         assert single_eval_pos is not None, 'Single eval pos is required now.'
         assert isinstance(src, tuple), 'the fused x/y input mode cannot be combined with single_eval_pos'
@@ -100,39 +153,75 @@ class TransformerModel(nn.Module):
             sep = max(sep + T, 0)
         sep = min(sep, T)
         precision = self.precision
-        dt = engine.act_dtype(precision)
-
-        if self._fused_embed_ok():
-            h = engine.EmbedFn.apply(x_src, y_src, self.encoder.weight, self.encoder.bias, self.y_encoder.weight,
-                                     self.y_encoder.bias, sep, precision)
-        else:
-            xs = self.encoder(x_src)
-            ys = self.y_encoder(y_src.unsqueeze(-1) if y_src.dim() == 2 else y_src)
-            h = torch.cat([xs[:sep] + ys[:sep], xs[sep:]], 0)
-            if self.input_ln is not None:
-                h = self.input_ln(h)
-            if self.pos_encoder is not None:
-                h = self.pos_encoder(h)
-            h = h.reshape(T * B, self.ninp).to(dt)
-
-        params = []
-        for layer in self.transformer_encoder.layers:
-            params.extend(engine.layer_params(layer))
+        h = self._embed(x_src, y_src, sep)
+        params = self._layer_params()
         drop = None
         if self.training and self.dropout > 0:
             # one seed per forward from torch's CPU generator (reproducible under torch.manual_seed, no device sync); the
             # kernels derive per-layer / per-site counter-based masks from it
             drop = (draw_seed(), L_drop_threshold(self.dropout))
         h = engine.EncoderStackFn.apply(h, T, B, sep, self.nhead, precision, torch.is_grad_enabled(), drop, *params)
+        return self._decode(h[sep * B:], T - sep, B)
 
-        hq = h[sep * B:]
-        if self._default_decoder():
-            out = engine.DecoderFn.apply(hq, self.decoder[0].weight, self.decoder[0].bias, self.decoder[2].weight,
-                                         self.decoder[2].bias, precision)
-        elif isinstance(self.decoder, (decoders.ScaledDecoder, decoders.FixedScaledDecoder)):
-            out = self.decoder.fused(hq, (T - sep, B), precision)
-        else:
-            # any other head runs as its own torch ops on the sequence-first [T - sep, B, E] rows, the shape the reference
-            # hands its decoder (reference transformer.py:85)
-            out = self.decoder(hq.float().view(T - sep, B, -1))
-        return out.reshape(T - sep, B, -1)
+    # ---- inference against a cached training set -------------------------------------------------------------
+    def _check_context_inference(self):
+        """Raise ValueError for a configuration in which a query row's result depends on more than the training rows and
+        itself, or is not the same in every call."""
+        if self.input_ln is not None:
+            raise ValueError("encode_context / predict: input_normalization=True is not supported: SeqBN normalises each "
+                             "feature over all rows of the sequence, so the training rows would depend on the queries")
+        if self.pos_encoder is not None and not isinstance(self.pos_encoder, NoPositionalEncoding):
+            raise ValueError(f"encode_context / predict: positional encoder {type(self.pos_encoder).__name__} is not "
+                             "supported: it adds a row of its table by position, so a query's result would depend on its "
+                             "index in the sequence (use None or NoPositionalEncoding)")
+        if self.training and self.dropout > 0:
+            raise ValueError("encode_context / predict: training-mode dropout is not supported: its masks are keyed by "
+                             "the row's position in the full sequence; call model.eval() first")
+
+    def encode_context(self, x_train, y_train):
+        """Run the n training rows x_train [n, B, F], y_train [n, B] (n >= 0) through the embedding and every encoder
+        layer on their own (they never attend to a query row) and return a `TrainingContext` holding each layer's K and
+        V of them.  No autograd.  With n = 0 a query attends only to itself, as in forward(..., single_eval_pos=0)."""
+        self._check_context_inference()
+        if x_train.dim() != 3 or y_train.shape[:2] != x_train.shape[:2]:
+            raise ValueError(f"encode_context: x_train must be [n, B, F] and y_train [n, B]; got {tuple(x_train.shape)} "
+                             f"and {tuple(y_train.shape)}")
+        if not x_train.is_cuda:
+            raise RuntimeError(
+                "TransformerModel.encode_context runs on hand-written sm_90a kernels only; inputs are on "
+                f"{x_train.device}. Move model and data to a CUDA device (there is no CPU fallback).")
+        n, B = x_train.shape[0], x_train.shape[1]
+        E, nlayers = self.ninp, len(self.transformer_encoder.layers)
+        dt = engine.act_dtype(self.precision)
+        with torch.no_grad():
+            if n == 0:
+                kv = torch.empty(nlayers, 0, 2 * E, device=x_train.device, dtype=dt)
+            else:
+                h = self._embed(x_train, y_train, n)
+                kv = engine.encode_context(h, n, B, self.nhead, self.precision, *self._layer_params())
+        return TrainingContext(kv, n, B, E, self.nhead, nlayers, self.precision, x_train.device)
+
+    def predict(self, ctx, x_query):
+        """Logits [m, B, n_out] of the query rows x_query [m, B, F] (m >= 1) given the training rows `ctx` holds: what
+        forward((cat(x_train, x_query), cat(y_train, anything)), single_eval_pos=n) returns.  No autograd; `ctx` is only
+        read, so one context serves any number of calls."""
+        self._check_context_inference()
+        if not isinstance(ctx, TrainingContext):
+            raise ValueError(f"predict: ctx must be a TrainingContext from encode_context, got {type(ctx).__name__}")
+        if x_query.dim() != 3 or x_query.shape[0] < 1:
+            raise ValueError(f"predict: x_query must be [m, B, F] with m >= 1; got {tuple(x_query.shape)}")
+        m, B = x_query.shape[0], x_query.shape[1]
+        want = {"B": B, "E": self.ninp, "nhead": self.nhead, "nlayers": len(self.transformer_encoder.layers),
+                "precision": self.precision, "device": x_query.device}
+        for name, value in want.items():
+            have = getattr(ctx, name)
+            if have != value:
+                raise ValueError(f"predict: the context's {name} is {have} but the model and queries have {value}")
+        if not x_query.is_cuda:
+            raise RuntimeError(
+                "TransformerModel.predict runs on hand-written sm_90a kernels only; inputs are on "
+                f"{x_query.device}. Move model and data to a CUDA device (there is no CPU fallback).")
+        with torch.no_grad():
+            h = self._embed(x_query, x_query.new_zeros(m, B), 0)
+            h = engine.query_stack(h, ctx.kv, ctx.n, B, self.nhead, self.precision, *self._layer_params())
+            return self._decode(h, m, B)
