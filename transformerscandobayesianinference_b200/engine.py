@@ -115,10 +115,48 @@ def _linear_wgrad(dy, x, dw, rows=None, cols=None):
            M=N, N=K, K=n_tok)
 
 
-def _layer_operands(params, li, dt):
-    """Layer li's parameters by name, and its four weight matrices in the activation dtype."""
-    P = dict(zip(LAYER_PARAM_NAMES, params[li * N_LAYER_PARAMS:(li + 1) * N_LAYER_PARAMS]))
-    return P, tuple(_cast(P[k], dt) for k in ("in_w", "out_w", "w1", "w2"))
+def _flat_grads(dev, *shapes):
+    """One zeroed fp32 buffer holding gradients of the given shapes back to back (a single all-reduce under DP), and
+    views of it in that order."""
+    sizes = [torch.Size(s).numel() for s in shapes]
+    flat = torch.zeros(sum(sizes), device=dev, dtype=torch.float32)
+    views, off = [], 0
+    for s, n in zip(shapes, sizes):
+        views.append(flat[off:off + n].view(s))
+        off += n
+    return flat, views
+
+
+def _bucket_ready(flat, wait=True):
+    """Hand a complete bucket of gradients to the data-parallel hook, if one is set.  `wait`: then wait for it
+    (stream-level) so autograd never touches a buffer NCCL is still writing; the encoder stack waits once, after its
+    last layer's bucket."""
+    if GRAD_BUCKET_HOOK is not None:
+        GRAD_BUCKET_HOOK(flat)
+        if wait:
+            GRAD_BUCKET_SYNC()
+
+
+def _stack_start(src, precision, nhead, params, kv=None):
+    """Checks of an encoder stack call; (activation dtype, number of layers, head dim, contiguous src)."""
+    L.require_cuda(src, kv, *params)
+    dt = act_dtype(precision)
+    assert src.dtype == dt and src.dim() == 2 and (kv is None or kv.dtype == dt)
+    return dt, len(params) // N_LAYER_PARAMS, src.shape[1] // nhead, src.contiguous()
+
+
+def _layer(seq, li):
+    """Layer li's entries of a sequence with one entry per stack parameter (the parameters, their gradients), by name."""
+    return dict(zip(LAYER_PARAM_NAMES, seq[li * N_LAYER_PARAMS:(li + 1) * N_LAYER_PARAMS]))
+
+
+def _layer_qkv(h, params, li, dt):
+    """Layer li's parameters by name, its four weight matrices in the activation dtype, its in-projection
+    qkv = h W_in^T + b_in, and an uninitialised attention output buffer."""
+    P = _layer(params, li)
+    in_w, out_w, w1, w2 = (_cast(P[k], dt) for k in ("in_w", "out_w", "w1", "w2"))
+    qkv = _linear_fwd(h, in_w, P["in_b"])
+    return P, (in_w, out_w, w1, w2), qkv, torch.empty_like(h)
 
 
 def _layer_tail(h, attn, P, out_w, w1, w2, drop, li):
@@ -160,20 +198,12 @@ class EncoderStackFn(torch.autograd.Function):
         `drop`: None or (seed, thr) — training-mode dropout with probability thr/256 at the reference layer's four sites
         (attention probabilities, attention block output, after the GELU, MLP block output; torch
         nn/modules/transformer.py:961-982).  Masks are counter-based and regenerated in backward (csrc/dropout.cuh)."""
-        L.require_cuda(src, *params)
-        dt = act_dtype(precision)
-        assert src.dtype == dt and src.dim() == 2
-        n_layers = len(params) // N_LAYER_PARAMS
-        N, E = src.shape
-        dh = E // nhead
+        dt, n_layers, dh, h = _stack_start(src, precision, nhead, params)
         keep = bool(keep) and any(ctx.needs_input_grad)
         saved = []
-        h = src.contiguous()
         thr = drop[1] if drop else 0
         for li in range(n_layers):
-            P, (in_w, out_w, w1, w2) = _layer_operands(params, li, dt)
-            qkv = _linear_fwd(h, in_w, P["in_b"])
-            attn = torch.empty(N, E, device=h.device, dtype=dt)
+            P, (in_w, out_w, w1, w2), qkv, attn = _layer_qkv(h, params, li, dt)
             lse = torch.empty(B * nhead, T, device=h.device, dtype=torch.float32)
             L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, sep, drop=(site_seed(drop[0], li, 0), thr) if thr else None)
             z1, mean1, rstd1, h1, u, u_is_grad, g, z2, mean2, rstd2, h2 = _layer_tail(h, attn, P, out_w, w1, w2, drop, li)
@@ -200,16 +230,11 @@ class EncoderStackFn(torch.autograd.Function):
         dev = dout.device
         N, E = dout.shape
         dh = E // nhead
-        sizes = [p.numel() for p in params]
-        flat = torch.zeros(sum(sizes), device=dev, dtype=torch.float32)
-        grads, off = [], 0
-        for p, n in zip(params, sizes):
-            grads.append(flat[off:off + n].view(p.shape))
-            off += n
+        flat, grads = _flat_grads(dev, *(p.shape for p in params))
+        end = flat.numel()
         dh2 = dout.contiguous().to(dt)
         for li in reversed(range(n_layers)):
-            P = dict(zip(LAYER_PARAM_NAMES, params[li * N_LAYER_PARAMS:(li + 1) * N_LAYER_PARAMS]))
-            G = dict(zip(LAYER_PARAM_NAMES, grads[li * N_LAYER_PARAMS:(li + 1) * N_LAYER_PARAMS]))
+            P, G = _layer(params, li), _layer(grads, li)
             h, qkv, attn, lse, z1, mean1, rstd1, h1, u, g, z2, mean2, rstd2, in_w, out_w, w1, w2 = ctx.saved_acts[li]
             ctx.saved_acts[li] = None
             # ---- LN2 and the MLP
@@ -270,9 +295,9 @@ class EncoderStackFn(torch.autograd.Function):
             _linear_wgrad(dqkv, h, G["in_w"])
             dh2 = _linear_dgrad(dqkv, in_w, aux=dz1)
             del dqkv, dz1, h
-            if GRAD_BUCKET_HOOK is not None:       # this layer's 12 gradients are one contiguous slice of the flat buffer
-                lo = sum(sizes[:li * N_LAYER_PARAMS])
-                GRAD_BUCKET_HOOK(flat[lo:lo + sum(sizes[li * N_LAYER_PARAMS:(li + 1) * N_LAYER_PARAMS])])
+            n = sum(t.numel() for t in G.values())     # this layer's 12 gradients are one contiguous slice of the flat buffer
+            _bucket_ready(flat[end - n:end], wait=False)
+            end -= n
         if GRAD_BUCKET_SYNC is not None:
             GRAD_BUCKET_SYNC()
         ctx.saved_acts = None
@@ -284,21 +309,14 @@ def encode_context(src, T, B, nhead, precision, *params):
     """The K/V cache of T training rows: src [T*B, E] (their embedding, activation dtype, T >= 1) runs through the encoder
     layers with sep = T, and kv [n_layers, T*B, 2E] keeps each layer's K | V of those rows, as the in-projection produced
     them.  The last layer's attention and MLP are not run: no later layer reads their output."""
-    L.require_cuda(src, *params)
-    dt = act_dtype(precision)
-    assert src.dtype == dt and src.dim() == 2
-    n_layers = len(params) // N_LAYER_PARAMS
-    N, E = src.shape
-    dh = E // nhead
+    dt, n_layers, dh, h = _stack_start(src, precision, nhead, params)
+    N, E = h.shape
     kv = torch.empty(n_layers, N, 2 * E, device=src.device, dtype=dt)
-    h = src.contiguous()
     for li in range(n_layers):
-        P, (in_w, out_w, w1, w2) = _layer_operands(params, li, dt)
-        qkv = _linear_fwd(h, in_w, P["in_b"])
+        P, (_, out_w, w1, w2), qkv, attn = _layer_qkv(h, params, li, dt)
         kv[li].copy_(qkv[:, E:])
         if li == n_layers - 1:
             break
-        attn = torch.empty(N, E, device=h.device, dtype=dt)
         lse = torch.empty(B * nhead, T, device=h.device, dtype=torch.float32)
         L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, T)
         h = _layer_tail(h, attn, P, out_w, w1, w2, None, li)[-1]
@@ -311,18 +329,10 @@ def query_stack(src, kv, n, B, nhead, precision, *params):
     attending to the n training rows whose K | V the cache kv [n_layers, n*B, 2E] holds (encode_context) and to itself:
     rows n .. n + m - 1 of EncoderStackFn on (training rows, query rows) with sep = n.  Per layer: the in-projection GEMM,
     the context attention, then the same out-projection, LayerNorm and MLP kernels as EncoderStackFn.forward."""
-    L.require_cuda(src, kv, *params)
-    dt = act_dtype(precision)
-    assert src.dtype == dt and kv.dtype == dt and src.dim() == 2
-    n_layers = len(params) // N_LAYER_PARAMS
-    N, E = src.shape
-    dh = E // nhead
-    h = src.contiguous()
+    dt, n_layers, dh, h = _stack_start(src, precision, nhead, params, kv)
     for li in range(n_layers):
-        P, (in_w, out_w, w1, w2) = _layer_operands(params, li, dt)
-        qkv = _linear_fwd(h, in_w, P["in_b"])
-        attn = torch.empty(N, E, device=h.device, dtype=dt)
-        L.attention_ctx_fwd(qkv, kv[li], attn, N // B, n, B, nhead, dh)
+        P, (_, out_w, w1, w2), qkv, attn = _layer_qkv(h, params, li, dt)
+        L.attention_ctx_fwd(qkv, kv[li], attn, h.shape[0] // B, n, B, nhead, dh)
         h = _layer_tail(h, attn, P, out_w, w1, w2, None, li)[-1]
     return h
 
@@ -357,6 +367,32 @@ class EmbedFn(torch.autograd.Function):
         return None, None, dWx, dbx, dwy.view(wy_shape), dby, None, None
 
 
+def _f32_rows(rows, n, dev):
+    """An uninitialised fp32 [rows, n] view whose row pitch is n rounded up to 4 (16-byte rows for the GEMM's stores)."""
+    return torch.empty(rows, (n + 3) // 4 * 4, device=dev, dtype=torch.float32)[:, :n]
+
+
+def _head_fwd(hq, w0, b0, w2, b2):
+    """The two GEMMs every decoder head runs: g = GELU(hq w0^T + b0), then z = g w2^T + b2 into padded fp32 rows.
+    Returns (g, u, u_is_grad, z) with u, u_is_grad as from _gelu_linear_fwd."""
+    g, u, u_is_grad = _gelu_linear_fwd(hq, w0, b0)
+    z = _f32_rows(hq.shape[0], w2.shape[0], hq.device)
+    L.gemm(g, w2, z, bias=b2.detach().contiguous())
+    return g, u, u_is_grad, z
+
+
+def _head_bwd(dz, hq, u, g, u_is_grad, w0, w2, grads):
+    """The backward of _head_fwd from dz = dL/dz (activation dtype): fills grads = (dW0, db0, dW2, db2) and returns
+    dL/dhq."""
+    dW0, db0, dW2, db2 = grads
+    L.colsum(dz, db2)
+    _linear_wgrad(dz, g, dW2)
+    du = _gelu_linear_dgrad(dz, w2, u, u_is_grad)
+    L.colsum(du, db0)
+    _linear_wgrad(du, hq, dW0)
+    return _linear_dgrad(du, w0)
+
+
 class DecoderFn(torch.autograd.Function):
     """hq [Nq, E] -> logits [Nq, n_out] fp32:  GELU(hq W0^T + b0) W2^T + b2  (reference transformer.py:23,85),
     applied to the query rows only (the reference computes all T rows and slices, transformer.py:91)."""
@@ -367,12 +403,7 @@ class DecoderFn(torch.autograd.Function):
         dt = act_dtype(precision)
         hq = hq.contiguous()
         w0, w2 = _cast(W0, dt), _cast(W2, dt)
-        n_out = W2.shape[0]
-        g, u, u_is_grad = _gelu_linear_fwd(hq, w0, b0)
-        ld = (n_out + 3) // 4 * 4
-        logits_buf = torch.empty(hq.shape[0], ld, device=hq.device, dtype=torch.float32)
-        logits = logits_buf[:, :n_out]
-        L.gemm(g, w2, logits, bias=b2.detach().contiguous())
+        g, u, u_is_grad, logits = _head_fwd(hq, w0, b0, w2, b2)
         ctx.save_for_backward(hq, u, g, W0, W2, w0, w2)
         ctx.u_is_grad = u_is_grad
         ctx.precision = precision
@@ -381,47 +412,14 @@ class DecoderFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dlogits):
         hq, u, g, W0, W2, w0, w2 = ctx.saved_tensors
-        dt = act_dtype(ctx.precision)
         dev = dlogits.device
         Nq, n_out = dlogits.shape
-        ld = (n_out + 7) // 8 * 8
-        dl = torch.zeros(Nq, ld, device=dev, dtype=dt)
+        dl = torch.zeros(Nq, (n_out + 7) // 8 * 8, device=dev, dtype=act_dtype(ctx.precision))
         dl[:, :n_out] = dlogits
-        dlv = dl[:, :n_out]
-        sizes = [W0.numel(), W0.shape[0], W2.numel(), n_out]
-        flat = torch.zeros(sum(sizes), device=dev, dtype=torch.float32)        # one bucket: a single all-reduce under DP
-        dW0 = flat[:sizes[0]].view(W0.shape)
-        db0 = flat[sizes[0]:sizes[0] + sizes[1]]
-        dW2 = flat[sizes[0] + sizes[1]:sizes[0] + sizes[1] + sizes[2]].view(W2.shape)
-        db2 = flat[sizes[0] + sizes[1] + sizes[2]:]
-        L.colsum(dlv, db2)
-        _linear_wgrad(dlv, g, dW2)
-        du = _gelu_linear_dgrad(dlv, w2, u, ctx.u_is_grad)
-        L.colsum(du, db0)
-        _linear_wgrad(du, hq, dW0)
-        dhq = _linear_dgrad(du, w0)
-        if GRAD_BUCKET_HOOK is not None:
-            GRAD_BUCKET_HOOK(flat)
-            GRAD_BUCKET_SYNC()     # 2 MB bucket: wait for it (stream-level) so autograd never touches a buffer NCCL is still writing
-        return dhq, dW0, db0, dW2, db2, None
-
-
-def _flat_grads(dev, *shapes):
-    """One zeroed fp32 buffer holding gradients of the given shapes back to back (a single all-reduce under DP), and
-    views of it in that order."""
-    sizes = [torch.Size(s).numel() for s in shapes]
-    flat = torch.zeros(sum(sizes), device=dev, dtype=torch.float32)
-    views, off = [], 0
-    for s, n in zip(shapes, sizes):
-        views.append(flat[off:off + n].view(s))
-        off += n
-    return flat, views
-
-
-def _bucket_ready(flat):
-    if GRAD_BUCKET_HOOK is not None:
-        GRAD_BUCKET_HOOK(flat)
-        GRAD_BUCKET_SYNC()     # a small bucket: wait for it (stream-level) so autograd never touches a buffer NCCL is still writing
+        flat, grads = _flat_grads(dev, W0.shape, W0.shape[:1], W2.shape, W2.shape[:1])
+        dhq = _head_bwd(dl[:, :n_out], hq, u, g, ctx.u_is_grad, w0, w2, grads)
+        _bucket_ready(flat)
+        return (dhq, *grads, None)
 
 
 def _head_grad_rows(dout, n_cols, dt):
@@ -444,14 +442,11 @@ class ScaledDecoderFn(torch.autograd.Function):
         dt = act_dtype(precision)
         hq = hq.contiguous()
         Nq, n_out = hq.shape[0], W1.shape[0]
-        nz = n_out + L.HEAD_TEMPS
         w = _cast(W, dt)
         w12 = torch.cat([W1.detach(), W2.detach()], 0).to(dt)
         b12 = torch.cat([b1.detach(), b2.detach()], 0).float()
-        g, u, u_is_grad = _gelu_linear_fwd(hq, w, b)
-        zz = torch.empty(Nq, (nz + 3) // 4 * 4, device=hq.device, dtype=torch.float32)[:, :nz]
-        L.gemm(g, w12, zz, bias=b12)
-        logits = torch.empty(Nq, (n_out + 3) // 4 * 4, device=hq.device, dtype=torch.float32)[:, :n_out]
+        g, u, u_is_grad, zz = _head_fwd(hq, w, b, w12, b12)
+        logits = _f32_rows(Nq, n_out, hq.device)
         temp = torch.empty(Nq, device=hq.device, dtype=torch.float32)
         L.scaled_head_fwd(zz, n_out, logits, temp)
         ctx.save_for_backward(hq, u, g, zz, temp, w, w12)
@@ -468,16 +463,11 @@ class ScaledDecoderFn(torch.autograd.Function):
         nz = n_out + L.HEAD_TEMPS
         dlogits, dzz = _head_grad_rows(dlogits, nz, act_dtype(precision))
         L.scaled_head_bwd(dlogits, zz, temp, n_out, dzz, dzz.shape[1])
-        dzv = dzz[:, :nz]
         # [W1; W2] and [b1; b2] are contiguous in the bucket, so the stacked GEMM writes both layers' gradients in place
-        flat, (dW, db, dW12, db12) = _flat_grads(hq.device, w_shape, w_shape[:1], (nz, nhid), (nz,))
-        L.colsum(dzv, db12)
-        _linear_wgrad(dzv, g, dW12)
-        du = _gelu_linear_dgrad(dzv, w12, u, ctx.u_is_grad)
-        L.colsum(du, db)
-        _linear_wgrad(du, hq, dW)
-        dhq = _linear_dgrad(du, w)
+        flat, grads = _flat_grads(hq.device, w_shape, w_shape[:1], (nz, nhid), (nz,))
+        dhq = _head_bwd(dzz[:, :nz], hq, u, g, ctx.u_is_grad, w, w12, grads)
         _bucket_ready(flat)
+        dW, db, dW12, db12 = grads
         return dhq, dW, db, dW12[:n_out], db12[:n_out], dW12[n_out:], db12[n_out:], None
 
 
@@ -493,11 +483,8 @@ class FixedScaledDecoderFn(torch.autograd.Function):
         hq = hq.contiguous()
         Nq, n_out = hq.shape[0], W2.shape[0]
         w0, w2 = _cast(W0, dt), _cast(W2, dt)
-        g, u, u_is_grad = _gelu_linear_fwd(hq, w0, b0)
-        ld = (n_out + 3) // 4 * 4
-        z = torch.empty(Nq, ld, device=hq.device, dtype=torch.float32)[:, :n_out]
-        L.gemm(g, w2, z, bias=b2.detach().contiguous())
-        logits = torch.empty(Nq, ld, device=hq.device, dtype=torch.float32)[:, :n_out]
+        g, u, u_is_grad, z = _head_fwd(hq, w0, b0, w2, b2)
+        logits = _f32_rows(Nq, n_out, hq.device)
         S = torch.empty(1, device=hq.device, dtype=torch.float32)
         L.fixed_scaled_head_fwd(z, n_out, T.detach().contiguous().float(), logits, S)
         ctx.save_for_backward(hq, u, g, z, S, w0, w2)
@@ -511,17 +498,11 @@ class FixedScaledDecoderFn(torch.autograd.Function):
         precision, w0_shape, w2_shape, t_shape = ctx.meta
         n_out = w2_shape[0]
         dlogits, dz = _head_grad_rows(dlogits, n_out, act_dtype(precision))
-        flat, (dW0, db0, dW2, db2, dT) = _flat_grads(hq.device, w0_shape, w0_shape[:1], w2_shape, w2_shape[:1], t_shape)
-        L.fixed_scaled_head_bwd(dlogits, z, S, n_out, dz, dT, dz.shape[1])
-        dzv = dz[:, :n_out]
-        L.colsum(dzv, db2)
-        _linear_wgrad(dzv, g, dW2)
-        du = _gelu_linear_dgrad(dzv, w2, u, ctx.u_is_grad)
-        L.colsum(du, db0)
-        _linear_wgrad(du, hq, dW0)
-        dhq = _linear_dgrad(du, w0)
+        flat, grads = _flat_grads(hq.device, w0_shape, w0_shape[:1], w2_shape, w2_shape[:1], t_shape)
+        L.fixed_scaled_head_bwd(dlogits, z, S, n_out, dz, grads[4], dz.shape[1])
+        dhq = _head_bwd(dz[:, :n_out], hq, u, g, ctx.u_is_grad, w0, w2, grads[:4])
         _bucket_ready(flat)
-        return dhq, dW0, db0, dW2, db2, dT, None
+        return (dhq, *grads, None)
 
 
 def conv_weight_operand(W, dgrad=False):

@@ -20,6 +20,13 @@ from .positional_encodings import NoPositionalEncoding
 from .utils import SeqBN
 
 
+def _require_cuda_input(x, method):
+    if not x.is_cuda:
+        raise RuntimeError(
+            f"TransformerModel.{method} runs on hand-written sm_90a kernels only; inputs are on "
+            f"{x.device}. Move model and data to a CUDA device (there is no CPU fallback).")
+
+
 class TrainingContext:
     """What `TransformerModel.encode_context` keeps of n training rows: `kv` [nlayers, n*B, 2*E] holds each layer's K | V
     of the rows (token row t*B + b, the model's activation dtype), plus the shapes and the precision it was made with.
@@ -143,10 +150,7 @@ class TransformerModel(nn.Module):
                 raise NotImplementedError(
                     "src_mask differs from generate_D_q_matrix(T, T - single_eval_pos): the sm_90a attention kernels "
                     "implement that mask implicitly and no other (reference transformer.py:60)")
-        if not x_src.is_cuda:
-            raise RuntimeError(
-                "TransformerModel.forward runs on hand-written sm_90a kernels only; inputs are on "
-                f"{x_src.device}. Move model and data to a CUDA device (there is no CPU fallback).")
+        _require_cuda_input(x_src, "forward")
         T, B = x_src.shape[0], x_src.shape[1]
         sep = int(single_eval_pos)
         if sep < 0:                      # python slicing semantics of the reference (priors/omniglot.py:75 uses -1)
@@ -186,10 +190,7 @@ class TransformerModel(nn.Module):
         if x_train.dim() != 3 or y_train.shape[:2] != x_train.shape[:2]:
             raise ValueError(f"encode_context: x_train must be [n, B, F] and y_train [n, B]; got {tuple(x_train.shape)} "
                              f"and {tuple(y_train.shape)}")
-        if not x_train.is_cuda:
-            raise RuntimeError(
-                "TransformerModel.encode_context runs on hand-written sm_90a kernels only; inputs are on "
-                f"{x_train.device}. Move model and data to a CUDA device (there is no CPU fallback).")
+        _require_cuda_input(x_train, "encode_context")
         n, B = x_train.shape[0], x_train.shape[1]
         E, nlayers = self.ninp, len(self.transformer_encoder.layers)
         dt = engine.act_dtype(self.precision)
@@ -217,10 +218,7 @@ class TransformerModel(nn.Module):
             have = getattr(ctx, name)
             if have != value:
                 raise ValueError(f"predict: the context's {name} is {have} but the model and queries have {value}")
-        if not x_query.is_cuda:
-            raise RuntimeError(
-                "TransformerModel.predict runs on hand-written sm_90a kernels only; inputs are on "
-                f"{x_query.device}. Move model and data to a CUDA device (there is no CPU fallback).")
+        _require_cuda_input(x_query, "predict")
         with torch.no_grad():
             h = self._embed(x_query, x_query.new_zeros(m, B), 0)
             h = engine.query_stack(h, ctx.kv, ctx.n, B, self.nhead, self.precision, *self._layer_params())
