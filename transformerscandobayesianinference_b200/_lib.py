@@ -5,6 +5,12 @@ library's own message is raised.  Tensors are passed as raw device pointers on t
 
 The header is restated here once: one ctypes Structure per descriptor, the mirrored enum constants, and one
 `_PROTOTYPES` line per entry point.  tests/test_cabi.py holds all three against the header.
+
+Each launching entry point has one thin wrapper below.  `@_guarded` rejects a tensor argument that is not on the call's
+one CUDA device before anything else happens and makes that device current; the wrapper body turns its arguments into
+the C arguments (`ptr`, `dtype_code`, `_set_ptrs` for descriptor pointer fields, `_u32` for seeds) and launches through
+`_call`, which counts the launches, passes torch's current stream and raises on a failed call.
+tests/test_lib_calls_host.py holds every wrapper's calls against a recorded log.
 """
 import ctypes
 import functools
@@ -271,11 +277,6 @@ def launch_count():
     return _launches
 
 
-def _count(n=1):
-    global _launches
-    _launches += n
-
-
 def declare(lib):
     """Check that the ctypes handle `lib` exports every entry point and give each its prototype; returns `lib`."""
     for name, argtypes in _PROTOTYPES.items():
@@ -385,21 +386,56 @@ def draw_seed(seed=None):
     return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if seed is None else int(seed)
 
 
+_Tensor = torch.Tensor     # bound once: the guard below runs on every library call
+
+
 def _guarded(fn):
-    """Run the wrapped library call with the device of its first tensor argument as the current device (so that
-    `stream_ptr()`, `num_sms()` and the launch itself all refer to the device that owns the data)."""
+    """Check that every tensor argument of the wrapped library call lives on one CUDA device (require_cuda), then run the
+    call with that device current (so that `stream_ptr()`, `num_sms()` and the launch itself all refer to the device
+    that owns the data).  The check comes first, so a rejected call neither reaches the library nor counts a launch.
+    A keyword argument may also be a tuple holding a tensor (gemm's `rowdot`)."""
     @functools.wraps(fn)
     def wrapper(*args, **kwargs):
-        dev = None
-        for a in args:
-            if torch.is_tensor(a) and a.is_cuda:
-                dev = a.device
-                break
+        tensors = [a for a in args if isinstance(a, _Tensor)]
+        for v in kwargs.values():
+            if isinstance(v, _Tensor):
+                tensors.append(v)
+            elif isinstance(v, tuple):
+                tensors += [t for t in v if isinstance(t, _Tensor)]
+        dev = require_cuda(*tensors)
         if dev is None:
             return fn(*args, **kwargs)
         with on_device(dev):
             return fn(*args, **kwargs)
     return wrapper
+
+
+def _call(name, *args, launches=1):
+    """Call entry point `name` with `args` and torch's current stream, adding the `launches` kernels it launches to
+    launch_count(); raises the library's error when the call fails.  `name` is looked up on the handle at every call."""
+    global _launches
+    _launches += launches
+    check(getattr(load(), name)(*(args + (stream_ptr(),))), name)     # one tuple: cheaper per call than f(*args, s)
+
+
+def _workspace(name, desc):
+    """The workspace size that query entry point `name` reports for `desc`; a negative size is the library's error."""
+    n = int(getattr(load(), name)(ctypes.byref(desc)))
+    if n < 0:
+        check(1, name)
+    return n
+
+
+def _set_ptrs(d, **tensors):
+    """Point each named field of the descriptor `d` at its tensor's data (None: NULL); returns `d`."""
+    for name, t in tensors.items():
+        setattr(d, name, None if t is None else t.data_ptr())
+    return d
+
+
+def _u32(seed):
+    """`seed` as the library's uint32_t seeds take it: its low 32 bits (two's complement for a negative seed)."""
+    return int(seed) & 0xFFFFFFFF
 
 
 # ------------------------------------------------------------------------------------------------
@@ -409,8 +445,6 @@ def _guarded(fn):
 def gemm(A, B, C, *, a_mn_major=False, b_mn_major=False, bias=None, aux=None, C2=None, epilogue=EPI_NONE,
          accumulate=False, k_splits=1, M=None, N=None, K=None, use_tc=None, rowdot=None, c2_gelu_grad=False):
     """C[M,N] (+)= epi(A . B^T-ish + bias) (+ aux).  Operands are 2-D row-major tensors (stride(1) == 1)."""
-    lib = load()
-    require_cuda(A, B, C, bias, aux, C2)
     if M is None:
         M = A.shape[1] if a_mn_major else A.shape[0]
     if K is None:
@@ -429,22 +463,19 @@ def gemm(A, B, C, *, a_mn_major=False, b_mn_major=False, bias=None, aux=None, C2
     d.ab_dtype = dtype_code(A)
     d.c2_gelu_grad = int(bool(c2_gelu_grad))
     if rowdot is not None:       # (fp32 [M, N // width] zeroed tensor, width): EPI_ROWDOT target
-        require_cuda(rowdot[0])
         d.rowdot_out, d.rowdot_width = rowdot[0].data_ptr(), int(rowdot[1])
     if use_tc is None:
         use_tc = tc_gemm_ok(A, B, C, aux, C2)
-    _count()
-    if use_tc:
-        if PROFILE_GEMM is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            check(lib.pfn_gemm_bf16_tc(ctypes.byref(d), stream_ptr()), "pfn_gemm_bf16_tc")
-            e1.record()
-            PROFILE_GEMM.append((2.0 * M * N * K, e0, e1, gemm_bytes(d)))
-        else:
-            check(lib.pfn_gemm_bf16_tc(ctypes.byref(d), stream_ptr()), "pfn_gemm_bf16_tc")
+    if not use_tc:
+        _call("pfn_gemm_simt", ctypes.byref(d))
+    elif PROFILE_GEMM is None:
+        _call("pfn_gemm_bf16_tc", ctypes.byref(d))
     else:
-        check(lib.pfn_gemm_simt(ctypes.byref(d), stream_ptr()), "pfn_gemm_simt")
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        _call("pfn_gemm_bf16_tc", ctypes.byref(d))
+        e1.record()
+        PROFILE_GEMM.append((2.0 * M * N * K, e0, e1, gemm_bytes(d)))
 
 
 def gemm_bytes(d):
@@ -472,7 +503,7 @@ def drop_threshold(p):
 def attention_desc(qkv, out, lse, T, B, H, dh, sep, dout=None, dqkv=None, delta=None, batch_major=False, drop=None):
     d = AttnDesc()
     if drop is not None:
-        d.drop_seed, d.drop_thr = int(drop[0]) & 0xFFFFFFFF, int(drop[1])
+        d.drop_seed, d.drop_thr = _u32(drop[0]), int(drop[1])
     d.batch_major = int(batch_major)
     d.T, d.B, d.H, d.dh, d.sep = T, B, H, dh, sep
     d.dtype = dtype_code(qkv)
@@ -494,14 +525,10 @@ def tc_attention_ok(qkv, dh, T=None):
 @_guarded
 def attention_fwd(qkv, out, lse, T, B, H, dh, sep, use_tc=None, batch_major=False, drop=None):
     """drop = (seed, thr): dropout on the attention probabilities (thr 0 / None = off)."""
-    _count(1)
-    lib = load()
-    require_cuda(qkv, out, lse)
     d = attention_desc(qkv, out, lse, T, B, H, dh, sep, batch_major=batch_major, drop=drop)
     if use_tc is None:
         use_tc = tc_attention_ok(qkv, dh)
-    fn = lib.pfn_attention_fwd_tc if use_tc else lib.pfn_attention_fwd_simt
-    check(fn(ctypes.byref(d), stream_ptr()), "pfn_attention_fwd")
+    _call("pfn_attention_fwd_tc" if use_tc else "pfn_attention_fwd_simt", ctypes.byref(d))
 
 
 @_guarded
@@ -509,9 +536,6 @@ def attention_bwd(qkv, out, lse, dout, dqkv, delta, T, B, H, dh, sep, use_tc=Non
                   dq_colsum=None, delta_token_major=False):
     """dq_colsum (fp32 [H*dh], tensor-core path only): += column sums of dQ, taken from the staged tiles inside the kernel.
     delta_token_major: `delta` is a [T*B, H] tensor that already holds rowsum(dO * O) (GEMM ROWDOT epilogue)."""
-    _count(2)
-    lib = load()
-    require_cuda(qkv, out, lse, dout, dqkv, delta, dq_colsum)
     d = attention_desc(qkv, out, lse, T, B, H, dh, sep, dout, dqkv, delta, batch_major=batch_major, drop=drop)
     if use_tc is None:
         use_tc = tc_attention_ok(qkv, dh)
@@ -521,8 +545,7 @@ def attention_bwd(qkv, out, lse, dout, dqkv, delta, T, B, H, dh, sep, use_tc=Non
     if delta_token_major:
         assert use_tc, "a precomputed token-major delta is consumed by the tensor-core backward only"
         d.delta_token_major = 1
-    fn = lib.pfn_attention_bwd_tc if use_tc else lib.pfn_attention_bwd_simt
-    check(fn(ctypes.byref(d), stream_ptr()), "pfn_attention_bwd")
+    _call("pfn_attention_bwd_tc" if use_tc else "pfn_attention_bwd_simt", ctypes.byref(d), launches=2)
 
 
 def attention_ctx_desc(qkv, kv, out, m, n, B, H, dh):
@@ -536,113 +559,86 @@ def attention_ctx_desc(qkv, kv, out, m, n, B, H, dh):
     return d
 
 
-@_guarded
 def attention_ctx_fwd(qkv, kv, out, m, n, B, H, dh, use_tc=None):
     """out [m*B, H*dh] <- the context attention of the m query rows (packed qkv [m*B, 3*H*dh]) against the n cached training
     rows of the same batch (kv [n*B, 2*H*dh], k | v; unused when n == 0) plus each row's own key."""
-    _count(1)
-    lib = load()
-    require_cuda(qkv, kv if n > 0 else None, out)
+    _attention_ctx_fwd(qkv, kv if n > 0 else None, out, m, n, B, H, dh, use_tc)     # an unread kv is not checked
+
+
+@_guarded
+def _attention_ctx_fwd(qkv, kv, out, m, n, B, H, dh, use_tc):
     if qkv.dtype != out.dtype or (n > 0 and kv.dtype != qkv.dtype):
         raise TypeError("attention_ctx_fwd: qkv, kv and out must share one dtype")
     d = attention_ctx_desc(qkv, kv, out, m, n, B, H, dh)
     if use_tc is None:
         use_tc = tc_attention_ok(qkv, dh)
-    fn = lib.pfn_attention_ctx_fwd_tc if use_tc else lib.pfn_attention_ctx_fwd_simt
-    check(fn(ctypes.byref(d), stream_ptr()), "pfn_attention_ctx_fwd")
+    _call("pfn_attention_ctx_fwd_tc" if use_tc else "pfn_attention_ctx_fwd_simt", ctypes.byref(d))
 
 
 @_guarded
 def embed_fwd(x, y, Wx, bx, wy, by, out, T, B, F, E, sep):
-    _count(1)
-    require_cuda(x, y, Wx, bx, wy, by, out)
-    check(load().pfn_embed_fwd(ptr(x), ptr(y), ptr(Wx), ptr(bx), ptr(wy), ptr(by), ptr(out), dtype_code(out), T, B, F,
-                               E, sep, stream_ptr()), "pfn_embed_fwd")
+    _call("pfn_embed_fwd", ptr(x), ptr(y), ptr(Wx), ptr(bx), ptr(wy), ptr(by), ptr(out), dtype_code(out), T, B, F, E, sep)
 
 
 @_guarded
 def embed_bwd(dout, x, y, dWx, dbx, dwy, dby, T, B, F, E, sep):
-    _count((F + 7) // 8)
-    require_cuda(dout, x, y, dWx, dbx, dwy, dby)
-    check(load().pfn_embed_bwd(ptr(dout), dtype_code(dout), ptr(x), ptr(y), ptr(dWx), ptr(dbx), ptr(dwy), ptr(dby), T,
-                               B, F, E, sep, stream_ptr()), "pfn_embed_bwd")
+    _call("pfn_embed_bwd", ptr(dout), dtype_code(dout), ptr(x), ptr(y), ptr(dWx), ptr(dbx), ptr(dwy), ptr(dby), T, B, F,
+          E, sep, launches=(F + 7) // 8)
 
 
 @_guarded
 def layernorm_fwd(z, gamma, beta, h, mean, rstd, eps=1e-5):
-    _count(1)
-    require_cuda(z, gamma, beta, h, mean, rstd)
     rows, E = z.shape
-    check(load().pfn_layernorm_fwd(ptr(z), z.stride(0), ptr(gamma), ptr(beta), ptr(h), h.stride(0), ptr(mean),
-                                   ptr(rstd), rows, E, eps, dtype_code(z), stream_ptr()), "pfn_layernorm_fwd")
+    _call("pfn_layernorm_fwd", ptr(z), z.stride(0), ptr(gamma), ptr(beta), ptr(h), h.stride(0), ptr(mean), ptr(rstd),
+          rows, E, eps, dtype_code(z))
 
 
 @_guarded
 def layernorm_bwd(dh, z, mean, rstd, gamma, dz, dgamma, dbeta, colsum_out=None):
-    _count(1)
-    require_cuda(dh, z, mean, rstd, gamma, dz, dgamma, dbeta, colsum_out)
     rows, E = z.shape
-    check(load().pfn_layernorm_bwd(ptr(dh), dh.stride(0), ptr(z), z.stride(0), ptr(mean), ptr(rstd), ptr(gamma),
-                                   ptr(dz), dz.stride(0), ptr(dgamma), ptr(dbeta), ptr(colsum_out), rows, E,
-                                   dtype_code(z), stream_ptr()), "pfn_layernorm_bwd")
+    _call("pfn_layernorm_bwd", ptr(dh), dh.stride(0), ptr(z), z.stride(0), ptr(mean), ptr(rstd), ptr(gamma), ptr(dz),
+          dz.stride(0), ptr(dgamma), ptr(dbeta), ptr(colsum_out), rows, E, dtype_code(z))
 
 
 @_guarded
 def colsum(X, out, N=None):
-    _count(1)
-    require_cuda(X, out)
     rows = X.shape[0]
     N = X.shape[1] if N is None else N
-    check(load().pfn_colsum(ptr(X), X.stride(0), dtype_code(X), ptr(out), rows, N, stream_ptr()), "pfn_colsum")
+    _call("pfn_colsum", ptr(X), X.stride(0), dtype_code(X), ptr(out), rows, N)
 
 
 @_guarded
 def bar_nll_fwd(logits, y, borders, n_bars, full_support, nll, idx, lse, oob_count):
-    _count(1)
-    require_cuda(logits, y, borders, nll, idx, lse, oob_count)
-    rows = logits.shape[0]
-    check(load().pfn_bar_nll_fwd(ptr(logits), logits.stride(0), dtype_code(logits), ptr(y), ptr(borders), n_bars,
-                                 int(full_support), ptr(nll), ptr(idx), ptr(lse), ptr(oob_count), rows, stream_ptr()),
-          "pfn_bar_nll_fwd")
+    _call("pfn_bar_nll_fwd", ptr(logits), logits.stride(0), dtype_code(logits), ptr(y), ptr(borders), n_bars,
+          int(full_support), ptr(nll), ptr(idx), ptr(lse), ptr(oob_count), logits.shape[0])
 
 
 @_guarded
 def bar_nll_bwd(logits, idx, lse, g, dlogits, n_bars, n_cols_pad=None):
-    _count(1)
-    require_cuda(logits, idx, lse, g, dlogits)
-    rows = logits.shape[0]
     n_cols_pad = n_bars if n_cols_pad is None else n_cols_pad
-    check(load().pfn_bar_nll_bwd(ptr(logits), logits.stride(0), dtype_code(logits), ptr(idx), ptr(lse), ptr(g),
-                                 ptr(dlogits), dlogits.stride(0), dtype_code(dlogits), n_bars, n_cols_pad, rows,
-                                 stream_ptr()), "pfn_bar_nll_bwd")
+    _call("pfn_bar_nll_bwd", ptr(logits), logits.stride(0), dtype_code(logits), ptr(idx), ptr(lse), ptr(g), ptr(dlogits),
+          dlogits.stride(0), dtype_code(dlogits), n_bars, n_cols_pad, logits.shape[0])
 
 
 @_guarded
 def bar_bucket_idx(y, borders, n_bars, idx):
-    _count(1)
-    require_cuda(y, borders, idx)
-    check(load().pfn_bar_bucket_idx(ptr(y), ptr(borders), n_bars, ptr(idx), y.numel(), stream_ptr()),
-          "pfn_bar_bucket_idx")
+    _call("pfn_bar_bucket_idx", ptr(y), ptr(borders), n_bars, ptr(idx), y.numel())
 
 
 @_guarded
 def dropout(x, out, seed, thr, residual=None):
     """out = dropout(x) (+ residual), mask regenerated from (seed, thr); in place when out is x."""
-    _count(1)
-    require_cuda(x, out, residual)
     rows, cols = x.shape
     assert out.shape == x.shape and out.dtype == x.dtype and (residual is None or residual.dtype == x.dtype)
-    check(load().pfn_dropout(ptr(x), x.stride(0), ptr(residual), residual.stride(0) if residual is not None else 0, ptr(out),
-                             out.stride(0), rows, cols, dtype_code(x), int(seed) & 0xFFFFFFFF, int(thr), stream_ptr()), "pfn_dropout")
+    _call("pfn_dropout", ptr(x), x.stride(0), ptr(residual), residual.stride(0) if residual is not None else 0, ptr(out),
+          out.stride(0), rows, cols, dtype_code(x), _u32(seed), int(thr))
 
 
 @_guarded
 def dropout_keep_mask(out, seed, thr):
     """out [rows, cols] uint8 <- keep bits of the site (tests: lets the oracle consume the kernels' mask)."""
-    _count(1)
-    require_cuda(out)
     rows, cols = out.shape
-    check(load().pfn_dropout_keep_mask(ptr(out), rows, cols, int(seed) & 0xFFFFFFFF, int(thr), stream_ptr()), "pfn_dropout_keep_mask")
+    _call("pfn_dropout_keep_mask", ptr(out), rows, cols, _u32(seed), int(thr))
 
 
 def adam_chunk_elems():
@@ -652,20 +648,16 @@ def adam_chunk_elems():
 @_guarded
 def adam_step(table, chunk_start, n_tensors, n_chunks, lr, beta1, beta2, eps, weight_decay, max_grad_norm, step, norm_sq):
     """Clip (max_grad_norm > 0) + Adam update of every tensor of the device-resident pointer table (optim.FusedClipAdam)."""
-    _count(2 if max_grad_norm > 0 else 1)
-    require_cuda(table, chunk_start, norm_sq)
-    check(load().pfn_adam_step(ptr(table), ptr(chunk_start), int(n_tensors), int(n_chunks), float(lr), float(beta1),
-                               float(beta2), float(eps), float(weight_decay), float(max_grad_norm), int(step), ptr(norm_sq),
-                               stream_ptr()), "pfn_adam_step")
+    _call("pfn_adam_step", ptr(table), ptr(chunk_start), int(n_tensors), int(n_chunks), float(lr), float(beta1),
+          float(beta2), float(eps), float(weight_decay), float(max_grad_norm), int(step), ptr(norm_sq),
+          launches=2 if max_grad_norm > 0 else 1)
 
 
 @_guarded
 def gp_sample(x, z, ls, os_, noise, jitter, kernel_type, y, work, info):
-    _count(1)
-    require_cuda(x, z, ls, os_, noise, y, work, info)
     Bn, T, F = x.shape
-    check(load().pfn_gp_sample(ptr(x), ptr(z), ptr(ls), ptr(os_), ptr(noise), float(jitter), int(kernel_type), ptr(y),
-                               ptr(work), ptr(info), Bn, T, F, stream_ptr()), "pfn_gp_sample")
+    _call("pfn_gp_sample", ptr(x), ptr(z), ptr(ls), ptr(os_), ptr(noise), float(jitter), int(kernel_type), ptr(y),
+          ptr(work), ptr(info), Bn, T, F)
 
 
 def _gp_problems(d, B, T, F, ts, kernel_type, hyper):
@@ -691,13 +683,9 @@ def gp_fit_desc(B, T, F, ts, kernel_type, hyper, noise_lb, noise_init, max_iter,
 def gp_fit(x, y, desc, theta, f, iters, nevals, status, theta0=None, grad=None, mean=None, var=None):
     """One launch fits every (prefix in desc.ts, dataset) problem.  x [B,T,F], y [B,T] fp32; outputs indexed by problem
     p = i * B + b: theta / grad [P, F+3], f / mean / var [P] fp64, iters / nevals / status [P] int32."""
-    _count(1)
-    require_cuda(x, y, theta, f, iters, nevals, status, theta0, grad, mean, var)
-    desc.x, desc.y = x.data_ptr(), y.data_ptr()
-    desc.theta, desc.f = theta.data_ptr(), f.data_ptr()
-    desc.iters, desc.nevals, desc.status = iters.data_ptr(), nevals.data_ptr(), status.data_ptr()
-    desc.theta0, desc.grad, desc.mean, desc.var = ptr(theta0), ptr(grad), ptr(mean), ptr(var)
-    check(load().pfn_gp_fit(ctypes.byref(desc), stream_ptr()), "pfn_gp_fit")
+    _set_ptrs(desc, x=x, y=y, theta=theta, f=f, iters=iters, nevals=nevals, status=status, theta0=theta0, grad=grad,
+              mean=mean, var=var)
+    _call("pfn_gp_fit", ctypes.byref(desc))
 
 
 def gp_mcmc_desc(B, T, F, ts, kernel_type, hyper, num_samples, warmup_steps, seed, max_tree_depth=GP_MCMC_MAX_DEPTH,
@@ -706,7 +694,7 @@ def gp_mcmc_desc(B, T, F, ts, kernel_type, hyper, num_samples, warmup_steps, see
     d = _gp_problems(GpMcmcDesc(), B, T, F, ts, kernel_type, hyper)
     d.num_samples, d.warmup_steps, d.max_tree_depth = int(num_samples), int(warmup_steps), int(max_tree_depth)
     d.n_pred = int(n_pred)
-    d.seed = int(seed) & 0xFFFFFFFF
+    d.seed = _u32(seed)
     return d
 
 
@@ -716,66 +704,49 @@ def gp_mcmc(x, y, desc, samples, step_size, accept, diag, init=None, log_samples
     """One launch runs a NUTS chain for every (prefix in desc.ts, dataset) problem.  x [B,T,F], y [B,T] fp32; outputs
     indexed by problem p = i * B + b: samples / log_samples [P, S', F+2], mean / var [P, S', n_pred], potential [P], grad [P, F+2],
     step_size / accept [P] fp64, diag [P, 6] int32 (GP_MCMC_DIAG_NAMES), trace [P, W + S, F+4]; S' = max(num_samples, 1)."""
-    _count(1)
-    require_cuda(x, y, samples, step_size, accept, diag, init, log_samples, mean, var, potential, grad, trace)
-    desc.x, desc.y = x.data_ptr(), y.data_ptr()
-    desc.samples, desc.step_size, desc.accept, desc.diag = (samples.data_ptr(), step_size.data_ptr(), accept.data_ptr(),
-                                                            diag.data_ptr())
-    desc.init, desc.log_samples, desc.mean, desc.var = ptr(init), ptr(log_samples), ptr(mean), ptr(var)
-    desc.potential, desc.grad, desc.trace = ptr(potential), ptr(grad), ptr(trace)
-    check(load().pfn_gp_mcmc(ctypes.byref(desc), stream_ptr()), "pfn_gp_mcmc")
+    _set_ptrs(desc, x=x, y=y, samples=samples, step_size=step_size, accept=accept, diag=diag, init=init,
+              log_samples=log_samples, mean=mean, var=var, potential=potential, grad=grad, trace=trace)
+    _call("pfn_gp_mcmc", ctypes.byref(desc))
 
 
 @_guarded
 def stroke_geometry(desc, seed, geom, turns, cap_flag):
     """geom [B, C, strokes_max, 4] int32, turns [B, C, strokes_max] fp64 <- the class strokes of B datasets; cap_flag [1]
     int32 is set to 1 (never cleared) when a stroke's rejection loop hits desc.max_iters."""
-    _count(1)
-    require_cuda(geom, turns, cap_flag)
-    check(load().pfn_stroke_geometry(ctypes.byref(desc), int(seed) & 0xFFFFFFFF, geom.shape[0], ptr(geom), ptr(turns),
-                                     ptr(cap_flag), stream_ptr()), "pfn_stroke_geometry")
+    _call("pfn_stroke_geometry", ctypes.byref(desc), _u32(seed), geom.shape[0], ptr(geom), ptr(turns), ptr(cap_flag))
 
 
 @_guarded
 def stroke_render(desc, seed, cls, geom, turns, x, normalize):
     """x [T, B, S*S] fp32 <- the images of the class table cls [T, B] int32."""
-    _count(1)
-    require_cuda(cls, geom, turns, x)
     T, B = cls.shape
-    check(load().pfn_stroke_render(ctypes.byref(desc), int(seed) & 0xFFFFFFFF, ptr(cls), ptr(geom), ptr(turns), ptr(x), T, B,
-                                   int(bool(normalize)), stream_ptr()), "pfn_stroke_render")
+    _call("pfn_stroke_render", ctypes.byref(desc), _u32(seed), ptr(cls), ptr(geom), ptr(turns), ptr(x), T, B,
+          int(bool(normalize)))
 
 
 @_guarded
 def stroke_raster(segs, nseg, widths, fill, mask, blurred, S):
     """Oracle hook: mask / blurred [N, S*S] uint8 <- segment sets segs [N, K, 4] int32 (nseg [N], widths [N] int32), ink
     filled with fill [N, S*S] uint8 (None: 128) before the blur."""
-    _count(1)
-    require_cuda(segs, nseg, widths, fill, mask, blurred)
     N, K, _ = segs.shape
-    check(load().pfn_stroke_raster(ptr(segs), ptr(nseg), ptr(widths), ptr(fill), ptr(mask), ptr(blurred), N, K, S,
-                                   stream_ptr()), "pfn_stroke_raster")
+    _call("pfn_stroke_raster", ptr(segs), ptr(nseg), ptr(widths), ptr(fill), ptr(mask), ptr(blurred), N, K, S)
 
 
 @_guarded
 def omniglot_episodes(desc, seed, bank, alpha_start, x, y, target_y):
     """x [T, B, S*S] fp32, y / target_y [T, B] int64 <- desc.B episodes drawn from bank [n_classes, 20, S, S] uint8
     (alpha_start [n_alpha] int32: first class of every alphabet of the split, Jonas mode only)."""
-    _count(1)
-    require_cuda(bank, alpha_start, x, y, target_y)
-    check(load().pfn_omniglot_episodes(ctypes.byref(desc), int(seed) & 0xFFFFFFFF, ptr(bank), ptr(alpha_start), ptr(x), ptr(y),
-                                       ptr(target_y), stream_ptr()), "pfn_omniglot_episodes")
+    _call("pfn_omniglot_episodes", ctypes.byref(desc), _u32(seed), ptr(bank), ptr(alpha_start), ptr(x), ptr(y),
+          ptr(target_y))
 
 
 @_guarded
 def bnn_prior(x, y, seed, E, dataset_offset=0, weights=None, x_raw=None, u=None):
     """x [T, B, F] fp32, y [T, B] fp32 <- B datasets of the Bayesian-NN prior with E hidden units.  The oracle hook:
     weights [B, E F + 3 E + 2] fp32, x_raw [T, B, F] fp32 (before the standardisation), u [T, B] fp64 (class uniforms)."""
-    _count(1)
-    require_cuda(x, y, weights, x_raw, u)
     T, B, F = x.shape
-    check(load().pfn_bnn_prior(int(seed) & 0xFFFFFFFF, int(dataset_offset), B, T, F, int(E), ptr(x), ptr(y), ptr(weights),
-                               ptr(x_raw), ptr(u), stream_ptr()), "pfn_bnn_prior")
+    _call("pfn_bnn_prior", _u32(seed), int(dataset_offset), B, T, F, int(E), ptr(x), ptr(y), ptr(weights), ptr(x_raw),
+          ptr(u))
 
 
 def bnn_mcmc_desc(N, n, n_test, F, E, num_samples, warmup_steps, seed, max_tree_depth=GP_MCMC_MAX_DEPTH):
@@ -783,16 +754,13 @@ def bnn_mcmc_desc(N, n, n_test, F, E, num_samples, warmup_steps, seed, max_tree_
     d = BnnMcmcDesc()
     d.N, d.n, d.n_test, d.F, d.E = int(N), int(n), int(n_test), int(F), int(E)
     d.num_samples, d.warmup_steps, d.max_tree_depth = int(num_samples), int(warmup_steps), int(max_tree_depth)
-    d.seed = int(seed) & 0xFFFFFFFF
+    d.seed = _u32(seed)
     return d
 
 
 def bnn_mcmc_workspace(desc):
     """Doubles of global workspace every chain of `desc` needs (0: the sampler state fits in shared memory)."""
-    w = int(load().pfn_bnn_mcmc_workspace(ctypes.byref(desc)))
-    if w < 0:
-        check(1, "pfn_bnn_mcmc_workspace")
-    return w
+    return _workspace("pfn_bnn_mcmc_workspace", desc)
 
 
 @_guarded
@@ -801,73 +769,54 @@ def bnn_mcmc(x_train, y_train, x_test, desc, samples, step_size, accept, diag, i
     """One launch runs a NUTS chain for every dataset.  x_train [N,n,F], y_train [N,n], x_test [N,n_test,F] fp32; outputs
     indexed by dataset: samples [N, S', d], probs [N, S', n_test] fp64, obs [N, S', n_test] fp32 (classes drawn from probs), potential [N], grad [N, d], step_size / accept [N] fp64,
     diag [N, 6] int32 (GP_MCMC_DIAG_NAMES), trace [N, W + S, d + 2]; workspace [N, bnn_mcmc_workspace(desc)] fp64."""
-    _count(1)
-    require_cuda(x_train, y_train, x_test, samples, step_size, accept, diag, init, probs, obs, potential, grad, trace, workspace)
-    desc.x_train, desc.y_train, desc.x_test = x_train.data_ptr(), y_train.data_ptr(), ptr(x_test)
-    desc.init = ptr(init)
-    desc.samples, desc.step_size, desc.accept, desc.diag = (samples.data_ptr(), step_size.data_ptr(), accept.data_ptr(),
-                                                            diag.data_ptr())
-    desc.probs, desc.obs, desc.potential, desc.grad = ptr(probs), ptr(obs), ptr(potential), ptr(grad)
-    desc.trace, desc.workspace = ptr(trace), ptr(workspace)
-    check(load().pfn_bnn_mcmc(ctypes.byref(desc), stream_ptr()), "pfn_bnn_mcmc")
+    _set_ptrs(desc, x_train=x_train, y_train=y_train, x_test=x_test, samples=samples, step_size=step_size, accept=accept,
+              diag=diag, init=init, probs=probs, obs=obs, potential=potential, grad=grad, trace=trace, workspace=workspace)
+    _call("pfn_bnn_mcmc", ctypes.byref(desc))
 
 
 @_guarded
 def knn_cv(x, y, proba, k_best, cv_mean, status):
     """One launch runs the KNN grid-search CV and refit of every problem.  x [n+m, S, F], y [n, S] fp32; outputs
     proba [m, S] fp64, k_best [S] int32, cv_mean [S, min(5, n - 2)] fp64, status [S] int32 (KNN_*)."""
-    _count(1)
-    require_cuda(x, y, proba, k_best, cv_mean, status)
     d = KnnCvDesc()
     rows, d.S, d.F = x.shape
     d.n = y.shape[0]
     d.m = rows - d.n
-    d.x, d.y = x.data_ptr(), y.data_ptr()
-    d.proba, d.k_best, d.cv_mean, d.status = proba.data_ptr(), k_best.data_ptr(), cv_mean.data_ptr(), status.data_ptr()
-    check(load().pfn_knn_cv(ctypes.byref(d), stream_ptr()), "pfn_knn_cv")
+    _set_ptrs(d, x=x, y=y, proba=proba, k_best=k_best, cv_mean=cv_mean, status=status)
+    _call("pfn_knn_cv", ctypes.byref(d))
 
 
 @_guarded
 def ridge_prefix(x, y, target, alpha, pred, sq_err):
     """One launch fits sklearn's Ridge(alpha) to every prefix t = 1 .. T-1 of every dataset.  x [B,T,F], y / target [B,T]
     fp32; outputs pred / sq_err [B,T] fp64 (column 0 NaN)."""
-    _count(1)
-    require_cuda(x, y, target, pred, sq_err)
     d = RidgePrefixDesc()
     d.B, d.T, d.F = x.shape
     d.alpha = float(alpha)
-    d.x, d.y, d.target, d.pred, d.sq_err = x.data_ptr(), y.data_ptr(), target.data_ptr(), pred.data_ptr(), sq_err.data_ptr()
-    check(load().pfn_ridge_prefix(ctypes.byref(d), stream_ptr()), "pfn_ridge_prefix")
+    _set_ptrs(d, x=x, y=y, target=target, pred=pred, sq_err=sq_err)
+    _call("pfn_ridge_prefix", ctypes.byref(d))
 
 
-def _exact_gp_desc(x, mode, length_scale, alpha=0.0):
+def _exact_gp(x, mode, length_scale, alpha=0.0, **tensors):
+    """One pfn_exact_gp call in `mode` on x [B,T,F]; `tensors` sets the descriptor's other pointer fields."""
     d = ExactGpDesc()
     d.B, d.T, d.F = x.shape
     d.mode, d.length_scale, d.alpha = mode, float(length_scale), float(alpha)
-    d.x = x.data_ptr()
-    return d
+    _call("pfn_exact_gp", ctypes.byref(_set_ptrs(d, x=x, **tensors)))
 
 
 @_guarded
 def exact_gp_evaluate(x, y, length_scale, alpha, mean, var, status):
     """The RBF exact GP's predictive of row t given rows < t, every t = 1 .. T-1 and dataset, from one factor per dataset.
     x [B,T,F], y [B,T] fp32; outputs mean / var [B,T] fp64 (column 0 NaN), status [B] int32 (0 or the failing prefix)."""
-    _count(1)
-    require_cuda(x, y, mean, var, status)
-    d = _exact_gp_desc(x, EXACT_GP_EVALUATE, length_scale, alpha)
-    d.y, d.mean, d.var, d.status = y.data_ptr(), mean.data_ptr(), var.data_ptr(), status.data_ptr()
-    check(load().pfn_exact_gp(ctypes.byref(d), stream_ptr()), "pfn_exact_gp")
+    _exact_gp(x, EXACT_GP_EVALUATE, length_scale, alpha, y=y, mean=mean, var=var, status=status)
 
 
 @_guarded
 def exact_gp_sample(x, z, length_scale, sample, rank, factor=None, perm=None):
     """sample [B,T] fp32 = P L z[:, :r] with P L L^T P^T = RBF(x, x) (pivoted Cholesky to the numerical rank r); rank [B]
     int32; optional factor [B,T,T] fp64 (P L) and perm [B,T] int32 (pivot order)."""
-    _count(1)
-    require_cuda(x, z, sample, rank, factor, perm)
-    d = _exact_gp_desc(x, EXACT_GP_SAMPLE, length_scale)
-    d.z, d.sample, d.rank, d.factor, d.perm = z.data_ptr(), sample.data_ptr(), rank.data_ptr(), ptr(factor), ptr(perm)
-    check(load().pfn_exact_gp(ctypes.byref(d), stream_ptr()), "pfn_exact_gp")
+    _exact_gp(x, EXACT_GP_SAMPLE, length_scale, z=z, sample=sample, rank=rank, factor=factor, perm=perm)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -891,61 +840,45 @@ def mcmc_trouble(diag):
     return int(diag[..., col("div_sampling")].sum()), int(diag[..., col("max_depth_hits")].sum())
 
 
-def _conv_desc(N, S, C_in, dtype, x=None, w=None, bias=None, g=None, y=None, dw=None, db=None, workspace=None):
-    """Descriptor of one 3x3 layer of the conv encoder (include/pfn_b200.h, pfn_conv_desc); S is the layer's input side."""
-    require_cuda(x, w, bias, g, y, dw, db, workspace)
+def _conv_desc(N, S, C_in, dtype, **tensors):
+    """Descriptor of one 3x3 layer of the conv encoder (include/pfn_b200.h, pfn_conv_desc); S is the layer's input side,
+    `tensors` sets its pointer fields (x, w, bias, g, y, dw, db, workspace; the others stay NULL)."""
     d = ConvDesc()
     d.N, d.S, d.C_in, d.dtype = N, S, C_in, dtype_code(dtype) if torch.is_tensor(dtype) else dtype
-    for name, t in (("x", x), ("w", w), ("bias", bias), ("g", g), ("y", y), ("dw", dw), ("db", db),
-                    ("workspace", workspace)):
-        setattr(d, name, None if t is None else t.data_ptr())
-    return d
+    return _set_ptrs(d, **tensors)
 
 
 @_guarded
 def conv_fwd(x, w, bias, y, N, S, C_in):
     """y [N, S-2, S-2, 64] = relu(conv3x3(x) + bias); y's dtype is the activation dtype."""
-    _count()
-    check(load().pfn_conv_fwd(ctypes.byref(_conv_desc(N, S, C_in, y, x=x, w=w, bias=bias, y=y)), stream_ptr()),
-          "pfn_conv_fwd")
+    _call("pfn_conv_fwd", ctypes.byref(_conv_desc(N, S, C_in, y, x=x, w=w, bias=bias, y=y)))
 
 
 @_guarded
 def conv_dgrad(g, w, x, out, N, S):
     """out (padded, side S + 4) interior = (input gradient of the 64 -> 64 layer with input x) * [x > 0]."""
-    _count()
-    check(load().pfn_conv_dgrad(ctypes.byref(_conv_desc(N, S, CONV_CH, out, x=x, w=w, g=g, y=out)), stream_ptr()),
-          "pfn_conv_dgrad")
+    _call("pfn_conv_dgrad", ctypes.byref(_conv_desc(N, S, CONV_CH, out, x=x, w=w, g=g, y=out)))
 
 
 def conv_wgrad_workspace(N, S, C_in):
-    n = load().pfn_conv_wgrad_workspace(ctypes.byref(_conv_desc(N, S, C_in, F32)))
-    if n < 0:
-        check(1, "pfn_conv_wgrad_workspace")
-    return n
+    return _workspace("pfn_conv_wgrad_workspace", _conv_desc(N, S, C_in, F32))
 
 
 @_guarded
 def conv_wgrad(g, x, dw, db, N, S, C_in):
     """dw [64, C_in, 3, 3], db [64] fp32 (overwritten) of the layer with input x and padded output gradient g."""
     ws = torch.empty(conv_wgrad_workspace(N, S, C_in), device=g.device, dtype=torch.float32)
-    _count(2)
-    check(load().pfn_conv_wgrad(ctypes.byref(_conv_desc(N, S, C_in, g, x=x, g=g, dw=dw, db=db, workspace=ws)),
-                                stream_ptr()), "pfn_conv_wgrad")
+    _call("pfn_conv_wgrad", ctypes.byref(_conv_desc(N, S, C_in, g, x=x, g=g, dw=dw, db=db, workspace=ws)), launches=2)
 
 
 @_guarded
 def conv_mean_fwd(y, feat, N, s):
-    require_cuda(y, feat)
-    _count()
-    check(load().pfn_conv_mean_fwd(ptr(y), N, s, dtype_code(y), ptr(feat), stream_ptr()), "pfn_conv_mean_fwd")
+    _call("pfn_conv_mean_fwd", ptr(y), N, s, dtype_code(y), ptr(feat))
 
 
 @_guarded
 def conv_mean_bwd(dfeat, y, g, N, s):
-    require_cuda(dfeat, y, g)
-    _count()
-    check(load().pfn_conv_mean_bwd(ptr(dfeat), ptr(y), N, s, dtype_code(y), ptr(g), stream_ptr()), "pfn_conv_mean_bwd")
+    _call("pfn_conv_mean_bwd", ptr(dfeat), ptr(y), N, s, dtype_code(y), ptr(g))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -954,41 +887,31 @@ def conv_mean_bwd(dfeat, y, g, N, s):
 @_guarded
 def scaled_head_fwd(zz, n_out, out, temp):
     """out [rows, n_out] = zz[:, :n_out] / temp, temp [rows] = softmax(zz[:, n_out:n_out + 10]) . c; zz, out, temp fp32."""
-    _count()
-    require_cuda(zz, out, temp)
-    check(load().pfn_scaled_head_fwd(ptr(zz), zz.stride(0), int(n_out), ptr(out), out.stride(0), ptr(temp), zz.shape[0],
-                                     stream_ptr()), "pfn_scaled_head_fwd")
+    _call("pfn_scaled_head_fwd", ptr(zz), zz.stride(0), int(n_out), ptr(out), out.stride(0), ptr(temp), zz.shape[0])
 
 
 @_guarded
 def scaled_head_bwd(g, zz, temp, n_out, dzz, n_cols_pad=None):
     """dzz [rows, n_cols_pad] (activation dtype) <- g [rows, n_out] fp32, the forward's zz and temp."""
-    _count()
-    require_cuda(g, zz, temp, dzz)
     n_cols_pad = n_out + HEAD_TEMPS if n_cols_pad is None else n_cols_pad
-    check(load().pfn_scaled_head_bwd(ptr(g), g.stride(0), ptr(zz), zz.stride(0), ptr(temp), int(n_out), ptr(dzz),
-                                     dzz.stride(0), dtype_code(dzz), int(n_cols_pad), g.shape[0], stream_ptr()),
-          "pfn_scaled_head_bwd")
+    _call("pfn_scaled_head_bwd", ptr(g), g.stride(0), ptr(zz), zz.stride(0), ptr(temp), int(n_out), ptr(dzz),
+          dzz.stride(0), dtype_code(dzz), int(n_cols_pad), g.shape[0])
 
 
 @_guarded
 def fixed_scaled_head_fwd(z, n_out, T, out, S):
     """out [rows, n_out] = z[:, :n_out] / S with S [1] = sum(T), all fp32."""
-    _count()
-    require_cuda(z, T, out, S)
-    check(load().pfn_fixed_scaled_head_fwd(ptr(z), z.stride(0), int(n_out), ptr(T), T.numel(), ptr(out), out.stride(0),
-                                           ptr(S), z.shape[0], stream_ptr()), "pfn_fixed_scaled_head_fwd")
+    _call("pfn_fixed_scaled_head_fwd", ptr(z), z.stride(0), int(n_out), ptr(T), T.numel(), ptr(out), out.stride(0),
+          ptr(S), z.shape[0])
 
 
 @_guarded
 def fixed_scaled_head_bwd(g, z, S, n_out, dz, dT, n_cols_pad=None, row_dot=None):
     """dz [rows, n_cols_pad] (activation dtype) = g / S; every dT [n_t] = -sum(g z) / S^2 (fp32)."""
-    require_cuda(g, z, S, dz, dT, row_dot)
     rows = g.shape[0]
-    _count(2 if rows else 1)
     if row_dot is None:
         row_dot = torch.empty(rows, device=g.device, dtype=torch.float32)
     n_cols_pad = n_out if n_cols_pad is None else n_cols_pad
-    check(load().pfn_fixed_scaled_head_bwd(ptr(g), g.stride(0), ptr(z), z.stride(0), ptr(S), int(n_out), ptr(dz),
-                                           dz.stride(0), dtype_code(dz), int(n_cols_pad), ptr(row_dot), ptr(dT), dT.numel(),
-                                           rows, stream_ptr()), "pfn_fixed_scaled_head_bwd")
+    _call("pfn_fixed_scaled_head_bwd", ptr(g), g.stride(0), ptr(z), z.stride(0), ptr(S), int(n_out), ptr(dz),
+          dz.stride(0), dtype_code(dz), int(n_cols_pad), ptr(row_dot), ptr(dT), dT.numel(), rows,
+          launches=2 if rows else 1)
