@@ -47,8 +47,9 @@ struct GemmTcParams {
   int rowdot_width, rowdot_groups;
 };
 
-// Epilogue kinds, one kernel instantiation each: the epilogue is unrolled over the 128 accumulators of a thread, and
-// keeping only the active variant keeps the kernel's code inside the instruction cache.
+// Epilogue kinds, one kernel instantiation each (two where aux is an optional residual: with and without it): the
+// epilogue is unrolled over the 128 accumulators of a thread, and keeping only the active variant keeps the kernel's
+// code inside the instruction cache.
 enum EpiKind : int { kEpiNone, kEpiGelu, kEpiGeluPre, kEpiGeluGrad, kEpiGeluBwd, kEpiRowdot, kEpiMul };
 
 constexpr int kBlockM = 128;
@@ -82,16 +83,24 @@ __device__ __forceinline__ Unit unit_at(const GemmTcParams& p, int u) {
 }
 
 // The epilogue math of one accumulator pair (columns col, col + 1 of one row), in the order of the reference formula.
-// `ep` is the pair's slot in the staging buffer: it holds aux on entry and receives C2.
-template <int EPI>
-__device__ __forceinline__ void epi_pair(const GemmTcParams& p, float& f0, float& f1, float2 b, bool add_bias,
-                                         bool use_aux, uint8_t* ep, int col, float& rowdot) {
-  float a0 = 0.f, a1 = 0.f;
-  if (use_aux) {
+// `ep` is the pair's slot in the staging buffer: it holds aux on entry and receives C2.  The code is branch-free, so that
+// the compiler can issue the staging-buffer loads of many pairs ahead of their use:
+//   - the bias is always added: sBias holds -0.0f where no bias applies, and x + (-0.0f) == x for every x, -0.0f
+//     included;
+//   - with AUX the aux pair is always loaded (the slot lies inside the staging buffer whatever its contents) and then
+//     selected: where it does not apply (past N, or a split-K unit other than the first) it is -0.0f, again an exact
+//     identity for the residual add.  The other aux kinds (GELU', MUL, ROWDOT) use aux in every unit, and their columns
+//     past N are neither stored (the TMA clips them) nor summed (ROWDOT checks col).
+template <int EPI, bool AUX>
+__device__ __forceinline__ void epi_pair(const GemmTcParams& p, float& f0, float& f1, float2 b, bool use_aux,
+                                         uint8_t* ep, int col, float& rowdot) {
+  float a0 = -0.f, a1 = -0.f;
+  if constexpr (AUX) {
     const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep));
-    a0 = t.x; a1 = t.y;
+    a0 = use_aux ? t.x : -0.f;
+    a1 = use_aux ? t.y : -0.f;
   }
-  if (add_bias) { f0 += b.x; f1 += b.y; }
+  f0 += b.x; f1 += b.y;
   if constexpr (EPI == kEpiGeluPre || EPI == kEpiGeluGrad) {
     float s0 = f0, s1 = f1;
     if constexpr (EPI == kEpiGeluGrad) { gelu_and_grad_fast(f0, f0, s0); gelu_and_grad_fast(f1, f1, s1); }
@@ -100,7 +109,7 @@ __device__ __forceinline__ void epi_pair(const GemmTcParams& p, float& f0, float
   } else if constexpr (EPI == kEpiGelu) {
     f0 = gelu_fast(f0); f1 = gelu_fast(f1);
   }
-  if (use_aux) {
+  if constexpr (AUX) {
     if constexpr (EPI == kEpiGeluBwd) {
       f0 *= gelu_grad_fast(a0); f1 *= gelu_grad_fast(a1);
     } else if constexpr (EPI == kEpiMul) {
@@ -111,12 +120,13 @@ __device__ __forceinline__ void epi_pair(const GemmTcParams& p, float& f0, float
       if (col < p.N) rowdot = fmaf(__bfloat162float(__float2bfloat16_rn(f0)), a0, rowdot);
       if (col + 1 < p.N) rowdot = fmaf(__bfloat162float(__float2bfloat16_rn(f1)), a1, rowdot);
     } else {
-      f0 += a0; f1 += a1;
+      // __fadd_rn: never contracted into an FMA with the GELU's last multiply, so C rounds as a separate add
+      f0 = __fadd_rn(f0, a0); f1 = __fadd_rn(f1, a1);
     }
   }
 }
 
-template <bool A_MN, bool B_MN, int EPI>
+template <bool A_MN, bool B_MN, int EPI, bool AUX>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmAux, const __grid_constant__ CUtensorMap tmC,
@@ -216,7 +226,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const Unit w = unit_at(p, u);
     if ((i & 1) != g) { kb_count += w.nkb; continue; }
     const bool add_bias = p.bias != nullptr && w.split == 0;
-    const float bias_v = add_bias && w.n0 + tid < p.N ? __ldg(p.bias + w.n0 + tid) : 0.f;
+    const float bias_v = add_bias && w.n0 + tid < p.N ? __ldg(p.bias + w.n0 + tid) : -0.f;   // -0: see epi_pair
     // the other warpgroup has drained its main loop (and this warpgroup has left its previous epilogue: all 128 threads
     // take part in the barrier, so sBias is free)
     if (i > 0) tc::named_bar_sync(1 + g, 256);
@@ -279,7 +289,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           uint8_t* ep = wslab + (j >> 3) * 16384 + mh * 8192 + h * 1024 + (((j & 7) ^ rl) << 4) + 4 * q;
-          epi_pair<EPI>(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b, add_bias, aux_j, ep, col, rowdot[mh][h]);
+          epi_pair<EPI, AUX>(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b, aux_j, ep, col, rowdot[mh][h]);
         }
       }
     }
@@ -363,7 +373,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (lane == 0) tc::bulk_wait<0>();
 }
 
-template <bool A_MN, bool B_MN, int EPI>
+template <bool A_MN, bool B_MN, int EPI, bool AUX>
 static int launch_gemm_tc(const pfn_gemm_desc* d, cudaStream_t stream) {
   CUtensorMap tmA, tmB, tmAux, tmC, tmC2;
   memset(&tmAux, 0, sizeof(tmAux));
@@ -420,7 +430,7 @@ static int launch_gemm_tc(const pfn_gemm_desc* d, cudaStream_t stream) {
   PFN_CHECK_ARG(total < (1LL << 31), "gemm_tc: too many tiles");
   p.tiles = static_cast<int>(tiles);
   p.units = static_cast<int>(total);
-  auto kern = gemm_tc_kernel<A_MN, B_MN, EPI>;
+  auto kern = gemm_tc_kernel<A_MN, B_MN, EPI, AUX>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
     PFN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
@@ -431,14 +441,20 @@ static int launch_gemm_tc(const pfn_gemm_desc* d, cudaStream_t stream) {
   return 0;
 }
 
-template <int EPI>
+template <int EPI, bool AUX>
 static int launch_layout(const pfn_gemm_desc* d, cudaStream_t s) {
   switch ((d->a_mn_major ? 2 : 0) | (d->b_mn_major ? 1 : 0)) {
-    case 0: return launch_gemm_tc<false, false, EPI>(d, s);
-    case 1: return launch_gemm_tc<false, true, EPI>(d, s);
-    case 2: return launch_gemm_tc<true, false, EPI>(d, s);
-    default: return launch_gemm_tc<true, true, EPI>(d, s);
+    case 0: return launch_gemm_tc<false, false, EPI, AUX>(d, s);
+    case 1: return launch_gemm_tc<false, true, EPI, AUX>(d, s);
+    case 2: return launch_gemm_tc<true, false, EPI, AUX>(d, s);
+    default: return launch_gemm_tc<true, true, EPI, AUX>(d, s);
   }
+}
+
+// the epilogue kinds whose aux is optional (a residual added last) have one instantiation without it and one with it
+template <int EPI>
+static int launch_aux(const pfn_gemm_desc* d, cudaStream_t s) {
+  return d->aux != nullptr ? launch_layout<EPI, true>(d, s) : launch_layout<EPI, false>(d, s);
 }
 
 }  // namespace pfn
@@ -474,12 +490,12 @@ extern "C" int pfn_gemm_bf16_tc(const pfn_gemm_desc* d, void* stream) {
     default: break;
   }
   switch (epi) {
-    case kEpiGelu: return launch_layout<kEpiGelu>(d, s);
-    case kEpiGeluPre: return launch_layout<kEpiGeluPre>(d, s);
-    case kEpiGeluGrad: return launch_layout<kEpiGeluGrad>(d, s);
-    case kEpiGeluBwd: return launch_layout<kEpiGeluBwd>(d, s);
-    case kEpiRowdot: return launch_layout<kEpiRowdot>(d, s);
-    case kEpiMul: return launch_layout<kEpiMul>(d, s);
-    default: return launch_layout<kEpiNone>(d, s);
+    case kEpiGelu: return launch_aux<kEpiGelu>(d, s);
+    case kEpiGeluPre: return launch_aux<kEpiGeluPre>(d, s);
+    case kEpiGeluGrad: return launch_aux<kEpiGeluGrad>(d, s);
+    case kEpiGeluBwd: return launch_layout<kEpiGeluBwd, true>(d, s);      // aux is required (checked above)
+    case kEpiRowdot: return launch_layout<kEpiRowdot, true>(d, s);
+    case kEpiMul: return launch_layout<kEpiMul, true>(d, s);
+    default: return launch_aux<kEpiNone>(d, s);
   }
 }
