@@ -215,7 +215,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
       tc::tma_prefetch_desc(&tmDO);
-      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk, E, 2 * E, 4 * AB_TILE, [&](const AttUnit& unit) {
+      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, [&](const AttUnit&) { return nblk; }, E, 2 * E, 4 * AB_TILE,
+                      [&](const AttUnit& unit) {
         for (int g = 0; g < 2; ++g) {
           const int t0 = unit.tile * 128 + 64 * g;
           att_load_tile(sQ + g * AB_TILE, &tmQ, pp.q_full, unit.h * ATT_DH, unit.b, t0);

@@ -8,7 +8,7 @@
 #include "common.cuh"
 #include "dropout.cuh"
 #include "tc_common.cuh"
-#include "../../include/pfn_b200.h"
+#include "../../include/pfn_b200_ragged.h"
 
 namespace pfn {
 
@@ -19,6 +19,9 @@ constexpr int ATT_TILE = ATT_TILE_ROWS * ATT_ROW_BYTES;       // 16 KB
 
 int check_attn_desc_public(const pfn_attn_desc* d, bool bwd, const char* who);
 int check_attn_ctx_desc(const pfn_attn_ctx_desc* d, const char* who);
+// the descriptor of the same forward with sep = T and no lse / over the cache of n rows, checked; the key counts stay in d
+int attn_ragged_as_masked(const pfn_attn_ragged_desc* d, pfn_attn_desc* a, const char* who);
+int attn_ctx_ragged_as_ctx(const pfn_attn_ctx_ragged_desc* d, pfn_attn_ctx_desc* c, const char* who);
 
 // token row of (time t, batch b) in the [T*B, cols] activations
 __device__ __forceinline__ size_t att_tok(int t, int b, int T, int B, int batch_major) {
@@ -98,16 +101,18 @@ struct AttPipe {
   }
 };
 
-// The producer of the pipeline (one thread): for each of the CTA's units, the nblk key blocks of its (batch, head).  The
-// next tile's query operands go in once the consumers are done with the current ones, which is before its last key
-// block is (so the first key blocks of the next tile are already in flight by then): load_q(unit) issues q_bytes of
-// TMA loads on q_full.  k_col / v_col: the first column of head 0's K and V in the map tmKV.
-template <int STAGES, class LoadQ>
+// The producer of the pipeline (one thread): for each of the CTA's units, the nblk_of(unit) key blocks of its (batch,
+// head).  The next tile's query operands go in once the consumers are done with the current ones, which is before its
+// last key block is (so the first key blocks of the next tile are already in flight by then): load_q(unit) issues
+// q_bytes of TMA loads on q_full.  k_col / v_col: the first column of head 0's K and V in the map tmKV.
+template <int STAGES, class NBlk, class LoadQ>
 __device__ __forceinline__ void att_kv_producer(const AttPipe<STAGES>& pp, const CUtensorMap* tmKV, int n_units, int n_tiles,
-                                                int H, int nblk, int k_col, int v_col, uint32_t q_bytes, LoadQ&& load_q) {
+                                                int H, NBlk&& nblk_of, int k_col, int v_col, uint32_t q_bytes,
+                                                LoadQ&& load_q) {
   AttRing<STAGES> ring;
   for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
     const AttUnit unit = att_unit(u, n_tiles, H);
+    const int nblk = nblk_of(unit);
     auto claim_q = [&]() {
       if (it > 0) tc::mbar_wait_suspend(pp.q_empty, (it - 1) & 1);
       tc::mbar_expect_tx(pp.q_full, q_bytes);
@@ -197,13 +202,19 @@ __device__ __forceinline__ float quad_max(float v) {
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
 
-static inline int check_tc_attn(const pfn_attn_desc* d, bool bwd, const char* who) {
-  if (int rc = check_attn_desc_public(d, bwd, who)) return rc;
+// what the tensor-core kernels need of a checked descriptor's forward operands
+static inline int check_tc_operands(const pfn_attn_desc* d, const char* who) {
   PFN_CHECK_ARG(d->dtype == PFN_BF16, "%s: bf16 only", who);
   PFN_CHECK_ARG(d->dh == ATT_DH, "%s: head dim %d unsupported (built for 128)", who, d->dh);
   PFN_CHECK_ARG(d->ld_qkv % 8 == 0 && d->ld_out % 8 == 0, "%s: leading dims must be multiples of 8", who);
   PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->qkv) | reinterpret_cast<uintptr_t>(d->out)) & 15) == 0,
                 "%s: qkv/out must be 16-byte aligned", who);
+  return 0;
+}
+
+static inline int check_tc_attn(const pfn_attn_desc* d, bool bwd, const char* who) {
+  if (int rc = check_attn_desc_public(d, bwd, who)) return rc;
+  if (int rc = check_tc_operands(d, who)) return rc;
   if (bwd) {
     PFN_CHECK_ARG(d->ld_dout % 8 == 0 && d->ld_dqkv % 8 == 0, "%s: leading dims must be multiples of 8", who);
     PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->dout) | reinterpret_cast<uintptr_t>(d->dqkv)) & 15) == 0,

@@ -3,9 +3,11 @@
 // lanes, scores are reduced with warp shuffles, softmax is computed online.  The single_eval_pos mask of
 // reference transformer.py:35-41 is implicit:  keys(i) = [0, sep)  U  {i if i >= sep}.  The forward also serves the
 // context attention (pfn_attention_ctx_fwd_simt): there the sep keys come from the K/V cache and every row has its own key.
+// In the ragged forwards (pfn_attention_ragged_fwd_simt, pfn_attention_ctx_ragged_fwd_simt) dataset b has n_keys[b] keys
+// in place of sep.
 #include "common.cuh"
 #include "dropout.cuh"
-#include "../../include/pfn_b200.h"
+#include "../../include/pfn_b200_ragged.h"
 
 namespace pfn {
 
@@ -26,14 +28,16 @@ __device__ __forceinline__ void store_head(T* base, int dh, int lane, const floa
   }
 }
 
-// The sep keys shared by all rows of batch b: K of key j at kv + (j*B + b)*ld + h*dh, V at + v_off (the packed qkv itself for
-// the masked attention, the K/V cache for the context attention).  Rows i >= diag_from also attend to their own key; the key
-// order is the same in both uses, so a query row gets the same bits from either entry point.
+// The keys shared by all rows of batch b: its first sep_b keys, K of key j at kv + (j*B + b)*ld + h*dh, V at + v_off (the
+// packed qkv itself for the masked attention, the K/V cache for the context attention).  sep_b is sep, or in the ragged
+// kernel n_keys[b] clamped to [0, sep].  Rows i >= min(diag_from, sep_b) also attend to their own key; the key order is the
+// same in all uses, so a query row gets the same bits from any entry point.
 struct SharedKeys {
   const void* kv; int ld; int v_off; int diag_from;
+  const int* n_keys;
 };
 
-template <typename T, int DPL>
+template <typename T, int DPL, bool kRagged>
 __global__ void __launch_bounds__(256)
 attn_fwd_simt_kernel(const pfn_attn_desc d, const SharedKeys sk) {
   const int E = d.H * d.dh;
@@ -52,12 +56,13 @@ attn_fwd_simt_kernel(const pfn_attn_desc d, const SharedKeys sk) {
 #pragma unroll
     for (int c = 0; c < DPL; ++c) { q[c] *= d.scale; o[c] = 0.f; }
     float m = -INFINITY, l = 0.f;
-    const int nkeys = d.sep + (i >= sk.diag_from ? 1 : 0);
+    const int sep = kRagged ? min(max(__ldg(sk.n_keys + b), 0), d.sep) : d.sep;
+    const int nkeys = sep + (i >= (kRagged ? min(sk.diag_from, sep) : sk.diag_from) ? 1 : 0);
     for (int jj = 0; jj < nkeys; ++jj) {
-      const int j = jj < d.sep ? jj : i;
-      const T* krow = jj < d.sep ? reinterpret_cast<const T*>(sk.kv) + (static_cast<size_t>(j) * d.B + b) * sk.ld + h * d.dh
-                                 : qkv + (static_cast<size_t>(i) * d.B + b) * d.ld_qkv + E + h * d.dh;
-      const int v_off = jj < d.sep ? sk.v_off : E;
+      const int j = jj < sep ? jj : i;
+      const T* krow = jj < sep ? reinterpret_cast<const T*>(sk.kv) + (static_cast<size_t>(j) * d.B + b) * sk.ld + h * d.dh
+                               : qkv + (static_cast<size_t>(i) * d.B + b) * d.ld_qkv + E + h * d.dh;
+      const int v_off = jj < sep ? sk.v_off : E;
       float k[DPL], v[DPL];
       load_head<T, DPL>(krow, d.dh, lane, k);
       load_head<T, DPL>(krow + v_off, d.dh, lane, v);
@@ -205,7 +210,8 @@ static int launch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, co
   const long long max_grid = static_cast<long long>(num_sms()) * 16;
   if (grid > max_grid) grid = max_grid;
   if (!bwd) {
-    attn_fwd_simt_kernel<T, DPL><<<static_cast<int>(grid), 256, 0, s>>>(*d, sk);
+    if (sk.n_keys) attn_fwd_simt_kernel<T, DPL, true><<<static_cast<int>(grid), 256, 0, s>>>(*d, sk);
+    else attn_fwd_simt_kernel<T, DPL, false><<<static_cast<int>(grid), 256, 0, s>>>(*d, sk);
     PFN_LAUNCH_OK();
     return 0;
   }
@@ -230,10 +236,25 @@ static int dispatch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, 
   return launch_attn_simt<T, 8>(d, bwd, s, sk);
 }
 
-// the keys of the masked attention: [0, sep) of the packed qkv, and row i's own key for i >= sep
-static SharedKeys masked_keys(const pfn_attn_desc* d) {
+// the keys of the masked attention: [0, sep) (or [0, n_keys[b])) of the packed qkv, and row i's own key for i >= sep
+static SharedKeys masked_keys(const pfn_attn_desc* d, const int* n_keys = nullptr) {
   const size_t esz = d->dtype == PFN_F32 ? 4 : 2;
-  return {static_cast<const char*>(d->qkv) + esz * d->H * d->dh, d->ld_qkv, d->H * d->dh, d->sep};
+  return {static_cast<const char*>(d->qkv) + esz * d->H * d->dh, d->ld_qkv, d->H * d->dh, d->sep, n_keys};
+}
+
+// the keys of the context attention: [0, n) (or [0, n_keys[b])) of the cache, and every row's own key
+static SharedKeys cached_keys(const pfn_attn_ctx_desc* d, const int* n_keys = nullptr) {
+  return {d->kv, d->ld_kv, d->H * d->dh, 0, n_keys};
+}
+
+// rows of the masked-attention forward with T = m query rows and sep = n shared keys taken from the cache
+static pfn_attn_desc ctx_as_masked(const pfn_attn_ctx_desc* d) {
+  pfn_attn_desc a = {};
+  a.T = d->m; a.B = d->B; a.H = d->H; a.dh = d->dh; a.sep = d->n;
+  a.dtype = d->dtype; a.scale = d->scale;
+  a.qkv = d->qkv; a.ld_qkv = d->ld_qkv;
+  a.out = d->out; a.ld_out = d->ld_out;
+  return a;
 }
 
 static int dispatch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, const SharedKeys& sk) {
@@ -252,6 +273,33 @@ int check_attn_ctx_desc(const pfn_attn_ctx_desc* d, const char* who) {
                 "%s: leading dims too small", who);
   PFN_CHECK_ARG(static_cast<long long>(d->m + d->n) * d->B * d->H < (1LL << 31), "%s: too many rows", who);
   return 0;
+}
+
+int attn_ragged_as_masked(const pfn_attn_ragged_desc* d, pfn_attn_desc* a, const char* who) {
+  PFN_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
+  PFN_CHECK_ARG(d->n_keys != nullptr, "%s: null n_keys", who);
+  *a = pfn_attn_desc{};
+  a->T = d->T; a->B = d->B; a->H = d->H; a->dh = d->dh; a->sep = d->T;
+  a->dtype = d->dtype; a->scale = d->scale;
+  a->qkv = d->qkv; a->ld_qkv = d->ld_qkv;
+  a->out = d->out; a->ld_out = d->ld_out;
+  PFN_CHECK_ARG(d->T > 0 && d->B > 0 && d->H > 0 && d->dh > 0, "%s: bad shape T=%d B=%d H=%d dh=%d", who, d->T, d->B, d->H,
+                d->dh);
+  PFN_CHECK_ARG(d->dtype == PFN_F32 || d->dtype == PFN_BF16, "%s: bad dtype %d", who, d->dtype);
+  PFN_CHECK_ARG(d->qkv && d->out, "%s: null qkv/out", who);
+  PFN_CHECK_ARG(d->ld_qkv >= 3 * d->H * d->dh && d->ld_out >= d->H * d->dh, "%s: leading dims too small", who);
+  return 0;
+}
+
+int attn_ctx_ragged_as_ctx(const pfn_attn_ctx_ragged_desc* d, pfn_attn_ctx_desc* c, const char* who) {
+  PFN_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
+  PFN_CHECK_ARG(d->n_keys != nullptr, "%s: null n_keys", who);
+  c->m = d->m; c->n = d->n; c->B = d->B; c->H = d->H; c->dh = d->dh;
+  c->dtype = d->dtype; c->scale = d->scale;
+  c->qkv = d->qkv; c->ld_qkv = d->ld_qkv;
+  c->kv = d->kv; c->ld_kv = d->ld_kv;
+  c->out = d->out; c->ld_out = d->ld_out;
+  return check_attn_ctx_desc(c, who);
 }
 
 }  // namespace pfn
@@ -273,11 +321,19 @@ extern "C" int pfn_attention_bwd_simt(const pfn_attn_desc* d, void* stream) {
 
 extern "C" int pfn_attention_ctx_fwd_simt(const pfn_attn_ctx_desc* d, void* stream) {
   if (int rc = check_attn_ctx_desc(d, "attention_ctx_fwd_simt")) return rc;
-  // rows of the masked-attention forward with T = m query rows and sep = n shared keys taken from the cache
-  pfn_attn_desc a = {};
-  a.T = d->m; a.B = d->B; a.H = d->H; a.dh = d->dh; a.sep = d->n;
-  a.dtype = d->dtype; a.scale = d->scale;
-  a.qkv = d->qkv; a.ld_qkv = d->ld_qkv;
-  a.out = d->out; a.ld_out = d->ld_out;
-  return dispatch_attn_simt(&a, false, reinterpret_cast<cudaStream_t>(stream), SharedKeys{d->kv, d->ld_kv, d->H * d->dh, 0});
+  const pfn_attn_desc a = ctx_as_masked(d);
+  return dispatch_attn_simt(&a, false, reinterpret_cast<cudaStream_t>(stream), cached_keys(d));
+}
+
+extern "C" int pfn_attention_ragged_fwd_simt(const pfn_attn_ragged_desc* d, void* stream) {
+  pfn_attn_desc a;
+  if (int rc = attn_ragged_as_masked(d, &a, "attention_ragged_fwd_simt")) return rc;
+  return dispatch_attn_simt(&a, false, reinterpret_cast<cudaStream_t>(stream), masked_keys(&a, d->n_keys));
+}
+
+extern "C" int pfn_attention_ctx_ragged_fwd_simt(const pfn_attn_ctx_ragged_desc* d, void* stream) {
+  pfn_attn_ctx_desc c;
+  if (int rc = attn_ctx_ragged_as_ctx(d, &c, "attention_ctx_ragged_fwd_simt")) return rc;
+  const pfn_attn_desc a = ctx_as_masked(&c);
+  return dispatch_attn_simt(&a, false, reinterpret_cast<cudaStream_t>(stream), cached_keys(&c, d->n_keys));
 }

@@ -20,6 +20,11 @@
 // The context attention (kCtx, pfn_attention_ctx_fwd_tc) is the same kernel on other operands: the query tiles come from
 // the query rows' packed [m*B, 3E] qkv (T = m), the key blocks from the [n*B, 2E] K/V cache (sep = n), and every query row
 // has its diagonal key.  It writes no lse.
+//
+// Ragged datasets (kRagged, pfn_attention_ragged_fwd_tc / pfn_attention_ctx_ragged_fwd_tc): dataset b has its own key
+// count n_b = n_keys[b] <= sep in place of sep, in the three places sep enters: the unit's key-block count, the mask of
+// its last block, and which rows have their diagonal key (i >= n_b; every row in the context attention).  Keys in
+// [n_b, sep) are real rows of the operand and are masked like the keys past sep in the last block.
 #include "attention_common.cuh"
 
 namespace pfn {
@@ -42,9 +47,16 @@ struct AttnFwdParams {
   int n_tiles;        // 128-row query tiles per (batch, head)
   int batch_major;
   uint32_t drop_seed; int drop_thr;   // dropout on the probabilities (thr 0 = off), csrc/dropout.cuh
+  const int* n_keys;  // [B] per-dataset key counts (kRagged only)
 };
 
-template <bool kCtx>
+// the key count of dataset b: sep, or n_keys[b] clamped to [0, sep] in the ragged kernels
+template <bool kRagged>
+__device__ __forceinline__ int att_sep(const AttnFwdParams& p, int b) {
+  return kRagged ? min(max(__ldg(p.n_keys + b), 0), p.sep) : p.sep;
+}
+
+template <bool kCtx, bool kRagged>
 __global__ void __launch_bounds__(AF_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                 const __grid_constant__ CUtensorMap tmO, const AttnFwdParams p) {
@@ -69,7 +81,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if (threadIdx.x == 256) {
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
-      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk, p.k_col, p.v_col, 2 * ATT_TILE, [&](const AttUnit& unit) {
+      auto nblk_of = [&](const AttUnit& unit) {
+        return kRagged ? (att_sep<true>(p, unit.b) + ATT_TILE_ROWS - 1) / ATT_TILE_ROWS : nblk;
+      };
+      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk_of, p.k_col, p.v_col, 2 * ATT_TILE, [&](const AttUnit& unit) {
         for (int g = 0; g < 2; ++g)
           att_load_tile(sQ + g * ATT_TILE, &tmQ, pp.q_full, unit.h * ATT_DH, unit.b, unit.tile * 128 + 64 * g);
       });
@@ -90,6 +105,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const AttUnit unit = att_unit(u, p.n_tiles, p.H);
     const int t0 = unit.tile * 128 + 64 * g;
     const int i0 = t0 + 16 * wq + (lane >> 2);            // this lane's rows: i0, i0 + 8
+    const int sep = att_sep<kRagged>(p, unit.b);
+    const int unit_nblk = kRagged ? (sep + ATT_TILE_ROWS - 1) / ATT_TILE_ROWS : nblk;
 
     // Diagonal key first: o[4 j + 2 r + c] is row i0 + 8 r, column 8 j + 2 (lane & 3) + c.  A row i >= sep starts from
     // m = s_ii, l = 1 (this lane's share of l: 1 in lane 0 of the quad) and O = keep_ii v_i; the loads are in flight
@@ -99,7 +116,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int i = i0 + 8 * r;
-      const bool diag = i < p.T && (kCtx || i >= p.sep);
+      const bool diag = i < p.T && (kCtx || i >= sep);
       drow[r] = static_cast<uint32_t>(unit.bh) * p.T + i;
       const __nv_bfloat16* qrow = p.qkv + att_tok(diag ? i : 0, unit.b, p.T, p.B, p.batch_major) * p.ld_qkv + unit.h * ATT_DH;
       float sd = 0.f;
@@ -148,10 +165,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     // before dropout; s is left holding them after dropout.
     auto softmax = [&](int kb) {
       const int key0 = kb * ATT_TILE_ROWS + 2 * (lane & 3);
-      if (kb * ATT_TILE_ROWS + ATT_TILE_ROWS > p.sep) {
+      if (kb * ATT_TILE_ROWS + ATT_TILE_ROWS > sep) {
 #pragma unroll
         for (int e = 0; e < 32; ++e)
-          if (key0 + 8 * (e >> 2) + (e & 1) >= p.sep) s[e] = -INFINITY;
+          if (key0 + 8 * (e >> 2) + (e & 1) >= sep) s[e] = -INFINITY;
       }
       float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -177,7 +194,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
       for (int e = 0; e < 16; ++e) ap[e] = tc::pack_bf16x2(s[2 * e], s[2 * e + 1]);
     };
-    if (att_key_loop(pp, ring, it, nblk, issue_s, issue_pv, [&] { tc::wgmma_fence_regs(s); },
+    if (att_key_loop(pp, ring, it, unit_nblk, issue_s, issue_pv, [&] { tc::wgmma_fence_regs(s); },
                      [&] { tc::wgmma_fence_regs(o); }, softmax, rescale_pack, [] {})) {
       timed_out = true;
       break;
@@ -198,7 +215,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const uint32_t off = (j >> 3) * 8192 + rr * 128 + (((j & 7) ^ (rr & 7)) << 4) + (lane & 3) * 4;
         *reinterpret_cast<uint32_t*>(stg + off) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
       }
-      if (!kCtx && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+      if (!kCtx && !kRagged && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
     }
     tc::fence_proxy_async_smem();
     tc::named_bar_sync(1 + g, 128);
@@ -212,12 +229,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   if (timed_out) asm volatile("trap;");
 }
 
-}  // namespace pfn
-
-using namespace pfn;
-
-extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
-  if (int rc = check_tc_attn(d, false, "attention_fwd_tc")) return rc;
+// The masked forward over d (lse written unless ragged) with n_keys[b] keys for dataset b when kRagged
+template <bool kRagged>
+static int launch_attn_fwd_tc(const pfn_attn_desc* d, const int* n_keys, cudaStream_t stream, const char* who) {
   AttnFwdParams p;
   p.T = d->T; p.B = d->B; p.H = d->H; p.sep = d->sep;
   p.scale_log2 = d->scale * 1.4426950408889634f;
@@ -228,24 +242,26 @@ extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
   p.n_tiles = (d->T + 127) / 128;
   p.batch_major = d->batch_major;
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
+  p.n_keys = n_keys;
   CUtensorMap tmQ, tmKV, tmO;
   if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
   // out: rows past T are not written
   if (int rc = att_tensor_map(&tmO, d->out, E, d->ld_out, d->T, d->B, d->T, d->batch_major)) return rc;
-  return att_launch_persistent<attn_fwd_kernel<false>>("attention_fwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
-                                                AF_THREADS, AF_SMEM, reinterpret_cast<cudaStream_t>(stream), tmQ, tmKV, tmO, p);
+  return att_launch_persistent<attn_fwd_kernel<false, kRagged>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                                AF_THREADS, AF_SMEM, stream, tmQ, tmKV, tmO, p);
 }
 
-extern "C" int pfn_attention_ctx_fwd_tc(const pfn_attn_ctx_desc* d, void* stream) {
-  if (int rc = check_attn_ctx_desc(d, "attention_ctx_fwd_tc")) return rc;
-  PFN_CHECK_ARG(d->dtype == PFN_BF16, "attention_ctx_fwd_tc: bf16 only");
-  PFN_CHECK_ARG(d->dh == ATT_DH, "attention_ctx_fwd_tc: head dim %d unsupported (built for 128)", d->dh);
-  PFN_CHECK_ARG(d->ld_qkv % 8 == 0 && d->ld_kv % 8 == 0 && d->ld_out % 8 == 0,
-                "attention_ctx_fwd_tc: leading dims must be multiples of 8");
+// The context forward over d with n_keys[b] cached keys for dataset b when kRagged
+template <bool kRagged>
+static int launch_attn_ctx_fwd_tc(const pfn_attn_ctx_desc* d, const int* n_keys, cudaStream_t stream, const char* who) {
+  if (int rc = check_attn_ctx_desc(d, who)) return rc;
+  PFN_CHECK_ARG(d->dtype == PFN_BF16, "%s: bf16 only", who);
+  PFN_CHECK_ARG(d->dh == ATT_DH, "%s: head dim %d unsupported (built for 128)", who, d->dh);
+  PFN_CHECK_ARG(d->ld_qkv % 8 == 0 && d->ld_kv % 8 == 0 && d->ld_out % 8 == 0, "%s: leading dims must be multiples of 8", who);
   // with n == 0 no key block is loaded; the key map then only needs a valid base
   const void* kv = d->n > 0 ? d->kv : d->qkv;
   PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->qkv) | reinterpret_cast<uintptr_t>(kv) | reinterpret_cast<uintptr_t>(d->out)) &
-                 15) == 0, "attention_ctx_fwd_tc: qkv/kv/out must be 16-byte aligned");
+                 15) == 0, "%s: qkv/kv/out must be 16-byte aligned", who);
   AttnFwdParams p;
   p.T = d->m; p.B = d->B; p.H = d->H; p.sep = d->n;
   p.scale_log2 = d->scale * 1.4426950408889634f;
@@ -256,11 +272,38 @@ extern "C" int pfn_attention_ctx_fwd_tc(const pfn_attn_ctx_desc* d, void* stream
   p.n_tiles = (d->m + 127) / 128;
   p.batch_major = 0;
   p.drop_seed = 0; p.drop_thr = 0;
+  p.n_keys = n_keys;
   CUtensorMap tmQ, tmKV, tmO;
   if (int rc = att_tensor_map(&tmQ, d->qkv, 3 * E, d->ld_qkv, d->m, d->B, d->m, 0)) return rc;
   if (int rc = att_tensor_map(&tmKV, kv, d->n > 0 ? 2 * E : 3 * E, d->n > 0 ? d->ld_kv : d->ld_qkv, d->n, d->B,
                               d->n > 0 ? d->n : 1, 0)) return rc;
   if (int rc = att_tensor_map(&tmO, d->out, E, d->ld_out, d->m, d->B, d->m, 0)) return rc;
-  return att_launch_persistent<attn_fwd_kernel<true>>("attention_ctx_fwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
-                                                      AF_THREADS, AF_SMEM, reinterpret_cast<cudaStream_t>(stream), tmQ, tmKV, tmO, p);
+  return att_launch_persistent<attn_fwd_kernel<true, kRagged>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                               AF_THREADS, AF_SMEM, stream, tmQ, tmKV, tmO, p);
+}
+
+}  // namespace pfn
+
+using namespace pfn;
+
+extern "C" int pfn_attention_fwd_tc(const pfn_attn_desc* d, void* stream) {
+  if (int rc = check_tc_attn(d, false, "attention_fwd_tc")) return rc;
+  return launch_attn_fwd_tc<false>(d, nullptr, reinterpret_cast<cudaStream_t>(stream), "attention_fwd_tc");
+}
+
+extern "C" int pfn_attention_ctx_fwd_tc(const pfn_attn_ctx_desc* d, void* stream) {
+  return launch_attn_ctx_fwd_tc<false>(d, nullptr, reinterpret_cast<cudaStream_t>(stream), "attention_ctx_fwd_tc");
+}
+
+extern "C" int pfn_attention_ragged_fwd_tc(const pfn_attn_ragged_desc* d, void* stream) {
+  pfn_attn_desc a;
+  if (int rc = attn_ragged_as_masked(d, &a, "attention_ragged_fwd_tc")) return rc;
+  if (int rc = check_tc_operands(&a, "attention_ragged_fwd_tc")) return rc;
+  return launch_attn_fwd_tc<true>(&a, d->n_keys, reinterpret_cast<cudaStream_t>(stream), "attention_ragged_fwd_tc");
+}
+
+extern "C" int pfn_attention_ctx_ragged_fwd_tc(const pfn_attn_ctx_ragged_desc* d, void* stream) {
+  pfn_attn_ctx_desc c;
+  if (int rc = attn_ctx_ragged_as_ctx(d, &c, "attention_ctx_ragged_fwd_tc")) return rc;
+  return launch_attn_ctx_fwd_tc<true>(&c, d->n_keys, reinterpret_cast<cudaStream_t>(stream), "attention_ctx_ragged_fwd_tc");
 }

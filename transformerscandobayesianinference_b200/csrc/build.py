@@ -61,7 +61,8 @@ def _nvcc():
 
 def _headers():
     hs = [os.path.join(HERE, f) for f in os.listdir(HERE) if f.endswith((".cuh", ".h"))]
-    hs.append(os.path.join(ROOT, "include", "pfn_b200.h"))
+    inc = os.path.join(ROOT, "include")
+    hs += [os.path.join(inc, f) for f in os.listdir(inc) if f.endswith(".h")]
     return hs
 
 

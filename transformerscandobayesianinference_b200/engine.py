@@ -14,7 +14,7 @@ import os
 
 import torch
 
-from . import _lib as L
+from . import _lib as L, _lib_ragged as LR
 
 LAYER_PARAM_NAMES = ("in_w", "in_b", "out_w", "out_b", "w1", "b1", "w2", "b2", "g1", "be1", "g2", "be2")
 N_LAYER_PARAMS = len(LAYER_PARAM_NAMES)
@@ -305,10 +305,12 @@ class EncoderStackFn(torch.autograd.Function):
 
 
 @torch.no_grad()
-def encode_context(src, T, B, nhead, precision, *params):
+def encode_context(src, T, B, nhead, precision, *params, n_keys=None):
     """The K/V cache of T training rows: src [T*B, E] (their embedding, activation dtype, T >= 1) runs through the encoder
     layers with sep = T, and kv [n_layers, T*B, 2E] keeps each layer's K | V of those rows, as the in-projection produced
-    them.  The last layer's attention and MLP are not run: no later layer reads their output."""
+    them.  The last layer's attention and MLP are not run: no later layer reads their output.
+    n_keys (int32 [B] on the device, optional): dataset b has n_keys[b] training rows; in the attention its row i attends
+    to rows [0, n_keys[b]) and, when i >= n_keys[b] (a padding row), to itself."""
     dt, n_layers, dh, h = _stack_start(src, precision, nhead, params)
     N, E = h.shape
     kv = torch.empty(n_layers, N, 2 * E, device=src.device, dtype=dt)
@@ -317,22 +319,29 @@ def encode_context(src, T, B, nhead, precision, *params):
         kv[li].copy_(qkv[:, E:])
         if li == n_layers - 1:
             break
-        lse = torch.empty(B * nhead, T, device=h.device, dtype=torch.float32)
-        L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, T)
+        if n_keys is None:
+            lse = torch.empty(B * nhead, T, device=h.device, dtype=torch.float32)
+            L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, T)
+        else:
+            LR.attention_ragged_fwd(qkv, attn, T, B, nhead, dh, n_keys)
         h = _layer_tail(h, attn, P, out_w, w1, w2, None, li)[-1]
     return kv
 
 
 @torch.no_grad()
-def query_stack(src, kv, n, B, nhead, precision, *params):
+def query_stack(src, kv, n, B, nhead, precision, *params, n_keys=None):
     """src [m*B, E] (the query rows' embedding, activation dtype) -> their output of the encoder layers, each query row
     attending to the n training rows whose K | V the cache kv [n_layers, n*B, 2E] holds (encode_context) and to itself:
     rows n .. n + m - 1 of EncoderStackFn on (training rows, query rows) with sep = n.  Per layer: the in-projection GEMM,
-    the context attention, then the same out-projection, LayerNorm and MLP kernels as EncoderStackFn.forward."""
+    the context attention, then the same out-projection, LayerNorm and MLP kernels as EncoderStackFn.forward.
+    n_keys (int32 [B] on the device, optional): the query rows of dataset b attend to its first n_keys[b] cached rows only."""
     dt, n_layers, dh, h = _stack_start(src, precision, nhead, params, kv)
     for li in range(n_layers):
         P, (_, out_w, w1, w2), qkv, attn = _layer_qkv(h, params, li, dt)
-        L.attention_ctx_fwd(qkv, kv[li], attn, h.shape[0] // B, n, B, nhead, dh)
+        if n_keys is None:
+            L.attention_ctx_fwd(qkv, kv[li], attn, h.shape[0] // B, n, B, nhead, dh)
+        else:
+            LR.attention_ctx_ragged_fwd(qkv, kv[li], attn, h.shape[0] // B, n, B, nhead, dh, n_keys)
         h = _layer_tail(h, attn, P, out_w, w1, w2, None, li)[-1]
     return h
 

@@ -8,8 +8,12 @@ never called.  `forward()` routes embedding -> encoder stack -> decoder through 
 For inference against one training set, `encode_context(x_train, y_train)` runs the training rows once and keeps every
 layer's K and V of them; `predict(ctx, x_query)` then scores any number of query sets against that context.  Under the
 single_eval_pos mask a training row attends only to training rows and a query row to the training rows and itself, so
-`predict` returns what `forward` returns for the concatenated sequence at single_eval_pos = n.
+`predict` returns what `forward` returns for the concatenated sequence at single_eval_pos = n.  With
+`encode_context(x_train, y_train, n_train)` the datasets of one batch have training sets of their own sizes: dataset b
+uses rows [0, n_train[b]) and the rows after them are padding that never reaches an output.
 """
+import numbers
+
 import torch
 import torch.nn as nn
 from torch.nn import TransformerEncoder, TransformerEncoderLayer
@@ -30,12 +34,37 @@ def _require_cuda_input(x, method):
 class TrainingContext:
     """What `TransformerModel.encode_context` keeps of n training rows: `kv` [nlayers, n*B, 2*E] holds each layer's K | V
     of the rows (token row t*B + b, the model's activation dtype), plus the shapes and the precision it was made with.
+    `n_train` is None when every dataset has all n rows, else the int32 [B] device tensor of each dataset's row count.
     It holds no weights: `predict` uses the model it is called on.  `predict` never writes to it."""
-    __slots__ = ("kv", "n", "B", "E", "nhead", "nlayers", "precision", "device")
+    __slots__ = ("kv", "n", "B", "E", "nhead", "nlayers", "precision", "device", "n_train")
 
-    def __init__(self, kv, n, B, E, nhead, nlayers, precision, device):
+    def __init__(self, kv, n, B, E, nhead, nlayers, precision, device, n_train=None):
         self.kv, self.n, self.B, self.E, self.nhead, self.nlayers = kv, n, B, E, nhead, nlayers
         self.precision, self.device = precision, torch.device(device)
+        self.n_train = n_train
+
+
+def _training_set_sizes(n_train, n, B):
+    """n_train (B integers in [0, n]: a sequence or an integer tensor on any device) as a tuple of ints; ValueError
+    otherwise."""
+    if torch.is_tensor(n_train):
+        if n_train.dtype.is_floating_point or n_train.dtype.is_complex or n_train.dtype == torch.bool:
+            raise ValueError(f"encode_context: n_train must hold integers, got a {n_train.dtype} tensor")
+        if n_train.dim() != 1:
+            raise ValueError(f"encode_context: n_train must be one-dimensional, got shape {tuple(n_train.shape)}")
+        sizes = n_train.tolist()
+    else:
+        sizes = list(n_train)
+        for v in sizes:
+            if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+                raise ValueError(f"encode_context: n_train must hold integers, got {v!r}")
+        sizes = [int(v) for v in sizes]
+    if len(sizes) != B:
+        raise ValueError(f"encode_context: n_train holds {len(sizes)} sizes for a batch of {B} datasets")
+    bad = [v for v in sizes if not 0 <= v <= n]
+    if bad:
+        raise ValueError(f"encode_context: n_train values must lie in [0, {n}] (the rows of x_train), got {bad[0]}")
+    return tuple(sizes)
 
 
 class TransformerModel(nn.Module):
@@ -182,25 +211,41 @@ class TransformerModel(nn.Module):
             raise ValueError("encode_context / predict: training-mode dropout is not supported: its masks are keyed by "
                              "the row's position in the full sequence; call model.eval() first")
 
-    def encode_context(self, x_train, y_train):
+    def encode_context(self, x_train, y_train, n_train=None):
         """Run the n training rows x_train [n, B, F], y_train [n, B] (n >= 0) through the embedding and every encoder
         layer on their own (they never attend to a query row) and return a `TrainingContext` holding each layer's K and
-        V of them.  No autograd.  With n = 0 a query attends only to itself, as in forward(..., single_eval_pos=0)."""
+        V of them.  No autograd.  With n = 0 a query attends only to itself, as in forward(..., single_eval_pos=0).
+
+        n_train (optional): B integers in [0, n], a sequence or an integer tensor on any device.  Dataset b then has the
+        training rows [0, n_train[b]) and `predict` gives its queries what forward gives them on those rows alone, at
+        single_eval_pos = n_train[b]; rows t >= n_train[b] are padding, whatever values they hold.  None (or every size
+        equal to n) runs the same kernels as a call without it."""
         self._check_context_inference()
         if x_train.dim() != 3 or y_train.shape[:2] != x_train.shape[:2]:
             raise ValueError(f"encode_context: x_train must be [n, B, F] and y_train [n, B]; got {tuple(x_train.shape)} "
                              f"and {tuple(y_train.shape)}")
-        _require_cuda_input(x_train, "encode_context")
         n, B = x_train.shape[0], x_train.shape[1]
+        sizes = None if n_train is None else _training_set_sizes(n_train, n, B)
+        if sizes is not None and all(v == n for v in sizes):
+            sizes = None
+        _require_cuda_input(x_train, "encode_context")
         E, nlayers = self.ninp, len(self.transformer_encoder.layers)
         dt = engine.act_dtype(self.precision)
+        n_keys = None
         with torch.no_grad():
+            if sizes is not None:
+                # the padding rows are zeroed before the embedding: a NaN or Inf there would survive a masked key's zero
+                # probability inside the attention's P V product
+                n_keys = torch.tensor(sizes, dtype=torch.int32, device=x_train.device)
+                keep = torch.arange(n, device=x_train.device).unsqueeze(1) < n_keys
+                x_train = torch.where(keep.unsqueeze(-1), x_train, 0)
+                y_train = torch.where(keep.view(*keep.shape, *(1,) * (y_train.dim() - 2)), y_train, 0)
             if n == 0:
                 kv = torch.empty(nlayers, 0, 2 * E, device=x_train.device, dtype=dt)
             else:
                 h = self._embed(x_train, y_train, n)
-                kv = engine.encode_context(h, n, B, self.nhead, self.precision, *self._layer_params())
-        return TrainingContext(kv, n, B, E, self.nhead, nlayers, self.precision, x_train.device)
+                kv = engine.encode_context(h, n, B, self.nhead, self.precision, *self._layer_params(), n_keys=n_keys)
+        return TrainingContext(kv, n, B, E, self.nhead, nlayers, self.precision, x_train.device, n_keys)
 
     def predict(self, ctx, x_query):
         """Logits [m, B, n_out] of the query rows x_query [m, B, F] (m >= 1) given the training rows `ctx` holds: what
@@ -221,5 +266,6 @@ class TransformerModel(nn.Module):
         _require_cuda_input(x_query, "predict")
         with torch.no_grad():
             h = self._embed(x_query, x_query.new_zeros(m, B), 0)
-            h = engine.query_stack(h, ctx.kv, ctx.n, B, self.nhead, self.precision, *self._layer_params())
+            h = engine.query_stack(h, ctx.kv, ctx.n, B, self.nhead, self.precision, *self._layer_params(),
+                                   n_keys=ctx.n_train)
             return self._decode(h, m, B)
