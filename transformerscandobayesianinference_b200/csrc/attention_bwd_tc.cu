@@ -12,12 +12,14 @@
 //      while the dQ MMAs of block j-1 run.  For a query row (i >= sep) the diagonal key is attended by that row only, so
 //      dK_i = dS_ii q_i and dV_i = P_ii dO_i are complete: producer warps 9-11 compute them one tile ahead, together with
 //      every row's lse2 and delta, and hand lse2, delta and dS_ii to the consumers through a double-buffered array in
-//      shared memory; the consumers add dS_ii k_i to dQ.
+//      shared memory; the consumers add dS_ii k_i to dQ, which leaves through a staging tile and TMA stores.
 //
-//  (2) attn_bwd_dkv_kernel    one CTA per (batch, head, 128-key tile of the train keys), K and V resident, loop over 64-row
-//      Q/dO blocks:
+//  (2) attn_bwd_dkv_kernel    persistent: one CTA per SM walks the (batch, head, 128-key tile of the train keys) list,
+//      key tile fastest; per tile K and V resident, loop over 64-row Q/dO blocks:
 //          S^T = K Q_i^T       dP^T = V dO_i^T     (row = key, column = query row; m64n64k16)
 //          dV += (P^T . mask) dO_i ;   dK += dS^T Q_i                           (m64n128k16, A from registers)
+//      K/V are double-buffered across tiles, so the next tile's land while the current one runs; dK and dV are staged in
+//      the tile's own K/V buffer once its last MMAs are done and leave by TMA stores clipped at sep.
 //
 // Both are warp-specialised: warpgroup 2 (producer; 64 registers in (1), 40 in (2)) issues the TMA loads into a ring of
 // stages, warpgroups 0 and 1 (consumers; 208 registers in (1), 232 in (2)) each own 64 rows of the tile (query rows in
@@ -34,19 +36,25 @@ namespace pfn {
 constexpr int AB_ROWS = ATT_TILE_ROWS;                    // rows of one consumer warpgroup; key / query block size
 constexpr int AB_TILE = ATT_TILE;                         // 16 KB: 64 rows x 128 bf16 = two 8 KB boxes of 64 columns
 constexpr int AB_THREADS = 3 * 128;
-constexpr int AB_DQ_STAGES = 4;                           // K/V blocks in flight (dQ kernel)
+constexpr int AB_DQ_STAGES = 3;                           // K/V blocks in flight (dQ kernel)
 constexpr int AB_DKV_STAGES = 3;                          // Q/dO blocks in flight (dK/dV kernel)
 constexpr int AB_DQ_STAT_WARPS = 3;                       // producer warps 9-11: per-row statistics of the next tile
-// dQ kernel: Q, dO of the tile (2 x 2 x 16 KB), ring of (K, V), two buffers of per-row (lse2, delta, ds_ii), barriers
+constexpr int AB_DQ_ROW_SLOTS = 8;                        // diagonal rows in flight per statistics warp
+constexpr int AB_DQ_ROW_SLOT = 1024;                      // one row's q_i | dO_i (512 B), then k_i | v_i (512 B)
+// dQ kernel: Q, dO of the tile (2 x 2 x 16 KB), ring of (K, V), the dQ staging tile (2 x 16 KB), two buffers of
+// per-row (lse2, delta, ds_ii), the statistics warps' rings of diagonal rows, barriers
 constexpr int AB_DQ_OFF_RING = 4 * AB_TILE;
-constexpr int AB_DQ_OFF_STAT = AB_DQ_OFF_RING + AB_DQ_STAGES * 2 * AB_TILE;
-constexpr int AB_DQ_OFF_BAR = AB_DQ_OFF_STAT + 2 * 3 * 128 * 4;
+constexpr int AB_DQ_OFF_OUT = AB_DQ_OFF_RING + AB_DQ_STAGES * 2 * AB_TILE;
+constexpr int AB_DQ_OFF_STAT = AB_DQ_OFF_OUT + 2 * AB_TILE;
+constexpr int AB_DQ_OFF_ROWS = AB_DQ_OFF_STAT + 2 * 3 * 128 * 4;
+constexpr int AB_DQ_OFF_BAR = AB_DQ_OFF_ROWS + AB_DQ_STAT_WARPS * AB_DQ_ROW_SLOTS * AB_DQ_ROW_SLOT;
 constexpr int AB_DQ_SMEM = AB_DQ_OFF_BAR + (2 * AB_DQ_STAGES + 2 + 4) * 8 + 1024;   // + 1 KB alignment slack
-// dK/dV kernel: K, V of the tile (2 x 2 x 16 KB), ring of (Q, dO), ring of (lse2, delta), barriers
-constexpr int AB_DKV_OFF_RING = 4 * AB_TILE;
+// dK/dV kernel: two buffers of the tile's K, V (2 x 2 x 2 x 16 KB), ring of (Q, dO), ring of (lse2, delta), barriers
+constexpr int AB_DKV_KV = 4 * AB_TILE;
+constexpr int AB_DKV_OFF_RING = 2 * AB_DKV_KV;
 constexpr int AB_DKV_OFF_STAT = AB_DKV_OFF_RING + AB_DKV_STAGES * 2 * AB_TILE;
 constexpr int AB_DKV_OFF_BAR = AB_DKV_OFF_STAT + AB_DKV_STAGES * 2 * AB_ROWS * 4;
-constexpr int AB_DKV_SMEM = AB_DKV_OFF_BAR + (2 * AB_DKV_STAGES + 1) * 8 + 1024;
+constexpr int AB_DKV_SMEM = AB_DKV_OFF_BAR + (2 * AB_DKV_STAGES + 4) * 8 + 1024;
 static_assert(AB_DQ_SMEM <= 232448 && AB_DKV_SMEM <= 232448, "the tiles and rings must fit the 227 KB of shared memory");
 
 struct AttnBwdParams {
@@ -111,11 +119,13 @@ attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ out, int ld_out, const _
 // =====================================================================================================================
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
-                   const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
+                   const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDQ,
+                   const AttnBwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = att_smem_base(smem_raw);
   uint8_t* sQ = smem;                                     // warpgroup g's 64 rows at + g * 16 KB
   uint8_t* sD = smem + 2 * AB_TILE;
+  uint8_t* sOut = smem + AB_DQ_OFF_OUT;                   // warpgroup g's 64 rows of dQ at + g * 16 KB
   const AttPipe<AB_DQ_STAGES> pp(smem + AB_DQ_OFF_RING, reinterpret_cast<uint64_t*>(smem + AB_DQ_OFF_BAR));
   // tile it's statistics are in buffer it & 1: [0, 128) lse2, [128, 256) delta, [256, 384) ds_ii of the tile's rows
   float* sStat = reinterpret_cast<float*>(smem + AB_DQ_OFF_STAT);
@@ -138,20 +148,43 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
   if (warp >= 8) {
     // ------------------------------------------------------------------ producer: TMA (thread 256), statistics (warps 9-11)
-    // 64 registers: the statistics warps keep two rows in flight (with 40 or 48 they spill), so the consumers get 208:
-    // 2 x 128 x 208 + 128 x 64 <= 64 K
+    // 64 registers for the statistics warps' row arithmetic, so the consumers get 208: 2 x 128 x 208 + 128 x 64 <= 64 K
     tc::setmaxnreg_dec<64>();
     if (warp > 8) {
       // Per tile: lse2 and delta of its 128 rows, and for each row i >= sep its diagonal key: s_ii = q_i.k_i,
       // dp_ii = dO_i.v_i, ds_ii = P_ii (mask dp_ii - delta_i) scale, which completes dK_i = ds_ii q_i and dV_i = P_ii mask
       // dO_i (stored here) and leaves ds_ii k_i for the consumers' dQ.  Warp pw owns the rows r = pw (mod 3).  A row is
-      // read by the whole warp with 16-byte loads: lanes 0-15 take q_i and k_i, lanes 16-31 dO_i and v_i, eight columns
-      // each; the two halves then store dK_i and dV_i.  Two rows are in flight at a time.
+      // read by the whole warp in 16-byte pieces: lanes 0-15 take q_i and k_i, lanes 16-31 dO_i and v_i, eight columns
+      // each; the two halves then store dK_i and dV_i.  The pieces come through the warp's ring of AB_DQ_ROW_SLOTS rows
+      // in shared memory (cp.async, one commit group per row), so that many rows are in flight while one is finished.
+      // A lane reads back only the bytes its own copies wrote, so its cp.async wait is all the synchronisation needed.
       const int pw = warp - 9;
+      uint8_t* lane_rows = smem + AB_DQ_OFF_ROWS + pw * AB_DQ_ROW_SLOTS * AB_DQ_ROW_SLOT + 16 * lane;
       for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
         const AttUnit unit = att_unit(u, p.n_tiles, p.H);
         const int sb = it & 1;
         float* st = sStat + sb * 3 * 128;
+        // the warp's diagonal rows of the tile: row k is r0 + 3 k, k < n_rows, in slot k % AB_DQ_ROW_SLOTS
+        const int r_lo = max(0, p.sep - unit.tile * 128), r_hi = min(128, p.T - unit.tile * 128);
+        const int r0 = r_lo + (pw - r_lo % AB_DQ_STAT_WARPS + AB_DQ_STAT_WARPS) % AB_DQ_STAT_WARPS;
+        const int n_rows = r0 < r_hi ? (r_hi - r0 + AB_DQ_STAT_WARPS - 1) / AB_DQ_STAT_WARPS : 0;
+        // the lane's half and columns come from an opaque lane index in every row, so that the address arithmetic built on
+        // them is formed next to its copies instead of being hoisted out of the loops and held in registers throughout
+        auto tok_of = [&](int r) { return att_tok(unit.tile * 128 + r, unit.b, p.T, p.B, p.batch_major); };
+        // one commit group per row, empty past the last, so that the wait before row k is always for row k
+        auto issue_row = [&](int k) {
+          if (k < n_rows) {
+            const int l = static_cast<int>(att_opaque(lane)), half = l >> 4, c8 = (l & 15) * 8;
+            const size_t tok = tok_of(r0 + AB_DQ_STAT_WARPS * k);
+            const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + unit.h * ATT_DH + c8;
+            uint8_t* slot = lane_rows + (k % AB_DQ_ROW_SLOTS) * AB_DQ_ROW_SLOT;
+            tc::cp_async16(slot, half ? p.dout + tok * p.ld_dout + unit.h * ATT_DH + c8 : qrow);   // q_i | dO_i
+            tc::cp_async16(slot + AB_DQ_ROW_SLOT / 2, qrow + (1 + half) * E);                      // k_i | v_i
+          }
+          tc::cp_async_commit();
+        };
+        // the first rows are in flight while the consumers free the statistics buffer and lse2 / delta are read
+        for (int k = 0; k < AB_DQ_ROW_SLOTS; ++k) issue_row(k);
         tc::mbar_wait_suspend(&st_empty[sb], ((it >> 1) & 1) ^ 1);
 #pragma unroll 1
         for (int r = pw + AB_DQ_STAT_WARPS * lane; r < 128; r += 32 * AB_DQ_STAT_WARPS) {
@@ -161,16 +194,6 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           st[128 + r] = valid ? ab_delta(p, unit.b, unit.h, i) : 0.f;
         }
         __syncwarp();
-        // the lane's half and columns come from an opaque lane index in every row, so that the address arithmetic built on
-        // them is formed next to its loads instead of being hoisted out of the loops and held in registers throughout
-        auto tok_of = [&](int r) { return att_tok(unit.tile * 128 + r, unit.b, p.T, p.B, p.batch_major); };
-        auto load_row = [&](int r, uint4& xv, uint4& yv) {
-          const int l = static_cast<int>(att_opaque(lane)), half = l >> 4, c8 = (l & 15) * 8;
-          const size_t tok = tok_of(r);
-          const __nv_bfloat16* qrow = p.qkv + tok * p.ld_qkv + unit.h * ATT_DH + c8;
-          xv = *reinterpret_cast<const uint4*>(half ? p.dout + tok * p.ld_dout + unit.h * ATT_DH + c8 : qrow);   // q_i | dO_i
-          yv = *reinterpret_cast<const uint4*>(qrow + (1 + half) * E);                                      // k_i | v_i
-        };
         auto finish_row = [&](int r, uint4 xv, uint4 yv) {
           const int l = static_cast<int>(att_opaque(lane)), half = l >> 4, c8 = (l & 15) * 8;
           const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&xv);
@@ -199,15 +222,13 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           *reinterpret_cast<uint4*>(p.dqkv + tok_of(r) * p.ld_dqkv + unit.h * ATT_DH + (1 + half) * E + c8) = o;   // dK_i | dV_i
           if (lane == 0) st[256 + r] = ds;
         };
-        const int r_lo = max(0, p.sep - unit.tile * 128), r_hi = min(128, p.T - unit.tile * 128);
-        for (int r = r_lo + (pw - r_lo % AB_DQ_STAT_WARPS + AB_DQ_STAT_WARPS) % AB_DQ_STAT_WARPS; r < r_hi;
-             r += 2 * AB_DQ_STAT_WARPS) {
-          const int r2 = r + AB_DQ_STAT_WARPS < r_hi ? r + AB_DQ_STAT_WARPS : r;
-          uint4 xa, ya, xb, yb;
-          load_row(r, xa, ya);
-          load_row(r2, xb, yb);
-          finish_row(r, xa, ya);
-          if (r2 != r) finish_row(r2, xb, yb);
+#pragma unroll 1
+        for (int k = 0; k < n_rows; ++k) {
+          tc::cp_async_wait<AB_DQ_ROW_SLOTS - 1>();
+          const uint8_t* slot = lane_rows + (k % AB_DQ_ROW_SLOTS) * AB_DQ_ROW_SLOT;
+          const uint4 xv = *reinterpret_cast<const uint4*>(slot), yv = *reinterpret_cast<const uint4*>(slot + AB_DQ_ROW_SLOT / 2);
+          finish_row(r0 + AB_DQ_STAT_WARPS * k, xv, yv);
+          issue_row(k + AB_DQ_ROW_SLOTS);       // refills the slot just read: finish_row has consumed its values
         }
         tc::mbar_arrive(&st_full[sb]);
       }
@@ -215,6 +236,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
       tc::tma_prefetch_desc(&tmDO);
+      tc::tma_prefetch_desc(&tmDQ);
       att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, [&](const AttUnit&) { return nblk; }, E, 2 * E, 4 * AB_TILE,
                       [&](const AttUnit& unit) {
         for (int g = 0; g < 2; ++g) {
@@ -230,7 +252,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   // -------------------------------------------------------------------- consumer warpgroups
   tc::setmaxnreg_inc<208>();
   const int g = warp >> 2, wq = warp & 3;
+  const int tid = threadIdx.x & 127;
   const uint32_t q_tile = tc::smem_u32(sQ + g * AB_TILE), d_tile = tc::smem_u32(sD + g * AB_TILE);
+  uint8_t* out_tile = sOut + g * AB_TILE;
   AttRing<AB_DQ_STAGES> ring;
   bool timed_out = false;
   for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
@@ -312,16 +336,16 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       break;
     }
 
-    // dQ = dq + ds_ii k_i, stores, column sums over the bf16-rounded values
-    float cs[16][2];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) cs[j][0] = cs[j][1] = 0.f;
+    // dQ = dq + ds_ii k_i, staged in the warpgroup's dQ tile (once the TMA has read the previous tile's out of it) and
+    // stored by the TMA, which drops the rows >= T; the column sums are read back from the staged tile
+    if (tid == 0) tc::bulk_wait_read<0>();
+    tc::named_bar_sync(1 + g, 128);
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int i = i0 + 8 * r;
       if (i < p.T) {
         const bool diag = i >= p.sep;
-        __nv_bfloat16* grow = p.dqkv + att_tok(i, unit.b, p.T, p.B, p.batch_major) * p.ld_dqkv + unit.h * ATT_DH;
+        const int lr = 16 * wq + (lane >> 2) + 8 * r;              // row i in the warpgroup's 64
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           float x = nblk > 0 ? dq[4 * j + 2 * r] : 0.f, y = nblk > 0 ? dq[4 * j + 2 * r + 1] : 0.f;
@@ -330,26 +354,28 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             x = fmaf(dsd[r], k.x, x);
             y = fmaf(dsd[r], k.y, y);
           }
-          att_st2(grow, j, lane, x, y);
-          cs[j][0] += __bfloat162float(__float2bfloat16_rn(x));
-          cs[j][1] += __bfloat162float(__float2bfloat16_rn(y));
+          *reinterpret_cast<uint32_t*>(out_tile + att_tile_off2(lr, j, lane)) = tc::pack_bf16x2(x, y);
         }
       }
     }
-    if (p.dq_colsum != nullptr) {
-      // reduce over the eight row groups of the warp (lanes with equal lane & 3), then one atomic per column and warp
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float v = cs[j][e];
-          v += __shfl_xor_sync(0xffffffffu, v, 4);
-          v += __shfl_xor_sync(0xffffffffu, v, 8);
-          v += __shfl_xor_sync(0xffffffffu, v, 16);
-          if (lane < 4) atomicAdd(p.dq_colsum + unit.h * ATT_DH + 8 * j + 2 * lane + e, v);
-        }
+    tc::fence_proxy_async_smem();
+    tc::named_bar_sync(1 + g, 128);
+    if (tid == 0 && unit.tile * 128 + 64 * g < p.T) {
+      att_store_tile(&tmDQ, out_tile, unit.h * ATT_DH, unit.b, unit.tile * 128 + 64 * g);
+      tc::bulk_commit();
+    }
+    const int rows = min(64, p.T - (unit.tile * 128 + 64 * g));
+    if (p.dq_colsum != nullptr && rows > 0) {
+      // thread tid sums column tid of the warpgroup's staged rows < T (the bf16 values as stored): one atomic per column
+      const uint8_t* col = out_tile + (tid >> 6) * 8192 + 2 * (tid & 7);
+      float v = 0.f;
+#pragma unroll 8
+      for (int r = 0; r < rows; ++r)
+        v += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((((tid & 63) >> 3) ^ (r & 7)) << 4)));
+      atomicAdd(p.dq_colsum + unit.h * ATT_DH + tid, v);
     }
   }
+  if (tid == 0) tc::bulk_wait<0>();
   if (timed_out) asm volatile("trap;");
 }
 
@@ -358,26 +384,30 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // =====================================================================================================================
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
-                    const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
+                    const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDKV,
+                    const AttnBwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = att_smem_base(smem_raw);
-  uint8_t* sK = smem;                                     // warpgroup g's 64 keys at + g * 16 KB
-  uint8_t* sV = smem + 2 * AB_TILE;
+  // the CTA's it-th tile uses K/V buffer it & 1: warpgroup g's 64 keys of K at + g * 16 KB, of V at + (2 + g) * 16 KB
   uint8_t* sRing = smem + AB_DKV_OFF_RING;                // stage s: Q at + 2 s * 16 KB, dO at + (2 s + 1) * 16 KB
   float* sStat = reinterpret_cast<float*>(smem + AB_DKV_OFF_STAT);   // stage s: lse2 at [128 s], delta at [128 s + 64]
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + AB_DKV_OFF_BAR);
   uint64_t* empty = full + AB_DKV_STAGES;
-  uint64_t* kv_bar = empty + AB_DKV_STAGES;               // K, V of the tile have landed
+  uint64_t* kv_full = empty + AB_DKV_STAGES;              // [2] K, V of the buffer's tile have landed
+  uint64_t* kv_empty = kv_full + 2;                       // [2] both warpgroups' dK/dV stores have read the buffer
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const AttUnit unit = att_unit(blockIdx.x, p.n_tiles, p.H);
   const int E = p.H * ATT_DH;
   const int nqb = (p.T + AB_ROWS - 1) / AB_ROWS;
+  const int n_units = p.n_tiles * p.B * p.H;
   if (threadIdx.x == 0) {
     for (int s = 0; s < AB_DKV_STAGES; ++s) {
       tc::mbar_init(&full[s], 1 + AB_ROWS);              // the TMA thread's expect_tx + one arrival per statistics row
       tc::mbar_init(&empty[s], 2);
     }
-    tc::mbar_init(kv_bar, 1);
+    for (int s = 0; s < 2; ++s) {
+      tc::mbar_init(&kv_full[s], 1);
+      tc::mbar_init(&kv_empty[s], 2);
+    }
     tc::mbar_fence_init();
   }
   __syncthreads();
@@ -391,32 +421,50 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       tc::tma_prefetch_desc(&tmQ);
       tc::tma_prefetch_desc(&tmKV);
       tc::tma_prefetch_desc(&tmDO);
-      tc::mbar_expect_tx(kv_bar, 4 * AB_TILE);
-      for (int g = 0; g < 2; ++g) {
-        const int j0 = unit.tile * 128 + 64 * g;
-        att_load_tile(sK + g * AB_TILE, &tmKV, kv_bar, E + unit.h * ATT_DH, unit.b, j0);
-        att_load_tile(sV + g * AB_TILE, &tmKV, kv_bar, 2 * E + unit.h * ATT_DH, unit.b, j0);
-      }
-      for (int qb = 0; qb < nqb; ++qb) {
-        tc::mbar_wait_suspend(&empty[ring.stage], ring.phase ^ 1);
-        uint8_t* dst = sRing + ring.stage * 2 * AB_TILE;
-        tc::mbar_expect_tx(&full[ring.stage], 2 * AB_TILE);
-        att_load_tile(dst, &tmQ, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
-        att_load_tile(dst + AB_TILE, &tmDO, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
-        ring.advance();
+      tc::tma_prefetch_desc(&tmDKV);
+      // K and V of unit u, the CTA's j-th, into buffer j & 1 once the stores of tile j - 2 have read it
+      auto load_kv = [&](int u, int j) {
+        const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+        uint8_t* kv = smem + (j & 1) * AB_DKV_KV;
+        tc::mbar_wait_suspend(&kv_empty[j & 1], ((j >> 1) & 1) ^ 1);
+        tc::mbar_expect_tx(&kv_full[j & 1], 4 * AB_TILE);
+        for (int g = 0; g < 2; ++g) {
+          const int j0 = unit.tile * 128 + 64 * g;
+          att_load_tile(kv + g * AB_TILE, &tmKV, &kv_full[j & 1], E + unit.h * ATT_DH, unit.b, j0);
+          att_load_tile(kv + (2 + g) * AB_TILE, &tmKV, &kv_full[j & 1], 2 * E + unit.h * ATT_DH, unit.b, j0);
+        }
+      };
+      load_kv(blockIdx.x, 0);
+      // the next tile's K/V go in after the Q/dO of block claim_at, so that the wait for the buffer (released under the
+      // current tile's first block) leaves the consumers a block in hand; never before block 0, whose MMAs release it
+      const int claim_at = min(1, nqb - 1);
+      for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
+        const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+        for (int qb = 0; qb < nqb; ++qb) {
+          tc::mbar_wait_suspend(&empty[ring.stage], ring.phase ^ 1);
+          uint8_t* dst = sRing + ring.stage * 2 * AB_TILE;
+          tc::mbar_expect_tx(&full[ring.stage], 2 * AB_TILE);
+          att_load_tile(dst, &tmQ, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
+          att_load_tile(dst + AB_TILE, &tmDO, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
+          ring.advance();
+          if (qb == claim_at && u + static_cast<int>(gridDim.x) < n_units) load_kv(u + gridDim.x, it + 1);
+        }
       }
     } else if (pt >= 64) {
       const int r = pt - 64;
-      for (int qb = 0; qb < nqb; ++qb) {
-        const int i = qb * AB_ROWS + r;
-        const bool valid = i < p.T;
-        const float l2 = valid ? p.lse[static_cast<size_t>(unit.bh) * p.T + i] * 1.4426950408889634f : INFINITY;
-        const float dl = valid ? ab_delta(p, unit.b, unit.h, i) : 0.f;
-        tc::mbar_wait_suspend(&empty[ring.stage], ring.phase ^ 1);
-        sStat[ring.stage * 2 * AB_ROWS + r] = l2;
-        sStat[ring.stage * 2 * AB_ROWS + AB_ROWS + r] = dl;
-        tc::mbar_arrive(&full[ring.stage]);
-        ring.advance();
+      for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+        const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+        for (int qb = 0; qb < nqb; ++qb) {
+          const int i = qb * AB_ROWS + r;
+          const bool valid = i < p.T;
+          const float l2 = valid ? p.lse[static_cast<size_t>(unit.bh) * p.T + i] * 1.4426950408889634f : INFINITY;
+          const float dl = valid ? ab_delta(p, unit.b, unit.h, i) : 0.f;
+          tc::mbar_wait_suspend(&empty[ring.stage], ring.phase ^ 1);
+          sStat[ring.stage * 2 * AB_ROWS + r] = l2;
+          sStat[ring.stage * 2 * AB_ROWS + AB_ROWS + r] = dl;
+          tc::mbar_arrive(&full[ring.stage]);
+          ring.advance();
+        }
       }
     }
     return;
@@ -426,83 +474,105 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   tc::setmaxnreg_inc<232>();
   const int g = warp >> 2, wq = warp & 3;
   const int tid = threadIdx.x & 127;
-  const uint32_t k_tile = tc::smem_u32(sK + g * AB_TILE), v_tile = tc::smem_u32(sV + g * AB_TILE);
   const float dscale = p.drop_thr > 0 ? drop_scale(p.drop_thr) : 1.0f;
-  const int key_a = unit.tile * 128 + 64 * g + 16 * wq + (lane >> 2);   // this lane's keys: key_a, key_a + 8
-  const uint32_t drow_base = static_cast<uint32_t>(unit.bh) * p.T;
-  tc::mbar_wait(kv_bar, 0);
 
-  // The first MMAs write dk / dv (scale-d = 0), so nothing but wgmma defines them until the loop has drained.
+  // The first MMAs of a tile write dk / dv (scale-d = 0), so nothing but wgmma defines them until its loop has drained.
   float dk[64], dv[64];
   AttRing<AB_DKV_STAGES> ring;
   bool timed_out = false;
-  for (int qb = 0; qb < nqb; ++qb) {
-    if (!tc::mbar_wait_bounded(&full[ring.stage], ring.phase)) { timed_out = true; break; }
-    const uint32_t q_s = tc::smem_u32(sRing + ring.stage * 2 * AB_TILE);
-    const uint32_t d_s = q_s + AB_TILE;
-    const uint32_t k_s = att_opaque(k_tile), v_s = att_opaque(v_tile);
-    const float* st_lse = sStat + ring.stage * 2 * AB_ROWS;
-    const float* st_dl = st_lse + AB_ROWS;
-    float s[32], dp[32];
-    tc::wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) att_mma_n64(s, att_desc_k(k_s, kk), att_desc_k(q_s, kk), kk);
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) att_mma_n64(dp, att_desc_k(v_s, kk), att_desc_k(d_s, kk), kk);
-    tc::wgmma_commit();
-    tc::wgmma_wait<0>();
-    tc::wgmma_fence_regs(s);
-    tc::wgmma_fence_regs(dp);
+  for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
+    const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+    uint8_t* k_buf = smem + (it & 1) * AB_DKV_KV + g * AB_TILE;
+    uint8_t* v_buf = k_buf + 2 * AB_TILE;
+    const uint32_t k_tile = tc::smem_u32(k_buf), v_tile = tc::smem_u32(v_buf);
+    const int key_a = unit.tile * 128 + 64 * g + 16 * wq + (lane >> 2);   // this lane's keys: key_a, key_a + 8
+    const uint32_t drow_base = static_cast<uint32_t>(unit.bh) * p.T;
+    if (!tc::mbar_wait_bounded(&kv_full[it & 1], (it >> 1) & 1)) { timed_out = true; break; }
 
-    // element 4 j + e is (key key_a + 8 (e >> 1), query row qb * 64 + 8 j + 2 (lane & 3) + (e & 1)).  Per 16 query rows
-    // kk: P^T . mask -> ap, dS^T -> as, then dV += ap dO and dK += as Q for those rows, so the MMAs of one slice run while
-    // the next is computed and the A fragments take the registers that S^T and dP^T free.
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t ap[4], as[4];
-#pragma unroll
-      for (int jj = 0; jj < 2; ++jj)
-#pragma unroll
-        for (int e = 0; e < 4; e += 2) {
-          const int j = 2 * kk + jj;
-          float pm[2], ds[2];
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int ci = 8 * j + 2 * (lane & 3) + c;
-            const int i = qb * AB_ROWS + ci;
-            const float pr = fast_ex2(fmaf(s[4 * j + e + c], p.scale_log2, -st_lse[ci]));
-            const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow_base + i, key_a + 8 * (e >> 1), p.drop_thr) ? dscale : 0.f) : 1.f;
-            ds[c] = pr * fmaf(mk, dp[4 * j + e + c], -st_dl[ci]) * p.scale;
-            pm[c] = pr * mk;
-          }
-          ap[2 * jj + (e >> 1)] = tc::pack_bf16x2(pm[0], pm[1]);
-          as[2 * jj + (e >> 1)] = tc::pack_bf16x2(ds[0], ds[1]);
-        }
+    for (int qb = 0; qb < nqb; ++qb) {
+      if (!tc::mbar_wait_bounded(&full[ring.stage], ring.phase)) { timed_out = true; break; }
+      const uint32_t q_s = tc::smem_u32(sRing + ring.stage * 2 * AB_TILE);
+      const uint32_t d_s = q_s + AB_TILE;
+      const uint32_t k_s = att_opaque(k_tile), v_s = att_opaque(v_tile);
+      const float* st_lse = sStat + ring.stage * 2 * AB_ROWS;
+      const float* st_dl = st_lse + AB_ROWS;
+      float s[32], dp[32];
       tc::wgmma_fence();
-      tc::wgmma_m64n128k16_rs(dv, ap, att_desc_mn(d_s, kk), qb > 0 || kk > 0);
-      tc::wgmma_m64n128k16_rs(dk, as, att_desc_mn(q_s, kk), qb > 0 || kk > 0);
-    }
-    tc::wgmma_commit();
-    tc::wgmma_wait<0>();
-    if (tid == 0) tc::mbar_arrive(&empty[ring.stage]);
-    ring.advance();
-  }
-  tc::wgmma_fence_regs(dk);
-  tc::wgmma_fence_regs(dv);
-
-  // dk[4 j + 2 r + c] is key key_a + 8 r, column 8 j + 2 (lane & 3) + c
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int key = key_a + 8 * r;
-    if (key < p.sep) {
-      __nv_bfloat16* grow = p.dqkv + att_tok(key, unit.b, p.T, p.B, p.batch_major) * p.ld_dqkv + unit.h * ATT_DH;
+      for (int kk = 0; kk < 8; ++kk) att_mma_n64(s, att_desc_k(k_s, kk), att_desc_k(q_s, kk), kk);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) att_mma_n64(dp, att_desc_k(v_s, kk), att_desc_k(d_s, kk), kk);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      tc::wgmma_fence_regs(s);
+      tc::wgmma_fence_regs(dp);
+      // the previous tile's dK/dV stores have read its buffer by now (or shortly): release it to the producer
+      if (qb == 0 && it > 0 && tid == 0) {
+        tc::bulk_wait_read<0>();
+        tc::mbar_arrive(&kv_empty[(it - 1) & 1]);
+      }
+
+      // element 4 j + e is (key key_a + 8 (e >> 1), query row qb * 64 + 8 j + 2 (lane & 3) + (e & 1)).  Per 16 query
+      // rows kk: P^T . mask -> ap, dS^T -> as, then dV += ap dO and dK += as Q for those rows, so the MMAs of one slice
+      // run while the next is computed and the A fragments take the registers that S^T and dP^T free.
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        uint32_t ap[4], as[4];
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+          for (int e = 0; e < 4; e += 2) {
+            const int j = 2 * kk + jj;
+            float pm[2], ds[2];
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              const int ci = 8 * j + 2 * (lane & 3) + c;
+              const int i = qb * AB_ROWS + ci;
+              const float pr = fast_ex2(fmaf(s[4 * j + e + c], p.scale_log2, -st_lse[ci]));
+              const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow_base + i, key_a + 8 * (e >> 1), p.drop_thr) ? dscale : 0.f) : 1.f;
+              ds[c] = pr * fmaf(mk, dp[4 * j + e + c], -st_dl[ci]) * p.scale;
+              pm[c] = pr * mk;
+            }
+            ap[2 * jj + (e >> 1)] = tc::pack_bf16x2(pm[0], pm[1]);
+            as[2 * jj + (e >> 1)] = tc::pack_bf16x2(ds[0], ds[1]);
+          }
+        tc::wgmma_fence();
+        tc::wgmma_m64n128k16_rs(dv, ap, att_desc_mn(d_s, kk), qb > 0 || kk > 0);
+        tc::wgmma_m64n128k16_rs(dk, as, att_desc_mn(q_s, kk), qb > 0 || kk > 0);
+      }
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      if (tid == 0) tc::mbar_arrive(&empty[ring.stage]);
+      ring.advance();
+    }
+    tc::wgmma_fence_regs(dk);
+    tc::wgmma_fence_regs(dv);
+    if (timed_out) break;
+
+    // The warpgroup's K and V tiles are free (its last MMAs that read them have completed): dK and dV go there in the
+    // layout the TMA reads (128-byte swizzle: the 16-byte chunk index of a 128-byte row is XORed with row & 7), then
+    // leave by TMA stores that drop the keys >= sep.  dk[4 j + 2 r + c] is key row 16 wq + (lane >> 2) + 8 r of the
+    // warpgroup's 64, column 8 j + 2 (lane & 3) + c.
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int lr = 16 * wq + (lane >> 2) + 8 * r;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        att_st2(grow + E, j, lane, dk[4 * j + 2 * r], dk[4 * j + 2 * r + 1]);
-        att_st2(grow + 2 * E, j, lane, dv[4 * j + 2 * r], dv[4 * j + 2 * r + 1]);
+        const int off = att_tile_off2(lr, j, lane);
+        *reinterpret_cast<uint32_t*>(k_buf + off) = tc::pack_bf16x2(dk[4 * j + 2 * r], dk[4 * j + 2 * r + 1]);
+        *reinterpret_cast<uint32_t*>(v_buf + off) = tc::pack_bf16x2(dv[4 * j + 2 * r], dv[4 * j + 2 * r + 1]);
       }
     }
+    tc::fence_proxy_async_smem();
+    tc::named_bar_sync(1 + g, 128);
+    const int j0 = unit.tile * 128 + 64 * g;
+    if (tid == 0 && j0 < p.sep) {
+      att_store_tile(&tmDKV, k_buf, E + unit.h * ATT_DH, unit.b, j0);
+      att_store_tile(&tmDKV, v_buf, 2 * E + unit.h * ATT_DH, unit.b, j0);
+      tc::bulk_commit();
+    }
   }
+  if (tid == 0) tc::bulk_wait<0>();
   if (timed_out) asm volatile("trap;");
 }
 
@@ -523,12 +593,10 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
   p.batch_major = d->batch_major;
   const int E = d->H * ATT_DH;
-  CUtensorMap tmQ, tmKV, tmDO;
+  CUtensorMap tmQ, tmKV, tmDO, tmDQ;
   if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
   if (int rc = att_tensor_map(&tmDO, d->dout, E, d->ld_dout, d->T, d->B, d->T, d->batch_major)) return rc;
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set))
-    PFN_CUDA_OK(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_DKV_SMEM));
+  if (int rc = att_tensor_map(&tmDQ, d->dqkv, 3 * E, d->ld_dqkv, d->T, d->B, d->T, d->batch_major)) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!d->delta_token_major) {
     const long long rows = static_cast<long long>(d->T) * d->B;
@@ -540,13 +608,16 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
   }
   p.n_tiles = (d->T + 127) / 128;
   if (int rc = att_launch_persistent<attn_bwd_dq_kernel>("attention_bwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
-                                                         AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, p))
+                                                         AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, tmDQ, p))
     return rc;
   if (d->sep > 0) {
+    // dK/dV of the train keys, stored through a map whose t extent of sep drops the keys >= sep of the last tile
+    CUtensorMap tmDKV;
+    if (int rc = att_tensor_map(&tmDKV, d->dqkv, 3 * E, d->ld_dqkv, d->T, d->B, d->sep, d->batch_major)) return rc;
     p.n_tiles = (d->sep + 127) / 128;
-    const long long grid = static_cast<long long>(p.n_tiles) * d->B * d->H;
-    attn_bwd_dkv_kernel<<<static_cast<unsigned>(grid), AB_THREADS, AB_DKV_SMEM, s>>>(tmQ, tmKV, tmDO, p);
-    PFN_LAUNCH_OK();
+    if (int rc = att_launch_persistent<attn_bwd_dkv_kernel>("attention_bwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                            AB_THREADS, AB_DKV_SMEM, s, tmQ, tmKV, tmDO, tmDKV, p))
+      return rc;
   }
   return 0;
 }

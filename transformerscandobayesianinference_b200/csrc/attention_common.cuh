@@ -54,6 +54,18 @@ __device__ __forceinline__ void att_load_tile(uint8_t* dst, const CUtensorMap* m
   tc::tma_load_3d(dst + 8192, m, bar, col0 + 64, b, t0);
 }
 
+// TMA store of a 16 KB tile to rows [t0, t0 + 64) of one head (columns col0 .. col0 + 127); rows at t >= the map's t
+// extent are not written.  The caller commits the bulk group.
+__device__ __forceinline__ void att_store_tile(const CUtensorMap* m, const uint8_t* src, int col0, int b, int t0) {
+  tc::tma_store_3d(m, src, col0, b, t0);
+  tc::tma_store_3d(m, src + 8192, col0 + 64, b, t0);
+}
+// Byte offset in a 16 KB tile of the columns 8 j + 2 (lane & 3) + {0, 1} of row `row` (an m16n8 accumulator pair): the
+// 128-byte swizzle XORs the 16-byte chunk index within a 128-byte row with row & 7
+__device__ __forceinline__ int att_tile_off2(int row, int j, int lane) {
+  return (j >> 3) * 8192 + row * 128 + (((j & 7) ^ (row & 7)) << 4) + 4 * (lane & 3);
+}
+
 // A work unit: one 128-row tile of one (batch, head).  Unit u is tile u % n_tiles of (batch, head) bh = u / n_tiles, so
 // the tiles of one (batch, head) are neighbours and the CTAs that run them at the same time share its K/V in L2.
 struct AttUnit {
@@ -189,9 +201,6 @@ __device__ __forceinline__ bool att_key_loop(const AttPipe<STAGES>& pp, AttRing<
 // the 32 columns of a 128-wide head row that lane `lane` owns in an m16n8 accumulator row: 8 j + 2 (lane & 3) + {0, 1}
 __device__ __forceinline__ float2 att_ld2(const __nv_bfloat16* row, int j, int lane) {
   return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + 8 * j + 2 * (lane & 3)));
-}
-__device__ __forceinline__ void att_st2(__nv_bfloat16* row, int j, int lane, float x, float y) {
-  *reinterpret_cast<uint32_t*>(row + 8 * j + 2 * (lane & 3)) = tc::pack_bf16x2(x, y);
 }
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);

@@ -212,16 +212,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       const int rr = 16 * wq + (lane >> 2) + 8 * r;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        const uint32_t off = (j >> 3) * 8192 + rr * 128 + (((j & 7) ^ (rr & 7)) << 4) + (lane & 3) * 4;
-        *reinterpret_cast<uint32_t*>(stg + off) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+        *reinterpret_cast<uint32_t*>(stg + att_tile_off2(rr, j, lane)) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
       }
       if (!kCtx && !kRagged && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
     }
     tc::fence_proxy_async_smem();
     tc::named_bar_sync(1 + g, 128);
     if (tid == 0 && t0 < p.T) {
-      tc::tma_store_3d(&tmO, stg, unit.h * ATT_DH, unit.b, t0);
-      tc::tma_store_3d(&tmO, stg + 8192, unit.h * ATT_DH + 64, unit.b, t0);
+      att_store_tile(&tmO, stg, unit.h * ATT_DH, unit.b, t0);
       tc::bulk_commit();
     }
   }

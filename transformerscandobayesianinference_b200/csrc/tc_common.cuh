@@ -126,6 +126,15 @@ template <int N>
 __device__ __forceinline__ void bulk_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
+// 16-byte global -> shared copy through L2 (cp.async), its commit group, and the wait for all but the newest N groups
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
 // generic-proxy shared-memory writes become visible to the async proxy (TMA) that reads them next
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
