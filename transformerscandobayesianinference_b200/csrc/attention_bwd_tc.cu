@@ -29,6 +29,12 @@
 // (columns, batch, time) whose two row strides encode the token order; the TMA zero-fills rows past T (Q, dO) and keys
 // past sep (K, V).  One 128-byte-swizzled tile serves as a K-major operand (S = Q K^T) and as an MN-major one
 // (dQ += dS K), so nothing is transposed.  No atomics on dQKV: every element is written exactly once.
+//
+// Ragged datasets (kRagged, pfn_attention_ragged_train_bwd_tc): dataset b has its own separator s_b = n_keys[b] <= sep.
+// In the dQ kernel a unit runs ceil(s_b / 64) key blocks, masks keys >= s_b in its last one, and rows i >= s_b have their
+// diagonal key.  In the dK/dV kernel the key tiles at or past s_b have no work and are skipped by every role of the CTA
+// alike; a warpgroup whose 64 keys straddle s_b stores its rows < s_b directly instead of by the TMA, whose map clips
+// at sep only.  The keys [s_b, sep) are real rows of qkv, loaded and masked like the keys past sep.
 #include "attention_common.cuh"
 
 namespace pfn {
@@ -70,7 +76,14 @@ struct AttnBwdParams {
   uint32_t drop_seed; int drop_thr;   // dropout on the attention probabilities (thr 0 = off), csrc/dropout.cuh
   int n_tiles;           // 128-row tiles per (batch, head): query rows (dQ kernel) or train keys (dK/dV kernel)
   int batch_major;
+  const int* n_keys;     // [B] per-dataset separators (kRagged only)
 };
+
+// the separator of dataset b: sep, or n_keys[b] clamped to [0, sep] in the ragged kernels
+template <bool kRagged>
+__device__ __forceinline__ int ab_sep(const AttnBwdParams& p, int b) {
+  return kRagged ? min(max(__ldg(p.n_keys + b), 0), p.sep) : p.sep;
+}
 
 __device__ __forceinline__ float ab_delta(const AttnBwdParams& p, int b, int h, int i) {
   return p.delta_tm ? p.delta[att_tok(i, b, p.T, p.B, 0) * p.H + h] : p.delta[(static_cast<size_t>(b) * p.H + h) * p.T + i];
@@ -117,6 +130,7 @@ attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ out, int ld_out, const _
 // =====================================================================================================================
 // Kernel 1: dQ (+ dK, dV of the query rows' own keys)
 // =====================================================================================================================
+template <bool kRagged>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                    const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDQ,
@@ -165,7 +179,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         const int sb = it & 1;
         float* st = sStat + sb * 3 * 128;
         // the warp's diagonal rows of the tile: row k is r0 + 3 k, k < n_rows, in slot k % AB_DQ_ROW_SLOTS
-        const int r_lo = max(0, p.sep - unit.tile * 128), r_hi = min(128, p.T - unit.tile * 128);
+        const int r_lo = max(0, ab_sep<kRagged>(p, unit.b) - unit.tile * 128), r_hi = min(128, p.T - unit.tile * 128);
         const int r0 = r_lo + (pw - r_lo % AB_DQ_STAT_WARPS + AB_DQ_STAT_WARPS) % AB_DQ_STAT_WARPS;
         const int n_rows = r0 < r_hi ? (r_hi - r0 + AB_DQ_STAT_WARPS - 1) / AB_DQ_STAT_WARPS : 0;
         // the lane's half and columns come from an opaque lane index in every row, so that the address arithmetic built on
@@ -237,7 +251,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       tc::tma_prefetch_desc(&tmKV);
       tc::tma_prefetch_desc(&tmDO);
       tc::tma_prefetch_desc(&tmDQ);
-      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, [&](const AttUnit&) { return nblk; }, E, 2 * E, 4 * AB_TILE,
+      auto nblk_of = [&](const AttUnit& unit) { return kRagged ? (ab_sep<true>(p, unit.b) + AB_ROWS - 1) / AB_ROWS : nblk; };
+      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk_of, E, 2 * E, 4 * AB_TILE,
                       [&](const AttUnit& unit) {
         for (int g = 0; g < 2; ++g) {
           const int t0 = unit.tile * 128 + 64 * g;
@@ -260,6 +275,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
     const AttUnit unit = att_unit(u, p.n_tiles, p.H);
     const int i0 = unit.tile * 128 + 64 * g + 16 * wq + (lane >> 2);    // this lane's rows: i0, i0 + 8
+    const int sep = ab_sep<kRagged>(p, unit.b);
+    const int unit_nblk = kRagged ? (sep + AB_ROWS - 1) / AB_ROWS : nblk;
 
     // per-row statistics of this lane's two rows (and ds_ii of its diagonal keys), prepared by the statistics warps
     const int sb = it & 1;
@@ -307,7 +324,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       for (int e = 0; e < 32; ++e) {
         const int r = (e >> 1) & 1;
         const int key = key0 + 8 * (e >> 2) + (e & 1);
-        const float pr = key < p.sep ? fast_ex2(fmaf(s[e], p.scale_log2, -lse2[r])) : 0.f;
+        const float pr = key < sep ? fast_ex2(fmaf(s[e], p.scale_log2, -lse2[r])) : 0.f;
         const float mk = p.drop_thr > 0 ? (drop_keep(p.drop_seed, drow[r], key, p.drop_thr) ? dscale : 0.f) : 1.f;
         s[e] = pr * fmaf(mk, dp[e], -dl[r]) * p.scale;
       }
@@ -323,14 +340,14 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int i = i0 + 8 * r;
-        const bool diag = i < p.T && i >= p.sep;
+        const bool diag = i < p.T && i >= sep;
         const __nv_bfloat16* krow = p.qkv + att_tok(diag ? i : 0, unit.b, p.T, p.B, p.batch_major) * p.ld_qkv + E + unit.h * ATT_DH;
 #pragma unroll
         for (int j = 0; j < 16; ++j)
           kd[r][j] = diag ? *reinterpret_cast<const uint32_t*>(krow + 8 * j + 2 * (lane & 3)) : 0u;
       }
     };
-    if (att_key_loop(pp, ring, it, nblk, issue_sdp, issue_dq, [&] { tc::wgmma_fence_regs(s); tc::wgmma_fence_regs(dp); },
+    if (att_key_loop(pp, ring, it, unit_nblk, issue_sdp, issue_dq, [&] { tc::wgmma_fence_regs(s); tc::wgmma_fence_regs(dp); },
                      [&] { tc::wgmma_fence_regs(dq); }, compute_ds, pack_ds, load_kd)) {
       timed_out = true;
       break;
@@ -344,11 +361,11 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int r = 0; r < 2; ++r) {
       const int i = i0 + 8 * r;
       if (i < p.T) {
-        const bool diag = i >= p.sep;
+        const bool diag = i >= sep;
         const int lr = 16 * wq + (lane >> 2) + 8 * r;              // row i in the warpgroup's 64
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          float x = nblk > 0 ? dq[4 * j + 2 * r] : 0.f, y = nblk > 0 ? dq[4 * j + 2 * r + 1] : 0.f;
+          float x = unit_nblk > 0 ? dq[4 * j + 2 * r] : 0.f, y = unit_nblk > 0 ? dq[4 * j + 2 * r + 1] : 0.f;
           if (diag) {
             const float2 k = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&kd[r][j]));
             x = fmaf(dsd[r], k.x, x);
@@ -382,6 +399,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // =====================================================================================================================
 // Kernel 2: dK, dV of the train keys
 // =====================================================================================================================
+template <bool kRagged>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                     const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDKV,
@@ -399,6 +417,25 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int E = p.H * ATT_DH;
   const int nqb = (p.T + AB_ROWS - 1) / AB_ROWS;
   const int n_units = p.n_tiles * p.B * p.H;
+  // Ragged: a live unit costs the same nqb query blocks whatever its dataset, so what balances the CTAs is how many live
+  // units each meets.  With the key tile fastest, a CTA's stride through the list meets only the tiles u % n_tiles takes
+  // on its residues, and the high tiles are the ones most often dead.  The tiles of every odd (batch, head) therefore run
+  // in reverse order, so that a CTA meets tile t and tile n_tiles - 1 - t alike; the tiles of one (batch, head) stay
+  // neighbours, so the CTAs that run them at the same time still share its Q and dO in L2.
+  auto unit_of = [&](int u) {
+    AttUnit unit = att_unit(u, p.n_tiles, p.H);
+    if (kRagged && (unit.bh & 1)) unit.tile = p.n_tiles - 1 - unit.tile;
+    return unit;
+  };
+  // the CTA's first unit at or after u that has keys below its dataset's separator (every unit when uniform)
+  auto live = [&](int u) {
+    if (kRagged)
+      for (; u < n_units; u += gridDim.x) {
+        const AttUnit unit = unit_of(u);
+        if (unit.tile * 128 < ab_sep<true>(p, unit.b)) break;
+      }
+    return u;
+  };
   if (threadIdx.x == 0) {
     for (int s = 0; s < AB_DKV_STAGES; ++s) {
       tc::mbar_init(&full[s], 1 + AB_ROWS);              // the TMA thread's expect_tx + one arrival per statistics row
@@ -424,7 +461,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       tc::tma_prefetch_desc(&tmDKV);
       // K and V of unit u, the CTA's j-th, into buffer j & 1 once the stores of tile j - 2 have read it
       auto load_kv = [&](int u, int j) {
-        const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+        const AttUnit unit = unit_of(u);
         uint8_t* kv = smem + (j & 1) * AB_DKV_KV;
         tc::mbar_wait_suspend(&kv_empty[j & 1], ((j >> 1) & 1) ^ 1);
         tc::mbar_expect_tx(&kv_full[j & 1], 4 * AB_TILE);
@@ -434,12 +471,14 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
           att_load_tile(kv + (2 + g) * AB_TILE, &tmKV, &kv_full[j & 1], 2 * E + unit.h * ATT_DH, unit.b, j0);
         }
       };
-      load_kv(blockIdx.x, 0);
+      const int first = live(blockIdx.x);
+      if (!kRagged || first < n_units) load_kv(first, 0);     // a uniform grid has a unit for every CTA
       // the next tile's K/V go in after the Q/dO of block claim_at, so that the wait for the buffer (released under the
       // current tile's first block) leaves the consumers a block in hand; never before block 0, whose MMAs release it
       const int claim_at = min(1, nqb - 1);
-      for (int u = blockIdx.x, it = 0; u < n_units; u += gridDim.x, ++it) {
-        const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+      for (int u = first, it = 0; u < n_units; ++it) {
+        const AttUnit unit = unit_of(u);
+        const int next = live(u + gridDim.x);
         for (int qb = 0; qb < nqb; ++qb) {
           tc::mbar_wait_suspend(&empty[ring.stage], ring.phase ^ 1);
           uint8_t* dst = sRing + ring.stage * 2 * AB_TILE;
@@ -447,13 +486,14 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
           att_load_tile(dst, &tmQ, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
           att_load_tile(dst + AB_TILE, &tmDO, &full[ring.stage], unit.h * ATT_DH, unit.b, qb * AB_ROWS);
           ring.advance();
-          if (qb == claim_at && u + static_cast<int>(gridDim.x) < n_units) load_kv(u + gridDim.x, it + 1);
+          if (qb == claim_at && next < n_units) load_kv(next, it + 1);
         }
+        u = next;
       }
     } else if (pt >= 64) {
       const int r = pt - 64;
-      for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+      for (int u = live(blockIdx.x); u < n_units; u = live(u + gridDim.x)) {
+        const AttUnit unit = unit_of(u);
         for (int qb = 0; qb < nqb; ++qb) {
           const int i = qb * AB_ROWS + r;
           const bool valid = i < p.T;
@@ -480,17 +520,29 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   float dk[64], dv[64];
   AttRing<AB_DKV_STAGES> ring;
   bool timed_out = false;
-  for (int u = blockIdx.x, it = 0; u < n_units && !timed_out; u += gridDim.x, ++it) {
-    const AttUnit unit = att_unit(u, p.n_tiles, p.H);
+  for (int u = live(blockIdx.x), it = 0; u < n_units && !timed_out; u = live(u + gridDim.x), ++it) {
+    const AttUnit unit = unit_of(u);
     uint8_t* k_buf = smem + (it & 1) * AB_DKV_KV + g * AB_TILE;
     uint8_t* v_buf = k_buf + 2 * AB_TILE;
     const uint32_t k_tile = tc::smem_u32(k_buf), v_tile = tc::smem_u32(v_buf);
     const int key_a = unit.tile * 128 + 64 * g + 16 * wq + (lane >> 2);   // this lane's keys: key_a, key_a + 8
     const uint32_t drow_base = static_cast<uint32_t>(unit.bh) * p.T;
     if (!tc::mbar_wait_bounded(&kv_full[it & 1], (it >> 1) & 1)) { timed_out = true; break; }
+    // ragged: a warpgroup whose 64 keys all lie at or past the separator has nothing to store; it only passes the
+    // query blocks on (its arrivals keep the barrier counts of the uniform kernel)
+    const bool idle = kRagged && unit.tile * 128 + 64 * g >= ab_sep<kRagged>(p, unit.b);
 
     for (int qb = 0; qb < nqb; ++qb) {
       if (!tc::mbar_wait_bounded(&full[ring.stage], ring.phase)) { timed_out = true; break; }
+      if (idle) {
+        if (qb == 0 && it > 0 && tid == 0) {
+          tc::bulk_wait_read<0>();
+          tc::mbar_arrive(&kv_empty[(it - 1) & 1]);
+        }
+        if (tid == 0) tc::mbar_arrive(&empty[ring.stage]);
+        ring.advance();
+        continue;
+      }
       const uint32_t q_s = tc::smem_u32(sRing + ring.stage * 2 * AB_TILE);
       const uint32_t d_s = q_s + AB_TILE;
       const uint32_t k_s = att_opaque(k_tile), v_s = att_opaque(v_tile);
@@ -553,6 +605,28 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     // layout the TMA reads (128-byte swizzle: the 16-byte chunk index of a 128-byte row is XORed with row & 7), then
     // leave by TMA stores that drop the keys >= sep.  dk[4 j + 2 r + c] is key row 16 wq + (lane >> 2) + 8 r of the
     // warpgroup's 64, column 8 j + 2 (lane & 3) + c.
+    const int j0 = unit.tile * 128 + 64 * g;
+    if (kRagged) {
+      const int sep = ab_sep<true>(p, unit.b);
+      if (j0 + AB_ROWS > sep) {
+        // the keys >= sep of this dataset are its own rows (their dK, dV came from the dQ kernel): only the keys < sep
+        // are stored, one accumulator pair at a time
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int key = j0 + 16 * wq + (lane >> 2) + 8 * r;
+          if (key < sep) {
+            __nv_bfloat16* row = p.dqkv + att_tok(key, unit.b, p.T, p.B, p.batch_major) * p.ld_dqkv + E + unit.h * ATT_DH +
+                                 2 * (lane & 3);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              *reinterpret_cast<uint32_t*>(row + 8 * j) = tc::pack_bf16x2(dk[4 * j + 2 * r], dk[4 * j + 2 * r + 1]);
+              *reinterpret_cast<uint32_t*>(row + E + 8 * j) = tc::pack_bf16x2(dv[4 * j + 2 * r], dv[4 * j + 2 * r + 1]);
+            }
+          }
+        }
+        continue;
+      }
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int lr = 16 * wq + (lane >> 2) + 8 * r;
@@ -565,7 +639,6 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     }
     tc::fence_proxy_async_smem();
     tc::named_bar_sync(1 + g, 128);
-    const int j0 = unit.tile * 128 + 64 * g;
     if (tid == 0 && j0 < p.sep) {
       att_store_tile(&tmDKV, k_buf, E + unit.h * ATT_DH, unit.b, j0);
       att_store_tile(&tmDKV, v_buf, 2 * E + unit.h * ATT_DH, unit.b, j0);
@@ -576,13 +649,11 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   if (timed_out) asm volatile("trap;");
 }
 
-}  // namespace pfn
-
-using namespace pfn;
-
-extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
-  if (int rc = check_tc_attn(d, true, "attention_bwd_tc")) return rc;
-  PFN_CHECK_ARG(!(d->delta_token_major && d->batch_major), "attention_bwd_tc: a token-major delta implies the reference token order");
+// The backward over d with separator n_keys[b] for dataset b when kRagged
+template <bool kRagged>
+static int launch_attn_bwd_tc(const pfn_attn_desc* d, const int* n_keys, cudaStream_t s, const char* who) {
+  if (int rc = check_tc_attn(d, true, who)) return rc;
+  PFN_CHECK_ARG(!(d->delta_token_major && d->batch_major), "%s: a token-major delta implies the reference token order", who);
   AttnBwdParams p;
   p.T = d->T; p.B = d->B; p.H = d->H; p.sep = d->sep;
   p.scale = d->scale; p.scale_log2 = d->scale * 1.4426950408889634f;
@@ -592,12 +663,12 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
   p.lse = d->lse; p.delta = d->delta; p.dq_colsum = d->dq_colsum; p.delta_tm = d->delta_token_major;
   p.drop_seed = d->drop_seed; p.drop_thr = d->drop_thr;
   p.batch_major = d->batch_major;
+  p.n_keys = n_keys;
   const int E = d->H * ATT_DH;
   CUtensorMap tmQ, tmKV, tmDO, tmDQ;
   if (int rc = att_qkv_maps(d, &tmQ, &tmKV)) return rc;
   if (int rc = att_tensor_map(&tmDO, d->dout, E, d->ld_dout, d->T, d->B, d->T, d->batch_major)) return rc;
   if (int rc = att_tensor_map(&tmDQ, d->dqkv, 3 * E, d->ld_dqkv, d->T, d->B, d->T, d->batch_major)) return rc;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!d->delta_token_major) {
     const long long rows = static_cast<long long>(d->T) * d->B;
     long long grid = (rows + 7) / 8;
@@ -607,17 +678,30 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
     PFN_LAUNCH_OK();
   }
   p.n_tiles = (d->T + 127) / 128;
-  if (int rc = att_launch_persistent<attn_bwd_dq_kernel>("attention_bwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
-                                                         AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, tmDQ, p))
+  if (int rc = att_launch_persistent<attn_bwd_dq_kernel<kRagged>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                                  AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, tmDQ, p))
     return rc;
   if (d->sep > 0) {
     // dK/dV of the train keys, stored through a map whose t extent of sep drops the keys >= sep of the last tile
     CUtensorMap tmDKV;
     if (int rc = att_tensor_map(&tmDKV, d->dqkv, 3 * E, d->ld_dqkv, d->T, d->B, d->sep, d->batch_major)) return rc;
     p.n_tiles = (d->sep + 127) / 128;
-    if (int rc = att_launch_persistent<attn_bwd_dkv_kernel>("attention_bwd_tc", static_cast<long long>(p.n_tiles) * d->B * d->H,
-                                                            AB_THREADS, AB_DKV_SMEM, s, tmQ, tmKV, tmDO, tmDKV, p))
+    if (int rc = att_launch_persistent<attn_bwd_dkv_kernel<kRagged>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                                     AB_THREADS, AB_DKV_SMEM, s, tmQ, tmKV, tmDO, tmDKV, p))
       return rc;
   }
   return 0;
+}
+
+}  // namespace pfn
+
+using namespace pfn;
+
+extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
+  return launch_attn_bwd_tc<false>(d, nullptr, reinterpret_cast<cudaStream_t>(stream), "attention_bwd_tc");
+}
+
+extern "C" int pfn_attention_ragged_train_bwd_tc(const pfn_attn_ragged_train_desc* d, void* stream) {
+  PFN_CHECK_ARG(d != nullptr && d->n_keys != nullptr, "attention_ragged_train_bwd_tc: null descriptor / n_keys");
+  return launch_attn_bwd_tc<true>(&d->a, d->n_keys, reinterpret_cast<cudaStream_t>(stream), "attention_ragged_train_bwd_tc");
 }

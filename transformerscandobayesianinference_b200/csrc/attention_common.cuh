@@ -9,6 +9,7 @@
 #include "dropout.cuh"
 #include "tc_common.cuh"
 #include "../../include/pfn_b200_ragged.h"
+#include "../../include/pfn_b200_ragged_train.h"
 
 namespace pfn {
 

@@ -3,11 +3,12 @@
 // lanes, scores are reduced with warp shuffles, softmax is computed online.  The single_eval_pos mask of
 // reference transformer.py:35-41 is implicit:  keys(i) = [0, sep)  U  {i if i >= sep}.  The forward also serves the
 // context attention (pfn_attention_ctx_fwd_simt): there the sep keys come from the K/V cache and every row has its own key.
-// In the ragged forwards (pfn_attention_ragged_fwd_simt, pfn_attention_ctx_ragged_fwd_simt) dataset b has n_keys[b] keys
-// in place of sep.
+// In the ragged entry points (pfn_attention_ragged_fwd_simt, pfn_attention_ctx_ragged_fwd_simt and the training pair
+// pfn_attention_ragged_train_{fwd,bwd}_simt) dataset b has n_keys[b] keys in place of sep.
 #include "common.cuh"
 #include "dropout.cuh"
 #include "../../include/pfn_b200_ragged.h"
+#include "../../include/pfn_b200_ragged_train.h"
 
 namespace pfn {
 
@@ -87,10 +88,16 @@ attn_fwd_simt_kernel(const pfn_attn_desc d, const SharedKeys sk) {
   }
 }
 
+// the key count of dataset b: sep, or n_keys[b] clamped to [0, sep] in the ragged kernels
+template <bool kRagged>
+__device__ __forceinline__ int simt_sep(const pfn_attn_desc& d, const int* n_keys, int b) {
+  return kRagged ? min(max(__ldg(n_keys + b), 0), d.sep) : d.sep;
+}
+
 // dQ (+ delta, + the diagonal-key contributions that are the ONLY gradient of k_i, v_i for query rows)
-template <typename T, int DPL>
+template <typename T, int DPL, bool kRagged>
 __global__ void __launch_bounds__(256)
-attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta) {
+attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta, const int* __restrict__ n_keys) {
   const int E = d.H * d.dh;
   const long long total = static_cast<long long>(d.B) * d.H * d.T;
   const int lane = threadIdx.x & 31;
@@ -114,9 +121,10 @@ attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta) {
     dl = warp_sum(dl);
     if (lane == 0) delta[static_cast<size_t>(bh) * d.T + i] = dl;
     const float lse = d.lse[static_cast<size_t>(bh) * d.T + i];
-    const int nkeys = d.sep + (i >= d.sep ? 1 : 0);
+    const int sep = simt_sep<kRagged>(d, n_keys, b);
+    const int nkeys = sep + (i >= sep ? 1 : 0);
     for (int jj = 0; jj < nkeys; ++jj) {
-      const int j = jj < d.sep ? jj : i;
+      const int j = jj < sep ? jj : i;
       const T* krow = qkv + (static_cast<size_t>(j) * d.B + b) * d.ld_qkv + E + h * d.dh;
       float k[DPL], v[DPL];
       load_head<T, DPL>(krow, d.dh, lane, k);
@@ -132,7 +140,7 @@ attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta) {
       const float ds = p * (mk * dp - dl) * d.scale;
 #pragma unroll
       for (int c = 0; c < DPL; ++c) dq[c] = fmaf(ds, k[c], dq[c]);
-      if (jj >= d.sep) {
+      if (jj >= sep) {
         float dk[DPL], dv[DPL];
 #pragma unroll
         for (int c = 0; c < DPL; ++c) { dk[c] = ds * q[c]; dv[c] = p * mk * dO[c]; }
@@ -144,10 +152,10 @@ attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta) {
   }
 }
 
-// dK, dV of the train keys j < sep: every row i attends to them.
-template <typename T, int DPL>
+// dK, dV of the train keys j < sep (j < n_keys[b] when ragged): every row i attends to them.
+template <typename T, int DPL, bool kRagged>
 __global__ void __launch_bounds__(256)
-attn_bwd_dkv_simt_kernel(const pfn_attn_desc d, const float* __restrict__ delta) {
+attn_bwd_dkv_simt_kernel(const pfn_attn_desc d, const float* __restrict__ delta, const int* __restrict__ n_keys) {
   const int E = d.H * d.dh;
   const long long total = static_cast<long long>(d.B) * d.H * d.sep;
   const int lane = threadIdx.x & 31;
@@ -159,6 +167,7 @@ attn_bwd_dkv_simt_kernel(const pfn_attn_desc d, const float* __restrict__ delta)
     const int j = static_cast<int>(task % d.sep);
     const int bh = static_cast<int>(task / d.sep);
     const int h = bh % d.H, b = bh / d.H;
+    if (kRagged && j >= simt_sep<true>(d, n_keys, b)) continue;     // a row of b's own: the dQ kernel wrote its dK, dV
     const size_t tokj = static_cast<size_t>(j) * d.B + b;
     float k[DPL], v[DPL], dk[DPL], dv[DPL];
     load_head<T, DPL>(qkv + tokj * d.ld_qkv + E + h * d.dh, d.dh, lane, k);
@@ -215,13 +224,15 @@ static int launch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, co
     PFN_LAUNCH_OK();
     return 0;
   }
-  attn_bwd_dq_simt_kernel<T, DPL><<<static_cast<int>(grid), 256, 0, s>>>(*d, d->delta);
+  if (sk.n_keys) attn_bwd_dq_simt_kernel<T, DPL, true><<<static_cast<int>(grid), 256, 0, s>>>(*d, d->delta, sk.n_keys);
+  else attn_bwd_dq_simt_kernel<T, DPL, false><<<static_cast<int>(grid), 256, 0, s>>>(*d, d->delta, nullptr);
   PFN_LAUNCH_OK();
   if (d->sep > 0) {
     const long long tasks2 = static_cast<long long>(d->B) * d->H * d->sep;
     long long grid2 = (tasks2 + 7) / 8;
     if (grid2 > max_grid) grid2 = max_grid;
-    attn_bwd_dkv_simt_kernel<T, DPL><<<static_cast<int>(grid2), 256, 0, s>>>(*d, d->delta);
+    if (sk.n_keys) attn_bwd_dkv_simt_kernel<T, DPL, true><<<static_cast<int>(grid2), 256, 0, s>>>(*d, d->delta, sk.n_keys);
+    else attn_bwd_dkv_simt_kernel<T, DPL, false><<<static_cast<int>(grid2), 256, 0, s>>>(*d, d->delta, nullptr);
     PFN_LAUNCH_OK();
   }
   return 0;
@@ -336,4 +347,24 @@ extern "C" int pfn_attention_ctx_ragged_fwd_simt(const pfn_attn_ctx_ragged_desc*
   if (int rc = attn_ctx_ragged_as_ctx(d, &c, "attention_ctx_ragged_fwd_simt")) return rc;
   const pfn_attn_desc a = ctx_as_masked(&c);
   return dispatch_attn_simt(&a, false, reinterpret_cast<cudaStream_t>(stream), cached_keys(&c, d->n_keys));
+}
+
+// the ragged training descriptor checked as the scalar one (its sep the bound of the key counts)
+static int check_ragged_train_simt(const pfn_attn_ragged_train_desc* d, bool bwd, const char* who) {
+  PFN_CHECK_ARG(d != nullptr && d->n_keys != nullptr, "%s: null descriptor / n_keys", who);
+  if (int rc = check_attn_desc(&d->a, bwd, who)) return rc;
+  PFN_CHECK_ARG(d->a.batch_major == 0, "%s: batch-major token order is only implemented by the tensor-core kernels", who);
+  PFN_CHECK_ARG(d->a.delta_token_major == 0, "%s: a precomputed token-major delta is only consumed by the tensor-core kernels",
+                who);
+  return 0;
+}
+
+extern "C" int pfn_attention_ragged_train_fwd_simt(const pfn_attn_ragged_train_desc* d, void* stream) {
+  if (int rc = check_ragged_train_simt(d, false, "attention_ragged_train_fwd_simt")) return rc;
+  return dispatch_attn_simt(&d->a, false, reinterpret_cast<cudaStream_t>(stream), masked_keys(&d->a, d->n_keys));
+}
+
+extern "C" int pfn_attention_ragged_train_bwd_simt(const pfn_attn_ragged_train_desc* d, void* stream) {
+  if (int rc = check_ragged_train_simt(d, true, "attention_ragged_train_bwd_simt")) return rc;
+  return dispatch_attn_simt(&d->a, true, reinterpret_cast<cudaStream_t>(stream), masked_keys(&d->a, d->n_keys));
 }

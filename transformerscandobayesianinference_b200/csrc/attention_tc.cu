@@ -24,7 +24,8 @@
 // Ragged datasets (kRagged, pfn_attention_ragged_fwd_tc / pfn_attention_ctx_ragged_fwd_tc): dataset b has its own key
 // count n_b = n_keys[b] <= sep in place of sep, in the three places sep enters: the unit's key-block count, the mask of
 // its last block, and which rows have their diagonal key (i >= n_b; every row in the context attention).  Keys in
-// [n_b, sep) are real rows of the operand and are masked like the keys past sep in the last block.
+// [n_b, sep) are real rows of the operand and are masked like the keys past sep in the last block.  The training
+// entry point (pfn_attention_ragged_train_fwd_tc) also writes lse and applies dropout.
 #include "attention_common.cuh"
 
 namespace pfn {
@@ -214,7 +215,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int j = 0; j < 16; ++j) {
         *reinterpret_cast<uint32_t*>(stg + att_tile_off2(rr, j, lane)) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
       }
-      if (!kCtx && !kRagged && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+      if (!kCtx && (!kRagged || p.lse != nullptr) && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
     }
     tc::fence_proxy_async_smem();
     tc::named_bar_sync(1 + g, 128);
@@ -227,7 +228,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   if (timed_out) asm volatile("trap;");
 }
 
-// The masked forward over d (lse written unless ragged) with n_keys[b] keys for dataset b when kRagged
+// The masked forward over d (lse written when d->lse is set) with n_keys[b] keys for dataset b when kRagged
 template <bool kRagged>
 static int launch_attn_fwd_tc(const pfn_attn_desc* d, const int* n_keys, cudaStream_t stream, const char* who) {
   AttnFwdParams p;
@@ -304,4 +305,10 @@ extern "C" int pfn_attention_ctx_ragged_fwd_tc(const pfn_attn_ctx_ragged_desc* d
   pfn_attn_ctx_desc c;
   if (int rc = attn_ctx_ragged_as_ctx(d, &c, "attention_ctx_ragged_fwd_tc")) return rc;
   return launch_attn_ctx_fwd_tc<true>(&c, d->n_keys, reinterpret_cast<cudaStream_t>(stream), "attention_ctx_ragged_fwd_tc");
+}
+
+extern "C" int pfn_attention_ragged_train_fwd_tc(const pfn_attn_ragged_train_desc* d, void* stream) {
+  PFN_CHECK_ARG(d != nullptr && d->n_keys != nullptr, "attention_ragged_train_fwd_tc: null descriptor / n_keys");
+  if (int rc = check_tc_attn(&d->a, false, "attention_ragged_train_fwd_tc")) return rc;
+  return launch_attn_fwd_tc<true>(&d->a, d->n_keys, reinterpret_cast<cudaStream_t>(stream), "attention_ragged_train_fwd_tc");
 }

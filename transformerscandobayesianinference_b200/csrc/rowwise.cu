@@ -3,7 +3,7 @@
 // gradients) are accumulated per lane across the rows a warp owns, combined per CTA in shared memory and
 // flushed with one atomicAdd per column per CTA.
 #include "common.cuh"
-#include "../../include/pfn_b200.h"
+#include "../../include/pfn_b200_ragged_train.h"
 
 namespace pfn {
 
@@ -44,11 +44,19 @@ template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16*
 // --------------------------------------------------------------------------------------------
 // Embedding forward: out[row,:] = x[row,:] Wx^T + bx + (t < sep ? y[row] wy + by : 0)
 // --------------------------------------------------------------------------------------------
-template <typename T>
+// Whether token row r = t*B + b is a training row: r < train_rows (= sep * B), or in the ragged kernels t < n_keys[b]
+// (clamped to [0, T])
+template <bool kRagged>
+__device__ __forceinline__ bool embed_train_row(int r, int train_rows, int B, int T, const int* n_keys) {
+  if (!kRagged) return r < train_rows;
+  return r / B < min(max(__ldg(n_keys + r % B), 0), T);
+}
+
+template <typename T, bool kRagged>
 __global__ void __launch_bounds__(256)
 embed_fwd_kernel(const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ Wx,
                  const float* __restrict__ bx, const float* __restrict__ wy, const float* __restrict__ by,
-                 T* __restrict__ out, int rows, int train_rows, int F, int E) {
+                 T* __restrict__ out, int rows, int train_rows, int F, int E, int B, const int* __restrict__ n_keys) {
   constexpr int ROWS = 8;
   extern __shared__ float sx[];  // [ROWS][F] + [ROWS] y
   float* sy = sx + ROWS * F;
@@ -59,7 +67,7 @@ embed_fwd_kernel(const float* __restrict__ x, const float* __restrict__ y, const
   }
   if (threadIdx.x < ROWS) {
     const int r = r0 + threadIdx.x;
-    sy[threadIdx.x] = (r < rows && r < train_rows) ? y[r] : 0.f;
+    sy[threadIdx.x] = (r < rows && embed_train_row<kRagged>(r, train_rows, B, rows / B, n_keys)) ? y[r] : 0.f;
   }
   __syncthreads();
   for (int e = threadIdx.x; e < E; e += blockDim.x) {
@@ -77,7 +85,7 @@ embed_fwd_kernel(const float* __restrict__ x, const float* __restrict__ y, const
       const int row = r0 + r;
       if (row < rows) {
         float v = acc[r];
-        if (row < train_rows) v += fmaf(sy[r], wye, bye);
+        if (embed_train_row<kRagged>(row, train_rows, B, rows / B, n_keys)) v += fmaf(sy[r], wye, bye);
         out[static_cast<size_t>(row) * E + e] = from_f32<T>(v);
       }
     }
@@ -85,11 +93,11 @@ embed_fwd_kernel(const float* __restrict__ x, const float* __restrict__ y, const
 }
 
 // Embedding backward: thread owns column e, loops over a chunk of rows.
-template <typename T, int FMAX>
+template <typename T, int FMAX, bool kRagged>
 __global__ void __launch_bounds__(128)
 embed_bwd_kernel(const T* __restrict__ dout, const float* __restrict__ x, const float* __restrict__ y,
                  float* __restrict__ dWx, float* __restrict__ dbx, float* __restrict__ dwy, float* __restrict__ dby,
-                 int rows, int train_rows, int F, int E, int rows_per_cta, int f0) {
+                 int rows, int train_rows, int F, int E, int rows_per_cta, int f0, int B, const int* __restrict__ n_keys) {
   const int e = blockIdx.y * blockDim.x + threadIdx.x;
   const int r_begin = blockIdx.x * rows_per_cta;
   const int r_end = min(r_begin + rows_per_cta, rows);
@@ -101,7 +109,7 @@ embed_bwd_kernel(const T* __restrict__ dout, const float* __restrict__ x, const 
     for (int r = r_begin; r < r_end; ++r) {
       const float d = to_f32<T>(dout[static_cast<size_t>(r) * E + e]);
       sd += d;
-      if (r < train_rows) { sdt += d; sdy = fmaf(d, y[r], sdy); }
+      if (embed_train_row<kRagged>(r, train_rows, B, rows / B, n_keys)) { sdt += d; sdy = fmaf(d, y[r], sdy); }
 #pragma unroll
       for (int f = 0; f < FMAX; ++f)
         if (f0 + f < F) accw[f] = fmaf(d, x[static_cast<size_t>(r) * F + f0 + f], accw[f]);
@@ -460,45 +468,79 @@ colsum_kernel(const T* __restrict__ X, int ld, float* __restrict__ out, int rows
 
 using namespace pfn;
 
+// The embedding forward with y on the rows t < sep, or t < n_keys[b] when kRagged
+template <bool kRagged>
+static int embed_fwd(const float* x, const float* y, const float* Wx, const float* bx, const float* wy, const float* by,
+                     void* out, int out_dtype, int T, int B, int F, int E, int sep, const int* n_keys, cudaStream_t s) {
+  const int rows = T * B, train_rows = sep * B;
+  const int grid = (rows + 7) / 8;
+  const size_t smem = (8 * F + 8) * sizeof(float);
+  if (out_dtype == PFN_F32)
+    embed_fwd_kernel<float, kRagged><<<grid, 256, smem, s>>>(x, y, Wx, bx, wy, by, reinterpret_cast<float*>(out), rows,
+                                                             train_rows, F, E, B, n_keys);
+  else
+    embed_fwd_kernel<__nv_bfloat16, kRagged><<<grid, 256, smem, s>>>(x, y, Wx, bx, wy, by,
+                                                                     reinterpret_cast<__nv_bfloat16*>(out), rows,
+                                                                     train_rows, F, E, B, n_keys);
+  PFN_LAUNCH_OK();
+  return 0;
+}
+
+template <bool kRagged>
+static int embed_bwd(const void* dout, int dtype, const float* x, const float* y, float* dWx, float* dbx, float* dwy,
+                     float* dby, int T, int B, int F, int E, int sep, const int* n_keys, cudaStream_t s) {
+  const int rows = T * B, train_rows = sep * B;
+  const int rows_per_cta = 512;
+  dim3 grid((rows + rows_per_cta - 1) / rows_per_cta, (E + 127) / 128);
+  constexpr int FMAX = 8;
+  for (int f0 = 0; f0 < F; f0 += FMAX) {
+    if (dtype == PFN_F32)
+      embed_bwd_kernel<float, FMAX, kRagged><<<grid, 128, 0, s>>>(reinterpret_cast<const float*>(dout), x, y, dWx, dbx,
+                                                                  dwy, dby, rows, train_rows, F, E, rows_per_cta, f0, B,
+                                                                  n_keys);
+    else
+      embed_bwd_kernel<__nv_bfloat16, FMAX, kRagged><<<grid, 128, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dout), x,
+                                                                          y, dWx, dbx, dwy, dby, rows, train_rows, F, E,
+                                                                          rows_per_cta, f0, B, n_keys);
+    PFN_LAUNCH_OK();
+  }
+  return 0;
+}
+
 extern "C" int pfn_embed_fwd(const float* x, const float* y, const float* Wx, const float* bx, const float* wy,
                              const float* by, void* out, int out_dtype, int T, int B, int F, int E, int sep,
                              void* stream) {
   PFN_CHECK_ARG(T > 0 && B > 0 && F > 0 && E > 0, "embed_fwd: bad shape T=%d B=%d F=%d E=%d", T, B, F, E);
   PFN_CHECK_ARG(sep >= 0 && sep <= T, "embed_fwd: sep %d outside [0,%d]", sep, T);
   PFN_CHECK_ARG(F <= 1024, "embed_fwd: F=%d too large for the fused kernel (route through the GEMM)", F);
-  const int rows = T * B, train_rows = sep * B;
-  const int grid = (rows + 7) / 8;
-  const size_t smem = (8 * F + 8) * sizeof(float);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (out_dtype == PFN_F32)
-    embed_fwd_kernel<float><<<grid, 256, smem, s>>>(x, y, Wx, bx, wy, by, reinterpret_cast<float*>(out), rows,
-                                                    train_rows, F, E);
-  else
-    embed_fwd_kernel<__nv_bfloat16><<<grid, 256, smem, s>>>(x, y, Wx, bx, wy, by,
-                                                            reinterpret_cast<__nv_bfloat16*>(out), rows, train_rows, F, E);
-  PFN_LAUNCH_OK();
-  return 0;
+  return embed_fwd<false>(x, y, Wx, bx, wy, by, out, out_dtype, T, B, F, E, sep, nullptr,
+                          reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int pfn_embed_bwd(const void* dout, int dtype, const float* x, const float* y, float* dWx, float* dbx,
                              float* dwy, float* dby, int T, int B, int F, int E, int sep, void* stream) {
   PFN_CHECK_ARG(T > 0 && B > 0 && F > 0 && E > 0, "embed_bwd: bad shape");
   PFN_CHECK_ARG(sep >= 0 && sep <= T, "embed_bwd: sep %d outside [0,%d]", sep, T);
-  const int rows = T * B, train_rows = sep * B;
-  const int rows_per_cta = 512;
-  dim3 grid((rows + rows_per_cta - 1) / rows_per_cta, (E + 127) / 128);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  constexpr int FMAX = 8;
-  for (int f0 = 0; f0 < F; f0 += FMAX) {
-    if (dtype == PFN_F32)
-      embed_bwd_kernel<float, FMAX><<<grid, 128, 0, s>>>(reinterpret_cast<const float*>(dout), x, y, dWx, dbx, dwy, dby,
-                                                         rows, train_rows, F, E, rows_per_cta, f0);
-    else
-      embed_bwd_kernel<__nv_bfloat16, FMAX><<<grid, 128, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dout), x, y, dWx,
-                                                                 dbx, dwy, dby, rows, train_rows, F, E, rows_per_cta, f0);
-    PFN_LAUNCH_OK();
-  }
-  return 0;
+  return embed_bwd<false>(dout, dtype, x, y, dWx, dbx, dwy, dby, T, B, F, E, sep, nullptr,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pfn_embed_ragged_fwd(const float* x, const float* y, const float* Wx, const float* bx, const float* wy,
+                                    const float* by, void* out, int out_dtype, int T, int B, int F, int E,
+                                    const int* n_keys, void* stream) {
+  PFN_CHECK_ARG(T > 0 && B > 0 && F > 0 && E > 0, "embed_ragged_fwd: bad shape T=%d B=%d F=%d E=%d", T, B, F, E);
+  PFN_CHECK_ARG(n_keys != nullptr, "embed_ragged_fwd: null n_keys");
+  PFN_CHECK_ARG(F <= 1024, "embed_ragged_fwd: F=%d too large for the fused kernel (route through the GEMM)", F);
+  return embed_fwd<true>(x, y, Wx, bx, wy, by, out, out_dtype, T, B, F, E, 0, n_keys,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pfn_embed_ragged_bwd(const void* dout, int dtype, const float* x, const float* y, float* dWx, float* dbx,
+                                    float* dwy, float* dby, int T, int B, int F, int E, const int* n_keys, void* stream) {
+  PFN_CHECK_ARG(T > 0 && B > 0 && F > 0 && E > 0, "embed_ragged_bwd: bad shape");
+  PFN_CHECK_ARG(n_keys != nullptr, "embed_ragged_bwd: null n_keys");
+  return embed_bwd<true>(dout, dtype, x, y, dWx, dbx, dwy, dby, T, B, F, E, 0, n_keys,
+                         reinterpret_cast<cudaStream_t>(stream));
 }
 
 // Vector-path launches: LnRing's CTAs per SM, no more than the rows need.  An SM has 228 KB of shared memory, of which

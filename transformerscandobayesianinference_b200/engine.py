@@ -14,7 +14,7 @@ import os
 
 import torch
 
-from . import _lib as L, _lib_ragged as LR
+from . import _lib as L, _lib_ragged as LR, _lib_ragged_train as LRT
 
 LAYER_PARAM_NAMES = ("in_w", "in_b", "out_w", "out_b", "w1", "b1", "w2", "b2", "g1", "be1", "g2", "be2")
 N_LAYER_PARAMS = len(LAYER_PARAM_NAMES)
@@ -137,6 +137,31 @@ def _bucket_ready(flat, wait=True):
             GRAD_BUCKET_SYNC()
 
 
+class RaggedSeps:
+    """One single_eval_pos per dataset, in place of the scalar `sep` of EncoderStackFn and EmbedFn: `n_keys` the int32 [B]
+    device tensor of the values, `s_min` / `s_max` their least and greatest value (host ints)."""
+    __slots__ = ("n_keys", "s_min", "s_max")
+
+    def __init__(self, n_keys, s_min, s_max):
+        self.n_keys, self.s_min, self.s_max = n_keys, int(s_min), int(s_max)
+
+
+def _attention_fwd(qkv, attn, lse, T, B, nhead, dh, sep, drop):
+    """The masked attention forward at the scalar sep, or at one separator per dataset (RaggedSeps)."""
+    if isinstance(sep, RaggedSeps):
+        LRT.attention_ragged_train_fwd(qkv, attn, lse, T, B, nhead, dh, sep.s_max, sep.n_keys, drop=drop)
+    else:
+        L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, sep, drop=drop)
+
+
+def _attention_bwd(qkv, attn, lse, dattn, dqkv, delta, T, B, nhead, dh, sep, **kw):
+    """The backward of _attention_fwd."""
+    if isinstance(sep, RaggedSeps):
+        LRT.attention_ragged_train_bwd(qkv, attn, lse, dattn, dqkv, delta, T, B, nhead, dh, sep.s_max, sep.n_keys, **kw)
+    else:
+        L.attention_bwd(qkv, attn, lse, dattn, dqkv, delta, T, B, nhead, dh, sep, **kw)
+
+
 def _stack_start(src, precision, nhead, params, kv=None):
     """Checks of an encoder stack call; (activation dtype, number of layers, head dim, contiguous src)."""
     L.require_cuda(src, kv, *params)
@@ -189,7 +214,8 @@ def _layer_tail(h, attn, P, out_w, w1, w2, drop, li):
 
 
 class EncoderStackFn(torch.autograd.Function):
-    """src [T*B, E] (activation dtype) -> output of `nlayers` post-norm encoder layers under the sep mask."""
+    """src [T*B, E] (activation dtype) -> output of `nlayers` post-norm encoder layers under the sep mask; `sep` is an int
+    or a RaggedSeps (dataset b's rows then attend under its own separator).  Only the attention depends on sep."""
 
     @staticmethod
     def forward(ctx, src, T, B, sep, nhead, precision, keep, drop, *params):
@@ -205,7 +231,7 @@ class EncoderStackFn(torch.autograd.Function):
         for li in range(n_layers):
             P, (in_w, out_w, w1, w2), qkv, attn = _layer_qkv(h, params, li, dt)
             lse = torch.empty(B * nhead, T, device=h.device, dtype=torch.float32)
-            L.attention_fwd(qkv, attn, lse, T, B, nhead, dh, sep, drop=(site_seed(drop[0], li, 0), thr) if thr else None)
+            _attention_fwd(qkv, attn, lse, T, B, nhead, dh, sep, (site_seed(drop[0], li, 0), thr) if thr else None)
             z1, mean1, rstd1, h1, u, u_is_grad, g, z2, mean2, rstd2, h2 = _layer_tail(h, attn, P, out_w, w1, w2, drop, li)
             if keep:
                 # the activation-dtype weight copies are kept for the backward as well (4 small tensors per layer) instead of
@@ -279,9 +305,9 @@ class EncoderStackFn(torch.autograd.Function):
             del da
             dqkv = torch.empty_like(qkv)
             fused_bias = (not drop) and tc_attn
-            L.attention_bwd(qkv, attn, lse, dattn, dqkv, delta, T, B, nhead, dh, sep,
-                            drop=(site_seed(drop[0], li, 0), drop[1]) if drop else None,
-                            dq_colsum=G["in_b"][:E] if fused_bias else None, delta_token_major=fuse_delta)
+            _attention_bwd(qkv, attn, lse, dattn, dqkv, delta, T, B, nhead, dh, sep,
+                           drop=(site_seed(drop[0], li, 0), drop[1]) if drop else None,
+                           dq_colsum=G["in_b"][:E] if fused_bias else None, delta_token_major=fuse_delta)
             del dattn, attn, qkv
             if fused_bias:
                 # in-projection bias gradient without re-reading dqkv (1.5 GB per layer at cfg 2): the q third comes out of
@@ -347,7 +373,8 @@ def query_stack(src, kv, n, B, nhead, precision, *params, n_keys=None):
 
 
 class EmbedFn(torch.autograd.Function):
-    """(x [T,B,F], y [T,B]) -> src [T*B, E]:  x Wx^T + bx + (t < sep)(y wy + by)   (reference transformer.py:68-74)."""
+    """(x [T,B,F], y [T,B]) -> src [T*B, E]:  x Wx^T + bx + (t < sep)(y wy + by)   (reference transformer.py:68-74);
+    with a RaggedSeps `sep`, (t < n_keys[b]) for dataset b."""
 
     @staticmethod
     def forward(ctx, x, y, Wx, bx, wy, by, sep, precision):
@@ -357,8 +384,12 @@ class EmbedFn(torch.autograd.Function):
         x = x.detach().contiguous().float()
         y = y.detach().contiguous().float()
         out = torch.empty(T * B, E, device=x.device, dtype=act_dtype(precision))
-        L.embed_fwd(x, y, Wx.detach().contiguous(), bx.detach().contiguous(), wy.detach().contiguous().view(-1),
-                    by.detach().contiguous(), out, T, B, F, E, sep)
+        args = (x, y, Wx.detach().contiguous(), bx.detach().contiguous(), wy.detach().contiguous().view(-1),
+                by.detach().contiguous(), out, T, B, F, E)
+        if isinstance(sep, RaggedSeps):
+            LRT.embed_ragged_fwd(*args, sep.n_keys)
+        else:
+            L.embed_fwd(*args, sep)
         ctx.save_for_backward(x, y)
         ctx.meta = (T, B, F, E, sep, wy.shape)
         return out
@@ -372,7 +403,10 @@ class EmbedFn(torch.autograd.Function):
         dbx = torch.zeros(E, device=dev)
         dwy = torch.zeros(E, device=dev)
         dby = torch.zeros(E, device=dev)
-        L.embed_bwd(dout.contiguous(), x, y, dWx, dbx, dwy, dby, T, B, F, E, sep)
+        if isinstance(sep, RaggedSeps):
+            LRT.embed_ragged_bwd(dout.contiguous(), x, y, dWx, dbx, dwy, dby, T, B, F, E, sep.n_keys)
+        else:
+            L.embed_bwd(dout.contiguous(), x, y, dWx, dbx, dwy, dby, T, B, F, E, sep)
         return None, None, dWx, dbx, dwy.view(wy_shape), dby, None, None
 
 

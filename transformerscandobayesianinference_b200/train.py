@@ -20,7 +20,7 @@ from torch import nn
 
 from . import encoders, positional_encodings, parallel
 from .bar_distribution import BarDistribution, FullSupportBarDistribution, get_bucket_limits  # noqa: F401
-from .transformer import TransformerModel
+from .transformer import TransformerModel, dataset_seps, is_per_dataset
 from .utils import (get_cosine_schedule_with_warmup, get_openai_lr, StoreDictKeyPair,  # noqa: F401
                     get_weighted_single_eval_pos_sampler, get_uniform_single_eval_pos_sampler)
 
@@ -63,6 +63,7 @@ class Trainer:
         print(f'Using {device} device')
         assert batch_size % world == 0, f'global batch {batch_size} must be divisible by the world size {world}'
         self.world, self.rank = world, parallel.rank()
+        self.batch_size = batch_size
         self.device = device
         self.bptt = bptt
         self.steps_per_epoch = steps_per_epoch
@@ -123,15 +124,46 @@ class Trainer:
         self.reducer = parallel.OverlappedGradReducer() if (world > 1 and on_cuda and aggregate_k_gradients == 1) else None
 
     # ------------------------------------------------------------------------------------------------------------
+    def local_seps(self, single_eval_pos, T):
+        """(single_eval_pos for this rank's forward, this rank's values, global number of query rows) of one step.
+        A scalar gives (itself, None, None).  B values for the global batch (batch_size of them, validated) give this
+        rank's slice of them; the forward takes the slice, or the common value when all B are equal (the scalar step,
+        whose loss is the mean: the count is then None).  A slice without a query row (every value T, while other ranks
+        have some) runs the forward at T - 1, so that the rank still takes part in the gradient reduction; its one row
+        per dataset is masked out of the loss."""
+        if not is_per_dataset(single_eval_pos):
+            return single_eval_pos, None, None
+        seps = dataset_seps(single_eval_pos, T, self.batch_size, "Trainer.step")
+        n_query = sum(T - s for s in seps)
+        if n_query == 0:
+            raise ValueError("Trainer.step: single_eval_pos leaves no query row in the batch")
+        local = self.batch_size // self.world
+        mine = seps[self.rank * local:(self.rank + 1) * local]
+        if len(set(seps)) == 1:
+            return seps[0], mine, None
+        return (T - 1 if min(mine) == T else mine), mine, n_query
+
+    @staticmethod
+    def query_mask(T, rows, seps, device):
+        """Bool [rows, len(seps)]: row r of the last `rows` sequence positions is a query of dataset b."""
+        pos = torch.arange(T - rows, T, device=device).unsqueeze(1)
+        return pos >= torch.tensor(seps, dtype=torch.long, device=device).unsqueeze(0)
+
     def step(self, data, targets, single_eval_pos):
         """One training step on one batch (reference train.py:64-97).  Returns (loss, losses) on the device; the
-        optimizer steps every `aggregate_k_gradients`-th call."""
+        optimizer steps every `aggregate_k_gradients`-th call.  single_eval_pos may be one value per dataset of the
+        global batch: the per-row losses are then kept on each dataset's query rows only, and the loss is their sum over
+        (global query rows / world), so that the data-parallel mean is the global batch's mean."""
         device, criterion, model, n_out = self.device, self.criterion, self.model, self.n_out
+        T = targets.shape[0]
+        single_eval_pos, mine, n_query = self.local_seps(single_eval_pos, T)
         data = tuple(e.to(device) for e in data) if isinstance(data, tuple) else data.to(device)
         output = model(data, single_eval_pos=single_eval_pos)
         self.forward_done_time = time.time()
 
-        if single_eval_pos is not None:
+        if n_query is not None:
+            targets = targets[T - output.shape[0]:]
+        elif single_eval_pos is not None:
             targets = targets[single_eval_pos:]
         if isinstance(criterion, nn.GaussianNLLLoss):
             assert output.shape[-1] == 2, \
@@ -145,7 +177,11 @@ class Trainer:
             losses = criterion(output.reshape(-1, n_out), targets.to(device).flatten())
         losses = losses.view(*output.shape[0:2]).squeeze(-1)
 
-        loss = losses.mean()
+        if n_query is not None:
+            query = self.query_mask(T, output.shape[0], mine, losses.device)
+            loss = torch.where(query, losses.view(query.shape), 0.).sum() / (n_query / self.world)
+        else:
+            loss = losses.mean()
         if self.reducer is not None:
             from . import engine
             self.reducer.install(engine)
@@ -185,17 +221,29 @@ class Trainer:
         seps = self.draw_single_eval_positions(len(dl))
         time_to_get_batch = forward_time = step_time = 0.
         self._micro = 0
+        ragged = False
         for batch, (data, targets) in enumerate(dl):
             time_to_get_batch = time.time() - before_get_batch
             before_forward = time.time()
             single_eval_pos = seps[batch]
             loss, losses = self.step(data, targets, single_eval_pos)
+            single_eval_pos, mine, _ = self.local_seps(single_eval_pos, targets.shape[0])
             forward_time = self.forward_done_time - before_forward
             step_time = time.time() - before_forward
 
             ld = loss.detach()
             total_loss += ld
-            if single_eval_pos is None:
+            if mine is not None:
+                # a step with one value per dataset: each dataset's mean query-row loss in the bucket of its own value
+                ragged = True
+                query = self.query_mask(targets.shape[0], losses.numel() // len(mine), mine, device)
+                n_q = query.sum(0)
+                mean = torch.where(query, losses.detach().view(query.shape), 0.).sum(0) / n_q.clamp(min=1)
+                idx = torch.tensor(mine, device=device)
+                has = n_q > 0
+                pos_loss.index_add_(0, idx[has], mean[has])
+                pos_count.index_add_(0, idx[has], torch.ones_like(mean[has]))
+            elif single_eval_pos is None:
                 pos_loss += losses.mean(1).detach()
                 pos_count += 1
             else:
@@ -207,6 +255,8 @@ class Trainer:
             self.criterion.check_support()
         total_loss = parallel.allreduce_mean_scalar(total_loss)
         pos_loss = parallel.allreduce_mean_scalar(pos_loss)
+        if ragged:      # the ranks' datasets fall in different buckets: the mean is their sum over the summed counts
+            pos_count = parallel.allreduce_mean_scalar(pos_count)
         return (total_loss.item() / self.steps_per_epoch, (pos_loss / pos_count).tolist(), time_to_get_batch,
                 forward_time, step_time)
 

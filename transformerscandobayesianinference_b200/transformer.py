@@ -11,6 +11,10 @@ single_eval_pos mask a training row attends only to training rows and a query ro
 `predict` returns what `forward` returns for the concatenated sequence at single_eval_pos = n.  With
 `encode_context(x_train, y_train, n_train)` the datasets of one batch have training sets of their own sizes: dataset b
 uses rows [0, n_train[b]) and the rows after them are padding that never reaches an output.
+
+`forward(src, single_eval_pos=seps)` with B values trains on datasets of different training-set sizes in one batch:
+dataset b's rows attend under its own separator seps[b], and `query_rows(T, seps)` marks which of the returned rows are
+its queries.
 """
 import numbers
 
@@ -44,27 +48,46 @@ class TrainingContext:
         self.n_train = n_train
 
 
+def _dataset_ints(values, n, B, who, name, noun, rows):
+    """values (B integers in [0, n]: a sequence or an integer tensor on any device) as a tuple of ints; ValueError
+    otherwise.  who, name: the caller and its argument; noun: what the values are; rows: what n counts."""
+    if torch.is_tensor(values):
+        if values.dtype.is_floating_point or values.dtype.is_complex or values.dtype == torch.bool:
+            raise ValueError(f"{who}: {name} must hold integers, got a {values.dtype} tensor")
+        if values.dim() != 1:
+            raise ValueError(f"{who}: {name} must be one-dimensional, got shape {tuple(values.shape)}")
+        ints = values.tolist()
+    else:
+        ints = list(values)
+        for v in ints:
+            if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+                raise ValueError(f"{who}: {name} must hold integers, got {v!r}")
+        ints = [int(v) for v in ints]
+    if len(ints) != B:
+        raise ValueError(f"{who}: {name} holds {len(ints)} {noun} for a batch of {B} datasets")
+    bad = [v for v in ints if not 0 <= v <= n]
+    if bad:
+        raise ValueError(f"{who}: {name} values must lie in [0, {n}] ({rows}), got {bad[0]}")
+    return tuple(ints)
+
+
 def _training_set_sizes(n_train, n, B):
     """n_train (B integers in [0, n]: a sequence or an integer tensor on any device) as a tuple of ints; ValueError
     otherwise."""
-    if torch.is_tensor(n_train):
-        if n_train.dtype.is_floating_point or n_train.dtype.is_complex or n_train.dtype == torch.bool:
-            raise ValueError(f"encode_context: n_train must hold integers, got a {n_train.dtype} tensor")
-        if n_train.dim() != 1:
-            raise ValueError(f"encode_context: n_train must be one-dimensional, got shape {tuple(n_train.shape)}")
-        sizes = n_train.tolist()
-    else:
-        sizes = list(n_train)
-        for v in sizes:
-            if isinstance(v, bool) or not isinstance(v, numbers.Integral):
-                raise ValueError(f"encode_context: n_train must hold integers, got {v!r}")
-        sizes = [int(v) for v in sizes]
-    if len(sizes) != B:
-        raise ValueError(f"encode_context: n_train holds {len(sizes)} sizes for a batch of {B} datasets")
-    bad = [v for v in sizes if not 0 <= v <= n]
-    if bad:
-        raise ValueError(f"encode_context: n_train values must lie in [0, {n}] (the rows of x_train), got {bad[0]}")
-    return tuple(sizes)
+    return _dataset_ints(n_train, n, B, "encode_context", "n_train", "sizes", "the rows of x_train")
+
+
+def is_per_dataset(single_eval_pos):
+    """True when single_eval_pos is one value per dataset (a sequence, or a tensor or array with a dimension) rather than
+    one for the whole batch."""
+    if torch.is_tensor(single_eval_pos) or hasattr(single_eval_pos, "ndim"):
+        return single_eval_pos.ndim >= 1
+    return isinstance(single_eval_pos, (list, tuple))
+
+
+def dataset_seps(single_eval_pos, T, B, who="forward"):
+    """The per-dataset single_eval_pos (B integers in [0, T]) as a tuple of ints; ValueError otherwise."""
+    return _dataset_ints(single_eval_pos, T, B, who, "single_eval_pos", "values", "the sequence length")
 
 
 class TransformerModel(nn.Module):
@@ -128,7 +151,7 @@ class TransformerModel(nn.Module):
 
     def _embed(self, x_src, y_src, sep):
         """[T*B, E] activation-dtype input of the encoder stack: the x embedding of every row plus the y embedding of the
-        rows t < sep."""
+        rows t < sep (t < n_keys[b] in dataset b for an engine.RaggedSeps)."""
         T, B = x_src.shape[0], x_src.shape[1]
         precision = self.precision
         if self._fused_embed_ok():
@@ -136,7 +159,11 @@ class TransformerModel(nn.Module):
                                         self.y_encoder.bias, sep, precision)
         xs = self.encoder(x_src)
         ys = self.y_encoder(y_src.unsqueeze(-1) if y_src.dim() == 2 else y_src)
-        h = torch.cat([xs[:sep] + ys[:sep], xs[sep:]], 0)
+        if isinstance(sep, engine.RaggedSeps):
+            train = torch.arange(T, device=xs.device).unsqueeze(1) < sep.n_keys.to(xs.device)
+            h = torch.where(train.unsqueeze(-1), xs + ys, xs)
+        else:
+            h = torch.cat([xs[:sep] + ys[:sep], xs[sep:]], 0)
         if self.input_ln is not None:
             h = self.input_ln(h)
         if self.pos_encoder is not None:
@@ -163,10 +190,40 @@ class TransformerModel(nn.Module):
             out = self.decoder(hq.float().view(rows, B, -1))
         return out.reshape(rows, B, -1)
 
+    @staticmethod
+    def query_rows(T, single_eval_pos):
+        """Bool [T - s_min, B] mask of the rows of forward(..., single_eval_pos)'s output that are queries: row r of
+        dataset b is sequence position s_min + r, a query when it is >= single_eval_pos[b].  s_min = min(single_eval_pos)
+        for B values (the mask is then on their device, the CPU for a sequence); for a scalar every row is a query and
+        the mask has one column."""
+        if not is_per_dataset(single_eval_pos):
+            sep = int(single_eval_pos)
+            sep = min(max(sep + T, 0) if sep < 0 else sep, T)
+            return torch.ones(T - sep, 1, dtype=torch.bool)
+        n = len(single_eval_pos)
+        seps = dataset_seps(single_eval_pos, T, n, "query_rows")
+        dev = single_eval_pos.device if torch.is_tensor(single_eval_pos) else torch.device("cpu")
+        s_min = min(seps) if seps else 0
+        pos = torch.arange(s_min, T, device=dev).unsqueeze(1)
+        return pos >= torch.tensor(seps, dtype=torch.long, device=dev).unsqueeze(0)
+
     def forward(self, src, src_mask=None, single_eval_pos=None):
+        """Logits [T - sep, B, n_out] of the rows t >= single_eval_pos.  single_eval_pos may also be B integers in [0, T],
+        one per dataset (a sequence, or an integer tensor on any device): dataset b's rows then attend under
+        generate_D_q_matrix at its own value, the y embedding is added to its rows t < single_eval_pos[b], and the
+        result has T - min(single_eval_pos) rows; `query_rows` marks which are the queries.  B equal values run the
+        scalar path."""
         assert single_eval_pos is not None, 'Single eval pos is required now.'
         assert isinstance(src, tuple), 'the fused x/y input mode cannot be combined with single_eval_pos'
         x_src, y_src = src
+        if is_per_dataset(single_eval_pos):
+            seps = dataset_seps(single_eval_pos, x_src.shape[0], x_src.shape[1])
+            if src_mask is not None:
+                raise NotImplementedError("forward: an explicit src_mask cannot be combined with one single_eval_pos per "
+                                          "dataset (the kernels build the per-dataset mask themselves)")
+            if len(set(seps)) > 1:
+                return self._forward_ragged(x_src, y_src, seps)
+            single_eval_pos = seps[0]
         if src_mask is not None:
             # The kernels implement exactly the mask the reference builds when none is given (transformer.py:62-65:
             # generate_D_q_matrix(T, T - single_eval_pos)).  A caller that passes that very mask gets the same fast path; any
@@ -195,6 +252,21 @@ class TransformerModel(nn.Module):
             drop = (draw_seed(), L_drop_threshold(self.dropout))
         h = engine.EncoderStackFn.apply(h, T, B, sep, self.nhead, precision, torch.is_grad_enabled(), drop, *params)
         return self._decode(h[sep * B:], T - sep, B)
+
+    def _forward_ragged(self, x_src, y_src, seps):
+        """forward with one separator per dataset (seps: B ints, not all equal): the embedding and the attention take
+        every value, the rest of the step runs on the rows from s_min = min(seps) as the scalar path does."""
+        _require_cuda_input(x_src, "forward")
+        T, B = x_src.shape[0], x_src.shape[1]
+        n_keys = torch.tensor(seps, dtype=torch.int32).to(x_src.device, non_blocking=True)
+        sep = engine.RaggedSeps(n_keys, min(seps), max(seps))
+        h = self._embed(x_src, y_src, sep)
+        drop = None
+        if self.training and self.dropout > 0:
+            drop = (draw_seed(), L_drop_threshold(self.dropout))
+        h = engine.EncoderStackFn.apply(h, T, B, sep, self.nhead, self.precision, torch.is_grad_enabled(), drop,
+                                        *self._layer_params())
+        return self._decode(h[sep.s_min * B:], T - sep.s_min, B)
 
     # ---- inference against a cached training set -------------------------------------------------------------
     def _check_context_inference(self):

@@ -65,6 +65,22 @@ def get_uniform_single_eval_pos_sampler(max_len):
     return _ChoiceSampler(max_len)
 
 
+class per_dataset_sampler:
+    """Callable drawing one single_eval_pos per dataset: `batch_size` calls of the scalar sampler `sampler` (such as
+    get_weighted_single_eval_pos_sampler(k)), returned as a list.  Used as `train(single_eval_pos_gen=...)`, it gives every
+    dataset of a step its own training-set size; the draws consume python's `random` as the scalar sampler does."""
+
+    def __init__(self, sampler, batch_size):
+        if not callable(sampler):
+            raise ValueError(f"per_dataset_sampler: sampler must be callable, got {type(sampler).__name__}")
+        if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
+            raise ValueError(f"per_dataset_sampler: batch_size must be a positive int, got {batch_size!r}")
+        self.sampler, self.batch_size = sampler, batch_size
+
+    def __call__(self):
+        return [self.sampler() for _ in range(self.batch_size)]
+
+
 # ---- modules / misc ---------------------------------------------------------------------------------------------------
 class SeqBN(nn.Module):
     """BatchNorm1d over all T*B token rows of a [T, B, d_model] tensor (reference utils.py:76-86).  Optional input
