@@ -35,6 +35,11 @@
 // diagonal key.  In the dK/dV kernel the key tiles at or past s_b have no work and are skipped by every role of the CTA
 // alike; a warpgroup whose 64 keys straddle s_b stores its rows < s_b directly instead of by the TMA, whose map clips
 // at sep only.  The keys [s_b, sep) are real rows of qkv, loaded and masked like the keys past sep.
+//
+// Context attention (kCtx, pfn_attention_ctx_bwd_tc): the dQ kernel alone, on the operands of the context forward.  Q and
+// dO are the query rows' [m*B, 3E] qkv and [m*B, E] dO (T = m), the key blocks come from the [n*B, 2E] K/V cache through
+// its own map (sep = n, or n_keys[b] when ragged), and every row has its diagonal key.  The cached keys are constants, so
+// no dK/dV kernel runs: dqkv receives dQ and the dK_i, dV_i of each row's own key.
 #include "attention_common.cuh"
 
 namespace pfn {
@@ -130,7 +135,7 @@ attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ out, int ld_out, const _
 // =====================================================================================================================
 // Kernel 1: dQ (+ dK, dV of the query rows' own keys)
 // =====================================================================================================================
-template <bool kRagged>
+template <bool kCtx, bool kRagged>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                    const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDQ,
@@ -179,7 +184,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         const int sb = it & 1;
         float* st = sStat + sb * 3 * 128;
         // the warp's diagonal rows of the tile: row k is r0 + 3 k, k < n_rows, in slot k % AB_DQ_ROW_SLOTS
-        const int r_lo = max(0, ab_sep<kRagged>(p, unit.b) - unit.tile * 128), r_hi = min(128, p.T - unit.tile * 128);
+        const int r_lo = kCtx ? 0 : max(0, ab_sep<kRagged>(p, unit.b) - unit.tile * 128), r_hi = min(128, p.T - unit.tile * 128);
         const int r0 = r_lo + (pw - r_lo % AB_DQ_STAT_WARPS + AB_DQ_STAT_WARPS) % AB_DQ_STAT_WARPS;
         const int n_rows = r0 < r_hi ? (r_hi - r0 + AB_DQ_STAT_WARPS - 1) / AB_DQ_STAT_WARPS : 0;
         // the lane's half and columns come from an opaque lane index in every row, so that the address arithmetic built on
@@ -252,7 +257,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       tc::tma_prefetch_desc(&tmDO);
       tc::tma_prefetch_desc(&tmDQ);
       auto nblk_of = [&](const AttUnit& unit) { return kRagged ? (ab_sep<true>(p, unit.b) + AB_ROWS - 1) / AB_ROWS : nblk; };
-      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk_of, E, 2 * E, 4 * AB_TILE,
+      att_kv_producer(pp, &tmKV, n_units, p.n_tiles, p.H, nblk_of, kCtx ? 0 : E, kCtx ? E : 2 * E, 4 * AB_TILE,
                       [&](const AttUnit& unit) {
         for (int g = 0; g < 2; ++g) {
           const int t0 = unit.tile * 128 + 64 * g;
@@ -340,7 +345,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int i = i0 + 8 * r;
-        const bool diag = i < p.T && i >= sep;
+        const bool diag = i < p.T && (kCtx || i >= sep);
         const __nv_bfloat16* krow = p.qkv + att_tok(diag ? i : 0, unit.b, p.T, p.B, p.batch_major) * p.ld_qkv + E + unit.h * ATT_DH;
 #pragma unroll
         for (int j = 0; j < 16; ++j)
@@ -361,7 +366,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int r = 0; r < 2; ++r) {
       const int i = i0 + 8 * r;
       if (i < p.T) {
-        const bool diag = i >= sep;
+        const bool diag = kCtx || i >= sep;
         const int lr = 16 * wq + (lane >> 2) + 8 * r;              // row i in the warpgroup's 64
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
@@ -678,8 +683,8 @@ static int launch_attn_bwd_tc(const pfn_attn_desc* d, const int* n_keys, cudaStr
     PFN_LAUNCH_OK();
   }
   p.n_tiles = (d->T + 127) / 128;
-  if (int rc = att_launch_persistent<attn_bwd_dq_kernel<kRagged>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
-                                                                  AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, tmDQ, p))
+  if (int rc = att_launch_persistent<attn_bwd_dq_kernel<false, kRagged>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                                         AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, tmDQ, p))
     return rc;
   if (d->sep > 0) {
     // dK/dV of the train keys, stored through a map whose t extent of sep drops the keys >= sep of the last tile
@@ -693,6 +698,48 @@ static int launch_attn_bwd_tc(const pfn_attn_desc* d, const int* n_keys, cudaStr
   return 0;
 }
 
+// The context backward over d (dQ kernel only) with n_keys[b] cached keys for dataset b when kRagged
+template <bool kRagged>
+static int launch_attn_ctx_bwd_tc(const pfn_attn_ctx_grad_desc* d, cudaStream_t s, const char* who) {
+  if (int rc = check_attn_ctx_grad_desc(d, true, who)) return rc;
+  const pfn_attn_ctx_desc& c = d->c;
+  PFN_CHECK_ARG(c.dtype == PFN_BF16, "%s: bf16 only", who);
+  PFN_CHECK_ARG(c.dh == ATT_DH, "%s: head dim %d unsupported (built for 128)", who, c.dh);
+  PFN_CHECK_ARG(c.ld_qkv % 8 == 0 && c.ld_kv % 8 == 0 && c.ld_out % 8 == 0 && d->ld_dout % 8 == 0 && d->ld_dqkv % 8 == 0,
+                "%s: leading dims must be multiples of 8", who);
+  // with n == 0 no key block is loaded; the key map then only needs a valid base
+  const void* kv = c.n > 0 ? c.kv : c.qkv;
+  PFN_CHECK_ARG(((reinterpret_cast<uintptr_t>(c.qkv) | reinterpret_cast<uintptr_t>(kv) | reinterpret_cast<uintptr_t>(c.out) |
+                  reinterpret_cast<uintptr_t>(d->dout) | reinterpret_cast<uintptr_t>(d->dqkv)) & 15) == 0,
+                "%s: qkv/kv/out/dout/dqkv must be 16-byte aligned", who);
+  AttnBwdParams p;
+  p.T = c.m; p.B = c.B; p.H = c.H; p.sep = c.n;
+  p.scale = c.scale; p.scale_log2 = c.scale * 1.4426950408889634f;
+  p.qkv = reinterpret_cast<const __nv_bfloat16*>(c.qkv); p.ld_qkv = c.ld_qkv;
+  p.dout = reinterpret_cast<const __nv_bfloat16*>(d->dout); p.ld_dout = d->ld_dout;
+  p.dqkv = reinterpret_cast<__nv_bfloat16*>(d->dqkv); p.ld_dqkv = d->ld_dqkv;
+  p.lse = d->lse; p.delta = d->delta; p.dq_colsum = nullptr; p.delta_tm = 0;
+  p.drop_seed = 0; p.drop_thr = 0;
+  p.batch_major = 0;
+  p.n_keys = d->n_keys;
+  const int E = c.H * ATT_DH;
+  CUtensorMap tmQ, tmKV, tmDO, tmDQ;
+  if (int rc = att_tensor_map(&tmQ, c.qkv, 3 * E, c.ld_qkv, c.m, c.B, c.m, 0)) return rc;
+  if (int rc = att_tensor_map(&tmKV, kv, c.n > 0 ? 2 * E : 3 * E, c.n > 0 ? c.ld_kv : c.ld_qkv, c.n, c.B, c.n > 0 ? c.n : 1, 0))
+    return rc;
+  if (int rc = att_tensor_map(&tmDO, d->dout, E, d->ld_dout, c.m, c.B, c.m, 0)) return rc;
+  if (int rc = att_tensor_map(&tmDQ, d->dqkv, 3 * E, d->ld_dqkv, c.m, c.B, c.m, 0)) return rc;
+  const long long rows = static_cast<long long>(c.m) * c.B;
+  long long grid = (rows + 7) / 8;
+  if (grid > 8LL * num_sms()) grid = 8LL * num_sms();
+  attn_bwd_delta_kernel<<<static_cast<int>(grid), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(c.out), c.ld_out,
+                                                               p.dout, p.ld_dout, d->delta, c.m, c.B, c.H, 0);
+  PFN_LAUNCH_OK();
+  p.n_tiles = (c.m + 127) / 128;
+  return att_launch_persistent<attn_bwd_dq_kernel<true, kRagged>>(who, static_cast<long long>(p.n_tiles) * c.B * c.H,
+                                                                   AB_THREADS, AB_DQ_SMEM, s, tmQ, tmKV, tmDO, tmDQ, p);
+}
+
 }  // namespace pfn
 
 using namespace pfn;
@@ -704,4 +751,11 @@ extern "C" int pfn_attention_bwd_tc(const pfn_attn_desc* d, void* stream) {
 extern "C" int pfn_attention_ragged_train_bwd_tc(const pfn_attn_ragged_train_desc* d, void* stream) {
   PFN_CHECK_ARG(d != nullptr && d->n_keys != nullptr, "attention_ragged_train_bwd_tc: null descriptor / n_keys");
   return launch_attn_bwd_tc<true>(&d->a, d->n_keys, reinterpret_cast<cudaStream_t>(stream), "attention_ragged_train_bwd_tc");
+}
+
+extern "C" int pfn_attention_ctx_bwd_tc(const pfn_attn_ctx_grad_desc* d, void* stream) {
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const char* who = "attention_ctx_bwd_tc";
+  PFN_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
+  return d->n_keys ? launch_attn_ctx_bwd_tc<true>(d, s, who) : launch_attn_ctx_bwd_tc<false>(d, s, who);
 }

@@ -10,6 +10,7 @@
 #include "tc_common.cuh"
 #include "../../include/pfn_b200_ragged.h"
 #include "../../include/pfn_b200_ragged_train.h"
+#include "../../include/pfn_b200_input_grad.h"
 
 namespace pfn {
 
@@ -23,6 +24,8 @@ int check_attn_ctx_desc(const pfn_attn_ctx_desc* d, const char* who);
 // the descriptor of the same forward with sep = T and no lse / over the cache of n rows, checked; the key counts stay in d
 int attn_ragged_as_masked(const pfn_attn_ragged_desc* d, pfn_attn_desc* a, const char* who);
 int attn_ctx_ragged_as_ctx(const pfn_attn_ctx_ragged_desc* d, pfn_attn_ctx_desc* c, const char* who);
+// the context-attention descriptor with lse (and, for the backward, dout / dqkv / delta), checked
+int check_attn_ctx_grad_desc(const pfn_attn_ctx_grad_desc* d, bool bwd, const char* who);
 
 // token row of (time t, batch b) in the [T*B, cols] activations
 __device__ __forceinline__ size_t att_tok(int t, int b, int T, int B, int batch_major) {

@@ -4,11 +4,13 @@
 // reference transformer.py:35-41 is implicit:  keys(i) = [0, sep)  U  {i if i >= sep}.  The forward also serves the
 // context attention (pfn_attention_ctx_fwd_simt): there the sep keys come from the K/V cache and every row has its own key.
 // In the ragged entry points (pfn_attention_ragged_fwd_simt, pfn_attention_ctx_ragged_fwd_simt and the training pair
-// pfn_attention_ragged_train_{fwd,bwd}_simt) dataset b has n_keys[b] keys in place of sep.
+// pfn_attention_ragged_train_{fwd,bwd}_simt) dataset b has n_keys[b] keys in place of sep.  The context attention also
+// has a backward (pfn_attention_ctx_bwd_simt): the dQ kernel on the cached keys, whose gradient is not formed.
 #include "common.cuh"
 #include "dropout.cuh"
 #include "../../include/pfn_b200_ragged.h"
 #include "../../include/pfn_b200_ragged_train.h"
+#include "../../include/pfn_b200_input_grad.h"
 
 namespace pfn {
 
@@ -94,10 +96,11 @@ __device__ __forceinline__ int simt_sep(const pfn_attn_desc& d, const int* n_key
   return kRagged ? min(max(__ldg(n_keys + b), 0), d.sep) : d.sep;
 }
 
-// dQ (+ delta, + the diagonal-key contributions that are the ONLY gradient of k_i, v_i for query rows)
+// dQ (+ delta, + the diagonal-key contributions that are the ONLY gradient of k_i, v_i for query rows), over the keys sk
+// in the order of the forward
 template <typename T, int DPL, bool kRagged>
 __global__ void __launch_bounds__(256)
-attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta, const int* __restrict__ n_keys) {
+attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta, const SharedKeys sk) {
   const int E = d.H * d.dh;
   const long long total = static_cast<long long>(d.B) * d.H * d.T;
   const int lane = threadIdx.x & 31;
@@ -121,14 +124,15 @@ attn_bwd_dq_simt_kernel(const pfn_attn_desc d, float* __restrict__ delta, const 
     dl = warp_sum(dl);
     if (lane == 0) delta[static_cast<size_t>(bh) * d.T + i] = dl;
     const float lse = d.lse[static_cast<size_t>(bh) * d.T + i];
-    const int sep = simt_sep<kRagged>(d, n_keys, b);
-    const int nkeys = sep + (i >= sep ? 1 : 0);
+    const int sep = simt_sep<kRagged>(d, sk.n_keys, b);
+    const int nkeys = sep + (i >= (kRagged ? min(sk.diag_from, sep) : sk.diag_from) ? 1 : 0);
     for (int jj = 0; jj < nkeys; ++jj) {
       const int j = jj < sep ? jj : i;
-      const T* krow = qkv + (static_cast<size_t>(j) * d.B + b) * d.ld_qkv + E + h * d.dh;
+      const T* krow = jj < sep ? reinterpret_cast<const T*>(sk.kv) + (static_cast<size_t>(j) * d.B + b) * sk.ld + h * d.dh
+                               : qkv + tok * d.ld_qkv + E + h * d.dh;
       float k[DPL], v[DPL];
       load_head<T, DPL>(krow, d.dh, lane, k);
-      load_head<T, DPL>(krow + E, d.dh, lane, v);
+      load_head<T, DPL>(krow + (jj < sep ? sk.v_off : E), d.dh, lane, v);
       float s = 0.f, dp = 0.f;
 #pragma unroll
       for (int c = 0; c < DPL; ++c) { s = fmaf(q[c], k[c], s); dp = fmaf(dO[c], v[c], dp); }
@@ -224,10 +228,12 @@ static int launch_attn_simt(const pfn_attn_desc* d, bool bwd, cudaStream_t s, co
     PFN_LAUNCH_OK();
     return 0;
   }
-  if (sk.n_keys) attn_bwd_dq_simt_kernel<T, DPL, true><<<static_cast<int>(grid), 256, 0, s>>>(*d, d->delta, sk.n_keys);
-  else attn_bwd_dq_simt_kernel<T, DPL, false><<<static_cast<int>(grid), 256, 0, s>>>(*d, d->delta, nullptr);
+  if (sk.n_keys) attn_bwd_dq_simt_kernel<T, DPL, true><<<static_cast<int>(grid), 256, 0, s>>>(*d, d->delta, sk);
+  else attn_bwd_dq_simt_kernel<T, DPL, false><<<static_cast<int>(grid), 256, 0, s>>>(*d, d->delta, sk);
   PFN_LAUNCH_OK();
-  if (d->sep > 0) {
+  // the shared keys are rows of qkv, which get dK / dV, when rows below diag_from exist: the masked attention with sep > 0
+  // (the context attention's cached keys have diag_from 0 and are constants)
+  if (sk.diag_from > 0) {
     const long long tasks2 = static_cast<long long>(d->B) * d->H * d->sep;
     long long grid2 = (tasks2 + 7) / 8;
     if (grid2 > max_grid) grid2 = max_grid;
@@ -302,6 +308,17 @@ int attn_ragged_as_masked(const pfn_attn_ragged_desc* d, pfn_attn_desc* a, const
   return 0;
 }
 
+int check_attn_ctx_grad_desc(const pfn_attn_ctx_grad_desc* d, bool bwd, const char* who) {
+  PFN_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
+  if (int rc = check_attn_ctx_desc(&d->c, who)) return rc;
+  PFN_CHECK_ARG(d->lse != nullptr, "%s: null lse", who);
+  if (bwd) {
+    PFN_CHECK_ARG(d->dout && d->dqkv && d->delta, "%s: null dout/dqkv/delta", who);
+    PFN_CHECK_ARG(d->ld_dqkv >= 3 * d->c.H * d->c.dh && d->ld_dout >= d->c.H * d->c.dh, "%s: leading dims too small", who);
+  }
+  return 0;
+}
+
 int attn_ctx_ragged_as_ctx(const pfn_attn_ctx_ragged_desc* d, pfn_attn_ctx_desc* c, const char* who) {
   PFN_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
   PFN_CHECK_ARG(d->n_keys != nullptr, "%s: null n_keys", who);
@@ -367,4 +384,26 @@ extern "C" int pfn_attention_ragged_train_fwd_simt(const pfn_attn_ragged_train_d
 extern "C" int pfn_attention_ragged_train_bwd_simt(const pfn_attn_ragged_train_desc* d, void* stream) {
   if (int rc = check_ragged_train_simt(d, true, "attention_ragged_train_bwd_simt")) return rc;
   return dispatch_attn_simt(&d->a, true, reinterpret_cast<cudaStream_t>(stream), masked_keys(&d->a, d->n_keys));
+}
+
+// the context attention with lse, as the masked attention with T = m, sep = n over the cached keys
+static pfn_attn_desc ctx_grad_as_masked(const pfn_attn_ctx_grad_desc* d) {
+  pfn_attn_desc a = ctx_as_masked(&d->c);
+  a.lse = d->lse;
+  a.dout = d->dout; a.ld_dout = d->ld_dout;
+  a.dqkv = d->dqkv; a.ld_dqkv = d->ld_dqkv;
+  a.delta = d->delta;
+  return a;
+}
+
+extern "C" int pfn_attention_ctx_grad_fwd_simt(const pfn_attn_ctx_grad_desc* d, void* stream) {
+  if (int rc = check_attn_ctx_grad_desc(d, false, "attention_ctx_grad_fwd_simt")) return rc;
+  const pfn_attn_desc a = ctx_grad_as_masked(d);
+  return dispatch_attn_simt(&a, false, reinterpret_cast<cudaStream_t>(stream), cached_keys(&d->c, d->n_keys));
+}
+
+extern "C" int pfn_attention_ctx_bwd_simt(const pfn_attn_ctx_grad_desc* d, void* stream) {
+  if (int rc = check_attn_ctx_grad_desc(d, true, "attention_ctx_bwd_simt")) return rc;
+  const pfn_attn_desc a = ctx_grad_as_masked(d);
+  return dispatch_attn_simt(&a, true, reinterpret_cast<cudaStream_t>(stream), cached_keys(&d->c, d->n_keys));
 }

@@ -19,7 +19,8 @@
 //
 // The context attention (kCtx, pfn_attention_ctx_fwd_tc) is the same kernel on other operands: the query tiles come from
 // the query rows' packed [m*B, 3E] qkv (T = m), the key blocks from the [n*B, 2E] K/V cache (sep = n), and every query row
-// has its diagonal key.  It writes no lse.
+// has its diagonal key.  It writes no lse, except in the instantiation with kLse (pfn_attention_ctx_grad_fwd_tc), whose lse
+// the context backward reads; the flag only adds the store, so the other instantiations compile as before.
 //
 // Ragged datasets (kRagged, pfn_attention_ragged_fwd_tc / pfn_attention_ctx_ragged_fwd_tc): dataset b has its own key
 // count n_b = n_keys[b] <= sep in place of sep, in the three places sep enters: the unit's key-block count, the mask of
@@ -57,7 +58,7 @@ __device__ __forceinline__ int att_sep(const AttnFwdParams& p, int b) {
   return kRagged ? min(max(__ldg(p.n_keys + b), 0), p.sep) : p.sep;
 }
 
-template <bool kCtx, bool kRagged>
+template <bool kCtx, bool kRagged, bool kLse = !kCtx>
 __global__ void __launch_bounds__(AF_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                 const __grid_constant__ CUtensorMap tmO, const AttnFwdParams p) {
@@ -215,7 +216,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int j = 0; j < 16; ++j) {
         *reinterpret_cast<uint32_t*>(stg + att_tile_off2(rr, j, lane)) = tc::pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
       }
-      if (!kCtx && (!kRagged || p.lse != nullptr) && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
+      if (kLse && (!kRagged || p.lse != nullptr) && i < p.T && (lane & 3) == 0) p.lse[static_cast<size_t>(unit.bh) * p.T + i] = (m[r] + __log2f(lr)) * 0.69314718055994531f;
     }
     tc::fence_proxy_async_smem();
     tc::named_bar_sync(1 + g, 128);
@@ -250,9 +251,10 @@ static int launch_attn_fwd_tc(const pfn_attn_desc* d, const int* n_keys, cudaStr
                                                                 AF_THREADS, AF_SMEM, stream, tmQ, tmKV, tmO, p);
 }
 
-// The context forward over d with n_keys[b] cached keys for dataset b when kRagged
-template <bool kRagged>
-static int launch_attn_ctx_fwd_tc(const pfn_attn_ctx_desc* d, const int* n_keys, cudaStream_t stream, const char* who) {
+// The context forward over d with n_keys[b] cached keys for dataset b when kRagged, writing lse when kLse
+template <bool kRagged, bool kLse = false>
+static int launch_attn_ctx_fwd_tc(const pfn_attn_ctx_desc* d, const int* n_keys, cudaStream_t stream, const char* who,
+                                  float* lse = nullptr) {
   if (int rc = check_attn_ctx_desc(d, who)) return rc;
   PFN_CHECK_ARG(d->dtype == PFN_BF16, "%s: bf16 only", who);
   PFN_CHECK_ARG(d->dh == ATT_DH, "%s: head dim %d unsupported (built for 128)", who, d->dh);
@@ -267,7 +269,7 @@ static int launch_attn_ctx_fwd_tc(const pfn_attn_ctx_desc* d, const int* n_keys,
   p.qkv = reinterpret_cast<const __nv_bfloat16*>(d->qkv); p.ld_qkv = d->ld_qkv;
   const int E = d->H * ATT_DH;
   p.k_col = 0; p.v_col = E;
-  p.lse = nullptr;
+  p.lse = lse;
   p.n_tiles = (d->m + 127) / 128;
   p.batch_major = 0;
   p.drop_seed = 0; p.drop_thr = 0;
@@ -277,8 +279,8 @@ static int launch_attn_ctx_fwd_tc(const pfn_attn_ctx_desc* d, const int* n_keys,
   if (int rc = att_tensor_map(&tmKV, kv, d->n > 0 ? 2 * E : 3 * E, d->n > 0 ? d->ld_kv : d->ld_qkv, d->n, d->B,
                               d->n > 0 ? d->n : 1, 0)) return rc;
   if (int rc = att_tensor_map(&tmO, d->out, E, d->ld_out, d->m, d->B, d->m, 0)) return rc;
-  return att_launch_persistent<attn_fwd_kernel<true, kRagged>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
-                                                               AF_THREADS, AF_SMEM, stream, tmQ, tmKV, tmO, p);
+  return att_launch_persistent<attn_fwd_kernel<true, kRagged, kLse>>(who, static_cast<long long>(p.n_tiles) * d->B * d->H,
+                                                                     AF_THREADS, AF_SMEM, stream, tmQ, tmKV, tmO, p);
 }
 
 }  // namespace pfn
@@ -311,4 +313,12 @@ extern "C" int pfn_attention_ragged_train_fwd_tc(const pfn_attn_ragged_train_des
   PFN_CHECK_ARG(d != nullptr && d->n_keys != nullptr, "attention_ragged_train_fwd_tc: null descriptor / n_keys");
   if (int rc = check_tc_attn(&d->a, false, "attention_ragged_train_fwd_tc")) return rc;
   return launch_attn_fwd_tc<true>(&d->a, d->n_keys, reinterpret_cast<cudaStream_t>(stream), "attention_ragged_train_fwd_tc");
+}
+
+extern "C" int pfn_attention_ctx_grad_fwd_tc(const pfn_attn_ctx_grad_desc* d, void* stream) {
+  const char* who = "attention_ctx_grad_fwd_tc";
+  if (int rc = check_attn_ctx_grad_desc(d, false, who)) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  return d->n_keys ? launch_attn_ctx_fwd_tc<true, true>(&d->c, d->n_keys, s, who, d->lse)
+                   : launch_attn_ctx_fwd_tc<false, true>(&d->c, nullptr, s, who, d->lse);
 }

@@ -4,6 +4,7 @@
 // flushed with one atomicAdd per column per CTA.
 #include "common.cuh"
 #include "../../include/pfn_b200_ragged_train.h"
+#include "../../include/pfn_b200_input_grad.h"
 
 namespace pfn {
 
@@ -121,6 +122,58 @@ embed_bwd_kernel(const T* __restrict__ dout, const float* __restrict__ x, const 
       atomicAdd(&dbx[e], sd);
       atomicAdd(&dwy[e], sdy);
       atomicAdd(&dby[e], sdt);
+    }
+  }
+}
+
+// Embedding input gradient: dx[row,:] = dout[row,:] Wx, dy[row] = (t < sep) dout[row,:] . wy  (F <= 64).  One warp per
+// EIG_ROWS rows: per 32-column chunk of dout, lane l holds column e0 + l of each row and the chunk's columns are handed
+// round by shuffles, so lane f sums dx[row, f] and dx[row, f + 32] over e in ascending order and each Wx row is read once
+// per EIG_ROWS rows; dy is summed per lane over its own columns, then across the warp in a fixed butterfly.
+constexpr int EIG_ROWS = 8;
+template <typename T, bool kRagged>
+__global__ void __launch_bounds__(256)
+embed_input_bwd_kernel(const T* __restrict__ dout, const float* __restrict__ Wx, const float* __restrict__ wy,
+                       float* __restrict__ dx, float* __restrict__ dy, int rows, int train_rows, int F, int E, int B,
+                       const int* __restrict__ n_keys) {
+  const int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int r0 = warp * EIG_ROWS; r0 < rows; r0 += nwarps * EIG_ROWS) {
+    float a0[EIG_ROWS], a1[EIG_ROWS], ay[EIG_ROWS];
+#pragma unroll
+    for (int r = 0; r < EIG_ROWS; ++r) { a0[r] = 0.f; a1[r] = 0.f; ay[r] = 0.f; }
+    for (int e0 = 0; e0 < E; e0 += 32) {
+      const int e = e0 + lane;
+      const float wye = e < E ? wy[e] : 0.f;
+      float dv[EIG_ROWS];
+#pragma unroll
+      for (int r = 0; r < EIG_ROWS; ++r) {
+        dv[r] = (e < E && r0 + r < rows) ? to_f32<T>(dout[static_cast<size_t>(r0 + r) * E + e]) : 0.f;
+        ay[r] = fmaf(dv[r], wye, ay[r]);
+      }
+      const int n = min(32, E - e0);
+      for (int k = 0; k < n; ++k) {
+        const float* wrow = Wx + static_cast<size_t>(e0 + k) * F;
+        const float w0 = lane < F ? wrow[lane] : 0.f;
+        const float w1 = lane + 32 < F ? wrow[lane + 32] : 0.f;
+#pragma unroll
+        for (int r = 0; r < EIG_ROWS; ++r) {
+          const float d = __shfl_sync(0xffffffffu, dv[r], k);
+          a0[r] = fmaf(d, w0, a0[r]);
+          a1[r] = fmaf(d, w1, a1[r]);
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < EIG_ROWS; ++r) {
+      const int row = r0 + r;
+      const float sy = warp_sum(ay[r]);
+      if (row < rows) {
+        if (lane < F) dx[static_cast<size_t>(row) * F + lane] = a0[r];
+        if (lane + 32 < F) dx[static_cast<size_t>(row) * F + lane + 32] = a1[r];
+        if (lane == 0) dy[row] = embed_train_row<kRagged>(row, train_rows, B, rows / B, n_keys) ? sy : 0.f;
+      }
     }
   }
 }
@@ -541,6 +594,32 @@ extern "C" int pfn_embed_ragged_bwd(const void* dout, int dtype, const float* x,
   PFN_CHECK_ARG(n_keys != nullptr, "embed_ragged_bwd: null n_keys");
   return embed_bwd<true>(dout, dtype, x, y, dWx, dbx, dwy, dby, T, B, F, E, 0, n_keys,
                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pfn_embed_input_bwd(const void* dout, int dtype, const float* Wx, const float* wy, float* dx, float* dy,
+                                   int T, int B, int F, int E, int sep, const int* n_keys, void* stream) {
+  PFN_CHECK_ARG(T > 0 && B > 0 && F > 0 && E > 0, "embed_input_bwd: bad shape T=%d B=%d F=%d E=%d", T, B, F, E);
+  PFN_CHECK_ARG(F <= 64, "embed_input_bwd: F=%d > 64 (the fused embedding's limit)", F);
+  PFN_CHECK_ARG(n_keys != nullptr || (sep >= 0 && sep <= T), "embed_input_bwd: sep %d outside [0,%d]", sep, T);
+  PFN_CHECK_ARG(dtype == PFN_F32 || dtype == PFN_BF16, "embed_input_bwd: bad dtype %d", dtype);
+  PFN_CHECK_ARG(dout && Wx && wy && dx && dy, "embed_input_bwd: null pointer");
+  PFN_CHECK_ARG(static_cast<long long>(T) * B * (E > F ? E : F) < (1LL << 31), "embed_input_bwd: too many rows");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int rows = T * B, train_rows = n_keys ? 0 : sep * B;
+  long long grid = (static_cast<long long>(rows) + 8 * EIG_ROWS - 1) / (8 * EIG_ROWS);
+  if (grid > 16LL * num_sms()) grid = 16LL * num_sms();
+  const int g = static_cast<int>(grid);
+  if (dtype == PFN_F32) {
+    const float* d = reinterpret_cast<const float*>(dout);
+    if (n_keys) embed_input_bwd_kernel<float, true><<<g, 256, 0, s>>>(d, Wx, wy, dx, dy, rows, train_rows, F, E, B, n_keys);
+    else embed_input_bwd_kernel<float, false><<<g, 256, 0, s>>>(d, Wx, wy, dx, dy, rows, train_rows, F, E, B, nullptr);
+  } else {
+    const __nv_bfloat16* d = reinterpret_cast<const __nv_bfloat16*>(dout);
+    if (n_keys) embed_input_bwd_kernel<__nv_bfloat16, true><<<g, 256, 0, s>>>(d, Wx, wy, dx, dy, rows, train_rows, F, E, B, n_keys);
+    else embed_input_bwd_kernel<__nv_bfloat16, false><<<g, 256, 0, s>>>(d, Wx, wy, dx, dy, rows, train_rows, F, E, B, nullptr);
+  }
+  PFN_LAUNCH_OK();
+  return 0;
 }
 
 // Vector-path launches: LnRing's CTAs per SM, no more than the rows need.  An SM has 228 KB of shared memory, of which

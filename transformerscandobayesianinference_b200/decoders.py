@@ -27,6 +27,11 @@ def _rows(x, precision):
     return x.reshape(-1, x.shape[-1]).to(engine.act_dtype(precision))
 
 
+def _frozen(params, frozen):
+    """The head's parameters in the order its engine function takes them, detached when frozen."""
+    return [p.detach() if frozen else p for p in params]
+
+
 class ScaledDecoder(nn.Module):
     """Logits divided by a per-row temperature, the softmax-weighted mean of TEMPERATURES under 10 learned logits.
 
@@ -45,10 +50,12 @@ class ScaledDecoder(nn.Module):
     def forward(self, x):
         return self.fused(_rows(x, engine.default_precision()), x.shape[:-1], engine.default_precision())
 
-    def fused(self, h, lead, precision):
-        """h [N, ninp] in the activation dtype of `precision` -> logits [*lead, nout] fp32."""
-        out, temp = engine.ScaledDecoderFn.apply(h, self.linear.weight, self.linear.bias, self.linear1.weight,
-                                                 self.linear1.bias, self.linear2.weight, self.linear2.bias, precision)
+    def fused(self, h, lead, precision, frozen=False):
+        """h [N, ninp] in the activation dtype of `precision` -> logits [*lead, nout] fp32.  frozen: the parameters are
+        constants of the call (a backward reaches h only)."""
+        params = _frozen((self.linear.weight, self.linear.bias, self.linear1.weight, self.linear1.bias, self.linear2.weight,
+                          self.linear2.bias), frozen)
+        out, temp = engine.ScaledDecoderFn.apply(h, *params, precision)
         temps = temp.view(lead)
         if random.random() > .99:
             print(temps.shape, temps[:, :2] if temps.dim() >= 2 else temps[:2])
@@ -66,8 +73,10 @@ class FixedScaledDecoder(nn.Module):
     def forward(self, x):
         return self.fused(_rows(x, engine.default_precision()), x.shape[:-1], engine.default_precision())
 
-    def fused(self, h, lead, precision):
-        """h [N, ninp] in the activation dtype of `precision` -> logits [*lead, nout] fp32."""
-        out = engine.FixedScaledDecoderFn.apply(h, self.mapper[0].weight, self.mapper[0].bias, self.mapper[2].weight,
-                                                self.mapper[2].bias, self.T, precision)
+    def fused(self, h, lead, precision, frozen=False):
+        """h [N, ninp] in the activation dtype of `precision` -> logits [*lead, nout] fp32.  frozen: the parameters are
+        constants of the call (a backward reaches h only)."""
+        params = _frozen((self.mapper[0].weight, self.mapper[0].bias, self.mapper[2].weight, self.mapper[2].bias, self.T),
+                         frozen)
+        out = engine.FixedScaledDecoderFn.apply(h, *params, precision)
         return out.view(*lead, out.shape[-1])

@@ -14,7 +14,7 @@ import os
 
 import torch
 
-from . import _lib as L, _lib_ragged as LR, _lib_ragged_train as LRT
+from . import _lib as L, _lib_input_grad as LIG, _lib_ragged as LR, _lib_ragged_train as LRT
 
 LAYER_PARAM_NAMES = ("in_w", "in_b", "out_w", "out_b", "w1", "b1", "w2", "b2", "g1", "be1", "g2", "be2")
 N_LAYER_PARAMS = len(LAYER_PARAM_NAMES)
@@ -372,9 +372,67 @@ def query_stack(src, kv, n, B, nhead, precision, *params, n_keys=None):
     return h
 
 
+class QueryStackFn(torch.autograd.Function):
+    """query_stack with a backward to its input only: src [m*B, E] -> the query rows' output of the encoder layers against
+    the cache kv.  The cache and every parameter are constants here: the backward runs the dgrad chain of each layer
+    (LayerNorm, MLP, out-projection, context attention, in-projection) and forms no weight or bias gradient, so a
+    parameter's .grad is left as it was.  The forward runs the kernels of query_stack, the context attention in its
+    variant that also writes lse, so its output is query_stack's bit for bit."""
+
+    @staticmethod
+    def forward(ctx, src, kv, n, B, nhead, precision, n_keys, *params):
+        dt, n_layers, dh, h = _stack_start(src, precision, nhead, params, kv)
+        m = h.shape[0] // B
+        saved = []
+        for li in range(n_layers):
+            P, (in_w, out_w, w1, w2), qkv, attn = _layer_qkv(h, params, li, dt)
+            lse = torch.empty(B * nhead, m, device=h.device, dtype=torch.float32)
+            LIG.attention_ctx_grad_fwd(qkv, kv[li], attn, lse, m, n, B, nhead, dh, n_keys)
+            z1, mean1, rstd1, h1, u, u_is_grad, g, z2, mean2, rstd2, h2 = _layer_tail(h, attn, P, out_w, w1, w2, None, li)
+            saved.append((qkv, attn, lse, z1, mean1, rstd1, u, z2, mean2, rstd2, in_w, out_w, w1, w2))
+            h = h2
+        ctx.saved_acts = saved
+        ctx.u_is_grad = u_is_grad if n_layers else False
+        ctx.params = params
+        ctx.meta = (kv, n, B, nhead, precision, n_keys)
+        return h
+
+    @staticmethod
+    def backward(ctx, dout):
+        if ctx.saved_acts is None:
+            raise RuntimeError("QueryStackFn: activations were already released by a previous backward "
+                               "(retain_graph=True is not supported)")
+        kv, n, B, nhead, precision, n_keys = ctx.meta
+        dh2 = dout.contiguous().to(act_dtype(precision))
+        N, E = dh2.shape
+        m, dh = N // B, E // nhead
+        for li in reversed(range(len(ctx.saved_acts))):
+            P = _layer(ctx.params, li)
+            qkv, attn, lse, z1, mean1, rstd1, u, z2, mean2, rstd2, in_w, out_w, w1, w2 = ctx.saved_acts[li]
+            ctx.saved_acts[li] = None
+            dz2 = torch.empty_like(z2)
+            L.layernorm_bwd(dh2, z2, mean2, rstd2, P["g2"], dz2, None, None)
+            du = _gelu_linear_dgrad(dz2, w2, u, ctx.u_is_grad)
+            dh1 = _linear_dgrad(du, w1, aux=dz2)
+            del dz2, du, u, z2
+            dz1 = torch.empty_like(z1)
+            L.layernorm_bwd(dh1, z1, mean1, rstd1, P["g1"], dz1, None, None)
+            dattn = _linear_dgrad(dz1, out_w)
+            del dh1, z1
+            dqkv = torch.empty_like(qkv)
+            delta = torch.empty_like(lse)
+            LIG.attention_ctx_bwd(qkv, kv[li], attn, lse, dattn, dqkv, delta, m, n, B, nhead, dh, n_keys)
+            del dattn, attn, qkv
+            dh2 = _linear_dgrad(dqkv, in_w, aux=dz1)
+            del dqkv, dz1
+        ctx.saved_acts = None
+        return (dh2,) + (None,) * (6 + len(ctx.params))
+
+
 class EmbedFn(torch.autograd.Function):
     """(x [T,B,F], y [T,B]) -> src [T*B, E]:  x Wx^T + bx + (t < sep)(y wy + by)   (reference transformer.py:68-74);
-    with a RaggedSeps `sep`, (t < n_keys[b]) for dataset b."""
+    with a RaggedSeps `sep`, (t < n_keys[b]) for dataset b.  The backward returns the gradients of x (every row) and y
+    (the rows with the y embedding, zero elsewhere) when they are asked for, and of the weights when those are."""
 
     @staticmethod
     def forward(ctx, x, y, Wx, bx, wy, by, sep, precision):
@@ -382,6 +440,7 @@ class EmbedFn(torch.autograd.Function):
         T, B, F = x.shape
         E = Wx.shape[0]
         x = x.detach().contiguous().float()
+        y_shape = y.shape
         y = y.detach().contiguous().float()
         out = torch.empty(T * B, E, device=x.device, dtype=act_dtype(precision))
         args = (x, y, Wx.detach().contiguous(), bx.detach().contiguous(), wy.detach().contiguous().view(-1),
@@ -390,24 +449,36 @@ class EmbedFn(torch.autograd.Function):
             LRT.embed_ragged_fwd(*args, sep.n_keys)
         else:
             L.embed_fwd(*args, sep)
-        ctx.save_for_backward(x, y)
-        ctx.meta = (T, B, F, E, sep, wy.shape)
+        ctx.save_for_backward(x, y, args[2], args[4])
+        ctx.meta = (T, B, F, E, sep, wy.shape, y_shape)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        x, y = ctx.saved_tensors
-        T, B, F, E, sep, wy_shape = ctx.meta
+        x, y, Wx, wy = ctx.saved_tensors
+        T, B, F, E, sep, wy_shape, y_shape = ctx.meta
         dev = dout.device
+        dout = dout.contiguous()
+        ragged = isinstance(sep, RaggedSeps)
+        dx = dy = None
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            dx = torch.empty(T, B, F, device=dev)
+            dy = torch.empty(T * B, device=dev)
+            LIG.embed_input_bwd(dout, Wx, wy, dx, dy, T, B, F, E, sep.s_max if ragged else sep,
+                                sep.n_keys if ragged else None)
+            dx = dx if ctx.needs_input_grad[0] else None
+            dy = dy.view(y_shape) if ctx.needs_input_grad[1] else None
+        if not any(ctx.needs_input_grad[2:6]):
+            return dx, dy, None, None, None, None, None, None
         dWx = torch.zeros(E, F, device=dev)
         dbx = torch.zeros(E, device=dev)
         dwy = torch.zeros(E, device=dev)
         dby = torch.zeros(E, device=dev)
-        if isinstance(sep, RaggedSeps):
-            LRT.embed_ragged_bwd(dout.contiguous(), x, y, dWx, dbx, dwy, dby, T, B, F, E, sep.n_keys)
+        if ragged:
+            LRT.embed_ragged_bwd(dout, x, y, dWx, dbx, dwy, dby, T, B, F, E, sep.n_keys)
         else:
-            L.embed_bwd(dout.contiguous(), x, y, dWx, dbx, dwy, dby, T, B, F, E, sep)
-        return None, None, dWx, dbx, dwy.view(wy_shape), dby, None, None
+            L.embed_bwd(dout, x, y, dWx, dbx, dwy, dby, T, B, F, E, sep)
+        return dx, dy, dWx, dbx, dwy.view(wy_shape), dby, None, None
 
 
 def _f32_rows(rows, n, dev):
@@ -436,6 +507,12 @@ def _head_bwd(dz, hq, u, g, u_is_grad, w0, w2, grads):
     return _linear_dgrad(du, w0)
 
 
+def _head_dgrad(dz, u, u_is_grad, w0, w2):
+    """dL/dhq of _head_fwd with its weights held constant (a head called with frozen parameters): the two dgrad GEMMs of
+    _head_bwd alone, no weight gradient and no gradient bucket."""
+    return _linear_dgrad(_gelu_linear_dgrad(dz, w2, u, u_is_grad), w0)
+
+
 class DecoderFn(torch.autograd.Function):
     """hq [Nq, E] -> logits [Nq, n_out] fp32:  GELU(hq W0^T + b0) W2^T + b2  (reference transformer.py:23,85),
     applied to the query rows only (the reference computes all T rows and slices, transformer.py:91)."""
@@ -459,6 +536,8 @@ class DecoderFn(torch.autograd.Function):
         Nq, n_out = dlogits.shape
         dl = torch.zeros(Nq, (n_out + 7) // 8 * 8, device=dev, dtype=act_dtype(ctx.precision))
         dl[:, :n_out] = dlogits
+        if not any(ctx.needs_input_grad[1:5]):
+            return (_head_dgrad(dl[:, :n_out], u, ctx.u_is_grad, w0, w2),) + (None,) * 5
         flat, grads = _flat_grads(dev, W0.shape, W0.shape[:1], W2.shape, W2.shape[:1])
         dhq = _head_bwd(dl[:, :n_out], hq, u, g, ctx.u_is_grad, w0, w2, grads)
         _bucket_ready(flat)
@@ -506,6 +585,8 @@ class ScaledDecoderFn(torch.autograd.Function):
         nz = n_out + L.HEAD_TEMPS
         dlogits, dzz = _head_grad_rows(dlogits, nz, act_dtype(precision))
         L.scaled_head_bwd(dlogits, zz, temp, n_out, dzz, dzz.shape[1])
+        if not any(ctx.needs_input_grad[1:7]):
+            return (_head_dgrad(dzz[:, :nz], u, ctx.u_is_grad, w, w12),) + (None,) * 7
         # [W1; W2] and [b1; b2] are contiguous in the bucket, so the stacked GEMM writes both layers' gradients in place
         flat, grads = _flat_grads(hq.device, w_shape, w_shape[:1], (nz, nhid), (nz,))
         dhq = _head_bwd(dzz[:, :nz], hq, u, g, ctx.u_is_grad, w, w12, grads)
@@ -541,8 +622,12 @@ class FixedScaledDecoderFn(torch.autograd.Function):
         precision, w0_shape, w2_shape, t_shape = ctx.meta
         n_out = w2_shape[0]
         dlogits, dz = _head_grad_rows(dlogits, n_out, act_dtype(precision))
-        flat, grads = _flat_grads(hq.device, w0_shape, w0_shape[:1], w2_shape, w2_shape[:1], t_shape)
-        L.fixed_scaled_head_bwd(dlogits, z, S, n_out, dz, grads[4], dz.shape[1])
+        frozen = not any(ctx.needs_input_grad[1:6])
+        flat, grads = _flat_grads(hq.device, *((t_shape,) if frozen else (w0_shape, w0_shape[:1], w2_shape, w2_shape[:1],
+                                                                          t_shape)))
+        L.fixed_scaled_head_bwd(dlogits, z, S, n_out, dz, grads[-1], dz.shape[1])
+        if frozen:
+            return (_head_dgrad(dz[:, :n_out], u, ctx.u_is_grad, w0, w2),) + (None,) * 6
         dhq = _head_bwd(dz[:, :n_out], hq, u, g, ctx.u_is_grad, w0, w2, grads[:4])
         _bucket_ready(flat)
         return (dhq, *grads, None)

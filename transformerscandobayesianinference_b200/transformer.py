@@ -8,7 +8,9 @@ never called.  `forward()` routes embedding -> encoder stack -> decoder through 
 For inference against one training set, `encode_context(x_train, y_train)` runs the training rows once and keeps every
 layer's K and V of them; `predict(ctx, x_query)` then scores any number of query sets against that context.  Under the
 single_eval_pos mask a training row attends only to training rows and a query row to the training rows and itself, so
-`predict` returns what `forward` returns for the concatenated sequence at single_eval_pos = n.  With
+`predict` returns what `forward` returns for the concatenated sequence at single_eval_pos = n.  `predict` is
+differentiable in x_query (with the context and the parameters held constant), so candidate points can be optimised by
+gradient against one cached context; `forward` is differentiable in x and y as the reference's module is.  With
 `encode_context(x_train, y_train, n_train)` the datasets of one batch have training sets of their own sizes: dataset b
 uses rows [0, n_train[b]) and the rows after them are padding that never reaches an output.
 
@@ -39,7 +41,9 @@ class TrainingContext:
     """What `TransformerModel.encode_context` keeps of n training rows: `kv` [nlayers, n*B, 2*E] holds each layer's K | V
     of the rows (token row t*B + b, the model's activation dtype), plus the shapes and the precision it was made with.
     `n_train` is None when every dataset has all n rows, else the int32 [B] device tensor of each dataset's row count.
-    It holds no weights: `predict` uses the model it is called on.  `predict` never writes to it."""
+    It holds no weights: `predict` uses the model it is called on.  `predict` never writes to it, and a backward through
+    `predict` treats it as a constant: no gradient reaches the training rows through it (differentiate `forward` on the
+    concatenated sequence for that)."""
     __slots__ = ("kv", "n", "B", "E", "nhead", "nlayers", "precision", "device", "n_train")
 
     def __init__(self, kv, n, B, E, nhead, nlayers, precision, device, n_train=None):
@@ -88,6 +92,18 @@ def is_per_dataset(single_eval_pos):
 def dataset_seps(single_eval_pos, T, B, who="forward"):
     """The per-dataset single_eval_pos (B integers in [0, T]) as a tuple of ints; ValueError otherwise."""
     return _dataset_ints(single_eval_pos, T, B, who, "single_eval_pos", "values", "the sequence length")
+
+
+def _call_params(linear, frozen):
+    """(weight, bias) of an nn.Linear, detached when frozen."""
+    return (linear.weight.detach(), linear.bias.detach()) if frozen else (linear.weight, linear.bias)
+
+
+def _call_module(module, frozen, x):
+    """module(x), with every parameter of the module detached for the call when frozen."""
+    if not frozen:
+        return module(x)
+    return torch.func.functional_call(module, {k: p.detach() for k, p in module.named_parameters()}, (x,))
 
 
 class TransformerModel(nn.Module):
@@ -149,16 +165,17 @@ class TransformerModel(nn.Module):
                 and isinstance(d[1], nn.GELU) and getattr(d[1], 'approximate', 'none') == 'none'
                 and isinstance(d[2], nn.Linear) and d[0].bias is not None and d[2].bias is not None)
 
-    def _embed(self, x_src, y_src, sep):
+    def _embed(self, x_src, y_src, sep, frozen=False):
         """[T*B, E] activation-dtype input of the encoder stack: the x embedding of every row plus the y embedding of the
-        rows t < sep (t < n_keys[b] in dataset b for an engine.RaggedSeps)."""
+        rows t < sep (t < n_keys[b] in dataset b for an engine.RaggedSeps).  frozen: the encoders' parameters are
+        constants of the call, so a backward reaches the inputs only."""
         T, B = x_src.shape[0], x_src.shape[1]
         precision = self.precision
         if self._fused_embed_ok():
-            return engine.EmbedFn.apply(x_src, y_src, self.encoder.weight, self.encoder.bias, self.y_encoder.weight,
-                                        self.y_encoder.bias, sep, precision)
-        xs = self.encoder(x_src)
-        ys = self.y_encoder(y_src.unsqueeze(-1) if y_src.dim() == 2 else y_src)
+            return engine.EmbedFn.apply(x_src, y_src, *_call_params(self.encoder, frozen),
+                                        *_call_params(self.y_encoder, frozen), sep, precision)
+        xs = _call_module(self.encoder, frozen, x_src)
+        ys = _call_module(self.y_encoder, frozen, y_src.unsqueeze(-1) if y_src.dim() == 2 else y_src)
         if isinstance(sep, engine.RaggedSeps):
             train = torch.arange(T, device=xs.device).unsqueeze(1) < sep.n_keys.to(xs.device)
             h = torch.where(train.unsqueeze(-1), xs + ys, xs)
@@ -176,18 +193,19 @@ class TransformerModel(nn.Module):
             params.extend(engine.layer_params(layer))
         return params
 
-    def _decode(self, hq, rows, B):
-        """Logits [rows, B, n_out] of the decoder on the output hq [rows*B, E] of the query rows."""
+    def _decode(self, hq, rows, B, frozen=False):
+        """Logits [rows, B, n_out] of the decoder on the output hq [rows*B, E] of the query rows.  frozen: the decoder's
+        parameters are constants of the call."""
         precision = self.precision
         if self._default_decoder():
-            out = engine.DecoderFn.apply(hq, self.decoder[0].weight, self.decoder[0].bias, self.decoder[2].weight,
-                                         self.decoder[2].bias, precision)
+            out = engine.DecoderFn.apply(hq, *_call_params(self.decoder[0], frozen), *_call_params(self.decoder[2], frozen),
+                                         precision)
         elif isinstance(self.decoder, (decoders.ScaledDecoder, decoders.FixedScaledDecoder)):
-            out = self.decoder.fused(hq, (rows, B), precision)
+            out = self.decoder.fused(hq, (rows, B), precision, frozen)
         else:
             # any other head runs as its own torch ops on the sequence-first [T - sep, B, E] rows, the shape the reference
             # hands its decoder (reference transformer.py:85)
-            out = self.decoder(hq.float().view(rows, B, -1))
+            out = _call_module(self.decoder, frozen, hq.float().view(rows, B, -1))
         return out.reshape(rows, B, -1)
 
     @staticmethod
@@ -212,7 +230,8 @@ class TransformerModel(nn.Module):
         one per dataset (a sequence, or an integer tensor on any device): dataset b's rows then attend under
         generate_D_q_matrix at its own value, the y embedding is added to its rows t < single_eval_pos[b], and the
         result has T - min(single_eval_pos) rows; `query_rows` marks which are the queries.  B equal values run the
-        scalar path."""
+        scalar path.  The logits are differentiable in x and y (src) as well as in the parameters: y's gradient is zero
+        on the query rows t >= single_eval_pos[b], which have no y embedding."""
         assert single_eval_pos is not None, 'Single eval pos is required now.'
         assert isinstance(src, tuple), 'the fused x/y input mode cannot be combined with single_eval_pos'
         x_src, y_src = src
@@ -286,7 +305,7 @@ class TransformerModel(nn.Module):
     def encode_context(self, x_train, y_train, n_train=None):
         """Run the n training rows x_train [n, B, F], y_train [n, B] (n >= 0) through the embedding and every encoder
         layer on their own (they never attend to a query row) and return a `TrainingContext` holding each layer's K and
-        V of them.  No autograd.  With n = 0 a query attends only to itself, as in forward(..., single_eval_pos=0).
+        V of them.  No autograd: the context is a constant of every `predict`.  With n = 0 a query attends only to itself, as in forward(..., single_eval_pos=0).
 
         n_train (optional): B integers in [0, n], a sequence or an integer tensor on any device.  Dataset b then has the
         training rows [0, n_train[b]) and `predict` gives its queries what forward gives them on those rows alone, at
@@ -321,8 +340,13 @@ class TransformerModel(nn.Module):
 
     def predict(self, ctx, x_query):
         """Logits [m, B, n_out] of the query rows x_query [m, B, F] (m >= 1) given the training rows `ctx` holds: what
-        forward((cat(x_train, x_query), cat(y_train, anything)), single_eval_pos=n) returns.  No autograd; `ctx` is only
-        read, so one context serves any number of calls."""
+        forward((cat(x_train, x_query), cat(y_train, anything)), single_eval_pos=n) returns.  `ctx` is only read, so one
+        context serves any number of calls.
+
+        With grad mode on and x_query.requires_grad the call builds a graph whose backward reaches x_query only: the
+        context and every parameter of the model are constants of it, so a parameter's .grad is left as it was (with the
+        cached K / V held fixed a weight gradient would only be a partial derivative).  The logits are the same bits
+        either way; otherwise no graph is built."""
         self._check_context_inference()
         if not isinstance(ctx, TrainingContext):
             raise ValueError(f"predict: ctx must be a TrainingContext from encode_context, got {type(ctx).__name__}")
@@ -336,6 +360,11 @@ class TransformerModel(nn.Module):
             if have != value:
                 raise ValueError(f"predict: the context's {name} is {have} but the model and queries have {value}")
         _require_cuda_input(x_query, "predict")
+        if torch.is_grad_enabled() and x_query.requires_grad:
+            h = self._embed(x_query, x_query.new_zeros(m, B), 0, frozen=True)
+            h = engine.QueryStackFn.apply(h, ctx.kv, ctx.n, B, self.nhead, self.precision, ctx.n_train,
+                                          *(p.detach() for p in self._layer_params()))
+            return self._decode(h, m, B, frozen=True)
         with torch.no_grad():
             h = self._embed(x_query, x_query.new_zeros(m, B), 0)
             h = engine.query_stack(h, ctx.kv, ctx.n, B, self.nhead, self.precision, *self._layer_params(),
